@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- Diffuman4D window denoise-steps/sec on B200 (BASELINE.json metric).
+"""bench.py -- Diffuman4D window denoise-steps/sec on one H100 (BASELINE.json metric).
 
 A "step" is ONE window denoise step of the reference's sliding-window sampler
 (pipeline_diffuman4d.py:369-425): input assembly -> UNet forward on 2F images (CFG) -> CFG combine -> F per-frame
@@ -13,8 +13,10 @@ weights of the real architecture (no network for the checkpoint).
         the line also carries a `sharded` object: ONE window frame-sharded over the N ranks, SURVEY 8e.2)
     python bench.py --impl reference ...   (the CPU oracle -- the reference's torch graph restated -- on host cores,
         REAL W16 window steps, as many of the requested --steps as fit the time budget)
+    python bench.py --gpus 1 --steps 10 --warmup 3 --dump-outputs DIR   (also writes the last timed step's outputs as
+        DIR/<name>.npy, so that two builds can be compared output for output on identical seeded inputs)
 
-Everything printed is measured in this run; figures that come from a committed profile name the file they were read from.
+Everything printed is measured in this run.
 """
 from __future__ import annotations
 
@@ -22,7 +24,6 @@ import argparse
 import ctypes as C
 import json
 import os
-import re
 import subprocess
 import sys
 import threading
@@ -37,13 +38,13 @@ WORKLOAD = dict(name="demo_4d_tiny spatial window W16 (4 cond + 12 target frames
                 F=16, n_cond=4, h=64, w=64, guidance=2.0, domain="spatial", n_steps=18)
 # other BASELINE configurations, timed at N=1 as `also` entries (not the headline)
 ALSO = [dict(key="W24_temporal_64", name="temporal window W24 (12 cond + 12 target frames), CFG 2.0, latents 64x64",
-             F=24, n_cond=12, h=64, w=64, domain="temporal", steps=5),
+             F=24, n_cond=12, h=64, w=64, domain="temporal"),
         dict(key="W16_spatial_128", name="spatial window W16, CFG 2.0, latents 128x128 (reference default, 1024^2 px)",
-             F=16, n_cond=4, h=128, w=128, domain="spatial", steps=3)]
+             F=16, n_cond=4, h=128, w=128, domain="spatial")]
 METRIC = "unet_window_denoise_steps_per_sec"
 UNIT = "window-steps/s"
-# ncu --set full capture of the dominant kernel (tools/gpu_profile.sh -> tools/ncu_summary.py); parsed at run time
-NCU_SUMMARIES = ["profiles/r02_ncu_attention.txt", "profiles/r01d_ncu_attention.txt"]
+# NVIDIA's data-sheet dense BF16 rate of the H100 SXM (700 W); a card with a lower power limit sustains less
+H100_BF16_DENSE_TFLOPS = 989.0
 
 
 def synth_inputs(F, n_cond, h, w, pose=True, seed=0):
@@ -91,23 +92,25 @@ class ClockSampler(threading.Thread):
                 "samples": len(self.samples)}
 
 
-def ncu_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum of the dominant kernel, read from the newest committed ncu summary
-    (never a literal): returns (bytes, file) or (None, None)."""
-    for rel in NCU_SUMMARIES:
-        path = os.path.join(ROOT, rel)
-        if not os.path.exists(path):
-            continue
-        tot, found = 0.0, 0
-        for line in open(path):
-            m = re.match(r"\s*dram__bytes_(read|write)\.sum\s+([0-9.]+)\s+(\w+)", line)
-            if m and found < 2:   # first kernel block of the file
-                mult = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}.get(m.group(3), 1.0)
-                tot += float(m.group(2)) * mult
-                found += 1
-        if found == 2:
-            return int(tot), rel
-    return None, None
+def gpu_identity(index):
+    """Name, power limit and maximum SM clock of the measured card (they are part of every number of this run)."""
+    try:
+        o = subprocess.run(["nvidia-smi", f"--id={index}", "--query-gpu=name,power.limit,clocks.max.sm",
+                            "--format=csv,noheader"], capture_output=True, text=True, timeout=10).stdout
+        name, power, clock = [x.strip() for x in o.strip().split(",")][:3]
+        return {"name": name, "power_limit": power, "sm_max_clock": clock}
+    except Exception:  # noqa: BLE001
+        return {"name": torch.cuda.get_device_name(index), "power_limit": None, "sm_max_clock": None}
+
+
+def dump_outputs(out_dir, arrays):
+    """Write each array as out_dir/<name>.npy (float32, or float64 for integer arrays)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        t = t.detach().cpu()
+        a = t.double().numpy() if not t.dtype.is_floating_point else t.float().numpy()
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 # ------------------------------------------------------------------------------------------------------- CPU arm
@@ -218,12 +221,12 @@ def run_ours(args):
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200: there is no CPU fallback for the product path")
+        raise SystemExit("bench.py needs an H100: there is no CPU fallback for the product path")
     torch.cuda.set_device(local)
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     if not os.path.exists(os.path.join(ROOT, "diffuman4d_b200", "libd4d.so")):
-        d4d_build.build(test_lib=False)
+        d4d_build.build()
     dev = torch.device("cuda", local)
     cfg = UNetConfig.sd21()
     wl = WORKLOAD
@@ -237,7 +240,7 @@ def run_ours(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:  # noqa: BLE001
         pass
-    peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)
+    peak_tf = peaks.get("bf16_tflops_sustained", H100_BF16_DENSE_TFLOPS)
 
     def barrier():
         if world > 1:
@@ -280,7 +283,7 @@ def run_ours(args):
     # ================= headline: replicas (N=1: the single window) =================
     full_inputs = synth_inputs(F, wl["n_cond"], h, w, seed=rank)
     host = {k: (v.to(torch.bfloat16) if v.dtype.is_floating_point else v).pin_memory() for k, v in full_inputs.items()}
-    step_resident, lat_res, _ = make_stepper(pipe, full_inputs, wl["domain"])
+    step_resident, lat_res, ts_res = make_stepper(pipe, full_inputs, wl["domain"])
 
     out_host = torch.empty_like(host["latents"]).pin_memory()
     ts_host = torch.empty_like(host["ts"]).pin_memory()
@@ -320,6 +323,9 @@ def run_ours(args):
     sampler.start()
     ms_res = timed(step_resident, args.steps, max(args.warmup, 3))
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        # what the timed path returned in its last step: the updated latents and timestep indices of the window
+        dump_outputs(args.dump_outputs, {"latents": lat_res, "timestep_indices": ts_res})
     ms_e2e = timed(step_e2e, args.steps, 1)
     assert torch.isfinite(out_host.float()).all(), "non-finite latents out of the window step"
 
@@ -348,14 +354,10 @@ def run_ours(args):
     achieved = alg[top] / (kind_ms[top] * 1e-3) / 1e12
     launches_fwd = unet.forward_launches(2, B, F, h, w)
     launches_step = launches_fwd + 3   # + assemble, cfg-skeleton, cfg+ddim kernels (2 memcpys not counted)
-    traffic, traffic_file = (ncu_traffic() if (world == 1 and names[top] == "attention") else (None, None))
     roofline = {"bound": "tensor", "kernel": names[top], "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s",
                 "frac": achieved / peak_tf,
-                "traffic": traffic,
-                "traffic_note": (f"dram__bytes_read.sum + dram__bytes_write.sum of ONE captured launch, parsed at run time from "
-                                 f"{traffic_file} (ncu --set full); not re-measured in this run" if traffic_file else
-                                 "no ncu capture consulted in this run"),
-                "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else "fallback 1.4 PFLOP/s sustained",
+                "peak_source": ("MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else
+                                "H100 SXM data-sheet dense BF16 (700 W); not reached"),
                 "launches_per_forward": int(n_k[top]), "ms_per_forward": kind_ms[top],
                 "by_kind_ms": {names[k]: round(kind_ms[k], 4) for k in range(6)},
                 "by_kind_tflops": {names[k]: round(alg[k] / (kind_ms[k] * 1e-3) / 1e12, 1) for k in (0, 1, 2)},
@@ -376,11 +378,11 @@ def run_ours(args):
                    "(pose encoder + frame-index embedding), no attn2", "images_per_step": B,
                    "parallelism": (f"replicas x{world} (independent windows, no collective)" if world > 1 else "single GPU"),
                    "l2": f"no explicit flush: one step streams ~{unet.workspace_bytes(2, B, F, h, w) / 2**30:.1f} GiB of "
-                         "activations + 1.6 GB of weights through a 126 MB L2"},
+                         "activations + 1.6 GB of weights through a 50 MB L2"},
         "tflops_per_step": fl["total"] / 1e12,
         "unet_tflops_achieved": fl["total"] / (ms_res / args.steps * 1e-3) / 1e12,
         "unet_roofline_frac": fl["total"] / (ms_res / args.steps * 1e-3) / 1e12 / peak_tf,
-        "roofline": roofline, "clocks": clocks,
+        "roofline": roofline, "clocks": clocks, "gpu": gpu_identity(local),
         "e2e": {"value": e2e_val, "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                 "ms_per_step": ms_e2e / args.steps},
         "gpu_launches": launches_step * args.steps,
@@ -425,11 +427,11 @@ def run_ours(args):
                 Fa, ha, wa = a["F"], a["h"], a["w"]
                 pipe.parepare_schedulers(wl["n_steps"], Fa)
                 stp, _, _ = make_stepper(pipe, synth_inputs(Fa, a["n_cond"], ha, wa, seed=1), a["domain"])
-                ms_a = timed(stp, a["steps"], 2)
+                ms_a = timed(stp, args.steps, 2)
                 fa = unet_flops(cfg, 2 * Fa, Fa, ha, wa)["total"]
-                also[a["key"]] = {"workload": a["name"], "value": a["steps"] / (ms_a * 1e-3), "unit": UNIT,
-                                  "ms_per_step": ms_a / a["steps"], "steps": a["steps"], "tflops_per_step": fa / 1e12,
-                                  "unet_roofline_frac": fa / (ms_a / a["steps"] * 1e-3) / 1e12 / peak_tf}
+                also[a["key"]] = {"workload": a["name"], "value": args.steps / (ms_a * 1e-3), "unit": UNIT,
+                                  "ms_per_step": ms_a / args.steps, "steps": args.steps, "tflops_per_step": fa / 1e12,
+                                  "unet_roofline_frac": fa / (ms_a / args.steps * 1e-3) / 1e12 / peak_tf}
                 del stp
                 torch.cuda.empty_cache()
             except Exception as e:  # noqa: BLE001
@@ -470,7 +472,7 @@ def gpu_eager_baseline(cfg, sd, inputs, dev, steps):
             denoise_window_oracle(unet, sched, latents=d["latents"].clone(), pixel_latents=d["pixel"], plucker=d["plucker"],
                                   skeletons=d["skel"], cond_mask=d["mask"], timestep_indices=d["ts"], domain=WORKLOAD["domain"],
                                   guidance_scale=WORKLOAD["guidance"])
-        n = max(3, min(steps, 10))
+        n = steps
         for _ in range(2):
             step()
         torch.cuda.synchronize()
@@ -493,13 +495,16 @@ def gpu_eager_baseline(cfg, sd, inputs, dev, steps):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--steps", type=int, default=10,
+                    help="timed steps of the headline, e2e, `also` and GPU eager-baseline loops (the CPU baseline times one step)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-eager-baseline", action="store_true")
     ap.add_argument("--no-sharded", action="store_true", help="N>1: skip the frame-sharded `sharded` object")
     ap.add_argument("--quick", action="store_true", help="N=1: headline only (no `also`, no baselines)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (latents, timestep indices) as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -16,9 +16,6 @@ EXPORTS = [
     "d4d_op_attention", "d4d_op_groupnorm", "d4d_op_conv3x3_groupnorm", "d4d_op_conv_resample", "d4d_op_layernorm", "d4d_debug_tap", "d4d_exchange_alloc",
     "d4d_exchange_open", "d4d_unet_forward_sharded", "d4d_denoise_window_sharded",
 ]
-# extra symbols of the tools build libd4d_test.so (include/d4d_test.h): never part of the product library
-TEST_EXPORTS = ["d4d_op_probe_umma", "d4d_microbench"]
-TEST_LIB_PATH = os.path.join(_HERE, "libd4d_test.so")
 
 
 class D4DConfig(C.Structure):
@@ -44,37 +41,23 @@ class D4DError(RuntimeError):
 
 
 _lib = None
-_test_lib = None
 
 
 def lib() -> C.CDLL:
-    """Load libd4d.so (built by ``python -m diffuman4d_b200.build`` / ``__graft_entry__.build()``).
-    ``D4D_USE_TEST_LIB=1`` (tools/ablate_*.py, tools/microbench.py) swaps in the tools build for the whole process."""
+    """Load libd4d.so (built by ``python -m diffuman4d_b200.build`` / ``__graft_entry__.build()``)."""
     global _lib
-    if _lib is not None:
-        return _lib
-    if os.environ.get("D4D_USE_TEST_LIB") == "1":
-        _lib = test_lib()
-        return _lib
-    _lib = _load(LIB_PATH, False)
+    if _lib is None:
+        _lib = _load(LIB_PATH)
     return _lib
 
 
-def test_lib() -> C.CDLL:
-    """libd4d_test.so: same ABI plus the probe / microbenchmark kernels and the ablation switches."""
-    global _test_lib
-    if _test_lib is None:
-        _test_lib = _load(TEST_LIB_PATH, True)
-    return _test_lib
-
-
-def _load(path: str, with_test: bool) -> C.CDLL:
+def _load(path: str) -> C.CDLL:
     if not os.path.exists(path):
         raise ImportError(
             f"{path} not found: the CUDA extension is the product and there is no CPU fallback. "
             "Build it with `python -m diffuman4d_b200.build`.")
     l = C.CDLL(path)
-    vp, i32, i64p, f32, f32p, u32 = C.c_void_p, C.c_int, C.POINTER(C.c_int64), C.c_float, C.c_void_p, C.c_uint32
+    vp, i32, i64p, f32, f32p = C.c_void_p, C.c_int, C.POINTER(C.c_int64), C.c_float, C.c_void_p
     l.d4d_last_error.restype = C.c_char_p
     l.d4d_last_error.argtypes = []
     l.d4d_version.restype = C.c_int
@@ -104,11 +87,6 @@ def _load(path: str, with_test: bool) -> C.CDLL:
     l.d4d_op_layernorm.argtypes = [vp, i32, i32, f32, f32p, f32p, vp, vp]
     l.d4d_debug_tap.argtypes = [vp, vp, vp, vp, C.POINTER(C.c_int32), i32, i32, i32, i32, i32, i32, vp, C.c_char_p,
                                 C.POINTER(C.c_int32), vp]
-    if with_test:
-        l.d4d_op_probe_umma.argtypes = [vp, vp, vp, i32, i32, i32, i32, u32, u32, u32, vp]
-        l.d4d_op_probe_umma.restype = C.c_int
-        l.d4d_microbench.argtypes = [i32, i32, i32, i32, vp, vp, vp]
-        l.d4d_microbench.restype = C.c_int
     l.d4d_exchange_alloc.argtypes = [vp, C.c_size_t, vp]
     l.d4d_exchange_open.argtypes = [vp, i32, i32, vp]
     l.d4d_unet_forward_sharded.argtypes = [vp, vp, vp, vp, C.POINTER(C.c_int32), i32, i32, i32, i32, i32, i32, vp, vp]

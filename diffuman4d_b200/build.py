@@ -1,10 +1,5 @@
-"""Build libd4d.so (sm_100a) in-tree with nvcc.  No torch, no CPU fallback: the product is this library.
-
-Two libraries come out of the same sources:
-  libd4d.so       the product (include/d4d.h): no measurement kernels, no ablation switches, no environment reads
-                  on the data path
-  libd4d_test.so  tools build (-DD4D_TEST_KERNELS -DD4D_ABLATE): additionally exports the UMMA probe and the
-                  microbenchmarks (include/d4d_test.h) and honours D4D_GEMM_ABLATE / D4D_ATTN_ABLATE
+"""Build libd4d.so (sm_90a, H100) in-tree with nvcc.  No torch, no CPU fallback: the product is this library
+(include/d4d.h); it reads no environment variables on the data path.
 
     python -m diffuman4d_b200.build          # incremental
     python -m diffuman4d_b200.build --force
@@ -20,12 +15,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_obj")
 LIB = os.path.join(HERE, "libd4d.so")
-TEST_LIB = os.path.join(HERE, "libd4d_test.so")
-SOURCES = ["tmap.cu", "gemm_umma.cu", "attention_umma.cu", "attention_d64.cu", "norm.cu", "elementwise.cu", "unet.cu", "d4d_api.cu"]
-TEST_SOURCES = SOURCES + ["probe.cu", "microbench.cu"]
-TEST_DEFS = ["-DD4D_TEST_KERNELS", "-DD4D_ABLATE", "-DD4D_SPIN_LIMIT=(1u<<21)"]  # tools build: a protocol bug traps within seconds
+SOURCES = ["tmap.cu", "gemm_wgmma.cu", "attention_wgmma.cu", "norm.cu", "elementwise.cu", "unet.cu", "d4d_api.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-std=c++17", "-O3", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-Xcompiler", "-fPIC",
+FLAGS = ["-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-Xcompiler", "-fPIC",
          "-diag-suppress", "177"]
 
 
@@ -38,12 +30,12 @@ def _deps_mtime() -> float:
     return t
 
 
-def _compile(src: str, force: bool, hdr_t: float, test: bool = False) -> str:
-    obj = os.path.join(OBJ, src.replace(".cu", ".test.o" if test else ".o"))
+def _compile(src: str, force: bool, hdr_t: float) -> str:
+    obj = os.path.join(OBJ, src.replace(".cu", ".o"))
     s = os.path.join(CSRC, src)
     if not force and os.path.exists(obj) and os.path.getmtime(obj) >= max(os.path.getmtime(s), hdr_t):
         return obj
-    cmd = [NVCC, *FLAGS, *(TEST_DEFS if test else []), "-I", CSRC, "-c", s, "-o", obj]
+    cmd = [NVCC, *FLAGS, "-I", CSRC, "-c", s, "-o", obj]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"nvcc failed for {src}:\n{r.stdout}\n{r.stderr}")
@@ -53,7 +45,7 @@ def _compile(src: str, force: bool, hdr_t: float, test: bool = False) -> str:
 def _link(lib: str, objs, force: bool) -> bool:
     need_link = force or not os.path.exists(lib) or any(os.path.getmtime(o) > os.path.getmtime(lib) for o in objs)
     if need_link:
-        cmd = [NVCC, "-shared", "-o", lib, *objs, "-cudart", "static", "-gencode", "arch=compute_100a,code=sm_100a",
+        cmd = [NVCC, "-shared", "-o", lib, *objs, "-cudart", "static", "-gencode", "arch=compute_90a,code=sm_90a",
                "-Xlinker", "--exclude-libs,ALL"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
@@ -61,17 +53,14 @@ def _link(lib: str, objs, force: bool) -> bool:
     return need_link
 
 
-def build(force: bool = False, verbose: bool = True, test_lib: bool = True) -> str:
+def build(force: bool = False, verbose: bool = True) -> str:
     os.makedirs(OBJ, exist_ok=True)
     hdr_t = _deps_mtime()
-    jobs = [(s, False) for s in SOURCES] + ([(s, True) for s in TEST_SOURCES] if test_lib else [])
     with cf.ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 4)) as ex:
-        objs = list(ex.map(lambda j: _compile(j[0], force, hdr_t, j[1]), jobs))
-    linked = _link(LIB, objs[:len(SOURCES)], force)
-    if test_lib:
-        linked = _link(TEST_LIB, objs[len(SOURCES):], force) or linked
+        objs = list(ex.map(lambda s: _compile(s, force, hdr_t), SOURCES))
+    linked = _link(LIB, objs, force)
     if verbose:
-        print(f"[d4d] {'built' if linked else 'up to date'}: {LIB}" + (f" + {os.path.basename(TEST_LIB)}" if test_lib else ""))
+        print(f"[d4d] {'built' if linked else 'up to date'}: {LIB}")
     return LIB
 
 

@@ -1,5 +1,5 @@
-// Shared device/host helpers for the sm_100a kernels: PTX wrappers for mbarrier, TMA
-// (cp.async.bulk.tensor), tcgen05 (UMMA + TMEM), descriptors, and host-side error plumbing.
+// Shared device/host helpers for the sm_90a kernels: PTX wrappers for mbarrier, TMA (cp.async.bulk.tensor), register
+// reallocation, and host-side error plumbing.  The warpgroup MMA wrappers are in wgmma.cuh.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -88,20 +88,6 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Non-blocking probe (mbarrier.test_wait never suspends the thread).  A completed try_wait still costs ~200 cycles of
-// latency on sm_100 (microbench kind 18); probing the NEXT barrier before a long stretch of independent work and
-// falling back to mbar_wait only when the probe failed takes that latency off the critical path.
-__device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.b32 %0, 1, 0, p;\n\t}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
 // Bounded wait: a protocol bug must trap (-> cudaErrorLaunchFailure) instead of hanging the GPU box.
 #ifndef D4D_SPIN_LIMIT
 #define D4D_SPIN_LIMIT (1u << 26)
@@ -117,26 +103,17 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
-// Same bound without the printf: vprintf is a real call, and a call in a warp that holds > 128 live registers (the
-// head_dim-64 attention softmax) makes ptxas save them around it; the trap alone still turns a protocol bug into
-// cudaErrorLaunchFailure instead of a hang.
-__device__ __forceinline__ void mbar_wait_quiet(uint64_t* bar, uint32_t parity) {
-  uint32_t spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    if (++spins > D4D_SPIN_LIMIT) __trap();
-  }
-}
-
 // ---- proxies / fences ----------------------------------------------------------------------
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
 // programmatic dependent launch (see launch_pdl in kernels.h): wait for the predecessor grid's memory, then let the successor
 // grid become resident
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// warpgroup-wide register reallocation: producer warpgroups give registers back, MMA warpgroups take them
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // ---- TMA -----------------------------------------------------------------------------------
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* t) {
@@ -175,101 +152,6 @@ template <int N> __device__ __forceinline__ void bulk_wait_group() {  // <= N gr
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
-// ---- TMEM ----------------------------------------------------------------------------------
-// Allocation is warp-collective; the base address is written to *slot (shared memory).
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]      kind::f16 (bf16/fp16 inputs, fp32 accumulate)
-__device__ __forceinline__ void umma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]
-__device__ __forceinline__ void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-// (tcgen05.commit implies tcgen05.fence::before_thread_sync.)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// 32 lanes x 16 consecutive fp32 columns -> 16 registers per thread (thread i <-> TMEM lane base+i)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-      "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ---- descriptors -----------------------------------------------------------------------------
-// Instruction descriptor, kind::f16: bf16 x bf16 -> fp32, M x N tile, majors: 0 = K-major, 1 = MN-major.
-__host__ __device__ __forceinline__ uint32_t make_idesc_bf16(uint32_t M, uint32_t N, uint32_t a_mn_major,
-                                                             uint32_t b_mn_major) {
-  uint32_t d = 0;
-  d |= 1u << 4;                 // D format: F32
-  d |= 1u << 7;                 // A format: BF16
-  d |= 1u << 10;                // B format: BF16
-  d |= (a_mn_major & 1u) << 15;
-  d |= (b_mn_major & 1u) << 16;
-  d |= ((N >> 3) & 0x3Fu) << 17;
-  d |= ((M >> 4) & 0x1Fu) << 24;
-  return d;
-}
-// Shared-memory matrix descriptor (sm_100 format, version 1).  layout_type: 0 none, 2 = 128B swizzle,
-// 4 = 64B, 6 = 32B.  Offsets in bytes.
-__host__ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                            uint32_t layout_type) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFFu);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= 1ull << 46;  // descriptor version (sm_100)
-  d |= static_cast<uint64_t>(layout_type & 7u) << 61;
-  return d;
-}
-
 // ---- misc math ---------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
@@ -280,57 +162,18 @@ __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
   return __bfloat1622float2(v);
 }
 __device__ __forceinline__ float silu_f(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
-// ---- packed fp32x2 helpers (sm_100a FFMA2 / FMUL2 / FADD2) ----
-__device__ __forceinline__ uint64_t f2_pack(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void f2_unpack(uint64_t v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t f2_fma(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ uint64_t f2_mul(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ uint64_t f2_add(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ uint64_t f2_splat(float v) { return f2_pack(v, v); }
-
-// exact-erf GELU on a pair with ONE MUFU per element:  gelu(g) = relu(g) - 0.5 |g| erfc(|g| / sqrt 2), and
-// -log2 erfc(u / sqrt 2) is so close to a polynomial that  erfc(u / sqrt 2) = 2^-(d1 u + d2 u^2 + ... + d5 u^5)  holds to
-// 7e-7 absolute in the GELU (fit of tools/fit_gelu.py; the polynomial is increasing, so large |g| underflow to 0 cleanly).
-// 2 MUFU.EX2 + 8 packed FMA-pipe ops + 4 ALU ops per PAIR (Abramowitz-Stegun 7.1.26 needed 4 MUFU + 12 FMA and made the
-// GEGLU epilogue MUFU-bound).  Returns a * gelu(g) for both lanes.
-__device__ __forceinline__ uint64_t geglu2(uint64_t a2, uint64_t g2) {
-  float g0, g1;
-  f2_unpack(g2, g0, g1);
-  const uint64_t u = f2_pack(fabsf(g0), fabsf(g1));
-  uint64_t q = f2_fma(f2_splat(-4.8811754095e-04f), u, f2_splat(7.1988063864e-03f));  // negated: p = -(d1 u + ... + d5 u^5)
-  q = f2_fma(q, u, f2_splat(-5.2146803588e-02f));
-  q = f2_fma(q, u, f2_splat(-4.5959571004e-01f));
-  q = f2_fma(q, u, f2_splat(-1.1510006189e+00f));
-  float p0, p1, e0, e1;
-  f2_unpack(f2_mul(q, u), p0, p1);
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(p0));
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(p1));
-  const uint64_t relu = f2_pack(fmaxf(g0, 0.f), fmaxf(g1, 0.f));
-  const uint64_t gelu = f2_fma(f2_mul(u, f2_splat(-0.5f)), f2_pack(e0, e1), relu);
-  return f2_mul(a2, gelu);
-}
-__device__ __forceinline__ float gelu_erf_f(float x) {
-  float lo, hi;
-  f2_unpack(geglu2(f2_splat(1.0f), f2_splat(x)), lo, hi);
-  return lo;
+// exact-erf GELU with ONE MUFU:  gelu(g) = relu(g) - 0.5 |g| erfc(|g| / sqrt 2), and -log2 erfc(u / sqrt 2) is so close to a
+// polynomial that  erfc(u / sqrt 2) = 2^-(d1 u + d2 u^2 + ... + d5 u^5)  holds to 7e-7 absolute in the GELU (least-squares
+// fit; the polynomial is increasing, so large |g| underflow to 0 cleanly).
+__device__ __forceinline__ float gelu_erf_f(float g) {
+  const float u = fabsf(g);
+  float q = fmaf(-4.8811754095e-04f, u, 7.1988063864e-03f);  // negated: p = -(d1 u + ... + d5 u^5)
+  q = fmaf(q, u, -5.2146803588e-02f);
+  q = fmaf(q, u, -4.5959571004e-01f);
+  q = fmaf(q, u, -1.1510006189e+00f);
+  float e;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(q * u));
+  return fmaf(-0.5f * u, e, fmaxf(g, 0.f));
 }
 #endif  // __CUDACC__
 

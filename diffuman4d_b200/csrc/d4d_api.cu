@@ -81,8 +81,8 @@ int d4d_create(const d4d_config* cfg, int device, d4d_handle** out) {
   D4D_REQUIRE(device >= 0 && device < ndev, "device index out of range");
   cudaDeviceProp prop;
   D4D_CUDA_OK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    d4d::set_error("libd4d requires an sm_100a (Blackwell B200) device; found compute capability " +
+  if (prop.major != 9 || prop.minor != 0) {
+    d4d::set_error("libd4d requires an sm_90a (Hopper H100) device; found compute capability " +
                    std::to_string(prop.major) + "." + std::to_string(prop.minor));
     return 2;
   }
@@ -353,24 +353,6 @@ int d4d_debug_tap(d4d_handle* h, const void* sample, const int64_t* timestep, co
                              static_cast<bf16*>(out), name64, dims3, static_cast<cudaStream_t>(stream));
   D4D_API_END
 }
-
-#ifdef D4D_TEST_KERNELS  // libd4d_test.so only (include/d4d_test.h)
-int d4d_op_probe_umma(const void* A, const void* B, float* D, int N, int K, int a_src, int b_major, uint32_t b_lbo,
-                      uint32_t b_sbo, uint32_t b_kadv, void* stream) {
-  D4D_API_BEGIN
-  return d4d::probe_umma_run(static_cast<const bf16*>(A), static_cast<const bf16*>(B), D, N, K, a_src, b_major, b_lbo,
-                             b_sbo, b_kadv, static_cast<cudaStream_t>(stream));
-  D4D_API_END
-}
-
-int d4d_microbench(int kind, int warps, int iters, int blocks, uint64_t* cycles_dev, float* sink_dev, void* stream) {
-  D4D_API_BEGIN
-  return d4d::microbench_run(kind, warps, iters, blocks, reinterpret_cast<unsigned long long*>(cycles_dev), sink_dev,
-                             static_cast<cudaStream_t>(stream));
-  D4D_API_END
-}
-
-#endif  // D4D_TEST_KERNELS
 
 int d4d_unet_forward_sharded(d4d_handle* h, const void* sample, const int64_t* timestep, const void* skeletons,
                              const int32_t* domain_ids, int n_domains, int B_local, int F_local, int F_total, int height,

@@ -154,7 +154,7 @@ __global__ void pose_conv0_kernel(const bf16* __restrict__ x, int n, int H, int 
 // ---------------------------------------------------------------------------------------------
 // pose encoder, layers 1-4 (conv_layers.2/4/6/8: 3->16 k4 s2, 16->16 k3, 16->32 k4 s2, 32->32 k3; pad 1, SiLU): implicit
 // GEMM on the warp-level tensor-core path (mma.sync m16n8k16, bf16 x bf16 -> fp32).  These layers are 1-3 GMAC each on
-// 16/32 output channels - far too narrow for a tcgen05 tile (the UNet's convs use csrc/gemm_umma.cu) but, one thread per
+// 16/32 output channels - far too narrow for a wgmma tile (the UNet's convs use csrc/gemm_wgmma.cu) but, one thread per
 // pixel on the FMA pipe, they cost more than a whole 3x3 conv of the UNet.  Here a warp owns 32 output pixels (2 M tiles)
 // x all COUT channels; K = taps x CIN runs in chunks of 16.  The A fragment of m16n8k16 is, per lane, two adjacent
 // channels of one pixel at one tap = one 4-byte load straight from the NHWC activation (L1 keeps the 9-16x tap reuse);
@@ -463,7 +463,7 @@ int pose_conv_run(const bf16* x, int n, int Cin, int H, int W, const bf16* w, co
   const long long total = static_cast<long long>(n) * Ho * Wo;
   D4D_REQUIRE(static_cast<long long>(n) * H * W * Cin < (1ll << 31) && total * Cout < (1ll << 31), "pose conv: 32-bit offsets");
   D4D_REQUIRE(reinterpret_cast<uintptr_t>(w) % 16 == 0, "pose conv weights must be 16-byte aligned");
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int threads = 256;
@@ -508,12 +508,12 @@ int assemble_input_run(const AssembleArgs& a, cudaStream_t stream) {
 
 int broadcast_neg_images_run(const bf16* small, long long per_img, int F, bf16* full, cudaStream_t stream) {
   D4D_REQUIRE(per_img % 8 == 0 && F > 0, "broadcast_neg_images arguments");
-  broadcast_neg_images_kernel<<<148 * 8, 256, 0, stream>>>(small, per_img / 8, F, full);
+  broadcast_neg_images_kernel<<<132 * 8, 256, 0, stream>>>(small, per_img / 8, F, full);
   D4D_CUDA_OK(cudaGetLastError());
   return 0;
 }
 int fill_bf16_run(bf16* p, long long n, float v, cudaStream_t stream) {
-  fill_bf16_kernel<<<148 * 4, 256, 0, stream>>>(p, n, v);
+  fill_bf16_kernel<<<132 * 4, 256, 0, stream>>>(p, n, v);
   D4D_CUDA_OK(cudaGetLastError());
   return 0;
 }

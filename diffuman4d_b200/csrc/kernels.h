@@ -11,15 +11,14 @@
 namespace d4d {
 
 // --------------------------------------------------------------------------------------------
-// tcgen05 GEMM / implicit-GEMM conv3x3  (gemm_umma.cu)
+// wgmma GEMM / implicit-GEMM conv3x3  (gemm_wgmma.cu)
 // --------------------------------------------------------------------------------------------
 // fixed-point scales of the fused GroupNorm statistics: |sum| < 2^35 (|x| <= 2e6 over 16384 pixels), sum of squares < 2^39
-// (rms |x| <= 5800 over 16384 pixels); resolutions 3.7e-9 / 6e-8 per 32-row partial
+// (rms |x| <= 5800 over 16384 pixels); resolutions 3.7e-9 / 6e-8 per 16-row partial
 constexpr float kGnSumScale = 268435456.f;  // 2^28
 constexpr float kGnSqScale = 16777216.f;    // 2^24
 
 struct GemmKernelArgs {
-  int dbg;  // ablation switches (tools/ablate_gemm.py); 0 in production
   int M, N, k_blocks, block_n, n_tiles, m_tiles;
   int mode;      // 0 plain, 1 implicit-GEMM convolution over NHWC (tap table below; TMA zero fill = padding)
   int kb_split;  // plain: k-blocks served by A (rest by A2)
@@ -40,8 +39,6 @@ struct GemmKernelArgs {
   bf16* out;
   int ldo;
   int geglu;
-  int tma_store;    // 1: 32-row x 32-column epilogue units leave through TMA stores (tmap_out) instead of st.global
-  int stg_bufs;     // staging buffers per epilogue warp (1 or 2; the second one costs a ring stage, gemm_umma.cu)
   int act;          // 0 none, 1 SiLU applied to (acc + bias + rowvec) before scale/residual
   float out_scale;  // multiplies (acc + bias + rowvec) after the activation
   // fused GroupNorm statistics of the OUTPUT tensor: per (image, column) sum and sum of squares in 64-bit FIXED POINT
@@ -74,7 +71,7 @@ struct GemmDesc {
   int geglu = 0;
   int act = 0;
   float out_scale = 1.0f;
-  int block_n = 0;  // 0 = auto
+  int block_n = 0;  // 0 = auto (64, 128 or 256; the last N tile may overhang)
   // GroupNorm statistics of the output (see GemmKernelArgs::stats); plain GEMM: stats_rows = rows per image
   long long* stats = nullptr;
   int stats_rows = 0;
@@ -93,24 +90,17 @@ struct GemmDesc {
 };
 
 struct GemmLaunch {
-  CUtensorMap tmap_a, tmap_a2, tmap_b, tmap_out;
+  CUtensorMap tmap_a, tmap_a2, tmap_b;
   GemmKernelArgs args;
   int grid;
 };
 
-// largest divisor of N that is a multiple of `mult` and <= 256 (0 if none)
-inline int gemm_pick_block_n(int N, int mult) {
-  int best = 0;
-  for (int bn = mult; bn <= 256; bn += mult)
-    if (N % bn == 0) best = bn;
-  return best;
-}
 int gemm_prepare(const GemmDesc& d, GemmLaunch* L);
 int gemm_run(const GemmLaunch& L, cudaStream_t stream);
 double gemm_flops(const GemmLaunch& L);
 
 // --------------------------------------------------------------------------------------------
-// tcgen05 flash attention forward (attention_umma.cu)
+// wgmma flash attention forward (attention_wgmma.cu)
 //   q/k/v are column slices of one row-major [tokens, ld] bf16 matrix (the fused QKV GEMM output);
 //   head hd of batch b covers rows [b*S, (b+1)*S) and columns [hd*D, (hd+1)*D) of each slice.
 // --------------------------------------------------------------------------------------------
@@ -223,29 +213,6 @@ struct KvFlagArgs {
 int kv_signal_run(const KvFlagArgs& a, cudaStream_t stream);
 int kv_wait_run(const KvFlagArgs& a, cudaStream_t stream);
 
-#ifdef D4D_TEST_KERNELS  // measurement / probe kernels: only in libd4d_test.so (build.py), never in the product library
-// device microbenchmarks (microbench.cu)
-int microbench_run(int kind, int warps, int iters, int blocks, unsigned long long* cycles_dev, float* sink_dev, cudaStream_t s);
-
-// UMMA operand-encoding probe (probe.cu)
-int probe_umma_run(const bf16* A, const bf16* B, float* D, int N, int K, int a_src, int b_major, uint32_t b_lbo,
-                   uint32_t b_sbo, uint32_t b_kadv, cudaStream_t stream);
-#endif
-
-// Ablation switches (tools/ablate_*.py) exist only in the tools build (-DD4D_ABLATE, libd4d_test.so); in the product
-// library the tests below are compile-time false and no environment variable is read.
-#ifdef D4D_ABLATE
-#define D4D_DBG(args, bit) (((args).dbg & (bit)) != 0)
-#define D4D_DBGV(args) ((args).dbg)
-inline int ablate_env(const char* name) {
-  const char* e = getenv(name);
-  return e ? atoi(e) : 0;
-}
-#else
-#define D4D_DBG(args, bit) false
-#define D4D_DBGV(args) 0
-#endif
-
 // per-device "opt in to large dynamic smem" helper.  `once` holds one flag per device ordinal; the reference drives one
 // pipeline per GPU from its own thread (sampling_runner.py:36-43), so the first launches may race: std::call_once.
 struct PerDeviceOnce {
@@ -263,20 +230,9 @@ inline int ensure_dyn_smem(F func, int bytes, PerDeviceOnce& once) {
 }
 
 // Programmatic dependent launch: the kernel may become resident while its predecessor in the stream drains; it must
-// execute pdl_wait() (common.cuh) before touching anything a predecessor wrote.  Measured on the W16 step: 46.63 ms with the
-// attribute vs 46.55 ms without (the kernels are long enough that launch gaps do not show), so the product library leaves
-// it off; the tools build (libd4d_test.so) turns it on with D4D_PDL=1.
-inline bool pdl_enabled() {
-#ifdef D4D_ABLATE
-  static const bool on = [] {
-    const char* e = getenv("D4D_PDL");
-    return e && e[0] == '1';
-  }();  // thread-safe one-time initialisation
-  return on;
-#else
-  return false;
-#endif
-}
+// execute pdl_wait() (common.cuh) before touching anything a predecessor wrote.  The attribute is left off (serialised
+// launches): the kernels of a forward are long enough that launch gaps do not show.
+inline bool pdl_enabled() { return false; }
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
   cudaLaunchConfig_t cfg = {};

@@ -32,7 +32,7 @@ struct GnArgs {
   float* final_stats;   // [n_img][groups][2] = (mean, rstd), written by the last stats CTA of each image
   unsigned int* counters;  // [n_img] arrival counters (self-resetting)
   // fused-statistics mode (groupnorm_apply_run): per-(image, channel) {sum, sum of squares} of each source, accumulated by
-  // the epilogue of the GEMM / conv that produced it (gemm_umma.cu); the apply kernel derives (mean, rstd) itself
+  // the epilogue of the GEMM / conv that produced it (gemm_wgmma.cu); the apply kernel derives (mean, rstd) itself
   const long long* ch_stats1;  // fixed point (kGnSumScale, kGnSqScale)
   const long long* ch_stats2;
 };
@@ -413,7 +413,7 @@ int groupnorm_apply_run(const bf16* x1, int C1, const long long* stats1, const b
   // one wave of CTAs (2 per SM): every CTA pays the group-statistics prologue once, so fewer and longer CTAs than the
   // stand-alone path (which sizes its slabs for the partials it has to merge)
   {
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     int sp = (2 * sms) / n_img;

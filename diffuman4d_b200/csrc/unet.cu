@@ -3,7 +3,7 @@
 // Mirrors UNetMultiviewConditionModel.forward (reference unet_multiview_condition.py:501-598) and the block
 // wiring of unet_multiview_blocks.py:233-712 / transformer_multiview.py:79-232 / attention.py:22-153 as a
 // static launch plan per (domains, B, F, h, w): NHWC bf16 activations end to end, one arena, every FLOP in the
-// tcgen05 GEMM / conv / attention kernels, norms and layout glue in 128-bit HBM kernels.  The channel concat
+// wgmma GEMM / conv / attention kernels, norms and layout glue in 128-bit HBM kernels.  The channel concat
 // of the up path, the (b t) hw c <-> b (t hw) c rearranges and the NCHW<->token permutes of the reference are
 // address arithmetic here.
 #include "unet.h"
@@ -355,20 +355,17 @@ int Model::finalize() {
       x.a2 = attnw(b + ".attn2", C, heads, x.d, x.dpad);
     }
     x.ln3 = normw(b + ".norm3", C);
-    // GEGLU interleave: N tile t of width bn holds a[t*bn/2 .. ) | g[t*bn/2 .. )
-    const int N = 8 * C, bn = gemm_pick_block_n(N, 32), half = bn / 2;
-    x.ff1_bn = bn;
+    // GEGLU interleave in groups of 8 rows: rows 16p .. 16p+7 = a[8p .. 8p+7], rows 16p+8 .. 16p+15 = g[8p .. 8p+7]
+    const int N = 8 * C;
     const auto& w = T(b + ".ff.net.0.proj.weight");
     const auto& bb = T(b + ".ff.net.0.proj.bias");
     std::vector<float> wi(w.size()), bi(bb.size());
-    for (int t = 0; t < N / bn; ++t)
-      for (int j = 0; j < half; ++j) {
-        const int ra = t * half + j, rg = 4 * C + t * half + j;
-        memcpy(&wi[static_cast<size_t>(t * bn + j) * C], &w[static_cast<size_t>(ra) * C], sizeof(float) * C);
-        memcpy(&wi[static_cast<size_t>(t * bn + half + j) * C], &w[static_cast<size_t>(rg) * C], sizeof(float) * C);
-        bi[t * bn + j] = bb[ra];
-        bi[t * bn + half + j] = bb[rg];
-      }
+    for (int r = 0; r < N; ++r) {
+      const int p = r / 16, i = r % 16;
+      const int src = (i < 8 ? 0 : 4 * C) + 8 * p + (i & 7);
+      memcpy(&wi[static_cast<size_t>(r) * C], &w[static_cast<size_t>(src) * C], sizeof(float) * C);
+      bi[r] = bb[src];
+    }
     x.ff1.w = up_bf16(wi);
     x.ff1.b = up_f32(bi);
     x.ff1.in = C;
@@ -776,7 +773,7 @@ class PlanBuilder {
     {
       GemmDesc d;
       d.A = n; d.lda = C; d.K1 = C; d.Wt = x.ff1.w; d.M = M; d.N = 8 * C; d.bias = x.ff1.b; d.out = g; d.ldo = 4 * C;
-      d.geglu = 1; d.block_n = x.ff1_bn;
+      d.geglu = 1;
       gemm(d);
     }
     release(n);

@@ -31,7 +31,7 @@ struct XfW {
   LinW pin, pout, ff1, ff2;
   AttnW a1, a2;
   bool has2 = false;
-  int C = 0, heads = 0, d = 0, dpad = 0, ff1_bn = 0;
+  int C = 0, heads = 0, d = 0, dpad = 0;
 };
 struct PoseW {
   LinW conv[8];   // layers 0..5 direct layout [k*k][Cin][Cout]; 5 -> GEMM layout [Cout][16*Cin]; 6,7 conv3x3 layout

@@ -2,7 +2,7 @@
 
 Reference: src/samplers/utils/sampling_utils.py:17-51 (``_target_`` of configs/model/diffuman4d.yaml:1).  A config
 file ``configs/model/diffuman4d_b200.yaml`` with ``_target_: diffuman4d_b200.loader.load_pipelines`` makes the
-reference's ``inference.py`` build B200 pipelines without source edits (see INTEGRATION.md).
+reference's ``inference.py`` build the CUDA pipelines without source edits (see INTEGRATION.md).
 
 Reads the diffusers-layout checkpoint directory:  ``unet/config.json``, ``unet/diffusion_pytorch_model.safetensors``
 and ``scheduler/scheduler_config.json``.  No network access is attempted here; if ``huggingface_hub`` is importable the
@@ -24,11 +24,11 @@ from .unet import B200MultiviewUNet
 
 
 def unet_config_from_json(d: dict) -> UNetConfig:
-    """Map a diffusers ``unet/config.json`` onto ``UNetConfig``; refuse knobs the B200 path does not implement."""
+    """Map a diffusers ``unet/config.json`` onto ``UNetConfig``; refuse knobs the CUDA path does not implement."""
     def want(key, allowed, default):
         v = d.get(key, default)
         if v not in allowed:
-            raise NotImplementedError(f"unet config {key}={v!r} is not supported by the B200 path (supported: {allowed})")
+            raise NotImplementedError(f"unet config {key}={v!r} is not supported by the CUDA path (supported: {allowed})")
         return v
 
     want("act_fn", ("silu", "swish"), "silu")
@@ -63,7 +63,7 @@ def scheduler_config_from_json(d: dict) -> SchedulerConfig:
     cls = d.get("_class_name", "DDIMScheduler")
     if cls != "DDIMScheduler":
         raise NotImplementedError(
-            f"scheduler {cls} is not fused on the B200 path (DDIM epsilon / v_prediction / sample only); "
+            f"scheduler {cls} is not fused on the CUDA path (DDIM epsilon / v_prediction / sample only); "
             "run the reference's Python scheduler loop for other classes")
     if d.get("thresholding", False):
         raise NotImplementedError("dynamic thresholding is not supported")

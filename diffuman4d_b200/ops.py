@@ -6,7 +6,7 @@ from typing import Optional
 
 import torch
 
-from ._lib import check, lib, test_lib
+from ._lib import check, lib
 
 
 def _p(t: Optional[torch.Tensor]):
@@ -26,7 +26,8 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, 
          rowvec: Optional[torch.Tensor] = None, rows_per_image: int = 0, residual: Optional[torch.Tensor] = None,
          geglu: bool = False, act: int = 0, out_scale: float = 1.0, block_n: int = 0) -> torch.Tensor:
     """out = act((a | a2) @ w.T + bias + rowvec[row // rows_per_image]) * out_scale + residual   (bf16, fp32 accumulate).
-    With ``geglu`` the rows of ``w``/``bias`` must already be tile-interleaved (see ``interleave_geglu``)."""
+    With ``geglu`` the rows of ``w``/``bias`` must already be tile-interleaved (see ``interleave_geglu``);
+    ``block_n`` = 0 picks the tile width, otherwise it must be a multiple of 16 that divides N."""
     _bf16c(a, "a"), _bf16c(w, "w")
     M, K1 = a.shape
     K2 = 0 if a2 is None else a2.shape[1]
@@ -43,27 +44,17 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, 
     return out
 
 
-def pick_block_n(N: int, mult: int = 16) -> int:
-    best = 0
-    for bn in range(mult, 257, mult):
-        if N % bn == 0:
-            best = bn
-    return best
-
-
 def interleave_geglu(w: torch.Tensor, bias: torch.Tensor):
-    """Re-order the rows of a GEGLU projection [2*inner, C] (a rows then g rows) so that N tile t of width bn holds
-    a[t*bn/2:(t+1)*bn/2] followed by the matching g rows (same transform the C++ weight loader applies)."""
+    """Re-order the rows of a GEGLU projection [2*inner, C] (a rows then g rows) in groups of 8: rows 16p..16p+7 are
+    a[8p:8p+8], rows 16p+8..16p+15 the matching g rows (same transform the C++ weight loader applies).  The layout does
+    not depend on the GEMM tile width.  Returns the re-ordered weight and bias."""
     N = w.shape[0]
     inner = N // 2
-    bn = pick_block_n(N, 32)
-    half = bn // 2
     idx = []
-    for t in range(N // bn):
-        idx += list(range(t * half, (t + 1) * half))
-        idx += list(range(inner + t * half, inner + (t + 1) * half))
+    for p in range(inner // 8):
+        idx += list(range(8 * p, 8 * p + 8)) + list(range(inner + 8 * p, inner + 8 * p + 8))
     idx = torch.tensor(idx, device=w.device)
-    return w[idx].contiguous(), bias[idx].contiguous(), bn
+    return w[idx].contiguous(), bias[idx].contiguous()
 
 
 def conv3x3(x_nhwc: torch.Tensor, w_octi: torch.Tensor, bias: Optional[torch.Tensor] = None, *,
@@ -180,12 +171,3 @@ def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: flo
     check(lib().d4d_op_layernorm(_p(x), rows, C, float(eps), _p(gamma), _p(beta), _p(out), _stream()),
           "d4d_op_layernorm")
     return out
-
-
-def probe_umma(A: torch.Tensor, B: torch.Tensor, N: int, K: int, a_src: int, b_major: int, b_lbo: int, b_sbo: int,
-               b_kadv: int) -> torch.Tensor:
-    """UMMA operand-encoding probe: lives in the tools build libd4d_test.so, not in the product library."""
-    D = torch.empty(128, N, device=A.device, dtype=torch.float32)
-    check(test_lib().d4d_op_probe_umma(_p(A), _p(B), _p(D), N, K, a_src, b_major, b_lbo, b_sbo, b_kadv, _stream()),
-          "d4d_op_probe_umma")
-    return D

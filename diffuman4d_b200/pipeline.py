@@ -1,4 +1,4 @@
-"""``B200Diffuman4DPipeline`` -- the denoise part of the reference's ``Diffuman4DPipeline`` on one B200.
+"""``B200Diffuman4DPipeline`` -- the denoise part of the reference's ``Diffuman4DPipeline`` on one H100.
 
 Seams (SURVEY.md section 8b):
   B-3  ``denoise_window``  == ``Diffuman4DPipeline.__call__`` with latents given
@@ -129,7 +129,7 @@ class B200Diffuman4DPipeline:
                  schedulers=None, timesteps=None, timestep_indices=None, guidance_scale: float = 1.0,
                  output_type: str = "latent", **unused):
         if output_type != "latent":
-            raise ValueError("only output_type='latent' is on the B200 path (VAE decode is out of scope)")
+            raise ValueError("only output_type='latent' is on the CUDA path (VAE decode is out of scope)")
         if domains is None or len(domains) != 1:
             raise ValueError("domains must be a one-element list, e.g. ['spatial']")
         F_ = pixel_values_latents.shape[0]

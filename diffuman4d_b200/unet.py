@@ -45,7 +45,7 @@ def _c_config(cfg: UNetConfig) -> D4DConfig:
 
 
 class B200MultiviewUNet:
-    """The UNet of the Diffuman4D denoise step on one B200.  One instance per device (the reference drives one
+    """The UNet of the Diffuman4D denoise step on one H100.  One instance per device (the reference drives one
     pipeline per GPU from its own thread, src/samplers/sampling_runner.py:26-43)."""
 
     def __init__(self, config: UNetConfig, device: Union[int, str, torch.device] = 0):
@@ -70,14 +70,14 @@ class B200MultiviewUNet:
         return self._device
 
     def to(self, *args, **kwargs):
-        """Accepted for interface compatibility (``DiffusionPipeline.to``); the model is pinned to its B200."""
+        """Accepted for interface compatibility (``DiffusionPipeline.to``); the model is pinned to its GPU."""
         for a in list(args) + list(kwargs.values()):
             if isinstance(a, (str, torch.device)) and torch.device(a).type == "cuda":
                 idx = torch.device(a).index
                 if idx is not None and idx != self._device.index:
                     raise ValueError(f"this UNet was created on {self._device}; create a new one for {a}")
             if isinstance(a, torch.dtype) and a not in (torch.bfloat16,):
-                raise ValueError("the B200 path computes in bfloat16 only (reference default, configs/model/diffuman4d.yaml:4)")
+                raise ValueError("the CUDA path computes in bfloat16 only (reference default, configs/model/diffuman4d.yaml:4)")
         return self
 
     def eval(self):

@@ -1,11 +1,11 @@
-/* d4d.h -- C ABI of libd4d.so: the B200-native (sm_100a) replacement of the Diffuman4D denoise-step hot path.
+/* d4d.h -- C ABI of libd4d.so: the H100-native (sm_90a) replacement of the Diffuman4D denoise-step hot path.
  *
  * The reference is pure Python and has no FFI; the seams this ABI stands behind are (SURVEY.md section 8b):
  *   B-2  `pipeline.unet(sample, timestep, skeletons, domains, num_frames)`
- *        /root/reference/src/diffusers/pipelines/diffuman4d/pipeline_diffuman4d.py:398-405
- *        /root/reference/src/diffusers/models/unets/unet_multiview_condition.py:501-598      -> d4d_unet_forward
+ *        src/diffusers/pipelines/diffuman4d/pipeline_diffuman4d.py:398-405
+ *        src/diffusers/models/unets/unet_multiview_condition.py:501-598      -> d4d_unet_forward
  *   B-3  one window denoise step (input assembly + UNet + CFG + per-frame scheduler step)
- *        /root/reference/src/diffusers/pipelines/diffuman4d/pipeline_diffuman4d.py:369-425   -> d4d_denoise_window
+ *        src/diffusers/pipelines/diffuman4d/pipeline_diffuman4d.py:369-425   -> d4d_denoise_window
  *   weights: diffusers-layout state_dict keys of `unet/diffusion_pytorch_model.safetensors`
  *        (loaded by SUTIL load_pipelines, src/samplers/utils/sampling_utils.py:45-50)          -> d4d_load_weight
  * INTEGRATION.md shows the ctypes stub a maintainer of the reference would add.
@@ -122,7 +122,7 @@ int d4d_cfg_ddim_step(const void* noise, const void* latents, const void* cond_m
 
 /* ---- op-level entry points (each is one hot-path kernel; used by tests/ and bench.py) ------------------
  * d4d_op_gemm:   out[M,N] = act((A|A2)[M,K1+K2] . W[N,K]^T + bias + rowvec[row/rows_per_image]) * scale + residual
- *                geglu: W rows / bias interleaved per N tile (see DESIGN.md), out is [M, N/2].
+ *                geglu: W rows / bias interleaved in groups of 8 (a rows, then g rows), out is [M, N/2].
  * d4d_op_conv3x3: NHWC x [n,H,W,Cin], W [Cout][9][Cin] (tap = ky*3+kx), stride 1, pad 1.  */
 int d4d_op_gemm(const void* A, int lda, int K1, const void* A2, int lda2, int K2, const void* W, int M, int N,
                 const float* bias, const void* rowvec, int ld_rowvec, int rows_per_image, const void* residual,

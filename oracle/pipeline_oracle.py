@@ -1,7 +1,7 @@
 """CPU ORACLE (test infrastructure, NOT the product) for the window denoise step and the
 sliding-window loop of ``Diffuman4DPipeline``.
 
-Restates  PIPE = /root/reference/src/diffusers/pipelines/diffuman4d/pipeline_diffuman4d.py:
+Restates  PIPE = src/diffusers/pipelines/diffuman4d/pipeline_diffuman4d.py:
   * ``get_negative_latents``            PIPE:103-113
   * ``get_timestep``                    PIPE:273-278
   * ``__call__`` denoise loop           PIPE:345-425  (input assembly, CFG, per-frame scheduler step)

@@ -6,8 +6,8 @@ cpu_baseline / ``--impl reference`` legs may import this module.
 
 PARITY STATUS: the reference has no tests, golden vectors or fixtures for this path, and
 its leaf arithmetic lives in the un-vendored dependency ``diffusers==0.33.1`` (pinned in
-/root/reference/requirements.txt:5) which is not installed here (no network).  Pinned against
-code RUN from /root/reference (tests/golden/gen_golden.py, fixtures committed, tests in
+requirements.txt:5 of the reference) which is not installed here (no network).  Pinned against
+code RUN from the reference checkout (tests/golden/gen_golden.py, fixtures committed, tests in
 tests/test_oracle.py):
   * the whole UNet wiring -- the reference's own ``UNetMultiviewConditionModel`` constructor and
     forward, its block classes, ``TransformerMultiviewModel``, ``MultiviewTransformerBlock`` and
@@ -25,7 +25,7 @@ Module tree and ``state_dict`` keys follow the diffusers layout so a real checkp
 
 Citations: UNET = src/diffusers/models/unets/unet_multiview_condition.py,
 BLK = .../unets/unet_multiview_blocks.py, TRF = .../transformers/transformer_multiview.py,
-ATT = src/diffusers/models/attention.py, POSE = .../unets/pose_encoder.py (all under /root/reference).
+ATT = src/diffusers/models/attention.py, POSE = .../unets/pose_encoder.py (all in the reference checkout).
 """
 from __future__ import annotations
 

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a B200 GPU (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: test needs an H100 GPU (run with -m gpu on a GPU machine)")
 
 
 @pytest.fixture(scope="session")

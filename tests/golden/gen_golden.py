@@ -1,5 +1,5 @@
-"""Generate golden fixtures by RUNNING code from /root/reference (only possible in the build
-container -- /root/reference does not exist on the GPU box, so the outputs are committed).
+"""Generate golden fixtures by RUNNING code from a checkout of the reference (only possible in a
+container that has one; the GPU tests never read it, so the outputs are committed).
 
 Pinned here:
   pose_encoder.pt   -- the reference ``PoseEncoder`` (src/diffusers/models/unets/pose_encoder.py), imported
@@ -36,7 +36,7 @@ import types
 import torch
 import torch.nn as nn
 
-REF = "/root/reference"
+REF = os.environ.get("DIFFUMAN4D_REFERENCE", "reference")  # path of the reference checkout
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "..", ".."))
 
@@ -46,6 +46,43 @@ def load_by_path(name, path):
     mod = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(mod)
     return mod
+
+
+SHARD_MIN_BYTES = 100_000  # tensors at least this large leave the main file
+SHARD_MAX_BYTES = 900_000  # and are packed into shards of at most this many bytes: no stored file exceeds 1 MB
+
+
+def save_sharded(obj, name):
+    """Save `obj` as {HERE}/<name>.pt with its large tensors moved into {HERE}/<name>.inputs<i>.pt shards (a shard maps the
+    '/'-joined key path of a tensor to the tensor; its place in the main file holds None).  tests/test_oracle.py::_load_golden
+    puts them back.  Stale shards of an earlier run are removed first."""
+    import glob
+    for old in glob.glob(f"{HERE}/{name}.inputs*.pt"):
+        os.remove(old)
+    big = []
+
+    def walk(x, path):
+        if isinstance(x, dict):
+            for k in list(x.keys()):
+                v = x[k]
+                if torch.is_tensor(v) and v.numel() * v.element_size() > SHARD_MIN_BYTES:
+                    big.append(("/".join(path + [str(k)]), v))
+                    x[k] = None
+                else:
+                    walk(v, path + [str(k)])
+    walk(obj, [])
+    shards = []
+    for key, t in sorted(big, key=lambda e: -e[1].numel() * e[1].element_size()):  # first fit, largest first
+        size = t.numel() * t.element_size()
+        for sh in shards:
+            if sum(u.numel() * u.element_size() for _, u in sh) + size <= SHARD_MAX_BYTES:
+                sh.append((key, t))
+                break
+        else:
+            shards.append([(key, t)])
+    for i, sh in enumerate(shards):
+        torch.save({key: t.clone() for key, t in sh}, f"{HERE}/{name}.inputs{i}.pt")
+    torch.save(obj, f"{HERE}/{name}.pt")
 
 
 def gen_pose_encoder():
@@ -446,7 +483,7 @@ def gen_unet():
     except ValueError as e:
         out["num_frames_error"] = str(e)
     print("unet error ->", out["num_frames_error"])
-    torch.save(out, f"{HERE}/unet_ref.pt")
+    save_sharded(out, "unet_ref")
 
 
 _RANDN_CALLS = [0]
@@ -660,7 +697,7 @@ def gen_pipeline():
             errs[tag] = str(e)
         print("pipeline error", tag, "->", errs[tag])
     out["errors"] = errs
-    torch.save(out, f"{HERE}/pipeline_ref.pt")
+    save_sharded(out, "pipeline_ref")
 
 
 def gen_sampler():

@@ -1,4 +1,4 @@
-"""GPU parity tests of the individual sm_100a kernels, called through the C ABI (ctypes), against plain
+"""GPU parity tests of the individual sm_90a kernels, called through the C ABI (ctypes), against plain
 torch fp32 references evaluated on the SAME bf16 inputs.
 
 Tolerances (stated per the task contract): the kernels accumulate in fp32 and round ONCE to bf16, so the
@@ -33,23 +33,6 @@ def _rand(shape, seed, std=1.0, device="cuda"):
     return (torch.randn(shape, generator=g) * std).to(torch.bfloat16).to(device)
 
 
-# ------------------------------------------------------------------------------------------------ probe
-def test_umma_descriptor_conventions(cuda):
-    """Pins the operand encodings the kernels rely on: K-major SW128 A/B, A from TMEM, MN-major B (V)."""
-    from diffuman4d_b200 import ops
-    for N, K in [(64, 64), (128, 128)]:
-        A = _rand((128, K), 1)
-        Bk = _rand((N, K), 2)
-        for a_src in (0, 1):
-            D = ops.probe_umma(A, Bk, N, K, a_src, 0, 0, 1024, 32)
-            _close(D, A.float() @ Bk.float().t(), rtol=1e-4, afrac=1e-4)
-    for N, K in [(64, 128), (128, 128), (64, 64)]:
-        A = _rand((128, K), 3)
-        Bm = _rand((K, N), 4)
-        D = ops.probe_umma(A, Bm, N, K, 1, 1, 16384, 1024, 2048)  # the attention kernel's P.V encoding
-        _close(D, A.float() @ Bm.float(), rtol=1e-4, afrac=1e-4)
-
-
 # ------------------------------------------------------------------------------------------------ GEMM
 @pytest.mark.parametrize("M,N,K", [(128, 64, 64), (256, 320, 320), (1000, 640, 320), (32, 1280, 320),
                                    (4096, 1920, 640), (384, 160, 2880), (8192, 1280, 1280), (128, 16, 64)])
@@ -80,8 +63,8 @@ def test_gemm_epilogues(cuda):
 @pytest.mark.parametrize("M,N,K,bn", [(333, 240, 128, 240), (77, 48, 64, 48), (513, 400, 64, 80), (200, 96, 64, 32),
                                       (129, 320, 192, 160), (1, 16, 64, 16)])
 def test_gemm_staged_epilogue_tails(cuda, M, N, K, bn):
-    """The epilogue stages 32-column units (two 16-column TMEM chunks) per warp and stores 64-byte row segments: odd chunk
-    counts per tile (240, 48, 80 columns), ragged M (rows past M must not be written) and the in-place residual."""
+    """Tile widths that are not a wgmma width (240, 48, 80, 32, 160, 16 columns run on a wider kernel with the extra
+    columns masked), ragged M (rows past M must not be written) and the in-place residual."""
     from diffuman4d_b200 import ops
     a, w = _rand((M, K), 25), _rand((N, K), 26, std=K ** -0.5)
     bias = torch.randn(N, generator=torch.Generator().manual_seed(27)).cuda()
@@ -107,11 +90,11 @@ def test_gemm_geglu(cuda, C):
     x = _rand((M, C), 40)
     w = _rand((8 * C, C), 41, std=C ** -0.5)
     b = torch.randn(8 * C, generator=torch.Generator().manual_seed(42)).cuda()
-    wi, bi, bn = ops.interleave_geglu(w, b)
-    out = ops.gemm(x, wi, bi, geglu=True, block_n=bn)
+    wi, bi = ops.interleave_geglu(w, b)
     y = x.float() @ w.float().t() + b
     a, g = y.chunk(2, dim=-1)
-    _close(out, a * F.gelu(g))
+    for bn in (0, 32, 256):   # automatic width, a width narrower than the kernel's (masked), the widest
+        _close(ops.gemm(x, wi, bi, geglu=True, block_n=bn), a * F.gelu(g))
 
 
 # ------------------------------------------------------------------------------------------------ conv
@@ -145,7 +128,7 @@ def test_attention(cuda, batch, seq, heads, d):
 
 
 def test_attention_sharp_softmax(cuda):
-    """large logits: exercises the running-max rescale path (rows whose max grows by > 8 log2 units)."""
+    """large logits: the running max grows from tile to tile, so O and the row sums are rescaled many times."""
     from diffuman4d_b200 import ops
     batch, seq, heads, d = 1, 512, 2, 64
     qkv = _rand((batch * seq, 3 * heads * d), 61, std=3.0)

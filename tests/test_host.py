@@ -16,7 +16,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 @pytest.fixture(scope="module")
 def libd4d():
     from diffuman4d_b200 import build
-    build.build(verbose=False)          # nvcc cross-compiles sm_100a without a GPU
+    build.build(verbose=False)          # nvcc cross-compiles sm_90a without a GPU
     from diffuman4d_b200._lib import lib
     return lib()
 
@@ -32,19 +32,12 @@ def test_header_and_library_export_the_same_symbols(libd4d):
 
 
 def test_product_library_carries_no_test_kernels_or_ablation_switches(libd4d):
-    """Library hygiene: the measurement / probe kernels and the D4D_*_ABLATE environment switches exist only in the tools
-    build libd4d_test.so (include/d4d_test.h), never in the product library."""
+    """Library hygiene: no measurement / probe kernels and no D4D_*_ABLATE environment switches in the library."""
     import subprocess
-    from diffuman4d_b200._lib import LIB_PATH, TEST_EXPORTS, TEST_LIB_PATH, test_lib
-    hdr = open(os.path.join(ROOT, "include", "d4d_test.h")).read()
-    assert set(re.findall(r"\b(d4d_[a-z0-9_]+)\s*\(", hdr)) == set(TEST_EXPORTS)
-    for name in TEST_EXPORTS:
-        assert not hasattr(libd4d, name), f"product library exports {name}"
-        assert hasattr(test_lib(), name)
+    from diffuman4d_b200._lib import LIB_PATH
     prod = subprocess.run(["strings", LIB_PATH], capture_output=True, text=True).stdout
-    tools = subprocess.run(["strings", TEST_LIB_PATH], capture_output=True, text=True).stdout
     for sw in ("D4D_GEMM_ABLATE", "D4D_ATTN_ABLATE"):
-        assert sw not in prod and sw in tools
+        assert sw not in prod
     assert "microbench" not in prod and "probe_kernel" not in prod
 
 
@@ -199,7 +192,7 @@ def test_plucker_embeds_match_reference_ray_utils():
 
 
 def test_upsample_phase_weights_reproduce_nearest2x_conv3x3():
-    """The sub-pixel form the Upsample2D kernel executes (conv_kind 2 / 3, csrc/gemm_umma.cu) is an identity, not an
+    """The sub-pixel form the Upsample2D kernel executes (conv_kind 2 / 3, csrc/gemm_wgmma.cu) is an identity, not an
     approximation: with integer-valued inputs and weights (exact in bf16 and in the fp32 sums) the four 2x2 phase convs
     on the low-resolution tensor equal `F.interpolate(nearest, x2)` + 3x3 / pad 1 conv bit for bit (reference:
     diffusers Upsample2D as called at unet_multiview_blocks.py:620)."""

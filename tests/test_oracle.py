@@ -1,4 +1,4 @@
-"""CPU tests: the oracle against the golden vectors produced by code run from /root/reference
+"""CPU tests: the oracle against the golden vectors produced by code run from the reference project
 (tests/golden/gen_golden.py), and the oracle's own invariants (the reference's runtime checks, SURVEY.md section 4)."""
 import os
 
@@ -10,6 +10,23 @@ from oracle import unet_oracle as O
 from oracle.pipeline_oracle import (DDIMOracle, build_windows, denoise_window_oracle, sliding_iterative_denoise_oracle)
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
+
+
+def _load_golden(name):
+    """golden/<name>.pt with its large input tensors put back from the golden/<name>.inputs<i>.pt shards (kept apart so
+    that no stored file exceeds 1 MB); a shard maps the '/'-joined key path of a tensor to the tensor."""
+    g = torch.load(os.path.join(GOLD, f"{name}.pt"))
+    i = 0
+    while os.path.exists(os.path.join(GOLD, f"{name}.inputs{i}.pt")):
+        for path, t in torch.load(os.path.join(GOLD, f"{name}.inputs{i}.pt")).items():
+            *parents, leaf = path.split("/")
+            node = g
+            for k in parents:
+                node = node[k]
+            assert node[leaf] is None, path
+            node[leaf] = t
+        i += 1
+    return g
 
 
 def test_pose_encoder_matches_reference_golden():
@@ -122,7 +139,7 @@ def test_oracle_unet_matches_reference_unet_golden(tag):
     from diffuman4d_b200.config import UNetConfig
     from diffuman4d_b200.weights import random_state_dict, state_dict_spec
     from oracle.unet_oracle import OracleUNet
-    c = torch.load(os.path.join(GOLD, "unet_ref.pt"))["cases"][tag]
+    c = _load_golden("unet_ref")["cases"][tag]
     cfg = UNetConfig(**c["cfg"])
     spec = {k: tuple(v) for k, v in state_dict_spec(cfg).items()}
     assert spec == c["ref_state_dict_shapes"]          # product weight-key contract == reference module tree
@@ -138,7 +155,7 @@ def test_oracle_unet_matches_reference_unet_golden(tag):
 def test_oracle_unet_num_frames_error_matches_reference():
     from diffuman4d_b200.config import UNetConfig
     from oracle.unet_oracle import OracleUNet
-    g = torch.load(os.path.join(GOLD, "unet_ref.pt"))
+    g = _load_golden("unet_ref")
     cfg = UNetConfig(**g["cases"]["two_3d_levels"]["cfg"])
     m = OracleUNet(cfg)
     x = torch.zeros(4, cfg.in_channels, 8, 8)
@@ -158,7 +175,7 @@ def _fake_unet(cin):
 def test_window_step_matches_reference_pipeline_golden(tag):
     """The oracle's window step against the reference's own ``Diffuman4DPipeline.__call__`` (PIPE:345-425) run on stubs of
     the upstream surface (tests/golden/gen_golden.py::gen_pipeline): assembly, CFG negatives, cond aliasing, per-frame steps."""
-    c = torch.load(os.path.join(GOLD, "pipeline_ref.pt"))["cases"][tag]
+    c = _load_golden("pipeline_ref")["cases"][tag]
     i = c["in"]
     s = DDIMOracle(SchedulerConfig(prediction_type=c["prediction_type"]))
     s.set_timesteps(c["n_steps_table"])
@@ -177,7 +194,7 @@ def test_sliding_loop_matches_reference_pipeline_golden(tag):
     """Oracle AND product window schedule / sliding loop against the reference's ``sliding_iterative_denoise``
     (PIPE:439-559) run on the same stubs: visited windows, per-window timestep indices, final grid, bookkeeping."""
     from diffuman4d_b200.pipeline import build_windows as product_build_windows
-    c = torch.load(os.path.join(GOLD, "pipeline_ref.pt"))["cases"][tag]
+    c = _load_golden("pipeline_ref")["cases"][tag]
     i = c["in"]
     mask = i["cond_mask_latents"]
     tgt, inp = torch.where(mask[:, 0, 0, 0] != 0)[0], torch.where(mask[:, 0, 0, 0] == 0)[0]
@@ -200,7 +217,7 @@ def test_sliding_loop_matches_reference_pipeline_golden(tag):
 
 def test_sliding_argument_errors_match_reference_messages():
     """PIPE:464,481,486: same exception type and text as the reference raised in the generator run."""
-    errs = torch.load(os.path.join(GOLD, "pipeline_ref.pt"))["errors"]
+    errs = _load_golden("pipeline_ref")["errors"]
     n, h, w = 8, 8, 8
     mask = torch.ones(n, 1, h, w)
     mask[:2] = 0

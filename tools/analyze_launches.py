@@ -4,7 +4,7 @@ import re
 import sys
 from collections import defaultdict
 
-path = sys.argv[1] if len(sys.argv) > 1 else "gpurun_out/launches.csv"
+path = sys.argv[1] if len(sys.argv) > 1 else "launches.csv"
 rows = []
 with open(path) as f:
     lines = f.readlines()

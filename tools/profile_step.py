@@ -1,5 +1,5 @@
 """One warm window step, then ONE profiled window step (cudaProfilerStart/Stop) -- the command ncu wraps.
-    ncu --profile-from-start off --metrics gpu__time_duration.sum --clock-control none --csv --log-file gpurun_out/launches.csv python tools/profile_step.py
+    ncu --profile-from-start off --metrics gpu__time_duration.sum --clock-control none --csv --log-file launches.csv python tools/profile_step.py
 """
 import os
 import sys

@@ -4,10 +4,10 @@ CFG 2.0) driven by B200SlidingIterativeSampler (the device-resident mirror of sr
 through B200Diffuman4DPipeline.sliding_iterative_denoise on the SD-2.1 UNet layout with random weights, a synthetic dataset
 with the reference's get_item contract and a pooling stand-in for the VAE (the VAE is out of scope, SURVEY 8f-1).
 
-    python tools/run_grid.py [--latent 64] [--cams 48] [--frames 16] [--out gpurun_out/grid.json]
+    python tools/run_grid.py [--latent 64] [--cams 48] [--frames 16] [--out grid.json]
     torchrun --nproc-per-node N tools/run_grid.py ...     # replicas: tasks of a round sharded over the ranks
 
-Reports: window steps executed (W16 spatial / W24 temporal), device time inside denoise_window, wall time of execute_tasks.
+Prints one JSON line (and writes it to --out when given): window steps executed (W16 spatial / W24 temporal), device time inside denoise_window, wall time of execute_tasks.
 """
 import argparse
 import json
@@ -27,7 +27,7 @@ def main():
     ap.add_argument("--latent", type=int, default=64)
     ap.add_argument("--cams", type=int, default=48)
     ap.add_argument("--frames", type=int, default=16)
-    ap.add_argument("--out", default="gpurun_out/grid.json")
+    ap.add_argument("--out", default=None, help="also write the JSON result to this file")
     ap.add_argument("--prefetch", action="store_true", help="load the next task's dataset item on a helper thread")
     args = ap.parse_args()
 
@@ -107,8 +107,9 @@ def main():
             res["window_steps_per_s_wall"] = round(tot / res["wall_s_execute_tasks"], 2)
         dist.destroy_process_group()
     if rank == 0:
-        os.makedirs(os.path.dirname(args.out) or ".", exist_ok=True)
-        json.dump(res, open(args.out, "w"), indent=1)
+        if args.out:
+            os.makedirs(os.path.dirname(args.out) or ".", exist_ok=True)
+            json.dump(res, open(args.out, "w"), indent=1)
         print(json.dumps(res))
 
 
