@@ -40,20 +40,6 @@ struct DeviceGuard {
     if (prev >= 0) cudaSetDevice(prev);
   }
 };
-// scratch for the op-level GroupNorm entry point (per thread, grown on demand)
-float* gn_scratch(size_t floats) {
-  static thread_local float* p = nullptr;
-  static thread_local size_t cap = 0;
-  if (floats > cap) {
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-    if (cudaMalloc(&p, floats * sizeof(float)) != cudaSuccess) return nullptr;
-    if (cudaMemset(p, 0, floats * sizeof(float)) != cudaSuccess) return nullptr;
-    cap = floats;
-  }
-  return p;
-}
 }  // namespace
 
 extern "C" {
@@ -273,19 +259,19 @@ int d4d_op_attention(const void* q, const void* k, const void* v, int ld_qkv, vo
 }
 
 int d4d_op_groupnorm(const void* x1, int C1, const void* x2, int C2, int n_img, int hw, int groups, float eps,
-                     const float* gamma, const float* beta, int silu, void* out, void* stream) {
+                     const float* gamma, const float* beta, int silu, void* out, int64_t* stats, void* stream) {
   D4D_API_BEGIN
   D4D_REQUIRE(n_img > 0 && hw > 0 && groups > 0, "empty GroupNorm");
-  float* part = gn_scratch(d4d::groupnorm_scratch_floats(n_img, groups));
-  if (!part) {
-    d4d::set_error("GroupNorm scratch allocation failed");
-    return 2;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (x2 == nullptr) C2 = 0;
+  long long* s1 = reinterpret_cast<long long*>(stats);
+  long long* s2 = C2 > 0 ? s1 + static_cast<size_t>(n_img) * C1 * 2 : nullptr;
+  if (int rc = d4d::groupnorm_stats_run(static_cast<const bf16*>(x1), C1, n_img, hw, s1, st)) return rc;
+  if (C2 > 0) {
+    if (int rc = d4d::groupnorm_stats_run(static_cast<const bf16*>(x2), C2, n_img, hw, s2, st)) return rc;
   }
-  // the arrival counters live behind the (n_img-dependent) partial/final regions: zero them for this shape
-  const size_t ctr_off = static_cast<size_t>(n_img) * 32 * groups * 2 + static_cast<size_t>(n_img) * groups * 2;
-  D4D_CUDA_OK(cudaMemsetAsync(part + ctr_off, 0, sizeof(unsigned int) * n_img, static_cast<cudaStream_t>(stream)));
-  return d4d::groupnorm_run(static_cast<const bf16*>(x1), C1, static_cast<const bf16*>(x2), C2, n_img, hw, groups, eps,
-                            gamma, beta, silu, static_cast<bf16*>(out), part, static_cast<cudaStream_t>(stream));
+  return d4d::groupnorm_apply_run(static_cast<const bf16*>(x1), C1, s1, static_cast<const bf16*>(x2), C2, s2, n_img, hw, groups,
+                                  eps, gamma, beta, silu, static_cast<bf16*>(out), st);
   D4D_API_END
 }
 
@@ -306,30 +292,21 @@ int d4d_op_conv_resample(const void* x_nhwc, int n_img, int H, int W, int Cin, c
 
 int d4d_op_conv3x3_groupnorm(const void* x_nhwc, int n_img, int H, int W, int Cin, const void* Wt, int Cout, const float* bias,
                              const void* residual, int groups, float eps, const float* gamma, const float* beta, int silu,
-                             void* conv_out, void* gn_out, void* stream) {
+                             void* conv_out, void* gn_out, int64_t* stats, void* stream) {
   D4D_API_BEGIN
   D4D_REQUIRE(n_img > 0 && H > 0 && W > 0 && groups > 0, "empty conv");
+  D4D_REQUIRE(stats != nullptr, "null statistics workspace");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const size_t floats = static_cast<size_t>(n_img) * Cout * 2 * 2;  // [n_img][Cout][2] 64-bit {sum, sumsq}
-  // accumulated by the conv epilogue; lives behind the stand-alone kernel's scratch (16-byte aligned for the 128-bit loads)
-  const size_t off = (d4d::groupnorm_scratch_floats(n_img, groups) + 3) & ~size_t(3);
-  float* base = gn_scratch(off + floats);
-  if (!base) {
-    d4d::set_error("GroupNorm scratch allocation failed");
-    return 2;
-  }
-  long long* stats = reinterpret_cast<long long*>(base + off);
-  D4D_CUDA_OK(cudaMemsetAsync(stats, 0, floats * sizeof(float), st));
   d4d::GemmDesc d;
   d.conv = 1; d.A = static_cast<const bf16*>(x_nhwc); d.n_img = n_img; d.H = H; d.W = W; d.Cin = Cin;
   d.Wt = static_cast<const bf16*>(Wt); d.N = Cout; d.bias = bias;
   d.residual = static_cast<const bf16*>(residual); d.ld_res = Cout;
   d.out = static_cast<bf16*>(conv_out); d.ldo = Cout;
-  d.stats = stats;
+  d.stats = reinterpret_cast<long long*>(stats);
   d4d::GemmLaunch L;
   if (int rc = d4d::gemm_prepare(d, &L)) return rc;
   if (int rc = d4d::gemm_run(L, st)) return rc;
-  return d4d::groupnorm_apply_run(static_cast<const bf16*>(conv_out), Cout, stats, nullptr, 0, nullptr, n_img, H * W, groups, eps,
+  return d4d::groupnorm_apply_run(static_cast<const bf16*>(conv_out), Cout, d.stats, nullptr, 0, nullptr, n_img, H * W, groups, eps,
                                   gamma, beta, silu, static_cast<bf16*>(gn_out), st);
   D4D_API_END
 }

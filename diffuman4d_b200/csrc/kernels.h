@@ -13,8 +13,8 @@ namespace d4d {
 // --------------------------------------------------------------------------------------------
 // wgmma GEMM / implicit-GEMM conv3x3  (gemm_wgmma.cu)
 // --------------------------------------------------------------------------------------------
-// fixed-point scales of the fused GroupNorm statistics: |sum| < 2^35 (|x| <= 2e6 over 16384 pixels), sum of squares < 2^39
-// (rms |x| <= 5800 over 16384 pixels); resolutions 3.7e-9 / 6e-8 per 16-row partial
+// fixed-point scales of the GroupNorm statistics (GEMM / conv epilogue, groupnorm_stats_run): |sum| < 2^35 (|x| <= 2e6
+// over 16384 pixels), sum of squares < 2^39 (rms |x| <= 5800 over 16384 pixels); resolutions 3.7e-9 / 6e-8 per 16-row partial
 constexpr float kGnSumScale = 268435456.f;  // 2^28
 constexpr float kGnSqScale = 16777216.f;    // 2^24
 
@@ -129,18 +129,13 @@ double attn_flops(const AttnDesc& d);
 // --------------------------------------------------------------------------------------------
 // HBM-bound kernels (norm.cu, elementwise.cu)
 // --------------------------------------------------------------------------------------------
-// GroupNorm over NHWC tokens [n_img, hw, C1 (+C2)] (optional virtual channel concat of two sources),
-// fused affine + optional SiLU; writes bf16 [n_img*hw, C1+C2].  scratch: groupnorm_scratch_floats(n_img, groups) floats,
-// zero-initialised once (slab partials | final mean/rstd | self-resetting arrival counters).
-int groupnorm_splits(int hw);
-inline size_t groupnorm_scratch_floats(int n_img, int groups) {
-  return static_cast<size_t>(n_img) * 32 * groups * 2 + static_cast<size_t>(n_img) * groups * 2 + n_img + 16;
-}
-int groupnorm_run(const bf16* x1, int C1, const bf16* x2, int C2, int n_img, int hw, int groups, float eps,
-                  const float* gamma, const float* beta, int silu, bf16* out, float* partials, cudaStream_t stream);
-// Same normalisation with the statistics taken from the per-(image, channel) {sum, sum of squares} arrays that the
-// producing GEMM / conv epilogue accumulated (GemmDesc::stats): one launch, one read of x, no statistics pass.
-// stats1: [n_img][C1][2], stats2: [n_img][C2][2] (null when C2 == 0), fixed point (kGnSumScale, kGnSqScale).
+// GroupNorm statistics of an NHWC tensor [n_img, hw, C] in the format the GEMM / conv epilogue writes (GemmDesc::stats):
+// per-(image, channel) {sum, sum of squares}, fixed point (kGnSumScale, kGnSqScale), added into stats [n_img][C][2],
+// which the caller zeroes.  For tensors whose producer cannot accumulate them in its epilogue.
+int groupnorm_stats_run(const bf16* x, int C, int n_img, int hw, long long* stats, cudaStream_t stream);
+// GroupNorm over NHWC tokens [n_img, hw, C1 (+C2)] (optional virtual channel concat of two sources), fused affine +
+// optional SiLU; writes bf16 [n_img*hw, C1+C2].  The group (mean, rstd) come from the statistics of each source
+// (stats1: [n_img][C1][2], stats2: [n_img][C2][2], null when C2 == 0): one launch, one read of x.  32 <= C1 + C2 <= 4096.
 int groupnorm_apply_run(const bf16* x1, int C1, const long long* stats1, const bf16* x2, int C2, const long long* stats2, int n_img,
                         int hw, int groups, float eps, const float* gamma, const float* beta, int silu, bf16* out,
                         cudaStream_t stream);

@@ -502,31 +502,39 @@ int Model::finalize() {
 // plan builder
 // =================================================================================================
 class PlanBuilder {
-  static long long* dry_stats_marker() {  // dry run: "has statistics" marker, never dereferenced
-    static long long marker;
-    return &marker;
-  }
  public:
   PlanBuilder(Model& m, Plan& p, bool dry, char* base) : m_(m), p_(p), dry_(dry), base_(base) {}
 
-  struct Act { bf16* p; int C, H, W; long long* stats = nullptr; };  // stats: [B][C][2] {sum, sumsq} filled by the producer's epilogue
+  struct Act { bf16* p; int C, H, W; long long* stats = nullptr; };  // stats: [B][C][2] {sum, sumsq} when a GroupNorm reads p
 
   size_t peak() const { return peak_; }
   size_t stats_words() const { return stats_used_; }
   // per-(image, channel) statistics of a GEMM / conv output that a GroupNorm will read: a slice of one pool that a single
   // memset at the head of the plan zeroes
-  // (only when every 32-row warp of the producer's tiles stays inside one image: true for every level of a >= 32x32
-  //  latent; smaller test shapes fall back to the stand-alone statistics kernel)
-  long long* stats_alloc(int n_img, int C, int H, int W) {
+  long long* stats_alloc(int n_img, int C) {
+    long long* p = stats_pool_ ? stats_pool_ + stats_used_ : nullptr;  // (the dry run only counts)
+    stats_used_ += static_cast<size_t>(n_img) * C * 2;
+    return p;
+  }
+  // Runs the producer of `out` (d writes out.p) so that out.stats holds its statistics.  The epilogue accumulates them
+  // when every 32-row warp of the producer's tiles (grid H x W) stays inside one image: true at every level of the
+  // 64x64 and 128x128 latents.  Otherwise a statistics launch follows the producer.  Eager, not at the norm: a down-path
+  // output is read by two GroupNorms (the next block's and the up-path concat's) and must be summed once.
+  void gemm_stats(GemmDesc d, const Act& out, int n_img, int H, int W) {
     int bw = 16;
     while (bw > W) bw >>= 1;
     int bh = 128 / bw;
     while (bh > H && bh > 1) bh >>= 1;
-    if ((bw * bh) % 32 != 0 || (H * W) % 32 != 0) return nullptr;
-    const size_t n = static_cast<size_t>(n_img) * C * 2;
-    long long* p = stats_pool_ ? stats_pool_ + stats_used_ : dry_stats_marker();
-    stats_used_ += n;
-    return p;
+    if ((bw * bh) % 32 == 0 && (H * W) % 32 == 0) {
+      d.stats = out.stats;
+      gemm(d);
+      return;
+    }
+    gemm(d);
+    const bf16* x = out.p;
+    long long* st = out.stats;
+    const int C = out.C, hw = out.H * out.W;
+    op([=](cudaStream_t s) { return groupnorm_stats_run(x, C, n_img, hw, st, s); }, 1, 3);
   }
   int rc() const { return rc_; }
 
@@ -592,17 +600,12 @@ class PlanBuilder {
     if (int rc = attn_prepare(d, &L)) { if (!rc_) rc_ = rc; return; }
     op([L](cudaStream_t s) { return attn_run(L, s); }, 1, 2, attn_flops(d));
   }
-  // GroupNorm(+SiLU) of (a | b): statistics come from the producers' epilogues (Act::stats), one apply launch
+  // GroupNorm(+SiLU) of (a | b) from their statistics (Act::stats, see gemm_stats): one apply launch
   void groupnorm(const Act& xa, const Act* xb, int n_img, float eps, const NormW& n, int silu, bf16* out) {
     const int groups = m_.cfg_.norm_num_groups, hw = xa.H * xa.W;
     const bf16 *x1 = xa.p, *x2 = xb ? xb->p : nullptr;
     const int C1 = xa.C, C2 = xb ? xb->C : 0;
     const long long *s1 = xa.stats, *s2 = xb ? xb->stats : nullptr;
-    if (s1 == nullptr || (xb && s2 == nullptr)) {  // small shapes: stand-alone statistics pass
-      float* part = gn_partials_;
-      op([=](cudaStream_t s) { return groupnorm_run(x1, C1, x2, C2, n_img, hw, groups, eps, n.g, n.b, silu, out, part, s); }, 2, 3);
-      return;
-    }
     op([=](cudaStream_t s) { return groupnorm_apply_run(x1, C1, s1, x2, C2, s2, n_img, hw, groups, eps, n.g, n.b, silu, out, s); }, 1, 3);
   }
   void layernorm(const bf16* x, int rows, int C, const NormW& n, bf16* out) {
@@ -616,15 +619,14 @@ class PlanBuilder {
     const int Cin = xa.C + Cb;
     bf16* h0 = alloc(static_cast<size_t>(M) * Cin);
     groupnorm(xa, xb, B, m_.cfg_.norm_eps, r.n1, 1, h0);
-    Act h1{alloc(static_cast<size_t>(M) * r.cout), r.cout, xa.H, xa.W, stats_alloc(B, r.cout, xa.H, xa.W)};
+    Act h1{alloc(static_cast<size_t>(M) * r.cout), r.cout, xa.H, xa.W, stats_alloc(B, r.cout)};
     {
       GemmDesc d;
       d.conv = 1; d.A = h0; d.n_img = B; d.H = xa.H; d.W = xa.W; d.Cin = Cin;
       d.Wt = r.c1.w; d.N = r.cout; d.bias = r.c1.b;
       d.rowvec = temb_all + r.temb_off; d.ld_rowvec = ld_temb;
       d.out = h1.p; d.ldo = r.cout;
-      d.stats = h1.stats;
-      gemm(d);
+      gemm_stats(d, h1, B, xa.H, xa.W);
     }
     release(h0);
     bf16* h2 = alloc(static_cast<size_t>(M) * r.cout);
@@ -641,15 +643,14 @@ class PlanBuilder {
       gemm(d);
       res = sc;
     }
-    Act out{alloc(static_cast<size_t>(M) * r.cout), r.cout, xa.H, xa.W, stats_alloc(B, r.cout, xa.H, xa.W)};
+    Act out{alloc(static_cast<size_t>(M) * r.cout), r.cout, xa.H, xa.W, stats_alloc(B, r.cout)};
     {
       GemmDesc d;
       d.conv = 1; d.A = h2; d.n_img = B; d.H = xa.H; d.W = xa.W; d.Cin = r.cout;
       d.Wt = r.c2.w; d.N = r.cout; d.bias = r.c2.b;
       d.residual = res; d.ld_res = r.cout;
       d.out = out.p; d.ldo = r.cout;
-      d.stats = out.stats;
-      gemm(d);
+      gemm_stats(d, out, B, xa.H, xa.W);
     }
     release(h2);
     if (sc) release(sc);
@@ -786,26 +787,25 @@ class PlanBuilder {
     }
     release(g);
     release(t1);
-    Act out{alloc(static_cast<size_t>(M) * C), C, in.H, in.W, stats_alloc(B, C, in.H, in.W)};
+    Act out{alloc(static_cast<size_t>(M) * C), C, in.H, in.W, stats_alloc(B, C)};
     {
       GemmDesc d;
       d.A = t3; d.lda = C; d.K1 = C; d.Wt = x.pout.w; d.M = M; d.N = C; d.bias = x.pout.b;
       d.residual = in.p; d.ld_res = C; d.out = out.p; d.ldo = C;
-      d.stats = out.stats; d.stats_rows = hw;
-      gemm(d);
+      d.stats_rows = hw;
+      gemm_stats(d, out, B, in.H, in.W);
     }
     release(t3);
     return out;
   }
 
-  Act conv3x3(const LinW& w, Act in, int act = 0, int n_img = 0, bool want_stats = false) {
+  Act conv3x3(const LinW& w, Act in, int act = 0, int n_img = 0) {
     if (n_img <= 0) n_img = p_.B;
     const int M = n_img * in.H * in.W;
-    Act out{alloc(static_cast<size_t>(M) * w.out), w.out, in.H, in.W, want_stats ? stats_alloc(n_img, w.out, in.H, in.W) : nullptr};
+    Act out{alloc(static_cast<size_t>(M) * w.out), w.out, in.H, in.W};
     GemmDesc d;
     d.conv = 1; d.A = in.p; d.n_img = n_img; d.H = in.H; d.W = in.W; d.Cin = in.C;
     d.Wt = w.w; d.N = w.out; d.bias = w.b; d.out = out.p; d.ldo = w.out; d.act = act;
-    d.stats = out.stats;
     gemm(d);
     return out;
   }
@@ -819,11 +819,6 @@ class PlanBuilder {
     const int C0 = ch[0], TE = 4 * C0, L = cfg.layers_per_block;
     const int M0 = B * h * w;
 
-    {  // scratch of the stand-alone GroupNorm statistics kernel (small shapes only)
-      const size_t fl = groupnorm_scratch_floats(B, cfg.norm_num_groups);
-      gn_partials_ = reinterpret_cast<float*>(alloc(fl * 2));
-      if (!dry_ && cudaMemset(gn_partials_, 0, fl * sizeof(float)) != cudaSuccess) rc_ = 2;
-    }
     if (!dry_ && p_.stats_words > 0) {  // GroupNorm statistics pool (size from the dry run): zeroed once per forward
       stats_pool_ = reinterpret_cast<long long*>(alloc(p_.stats_words * 4));
       long long* pool = stats_pool_;
@@ -947,17 +942,15 @@ class PlanBuilder {
       const int KP = m.kp_in(), cp = m.cin_pad(), Cin = cfg.in_channels;
       bf16* col = alloc(static_cast<size_t>(M0) * KP);
       op([=](cudaStream_t s) { return im2col_nchw_run(pl->sample, B, Cin, h, w, cp, KP, col, s); });
-      bf16* x0 = alloc(static_cast<size_t>(M0) * C0);
-      long long* st0 = stats_alloc(B, C0, h, w);
+      x = {alloc(static_cast<size_t>(M0) * C0), C0, h, w, stats_alloc(B, C0)};
       GemmDesc d;
       d.A = col; d.lda = KP; d.K1 = KP; d.Wt = m.conv_in_.w; d.M = M0; d.N = C0; d.bias = m.conv_in_.b;
       if (pose_emb) { d.residual = pose_emb; d.ld_res = C0; }
-      d.out = x0; d.ldo = C0;
-      d.stats = st0; d.stats_rows = h * w;
-      gemm(d);
+      d.out = x.p; d.ldo = C0;
+      d.stats_rows = h * w;
+      gemm_stats(d, x, B, h, w);
       release(col);
       if (pose_emb) release(pose_emb);
-      x = {x0, C0, h, w, st0};
     }
     tap("conv_in", x);
 
@@ -978,14 +971,12 @@ class PlanBuilder {
       }
       if (i < 3) {  // Downsample2D: 3x3 stride-2 pad-1 conv, read in place through a strided tensor map
         const int Ho = x.H / 2, Wo = x.W / 2, Mo = B * Ho * Wo;
-        bf16* y = alloc(static_cast<size_t>(Mo) * x.C);
-        long long* sty = stats_alloc(B, x.C, Ho, Wo);
+        const Act y{alloc(static_cast<size_t>(Mo) * x.C), x.C, Ho, Wo, stats_alloc(B, x.C)};
         GemmDesc d;
         d.conv = 1; d.conv_kind = 1; d.A = x.p; d.n_img = B; d.H = x.H; d.W = x.W; d.Cin = x.C;
-        d.Wt = m.down_ds_[i].w; d.N = x.C; d.bias = m.down_ds_[i].b; d.out = y; d.ldo = x.C;
-        d.stats = sty;
-        gemm(d);
-        x = {y, x.C, Ho, Wo, sty};
+        d.Wt = m.down_ds_[i].w; d.N = x.C; d.bias = m.down_ds_[i].b; d.out = y.p; d.ldo = x.C;
+        gemm_stats(d, y, B, Ho, Wo);
+        x = y;
         skips.push_back(x);
       }
       tap("down_blocks." + std::to_string(i), x);
@@ -1018,14 +1009,13 @@ class PlanBuilder {
       }
       if (i < 3) {  // Upsample2D (nearest x2, then 3x3 conv) as four sub-pixel phases on the low-resolution tensor
         const int H2 = 2 * x.H, W2 = 2 * x.W;
-        Act y{alloc(static_cast<size_t>(B) * H2 * W2 * x.C), x.C, H2, W2, stats_alloc(B, x.C, x.H, x.W)};
+        Act y{alloc(static_cast<size_t>(B) * H2 * W2 * x.C), x.C, H2, W2, stats_alloc(B, x.C)};
         {
           GemmDesc d;
           d.conv = 1; d.conv_kind = 3;
           d.A = x.p; d.n_img = B; d.H = x.H; d.W = x.W; d.Cin = x.C;
           d.Wt = m.up_us_[i].w; d.N = x.C; d.bias = m.up_us_[i].b; d.out = y.p; d.ldo = x.C;
-          d.stats = y.stats;
-          gemm(d);
+          gemm_stats(d, y, B, x.H, x.W);  // (tiles walk the low-resolution grid)
         }
         release(x.p);
         x = y;
@@ -1057,7 +1047,6 @@ class PlanBuilder {
   size_t bump_ = 0, peak_ = 0;
   std::vector<std::pair<size_t, size_t>> free_;
   std::map<size_t, size_t> live_;
-  float* gn_partials_ = nullptr;
   long long* stats_pool_ = nullptr;
   size_t stats_used_ = 0;
   int rc_ = 0;

@@ -48,7 +48,7 @@ struct Plan {
   // frame-sharded window (DESIGN.md section 7): this rank owns F of F_total frames per CFG half
   int F_total = 0, rank = 0, world = 1;
   bool pose_shared_neg = false;  // skeleton batch = [1 CFG-negative image | F positive images] (window step)
-  size_t stats_words = 0;      // GroupNorm statistics pool: 64-bit fixed-point per-(image, channel) sums written by the producers' epilogues
+  size_t stats_words = 0;      // GroupNorm statistics pool: 64-bit fixed-point per-(image, channel) sums of every tensor a GroupNorm reads
   int n3d = 0;                 // number of 3-D attention layers (K/V exchanges) per forward
   unsigned int run_index = 0;  // forwards executed on this plan
   unsigned int epoch0 = 0;     // exchange counter at the start of the current forward (epoch / buffer parity per layer)

@@ -96,8 +96,9 @@ def groupnorm(x1: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, groups:
     n_img, hw, C1 = x1.shape
     C2 = 0 if x2 is None else x2.shape[2]
     out = torch.empty(n_img, hw, C1 + C2, device=x1.device, dtype=torch.bfloat16)
+    stats = torch.zeros(n_img, C1 + C2, 2, device=x1.device, dtype=torch.int64)
     check(lib().d4d_op_groupnorm(_p(x1), C1, _p(x2), C2, n_img, hw, groups, float(eps), _p(gamma), _p(beta),
-                                 int(silu), _p(out), _stream()), "d4d_op_groupnorm")
+                                 int(silu), _p(out), _p(stats), _stream()), "d4d_op_groupnorm")
     return out
 
 
@@ -158,9 +159,10 @@ def conv3x3_groupnorm(x_nhwc: torch.Tensor, w_octi: torch.Tensor, bias: Optional
     Cout = w_octi.shape[0]
     conv_out = torch.empty(n, H, W, Cout, device=x_nhwc.device, dtype=torch.bfloat16)
     gn_out = torch.empty_like(conv_out)
+    stats = torch.zeros(n, Cout, 2, device=x_nhwc.device, dtype=torch.int64)
     check(lib().d4d_op_conv3x3_groupnorm(_p(x_nhwc), n, H, W, Cin, _p(w_octi), Cout, _p(bias), _p(residual), groups,
-                                         float(eps), _p(gamma), _p(beta), int(silu), _p(conv_out), _p(gn_out), _stream()),
-          "d4d_op_conv3x3_groupnorm")
+                                         float(eps), _p(gamma), _p(beta), int(silu), _p(conv_out), _p(gn_out), _p(stats),
+                                         _stream()), "d4d_op_conv3x3_groupnorm")
     return conv_out, gn_out
 
 

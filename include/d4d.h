@@ -133,8 +133,12 @@ int d4d_op_conv3x3(const void* x_nhwc, int n_img, int H, int W, int Cin, const v
 /* q, k, v: column slices of one row-major [batch*seq, ld_qkv] matrix; head hd = columns [hd*D, (hd+1)*D). */
 int d4d_op_attention(const void* q, const void* k, const void* v, int ld_qkv, void* out, int ld_out, int batch,
                      int seq, int heads, int head_dim, float scale, void* stream);
+/* GroupNorm(+SiLU) of NHWC x1 [n_img, hw, C1], virtually concatenated on channels with x2 [n_img, hw, C2] when x2 is not
+ * NULL, into out [n_img, hw, C1+C2]; 32 <= C1 + C2 <= 4096, C1 and C2 multiples of 8.  One statistics launch per source
+ * fills `stats`, then one launch normalises.  stats: caller-allocated, ZEROED int64 workspace [n_img][C1+C2][2] (x1's
+ * channels, then x2's) that receives the per-(image, channel) fixed-point {sum, sum of squares}. */
 int d4d_op_groupnorm(const void* x1, int C1, const void* x2, int C2, int n_img, int hw, int groups, float eps,
-                     const float* gamma, const float* beta, int silu, void* out, void* stream);
+                     const float* gamma, const float* beta, int silu, void* out, int64_t* stats, void* stream);
 /* The two resampling convolutions of the UNet, read / written in place (no im2col, no materialised upsampled tensor):
  *   kind 1: 3x3 stride-2 pad-1 conv (diffusers Downsample2D): x [n,H,W,Cin] -> out [n,H/2,W/2,Cout], Wt [Cout][9][Cin];
  *   kind 2: one sub-pixel phase (up_a, up_b in {0,1}) of "nearest x2 upsample, then 3x3 pad-1 conv" (Upsample2D): a 2x2 conv on
@@ -145,10 +149,11 @@ int d4d_op_conv_resample(const void* x_nhwc, int n_img, int H, int W, int Cin, c
                          int kind, int up_a, int up_b, void* out, void* stream);
 /* conv3x3 (+bias, +residual) whose epilogue accumulates the per-(image, channel) sums of its output, followed by the
  * GroupNorm(+SiLU) that reads those sums instead of running a statistics pass: the pair every ResnetBlock2D of the UNet
- * executes (needs H*W % 32 == 0).  conv_out [n,H,W,Cout] and gn_out [n,H,W,Cout] are both written. */
+ * executes (needs H*W % 32 == 0).  conv_out [n,H,W,Cout] and gn_out [n,H,W,Cout] are both written.  stats:
+ * caller-allocated, ZEROED int64 workspace [n][Cout][2] for the sums (same format as d4d_op_groupnorm's). */
 int d4d_op_conv3x3_groupnorm(const void* x_nhwc, int n_img, int H, int W, int Cin, const void* Wt, int Cout,
                              const float* bias, const void* residual, int groups, float eps, const float* gamma,
-                             const float* beta, int silu, void* conv_out, void* gn_out, void* stream);
+                             const float* beta, int silu, void* conv_out, void* gn_out, int64_t* stats, void* stream);
 int d4d_op_layernorm(const void* x, int rows, int C, float eps, const float* gamma, const float* beta, void* out,
                      void* stream);
 /* Debug tap (per-level drift reports in tests/): runs the forward of d4d_unet_forward up to intermediate activation

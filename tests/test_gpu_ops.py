@@ -28,6 +28,16 @@ def _close(out, ref, rtol=8e-3, afrac=2e-3):
     assert not bad.any(), f"max err {err.max().item():.4g} (scale {scale:.4g}), {int(bad.sum())} / {bad.numel()} out of tolerance"
 
 
+def _within_bf16_ulp(out, ref):
+    """|out - ref| <= one bf16 ulp of the larger magnitude, everywhere.  Magnitudes below 2^-8 count as 2^-8: a normalised
+    value near zero is the difference of two O(1) fp32 terms and keeps their absolute rounding error."""
+    out, ref = out.float(), ref.float()
+    mag = torch.maximum(out.abs(), ref.abs()).clamp_min(2.0 ** -8)
+    ulp = torch.exp2(torch.floor(torch.log2(mag)) - 7)
+    err = (out - ref).abs()
+    assert (err <= ulp).all(), f"max err {err.max().item():.4g}, {int((err > ulp).sum())} / {err.numel()} beyond one ulp"
+
+
 def _rand(shape, seed, std=1.0, device="cuda"):
     g = torch.Generator().manual_seed(seed)
     return (torch.randn(shape, generator=g) * std).to(torch.bfloat16).to(device)
@@ -195,6 +205,9 @@ def test_conv3x3_fused_groupnorm_stats(cuda, n, H, W, Cin, Cout, silu):
     if silu:
         ref = F.silu(ref)
     _close(gn_out, ref)
+    # the stand-alone statistics kernel produces the epilogue's format: same normalisation to within one bf16 ulp
+    sa = ops.groupnorm(conv_out.view(n, H * W, Cout), gamma, beta, 32, 1e-5, silu).view(n, H, W, Cout)
+    _within_bf16_ulp(sa, gn_out)
 
 
 @pytest.mark.parametrize("rows,C", [(100, 64), (4096, 320), (1000, 640), (77, 1280)])
