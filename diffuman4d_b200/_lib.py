@@ -78,13 +78,13 @@ def _load(path: str) -> C.CDLL:
     l.d4d_assemble_input.argtypes = [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]
     l.d4d_cfg_ddim_step.argtypes = [vp, vp, vp, vp, vp, C.POINTER(D4DSched), f32, i32, i32, i32, i32, vp, vp]
     l.d4d_op_gemm.argtypes = [vp, i32, i32, vp, i32, i32, vp, i32, i32, f32p, vp, i32, i32, vp, i32, vp, i32, i32,
-                              i32, f32, i32, vp]
-    l.d4d_op_conv3x3.argtypes = [vp, i32, i32, i32, i32, vp, i32, f32p, vp, i32, vp, i32, vp, i32, vp]
-    l.d4d_op_attention.argtypes = [vp, vp, vp, i32, vp, i32, i32, i32, i32, i32, f32, vp]
+                              i32, f32, i32, vp, i32, vp]
+    l.d4d_op_conv3x3.argtypes = [vp, i32, i32, i32, i32, vp, i32, f32p, vp, i32, vp, i32, vp, i32, vp, vp]
+    l.d4d_op_attention.argtypes = [vp, vp, vp, i32, vp, i32, i32, i32, i32, i32, f32, i32, i32, vp]
     l.d4d_op_groupnorm.argtypes = [vp, i32, vp, i32, i32, i32, i32, f32, f32p, f32p, i32, vp, vp, vp]
     l.d4d_op_conv3x3_groupnorm.argtypes = [vp, i32, i32, i32, i32, vp, i32, f32p, vp, i32, f32, f32p, f32p, i32, vp, vp, vp,
                                            vp]
-    l.d4d_op_conv_resample.argtypes = [vp, i32, i32, i32, i32, vp, i32, f32p, i32, i32, i32, vp, vp]
+    l.d4d_op_conv_resample.argtypes = [vp, i32, i32, i32, i32, vp, i32, f32p, i32, i32, i32, vp, vp, vp]
     l.d4d_op_layernorm.argtypes = [vp, i32, i32, f32, f32p, f32p, vp, vp]
     l.d4d_debug_tap.argtypes = [vp, vp, vp, vp, C.POINTER(C.c_int32), i32, i32, i32, i32, i32, i32, vp, C.c_char_p,
                                 C.POINTER(C.c_int32), vp]

@@ -45,7 +45,7 @@ struct DeviceGuard {
 extern "C" {
 
 const char* d4d_last_error(void) { return d4d::g_last_error.c_str(); }
-int d4d_version(void) { return 100; }
+int d4d_version(void) { return 101; }
 
 int d4d_create(const d4d_config* cfg, int device, d4d_handle** out) {
   D4D_API_BEGIN
@@ -212,7 +212,8 @@ int d4d_cfg_ddim_step(const void* noise, const void* latents, const void* cond_m
 
 int d4d_op_gemm(const void* A, int lda, int K1, const void* A2, int lda2, int K2, const void* W, int M, int N,
                 const float* bias, const void* rowvec, int ld_rowvec, int rows_per_image, const void* residual,
-                int ld_res, void* out, int ldo, int geglu, int act, float out_scale, int block_n, void* stream) {
+                int ld_res, void* out, int ldo, int geglu, int act, float out_scale, int block_n, int64_t* stats,
+                int stats_rows, void* stream) {
   D4D_API_BEGIN
   d4d::GemmDesc d;
   d.A = static_cast<const bf16*>(A); d.lda = lda; d.K1 = K1;
@@ -221,6 +222,7 @@ int d4d_op_gemm(const void* A, int lda, int K1, const void* A2, int lda2, int K2
   d.rowvec = static_cast<const bf16*>(rowvec); d.ld_rowvec = ld_rowvec; d.rows_per_image = rows_per_image;
   d.residual = static_cast<const bf16*>(residual); d.ld_res = ld_res;
   d.out = static_cast<bf16*>(out); d.ldo = ldo; d.geglu = geglu; d.act = act; d.out_scale = out_scale; d.block_n = block_n;
+  d.stats = reinterpret_cast<long long*>(stats); d.stats_rows = stats_rows;
   D4D_REQUIRE(M > 0, "empty GEMM");
   d4d::GemmLaunch L;
   if (int rc = d4d::gemm_prepare(d, &L)) return rc;
@@ -230,7 +232,7 @@ int d4d_op_gemm(const void* A, int lda, int K1, const void* A2, int lda2, int K2
 
 int d4d_op_conv3x3(const void* x_nhwc, int n_img, int H, int W, int Cin, const void* Wt, int Cout, const float* bias,
                    const void* rowvec, int ld_rowvec, const void* residual, int act, void* out, int block_n,
-                   void* stream) {
+                   int64_t* stats, void* stream) {
   D4D_API_BEGIN
   D4D_REQUIRE(n_img > 0 && H > 0 && W > 0, "empty conv");
   d4d::GemmDesc d;
@@ -239,6 +241,7 @@ int d4d_op_conv3x3(const void* x_nhwc, int n_img, int H, int W, int Cin, const v
   d.rowvec = static_cast<const bf16*>(rowvec); d.ld_rowvec = ld_rowvec;
   d.residual = static_cast<const bf16*>(residual); d.ld_res = Cout;
   d.out = static_cast<bf16*>(out); d.ldo = Cout; d.act = act; d.block_n = block_n;
+  d.stats = reinterpret_cast<long long*>(stats);
   d4d::GemmLaunch L;
   if (int rc = d4d::gemm_prepare(d, &L)) return rc;
   return d4d::gemm_run(L, static_cast<cudaStream_t>(stream));
@@ -246,12 +249,13 @@ int d4d_op_conv3x3(const void* x_nhwc, int n_img, int H, int W, int Cin, const v
 }
 
 int d4d_op_attention(const void* q, const void* k, const void* v, int ld_qkv, void* out, int ld_out, int batch, int seq,
-                     int heads, int head_dim, float scale, void* stream) {
+                     int heads, int head_dim, float scale, int seq_kv, int ld_kv, void* stream) {
   D4D_API_BEGIN
   d4d::AttnDesc d;
   d.q = static_cast<const bf16*>(q); d.k = static_cast<const bf16*>(k); d.v = static_cast<const bf16*>(v);
   d.ld_qkv = ld_qkv; d.out = static_cast<bf16*>(out); d.ld_out = ld_out;
   d.batch = batch; d.seq = seq; d.heads = heads; d.head_dim = head_dim; d.scale = scale;
+  d.seq_kv = seq_kv; d.ld_kv = ld_kv;
   d4d::AttnLaunch L;
   if (int rc = d4d::attn_prepare(d, &L)) return rc;
   return d4d::attn_run(L, static_cast<cudaStream_t>(stream));
@@ -276,7 +280,7 @@ int d4d_op_groupnorm(const void* x1, int C1, const void* x2, int C2, int n_img, 
 }
 
 int d4d_op_conv_resample(const void* x_nhwc, int n_img, int H, int W, int Cin, const void* Wt, int Cout, const float* bias,
-                         int kind, int up_a, int up_b, void* out, void* stream) {
+                         int kind, int up_a, int up_b, void* out, int64_t* stats, void* stream) {
   D4D_API_BEGIN
   D4D_REQUIRE(n_img > 0 && H > 0 && W > 0 && kind >= 1 && kind <= 3, "conv_resample arguments");
   d4d::GemmDesc d;
@@ -284,6 +288,7 @@ int d4d_op_conv_resample(const void* x_nhwc, int n_img, int H, int W, int Cin, c
   d.A = static_cast<const bf16*>(x_nhwc); d.n_img = n_img; d.H = H; d.W = W; d.Cin = Cin;
   d.Wt = static_cast<const bf16*>(Wt); d.N = Cout; d.bias = bias;
   d.out = static_cast<bf16*>(out); d.ldo = Cout;
+  d.stats = reinterpret_cast<long long*>(stats);
   d4d::GemmLaunch L;
   if (int rc = d4d::gemm_prepare(d, &L)) return rc;
   return d4d::gemm_run(L, static_cast<cudaStream_t>(stream));

@@ -352,6 +352,8 @@ int gemm_prepare(const GemmDesc& d, GemmLaunch* L) {
   a.stats_rows = d.stats_rows > 0 ? d.stats_rows : 1;
   D4D_REQUIRE(d.stats == nullptr || (!d.geglu && d.kv_world == 0), "GroupNorm statistics: plain / conv epilogue only");
   D4D_REQUIRE(d.stats == nullptr || d.conv || (d.stats_rows > 0 && d.stats_rows % 32 == 0), "statistics need rows-per-image % 32 == 0");
+  // rows past the last whole image would add into image M / stats_rows, past the [M / stats_rows][N][2] workspace
+  D4D_REQUIRE(d.stats == nullptr || d.conv || d.M % d.stats_rows == 0, "statistics need M % rows-per-image == 0");
   a.kv_world = d.kv_world;
   a.kv_col0 = d.kv_col0;
   a.kv_ld = d.kv_ld;

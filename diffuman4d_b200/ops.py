@@ -22,12 +22,27 @@ def _bf16c(t: torch.Tensor, name: str):
         raise ValueError(f"{name} must be a contiguous CUDA bfloat16 tensor")
 
 
+def _stats_ws(stats: Optional[torch.Tensor], n_img: int, C: int):
+    """Pointer of a GroupNorm statistics workspace: contiguous CUDA int64 holding at least [n_img][C][2] words, which the
+    kernel ADDS into (pass it zeroed).  None passes NULL (no statistics)."""
+    if stats is None:
+        return None
+    if stats.dtype != torch.int64 or not stats.is_cuda or not stats.is_contiguous():
+        raise ValueError("stats must be a contiguous CUDA int64 tensor")
+    if stats.numel() < n_img * C * 2:
+        raise ValueError(f"stats needs at least {n_img} x {C} x 2 words")
+    return stats.data_ptr()
+
+
 def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, *, a2: Optional[torch.Tensor] = None,
          rowvec: Optional[torch.Tensor] = None, rows_per_image: int = 0, residual: Optional[torch.Tensor] = None,
-         geglu: bool = False, act: int = 0, out_scale: float = 1.0, block_n: int = 0) -> torch.Tensor:
+         geglu: bool = False, act: int = 0, out_scale: float = 1.0, block_n: int = 0, stats: Optional[torch.Tensor] = None,
+         stats_rows: int = 0) -> torch.Tensor:
     """out = act((a | a2) @ w.T + bias + rowvec[row // rows_per_image]) * out_scale + residual   (bf16, fp32 accumulate).
     With ``geglu`` the rows of ``w``/``bias`` must already be tile-interleaved (see ``interleave_geglu``);
-    ``block_n`` = 0 picks the tile width, otherwise it must be a multiple of 16 that divides N."""
+    ``block_n`` = 0 picks the tile width, otherwise it must be a multiple of 16 that divides N.
+    ``stats``: zeroed int64 [M // stats_rows, N, 2] that receives the GroupNorm statistics of ``out`` (image = row //
+    stats_rows; stats_rows a multiple of 32 that divides M)."""
     _bf16c(a, "a"), _bf16c(w, "w")
     M, K1 = a.shape
     K2 = 0 if a2 is None else a2.shape[1]
@@ -40,7 +55,9 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, 
     check(lib().d4d_op_gemm(_p(a), a.stride(0), K1, _p(a2), 0 if a2 is None else a2.stride(0), K2, _p(w), M, N,
                             _p(bias), _p(rowvec), 0 if rowvec is None else rowvec.stride(0), rows_per_image,
                             _p(residual), 0 if residual is None else residual.stride(0), _p(out), out.stride(0),
-                            int(geglu), act, float(out_scale), block_n, _stream()), "d4d_op_gemm")
+                            int(geglu), act, float(out_scale), block_n,
+                            _stats_ws(stats, M // stats_rows if stats_rows > 0 else 0, N), stats_rows, _stream()),
+          "d4d_op_gemm")
     return out
 
 
@@ -59,15 +76,16 @@ def interleave_geglu(w: torch.Tensor, bias: torch.Tensor):
 
 def conv3x3(x_nhwc: torch.Tensor, w_octi: torch.Tensor, bias: Optional[torch.Tensor] = None, *,
             rowvec: Optional[torch.Tensor] = None, residual: Optional[torch.Tensor] = None, act: int = 0,
-            block_n: int = 0) -> torch.Tensor:
-    """3x3 / stride 1 / pad 1 conv on NHWC activations.  ``w_octi``: [Cout, 9, Cin] (tap = ky*3+kx)."""
+            block_n: int = 0, stats: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """3x3 / stride 1 / pad 1 conv on NHWC activations.  ``w_octi``: [Cout, 9, Cin] (tap = ky*3+kx).
+    ``stats``: zeroed int64 [n, Cout, 2] that receives the GroupNorm statistics of the output."""
     _bf16c(x_nhwc, "x"), _bf16c(w_octi, "w")
     n, H, W, Cin = x_nhwc.shape
     Cout = w_octi.shape[0]
     out = torch.empty(n, H, W, Cout, device=x_nhwc.device, dtype=torch.bfloat16)
     check(lib().d4d_op_conv3x3(_p(x_nhwc), n, H, W, Cin, _p(w_octi), Cout, _p(bias), _p(rowvec),
                                0 if rowvec is None else rowvec.stride(0), _p(residual), act, _p(out), block_n,
-                               _stream()), "d4d_op_conv3x3")
+                               _stats_ws(stats, n, Cout), _stream()), "d4d_op_conv3x3")
     return out
 
 
@@ -76,40 +94,53 @@ def conv_weight_to_octi(w_oihw: torch.Tensor) -> torch.Tensor:
     return w_oihw.permute(0, 2, 3, 1).reshape(co, kh * kw, ci).contiguous()
 
 
-def attention(qkv: torch.Tensor, batch: int, seq: int, heads: int, head_dim: int, scale: float) -> torch.Tensor:
-    """qkv: [batch*seq, 3*heads*head_dim] (q | k | v column blocks, head-major inside each).  Returns [batch*seq, heads*head_dim]."""
+def attention(qkv: torch.Tensor, batch: int, seq: int, heads: int, head_dim: int, scale: float, *,
+              kv: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """qkv: [batch*seq, 3*heads*head_dim] (q | k | v column blocks, head-major inside each).  Returns [batch*seq, heads*head_dim].
+    ``kv``: keys and values from a separate [batch*seq_kv, 2*heads*head_dim] matrix (k | v column blocks; batch entry b
+    owns rows [b*seq_kv, (b+1)*seq_kv)), as the frame-sharded window gathers them; qkv then supplies only the queries."""
     _bf16c(qkv, "qkv")
     C = heads * head_dim
     if qkv.shape != (batch * seq, 3 * C):
         raise ValueError("qkv shape")
     out = torch.empty(batch * seq, C, device=qkv.device, dtype=torch.bfloat16)
     base = qkv.data_ptr()
-    check(lib().d4d_op_attention(base, base + 2 * C, base + 4 * C, qkv.stride(0), _p(out), C, batch, seq, heads,
-                                 head_dim, float(scale), _stream()), "d4d_op_attention")
+    k, v, seq_kv, ld_kv = base + 2 * C, base + 4 * C, 0, 0
+    if kv is not None:
+        _bf16c(kv, "kv")
+        if kv.dim() != 2 or kv.shape[1] != 2 * C or kv.shape[0] % batch != 0 or kv.shape[0] == 0:
+            raise ValueError("kv must be [batch*seq_kv, 2*heads*head_dim]")
+        k, v, seq_kv, ld_kv = kv.data_ptr(), kv.data_ptr() + 2 * C, kv.shape[0] // batch, kv.stride(0)
+    check(lib().d4d_op_attention(base, k, v, qkv.stride(0), _p(out), C, batch, seq, heads, head_dim, float(scale),
+                                 seq_kv, ld_kv, _stream()), "d4d_op_attention")
     return out
 
 
 def groupnorm(x1: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, groups: int, eps: float, silu: bool,
-              x2: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """x1: [n_img, hw, C1] (+ x2 [n_img, hw, C2] virtually concatenated on channels) -> [n_img, hw, C1+C2]."""
+              x2: Optional[torch.Tensor] = None, *, stats: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """x1: [n_img, hw, C1] (+ x2 [n_img, hw, C2] virtually concatenated on channels) -> [n_img, hw, C1+C2].
+    ``stats``: zeroed int64 [n_img, C1+C2, 2] that keeps the statistics the norm computed (allocated when None)."""
     _bf16c(x1, "x1")
     n_img, hw, C1 = x1.shape
     C2 = 0 if x2 is None else x2.shape[2]
     out = torch.empty(n_img, hw, C1 + C2, device=x1.device, dtype=torch.bfloat16)
-    stats = torch.zeros(n_img, C1 + C2, 2, device=x1.device, dtype=torch.int64)
+    if stats is None:
+        stats = torch.zeros(n_img, C1 + C2, 2, device=x1.device, dtype=torch.int64)
     check(lib().d4d_op_groupnorm(_p(x1), C1, _p(x2), C2, n_img, hw, groups, float(eps), _p(gamma), _p(beta),
-                                 int(silu), _p(out), _p(stats), _stream()), "d4d_op_groupnorm")
+                                 int(silu), _p(out), _stats_ws(stats, n_img, C1 + C2), _stream()), "d4d_op_groupnorm")
     return out
 
 
-def conv3x3_stride2(x_nhwc: torch.Tensor, w_octi: torch.Tensor, bias: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """3x3 / stride 2 / pad 1 conv (Downsample2D) through a strided tensor map: [n,H,W,Cin] -> [n,H/2,W/2,Cout]."""
+def conv3x3_stride2(x_nhwc: torch.Tensor, w_octi: torch.Tensor, bias: Optional[torch.Tensor] = None, *,
+                    stats: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """3x3 / stride 2 / pad 1 conv (Downsample2D) through a strided tensor map: [n,H,W,Cin] -> [n,H/2,W/2,Cout].
+    ``stats``: zeroed int64 [n, Cout, 2] that receives the GroupNorm statistics of the output."""
     _bf16c(x_nhwc, "x"), _bf16c(w_octi, "w")
     n, H, W, Cin = x_nhwc.shape
     Cout = w_octi.shape[0]
     out = torch.empty(n, H // 2, W // 2, Cout, device=x_nhwc.device, dtype=torch.bfloat16)
-    check(lib().d4d_op_conv_resample(_p(x_nhwc), n, H, W, Cin, _p(w_octi), Cout, _p(bias), 1, 0, 0, _p(out), _stream()),
-          "d4d_op_conv_resample")
+    check(lib().d4d_op_conv_resample(_p(x_nhwc), n, H, W, Cin, _p(w_octi), Cout, _p(bias), 1, 0, 0, _p(out),
+                                     _stats_ws(stats, n, Cout), _stream()), "d4d_op_conv_resample")
     return out
 
 
@@ -132,37 +163,42 @@ def upsample_phase_weights(w_oihw: torch.Tensor):
 
 
 def upsample2x_conv3x3(x_nhwc: torch.Tensor, w_oihw: torch.Tensor, bias: Optional[torch.Tensor] = None,
-                       single_launch: bool = True) -> torch.Tensor:
-    """nearest x2 upsample followed by a 3x3 / pad 1 conv (Upsample2D) as four sub-pixel phases on the low-res input."""
+                       single_launch: bool = True, *, stats: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """nearest x2 upsample followed by a 3x3 / pad 1 conv (Upsample2D) as four sub-pixel phases on the low-res input.
+    ``stats``: zeroed int64 [n, Cout, 2] that receives the GroupNorm statistics of the output."""
     _bf16c(x_nhwc, "x")
     n, H, W, Cin = x_nhwc.shape
     Cout = w_oihw.shape[0]
     out = torch.empty(n, 2 * H, 2 * W, Cout, device=x_nhwc.device, dtype=torch.bfloat16)
     phases = upsample_phase_weights(w_oihw)
+    st = _stats_ws(stats, n, Cout)
     if single_launch:
         wp = torch.stack(phases).contiguous()                                          # [4, Cout, 4, Cin]
-        check(lib().d4d_op_conv_resample(_p(x_nhwc), n, H, W, Cin, _p(wp), Cout, _p(bias), 3, 0, 0, _p(out), _stream()),
-              "d4d_op_conv_resample")
+        check(lib().d4d_op_conv_resample(_p(x_nhwc), n, H, W, Cin, _p(wp), Cout, _p(bias), 3, 0, 0, _p(out), st,
+                                         _stream()), "d4d_op_conv_resample")
         return out
     for ph, wp in enumerate(phases):
         check(lib().d4d_op_conv_resample(_p(x_nhwc), n, H, W, Cin, _p(wp), Cout, _p(bias), 2, ph >> 1, ph & 1, _p(out),
-                                         _stream()), "d4d_op_conv_resample")
+                                         st, _stream()), "d4d_op_conv_resample")
     return out
 
 
 def conv3x3_groupnorm(x_nhwc: torch.Tensor, w_octi: torch.Tensor, bias: Optional[torch.Tensor], gamma: torch.Tensor,
-                      beta: torch.Tensor, groups: int, eps: float, silu: bool, residual: Optional[torch.Tensor] = None):
+                      beta: torch.Tensor, groups: int, eps: float, silu: bool, residual: Optional[torch.Tensor] = None, *,
+                      stats: Optional[torch.Tensor] = None):
     """conv3x3 whose epilogue accumulates the GroupNorm statistics of its output + the GroupNorm(+SiLU) that consumes them
-    (no statistics pass).  Returns (conv_out, gn_out), both [n, H, W, Cout]."""
+    (no statistics pass).  Returns (conv_out, gn_out), both [n, H, W, Cout].  ``stats``: zeroed int64 [n, Cout, 2] that
+    keeps the statistics (allocated when None)."""
     _bf16c(x_nhwc, "x"), _bf16c(w_octi, "w")
     n, H, W, Cin = x_nhwc.shape
     Cout = w_octi.shape[0]
     conv_out = torch.empty(n, H, W, Cout, device=x_nhwc.device, dtype=torch.bfloat16)
     gn_out = torch.empty_like(conv_out)
-    stats = torch.zeros(n, Cout, 2, device=x_nhwc.device, dtype=torch.int64)
+    if stats is None:
+        stats = torch.zeros(n, Cout, 2, device=x_nhwc.device, dtype=torch.int64)
     check(lib().d4d_op_conv3x3_groupnorm(_p(x_nhwc), n, H, W, Cin, _p(w_octi), Cout, _p(bias), _p(residual), groups,
-                                         float(eps), _p(gamma), _p(beta), int(silu), _p(conv_out), _p(gn_out), _p(stats),
-                                         _stream()), "d4d_op_conv3x3_groupnorm")
+                                         float(eps), _p(gamma), _p(beta), int(silu), _p(conv_out), _p(gn_out),
+                                         _stats_ws(stats, n, Cout), _stream()), "d4d_op_conv3x3_groupnorm")
     return conv_out, gn_out
 
 

@@ -123,16 +123,23 @@ int d4d_cfg_ddim_step(const void* noise, const void* latents, const void* cond_m
 /* ---- op-level entry points (each is one hot-path kernel; used by tests/ and bench.py) ------------------
  * d4d_op_gemm:   out[M,N] = act((A|A2)[M,K1+K2] . W[N,K]^T + bias + rowvec[row/rows_per_image]) * scale + residual
  *                geglu: W rows / bias interleaved in groups of 8 (a rows, then g rows), out is [M, N/2].
- * d4d_op_conv3x3: NHWC x [n,H,W,Cin], W [Cout][9][Cin] (tap = ky*3+kx), stride 1, pad 1.  */
+ * d4d_op_conv3x3: NHWC x [n,H,W,Cin], W [Cout][9][Cin] (tap = ky*3+kx), stride 1, pad 1.
+ * stats (gemm, conv3x3, conv_resample): NULL, or a caller-allocated, ZEROED int64 workspace that receives the GroupNorm
+ *   statistics of the stored output in d4d_op_groupnorm's format: per-(image, column) fixed-point {sum * 2^28, sum of
+ *   squares * 2^24}.  Conv: [n_img][Cout][2], needs tiles whose 32-row warps stay inside one image.  GEMM: [M /
+ *   stats_rows][N][2], image = row / stats_rows; needs stats_rows % 32 == 0 and M % stats_rows == 0, and no GEGLU.  */
 int d4d_op_gemm(const void* A, int lda, int K1, const void* A2, int lda2, int K2, const void* W, int M, int N,
                 const float* bias, const void* rowvec, int ld_rowvec, int rows_per_image, const void* residual,
-                int ld_res, void* out, int ldo, int geglu, int act, float out_scale, int block_n, void* stream);
+                int ld_res, void* out, int ldo, int geglu, int act, float out_scale, int block_n, int64_t* stats,
+                int stats_rows, void* stream);
 int d4d_op_conv3x3(const void* x_nhwc, int n_img, int H, int W, int Cin, const void* Wt, int Cout, const float* bias,
                    const void* rowvec, int ld_rowvec, const void* residual, int act, void* out, int block_n,
-                   void* stream);
-/* q, k, v: column slices of one row-major [batch*seq, ld_qkv] matrix; head hd = columns [hd*D, (hd+1)*D). */
+                   int64_t* stats, void* stream);
+/* q: column slice of a row-major [batch*seq, ld_qkv] matrix; head hd = columns [hd*D, (hd+1)*D).  k, v: column slices of a
+ * row-major [batch*seq_kv, ld_kv] matrix, the keys of batch entry b in rows [b*seq_kv, (b+1)*seq_kv).  seq_kv = 0 means
+ * seq and ld_kv = 0 means ld_qkv (k and v in the QKV matrix). */
 int d4d_op_attention(const void* q, const void* k, const void* v, int ld_qkv, void* out, int ld_out, int batch,
-                     int seq, int heads, int head_dim, float scale, void* stream);
+                     int seq, int heads, int head_dim, float scale, int seq_kv, int ld_kv, void* stream);
 /* GroupNorm(+SiLU) of NHWC x1 [n_img, hw, C1], virtually concatenated on channels with x2 [n_img, hw, C2] when x2 is not
  * NULL, into out [n_img, hw, C1+C2]; 32 <= C1 + C2 <= 4096, C1 and C2 multiples of 8.  One statistics launch per source
  * fills `stats`, then one launch normalises.  stats: caller-allocated, ZEROED int64 workspace [n_img][C1+C2][2] (x1's
@@ -146,7 +153,7 @@ int d4d_op_groupnorm(const void* x1, int C1, const void* x2, int C2, int n_img, 
  *           up_a = 1, same for columns), written to pixels (2y+up_a, 2x+up_b) of out [n,2H,2W,Cout].  Four calls fill out;
  *   kind 3: all four phases in one launch, Wt [4 (= up_a*2+up_b)][Cout][4][Cin] (what the UNet plan uses). */
 int d4d_op_conv_resample(const void* x_nhwc, int n_img, int H, int W, int Cin, const void* Wt, int Cout, const float* bias,
-                         int kind, int up_a, int up_b, void* out, void* stream);
+                         int kind, int up_a, int up_b, void* out, int64_t* stats, void* stream);
 /* conv3x3 (+bias, +residual) whose epilogue accumulates the per-(image, channel) sums of its output, followed by the
  * GroupNorm(+SiLU) that reads those sums instead of running a statistics pass: the pair every ResnetBlock2D of the UNet
  * executes (needs H*W % 32 == 0).  conv_out [n,H,W,Cout] and gn_out [n,H,W,Cout] are both written.  stats:

@@ -38,6 +38,18 @@ def _within_bf16_ulp(out, ref):
     assert (err <= ulp).all(), f"max err {err.max().item():.4g}, {int((err > ulp).sum())} / {err.numel()} beyond one ulp"
 
 
+def _stats_exact(stats, y):
+    """stats [n, C, 2] are the fixed-point {sum * 2^28, sum of squares * 2^24} of the stored y [n, ..., C]: within the fp32
+    rounding of 16-term partials (2^-20 relative) plus half a fixed-point unit per partial.  One missing or doubled
+    16-row partial misses by orders of magnitude."""
+    n, C = stats.shape[0], stats.shape[1]
+    y = y.reshape(n, -1, C).double()
+    hw = y.shape[1]
+    s, q = stats[..., 0].double() * 2.0 ** -28, stats[..., 1].double() * 2.0 ** -24
+    assert ((s - y.sum(1)).abs() <= 2.0 ** -20 * y.abs().sum(1) + hw * 2.0 ** -28).all(), "sums"
+    assert ((q - (y * y).sum(1)).abs() <= 2.0 ** -20 * (y * y).sum(1) + hw * 2.0 ** -24).all(), "sums of squares"
+
+
 def _rand(shape, seed, std=1.0, device="cuda"):
     g = torch.Generator().manual_seed(seed)
     return (torch.randn(shape, generator=g) * std).to(torch.bfloat16).to(device)
@@ -197,9 +209,13 @@ def test_conv3x3_fused_groupnorm_stats(cuda, n, H, W, Cin, Cout, silu):
     res = _rand((n, H, W, Cout), 73)
     gamma = (1 + 0.2 * torch.randn(Cout, generator=g)).cuda()
     beta = (0.1 * torch.randn(Cout, generator=g)).cuda()
-    conv_out, gn_out = ops.conv3x3_groupnorm(x, ops.conv_weight_to_octi(w), bias, gamma, beta, 32, 1e-5, silu, residual=res)
+    stats = torch.zeros(n, Cout, 2, dtype=torch.int64, device="cuda")
+    conv_out, gn_out = ops.conv3x3_groupnorm(x, ops.conv_weight_to_octi(w), bias, gamma, beta, 32, 1e-5, silu, residual=res,
+                                             stats=stats)
     ref_conv = F.conv2d(x.float().permute(0, 3, 1, 2), w.float(), bias, padding=1).permute(0, 2, 3, 1) + res.float()
     _close(conv_out, ref_conv)
+    # the epilogue's statistics are exact sums of what it stored (the normalised output below cannot see one lost partial)
+    _stats_exact(stats, conv_out)
     # GroupNorm reference on the bf16 tensor the kernel actually stored (what the next layer of the reference sees)
     ref = F.group_norm(conv_out.float().permute(0, 3, 1, 2), 32, gamma, beta, 1e-5).permute(0, 2, 3, 1)
     if silu:
