@@ -45,7 +45,7 @@ struct DeviceGuard {
 extern "C" {
 
 const char* d4d_last_error(void) { return d4d::g_last_error.c_str(); }
-int d4d_version(void) { return 101; }
+int d4d_version(void) { return 102; }
 
 int d4d_create(const d4d_config* cfg, int device, d4d_handle** out) {
   D4D_API_BEGIN
@@ -321,6 +321,24 @@ int d4d_op_layernorm(const void* x, int rows, int C, float eps, const float* gam
   D4D_API_BEGIN
   return d4d::layernorm_run(static_cast<const bf16*>(x), rows, C, eps, gamma, beta, static_cast<bf16*>(out),
                             static_cast<cudaStream_t>(stream));
+  D4D_API_END
+}
+
+int d4d_op_pose_conv0(const void* x_nchw, int n, int H, int W, const void* Wt, const float* bias, void* out_nhwc4,
+                      void* stream) {
+  D4D_API_BEGIN
+  D4D_REQUIRE(n > 0 && H > 0 && W > 0, "empty pose conv");
+  return d4d::pose_conv0_run(static_cast<const bf16*>(x_nchw), n, H, W, static_cast<const bf16*>(Wt), bias,
+                             static_cast<bf16*>(out_nhwc4), static_cast<cudaStream_t>(stream));
+  D4D_API_END
+}
+
+int d4d_op_pose_conv(const void* x_nhwc, int n, int Cin, int H, int W, const void* Wt, const float* bias, int Cout,
+                     int ksize, int stride, void* out, void* stream) {
+  D4D_API_BEGIN
+  D4D_REQUIRE(n > 0 && H > 0 && W > 0, "empty pose conv");
+  return d4d::pose_conv_run(static_cast<const bf16*>(x_nhwc), n, Cin, H, W, static_cast<const bf16*>(Wt), bias, Cout,
+                            ksize, stride, static_cast<bf16*>(out), static_cast<cudaStream_t>(stream));
   D4D_API_END
 }
 

@@ -459,6 +459,9 @@ int pose_conv0_run(const bf16* x_nchw, int n, int H, int W, const bf16* w, const
 
 int pose_conv_run(const bf16* x, int n, int Cin, int H, int W, const bf16* w, const float* bias, int Cout, int ksize,
                   int stride, bf16* out_nhwc, cudaStream_t stream) {
+  // pad 1 on each side: a kernel larger than the padded input has no output pixel (C's truncating division below
+  // would still count one)
+  D4D_REQUIRE(H + 2 >= ksize && W + 2 >= ksize, "pose conv: kernel larger than the padded input");
   const int Ho = (H + 2 - ksize) / stride + 1, Wo = (W + 2 - ksize) / stride + 1;
   const long long total = static_cast<long long>(n) * Ho * Wo;
   D4D_REQUIRE(static_cast<long long>(n) * H * W * Cin < (1ll << 31) && total * Cout < (1ll << 31), "pose conv: 32-bit offsets");

@@ -202,6 +202,54 @@ def conv3x3_groupnorm(x_nhwc: torch.Tensor, w_octi: torch.Tensor, bias: Optional
     return conv_out, gn_out
 
 
+def pose_conv_weights(w_oihw: torch.Tensor) -> torch.Tensor:
+    """The pose-encoder conv weight layouts of ``pose_conv0`` / ``pose_conv`` (same transform the C++ weight loader
+    applies, csrc/unet.cu).  conv_layers.0 ([3, 3, 3, 3]) -> [9, 3, 3] = [tap][Cin][Cout]; conv_layers.2/4/6/8 ->
+    [Cout, k*k*cp + 8] with column tap*cp + ci (tap = ky*k+kx), cp = max(Cin, 4): 4 for conv_layers.2 (Cin 3, zero
+    weights for the pad channel), Cin for the others; and 8 zero columns that skew the rows over the shared-memory banks."""
+    co, ci, k, _ = w_oihw.shape
+    w = w_oihw.float()
+    if (co, ci, k) == (3, 3, 3):
+        return w.permute(2, 3, 1, 0).reshape(9, 3, 3).to(torch.bfloat16).contiguous()
+    cp = max(ci, 4)
+    out = torch.zeros(co, k * k, cp, device=w.device)
+    out[:, :, :ci] = w.permute(0, 2, 3, 1).reshape(co, k * k, ci)
+    out = torch.cat([out.reshape(co, k * k * cp), torch.zeros(co, 8, device=w.device)], 1)
+    return out.to(torch.bfloat16).contiguous()
+
+
+def pose_conv0(x: torch.Tensor, w_packed: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
+    """Pose encoder conv_layers.0 + SiLU: NCHW skeletons x [n, 3, H, W] -> NHWC [n, H, W, 4] with channel 3 = 0.
+    ``w_packed`` from ``pose_conv_weights``; ``bias`` fp32 [3]."""
+    _bf16c(x, "x"), _bf16c(w_packed, "w")
+    if x.dim() != 4 or x.shape[1] != 3 or w_packed.numel() != 81:
+        raise ValueError("pose_conv0 needs x [n, 3, H, W] and packed weights [9, 3, 3]")
+    if bias.dtype != torch.float32 or bias.numel() != 3:
+        raise ValueError("bias must be float32 [3]")
+    n, _, H, W = x.shape
+    out = torch.empty(n, H, W, 4, device=x.device, dtype=torch.bfloat16)
+    check(lib().d4d_op_pose_conv0(_p(x), n, H, W, _p(w_packed), _p(bias), _p(out), _stream()), "d4d_op_pose_conv0")
+    return out
+
+
+def pose_conv(x: torch.Tensor, w_packed: torch.Tensor, bias: torch.Tensor, ksize: int, stride: int) -> torch.Tensor:
+    """Pose encoder conv_layers.2/4/6/8 + SiLU (pad 1) on NHWC x [n, H, W, Cin] -> [n, Ho, Wo, Cout].  Cin is 4 for
+    conv_layers.2, which reads conv_layers.0's padded pixels.  ``w_packed`` [Cout, k*k*Cin + 8] from
+    ``pose_conv_weights``; ``bias`` fp32 [Cout]."""
+    _bf16c(x, "x"), _bf16c(w_packed, "w")
+    n, H, W, Cin = x.shape
+    Cout = w_packed.shape[0]
+    if w_packed.dim() != 2 or w_packed.shape[1] != ksize * ksize * Cin + 8:
+        raise ValueError("w must be [Cout, ksize*ksize*Cin + 8]")
+    if bias.dtype != torch.float32 or bias.numel() != Cout:
+        raise ValueError("bias must be float32 [Cout]")
+    Ho, Wo = (H + 2 - ksize) // stride + 1, (W + 2 - ksize) // stride + 1
+    out = torch.empty(n, Ho, Wo, Cout, device=x.device, dtype=torch.bfloat16)
+    check(lib().d4d_op_pose_conv(_p(x), n, Cin, H, W, _p(w_packed), _p(bias), Cout, ksize, stride, _p(out), _stream()),
+          "d4d_op_pose_conv")
+    return out
+
+
 def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float = 1e-5) -> torch.Tensor:
     _bf16c(x, "x")
     rows, C = x.shape

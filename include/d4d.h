@@ -163,6 +163,17 @@ int d4d_op_conv3x3_groupnorm(const void* x_nhwc, int n_img, int H, int W, int Ci
                              const float* beta, int silu, void* conv_out, void* gn_out, int64_t* stats, void* stream);
 int d4d_op_layernorm(const void* x, int rows, int C, float eps, const float* gamma, const float* beta, void* out,
                      void* stream);
+/* Pose encoder, conv_layers.0: 3 -> 3 channels, 3x3, stride 1, pad 1, + bias, SiLU.  x_nchw [n,3,H,W] (the skeleton
+ * images), Wt [9][3][3] = [tap = ky*3+kx][Cin][Cout], bias fp32 [3], out_nhwc4 [n,H,W,4] with channel 3 written as 0. */
+int d4d_op_pose_conv0(const void* x_nchw, int n, int H, int W, const void* Wt, const float* bias, void* out_nhwc4,
+                      void* stream);
+/* Pose encoder, conv_layers.2/4/6/8: pad 1, + bias, SiLU, NHWC x [n,H,W,Cin] -> out [n,Ho,Wo,Cout],
+ * Ho = (H + 2 - ksize) / stride + 1 (Wo alike).  (Cin, Cout, ksize, stride) is one of (4,16,4,2) (conv_layers.2 reading
+ * conv_layers.0's 4-channel pixels), (16,16,3,1), (16,32,4,2), (32,32,3,1); anything else returns 1.  Wt: 16-byte aligned
+ * [Cout][ksize*ksize*Cin + 8], column tap*Cin + ci with tap = ky*ksize+kx; the 8 trailing columns of each row are not read
+ * for arithmetic, and for Cin 4 the weights of channel 3 must be 0.  bias fp32 [Cout]. */
+int d4d_op_pose_conv(const void* x_nhwc, int n, int Cin, int H, int W, const void* Wt, const float* bias, int Cout,
+                     int ksize, int stride, void* out, void* stream);
 /* Debug tap (per-level drift reports in tests/): runs the forward of d4d_unet_forward up to intermediate activation
  * `tap` (0 = conv_in(+pose), then down_blocks.0-3, mid_block, up_blocks.0-3) and copies it out as NCHW bf16
  * [B, C, H, W].  name64 (64 bytes) / dims3 (C, H, W) are filled when non-NULL; out == NULL only queries them.
