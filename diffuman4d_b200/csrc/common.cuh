@@ -38,9 +38,6 @@ void set_error(const std::string& msg);          // thread-local last error (d4d
 // 2-D row-major bf16 matrix [rows, cols] with leading dimension ld (elements); box = {box_cols, box_rows}.
 int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
                  uint32_t box_cols, uint32_t box_rows, int swizzle_bytes);
-// NHWC bf16 tensor [n, h, w, c] as the DESTINATION of 32-row x 32-channel epilogue boxes {32, box_w, box_h, box_n}
-int make_tmap_nhwc_store(CUtensorMap* out, void* base, uint64_t n, uint64_t h, uint64_t w, uint64_t c, uint32_t box_w,
-                         uint32_t box_h, uint32_t box_n);
 // 4-D NHWC bf16 tensor [n, h, w, c]; box = {box_c, box_w, box_h, box_n} ELEMENTS LOADED; `stride` > 1 loads every
 // stride-th pixel along w and h (elementStrides: the box then spans stride * box_w x stride * box_h pixels).
 int make_tmap_nhwc(CUtensorMap* out, const void* base, uint64_t n, uint64_t h, uint64_t w, uint64_t c,
@@ -107,6 +104,18 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
+// barrier over `threads` threads (a multiple of 32) on hardware barrier `id` (0 is __syncthreads)
+__device__ __forceinline__ void named_barrier_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
+}
 // programmatic dependent launch (see launch_pdl in kernels.h): wait for the predecessor grid's memory, then let the successor
 // grid become resident
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -139,10 +148,6 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* t, uin
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* t, const void* src, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
                ::"l"(reinterpret_cast<uint64_t>(t)), "r"(smem_u32(src)), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* t, const void* src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(t)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
 __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void bulk_wait_group_read() {  // <= N groups still READING shared memory

@@ -7,6 +7,9 @@
 //   warpgroups 1 and 2 each own 64 rows of the 128-row tile and issue wgmma.m64nBNk16 with fp32 accumulators in
 //   registers.  The kernel is persistent (grid = #SMs) and walks tiles n-fastest, so CTAs that run concurrently share
 //   the same A rows through L2; the producer runs ahead into the next tile while the MMA warpgroups run the epilogue.
+// * plain GEMMs stage the epilogue in shared memory: each MMA warpgroup writes its finished 64 x BN bf16 rows into 32-column
+//   slabs (64B-swizzled, conflict-free), and one thread TMA-stores them and goes on into the next tile's MMAs while the
+//   stores drain.  The residual tile is TMA-loaded into the same slabs during the first k-block.
 // * "conv" mode turns the A loader into an implicit-GEMM gather: the A tile for k-block (tap, c0) is a 4-D TMA box
 //   {64 ch, BW, BH, BN} of the NHWC activation at spatial offset (ky-1, kx-1); out-of-bounds rows/cols are zero-filled
 //   by TMA, which is exactly the conv's zero padding.  K = 9*Cin, weights are pre-laid-out as [Cout][tap][Cin].
@@ -33,13 +36,19 @@ constexpr int BAR_BYTES = 1024;                 // barrier block in front of the
 constexpr int NUM_THREADS = 384;                // warpgroup 0: TMA producer, warpgroups 1-2: MMA + epilogue
 constexpr int MAX_SMEM = 227 * 1024;
 
-// Tile width BN (the wgmma N) is a template parameter; the ring takes as many stages as fit (at most 8).
-template <int BN>
+// staged epilogue: a slab is 64 rows x 32 columns of bf16 (64 B per row, TMA box {32, 64}, 64-byte swizzle)
+constexpr int SLAB_COLS = 32;
+constexpr int SLAB_BYTES = 64 * SLAB_COLS * 2;
+
+// Tile width BN (the wgmma N) is a template parameter; after the staging slabs of both warpgroups (plain GEMM only), the
+// ring takes as many stages as fit (at most 8).
+template <int BN, bool kStaged>
 struct GemmCfg {
   static constexpr int STAGE_BYTES = A_BYTES + BN * BLOCK_K * 2;
-  static constexpr int STAGES_FIT = (MAX_SMEM - 1024 - BAR_BYTES) / STAGE_BYTES;
+  static constexpr int STAGING_BYTES = kStaged ? 2 * 64 * BN * 2 : 0;
+  static constexpr int STAGES_FIT = (MAX_SMEM - 1024 - BAR_BYTES - STAGING_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;
-  static constexpr int SMEM = 1024 + BAR_BYTES + STAGES * STAGE_BYTES;
+  static constexpr int SMEM = 1024 + BAR_BYTES + STAGES * STAGE_BYTES + STAGING_BYTES;
 };
 
 struct TileCoord {
@@ -93,18 +102,24 @@ __device__ __forceinline__ void row_of(const GemmKernelArgs& a, const TileCoord&
 // Epilogue feature bits of the kernel template: a CLEAR bit compiles the feature out, a set bit is still checked at run
 // time.  gemm_run picks the instantiation whose bits equal the launch's features, or the E_ALL one.
 enum : int { E_BIAS = 1, E_ROWVEC = 2, E_ACT = 4, E_RES = 8, E_STATS = 16, E_KV = 32, E_ALL = 63 };
+// Instantiations with the staged epilogue: plain GEMMs.  Convs store from registers (their output pixels are not a row
+// range), and so do the E_KV kernels (they serve the K/V scatter and, as E_ALL, the rare feature sets no other kernel has).
+__host__ __device__ constexpr bool gemm_staged(bool conv, int epi) { return !conv && !(epi & E_KV); }
 
 template <int BN, bool kGeglu, bool kConv, int kEpi>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_a2,
-                  const __grid_constant__ CUtensorMap tmap_b, const GemmKernelArgs a) {
-  using Cfg = GemmCfg<BN>;
+                  const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ CUtensorMap tmap_c,
+                  const __grid_constant__ CUtensorMap tmap_r, const GemmKernelArgs a) {
+  constexpr bool kStaged = gemm_staged(kConv, kEpi);
+  using Cfg = GemmCfg<BN, kStaged>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment for the 128B swizzle atoms
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full = reinterpret_cast<uint64_t*>(smem);  // [STAGES]
   uint64_t* empty = full + STAGES;                      // [STAGES]
+  uint64_t* res_full = empty + STAGES;                  // [2]: residual tile of MMA warpgroup 0 / 1 landed
   uint8_t* ring = smem + BAR_BYTES;
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);  // tells the compiler the role branches are warp-uniform
@@ -119,6 +134,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       mbar_init(&full[i], 1);
       mbar_init(&empty[i], 2);  // one arrival per MMA warpgroup
     }
+    mbar_init(&res_full[0], 1);
+    mbar_init(&res_full[1], 1);
     fence_mbar_init();
   }
   __syncthreads();
@@ -169,6 +186,16 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   const int r_base = wg * 64 + wq * 16 + (lane >> 2);  // tile rows r_base and r_base + 8 belong to this thread
   const int c_base = 2 * (lane & 3);                   // columns 8j + c_base, +1 of fragment j
   const uint32_t ring_u32 = smem_u32(ring);
+  // staged epilogue: this warpgroup's slabs, and the offset of this thread's (row r_base, columns c_base, +1) in a slab; the
+  // 64-byte swizzle moves the 16-byte chunk c of row r to c ^ ((r >> 1) & 3), which for rows r_base, r_base + 8 is
+  // (lane >> 3) & 3: the 8 rows of a warp store land in 8 different chunks, 32 different banks
+  const bool staged = kStaged && a.staged;
+  uint8_t* stg = ring + STAGES * Cfg::STAGE_BYTES + wg * 64 * BN * 2;
+  const uint32_t stg_u32 = smem_u32(stg) + (r_base - wg * 64) * 64 + c_base * 2;
+  const int stg_xor = (lane >> 3) & 3;
+  const bool has_res = (kEpi & E_RES) && !kGeglu && a.residual != nullptr;
+  const int out_cols = kGeglu ? a.N / 2 : a.N;
+  uint32_t res_phase = 0;
 
   int stage = 0;
   uint32_t phase = 0;
@@ -179,6 +206,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     TileCoord tc;
     tile_coords<kConv>(a, m_tile, tc);
     const int n0 = n_tile * a.block_n;
+    // staged: the output columns and slabs of this tile, and whether this warpgroup has any rows inside the tensor
+    const int ocol0 = kGeglu ? n0 / 2 : n0;
+    const int ocols = min(kGeglu ? a.block_n / 2 : a.block_n, out_cols - ocol0);
+    const int n_slabs = (ocols + SLAB_COLS - 1) / SLAB_COLS;
+    const int orow0 = tc.m0 + wg * 64;
+    const bool stg_live = staged && orow0 < a.M;
 
     // ---- main loop: one k-block in flight behind the one being issued; a stage is released once its MMAs retired
     int prev_stage = -1;
@@ -195,9 +228,22 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         const int scale_d = (kb | k) != 0 ? 1 : 0;
         if constexpr (BN == 64) wgmma_ss_n64(acc, adesc + 2 * k, bdesc + 2 * k, scale_d);
         else if constexpr (BN == 128) wgmma_ss_n128(acc, adesc + 2 * k, bdesc + 2 * k, scale_d);
+        else if constexpr (BN == 160) wgmma_ss_n160(acc, adesc + 2 * k, bdesc + 2 * k, scale_d);
+        else if constexpr (BN == 192) wgmma_ss_n192(acc, adesc + 2 * k, bdesc + 2 * k, scale_d);
         else wgmma_ss_n256(acc, adesc + 2 * k, bdesc + 2 * k, scale_d);
       }
       wgmma_commit();
+      if (kb == 0 && staged && wg_leader) {
+        // the previous tile's stores must have read the slabs before they are refilled (or rewritten by the epilogue,
+        // after the barrier there); then the residual tile comes in under this tile's MMAs.  A tile reads only the
+        // residual rows and columns it stores itself, so the residual may alias the output.
+        bulk_wait_group_read<0>();
+        if (has_res && stg_live) {
+          mbar_expect_tx(&res_full[wg], n_slabs * SLAB_BYTES);
+          for (int s = 0; s < n_slabs; ++s)
+            tma_load_2d(stg + s * SLAB_BYTES, &tmap_r, &res_full[wg], ocol0 + s * SLAB_COLS, orow0);
+        }
+      }
       wgmma_wait<1>();
       if (prev_stage >= 0 && wg_leader) mbar_arrive(&empty[prev_stage]);
       prev_stage = stage;
@@ -207,12 +253,23 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     wgmma_fence_regs(acc);
     if (wg_leader) mbar_arrive(&empty[prev_stage]);
 
-    // ---- epilogue: straight from the accumulator registers
+    // ---- epilogue: into the staging slabs, or straight from the accumulator registers to global memory
     long long rows[2];
     int imgs[2];
     bool valid[2];
     row_of<kConv>(a, tc, r_base, rows[0], imgs[0], valid[0]);
     row_of<kConv>(a, tc, r_base + 8, rows[1], imgs[1], valid[1]);
+    if (staged) {
+      named_barrier_sync(1 + wg, 128);  // orders the slab writes below after the leader's bulk_wait_group_read
+      if (has_res && stg_live) {
+        mbar_wait(&res_full[wg], res_phase);
+        res_phase ^= 1;
+      }
+    }
+    // shared address of this thread's pair (fragment j, row half h) in the slabs
+    auto stg_addr = [&](int j, int h) {
+      return stg_u32 + h * 8 * 64 + (j >> 2) * SLAB_BYTES + (((j & 3) ^ stg_xor) << 4);
+    };
 
     if constexpr (kGeglu) {
       // tile columns 16p .. 16p+7 are the a half, 16p+8 .. 16p+15 the g half of output columns n0/2 + 8p .. + 7
@@ -231,13 +288,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
           if (!valid[h]) continue;
           const float a0 = acc[8 * p + 2 * h] + ba.x, a1 = acc[8 * p + 2 * h + 1] + ba.y;
           const float g0 = acc[8 * p + 4 + 2 * h] + bg.x, g1 = acc[8 * p + 4 + 2 * h + 1] + bg.y;
-          *reinterpret_cast<uint32_t*>(a.out + static_cast<size_t>(rows[h]) * a.ldo + ocol) =
-              pack_bf16x2(a0 * gelu_erf_f(g0), a1 * gelu_erf_f(g1));
+          const uint32_t o = pack_bf16x2(a0 * gelu_erf_f(g0), a1 * gelu_erf_f(g1));
+          if (staged) st_shared_u32(stg_addr(p, h), o);  // output column 8p + c_base of the tile: fragment p
+          else *reinterpret_cast<uint32_t*>(a.out + static_cast<size_t>(rows[h]) * a.ldo + ocol) = o;
         }
       }
     } else {
       const bool has_bias = (kEpi & E_BIAS) && a.bias != nullptr, has_rv = (kEpi & E_ROWVEC) && a.rowvec != nullptr;
-      const bool has_res = (kEpi & E_RES) && a.residual != nullptr, has_stats = (kEpi & E_STATS) && a.stats != nullptr;
+      const bool has_stats = (kEpi & E_STATS) && a.stats != nullptr;
       const bool has_act = (kEpi & E_ACT) && a.act == 1, has_scale = (kEpi & E_ACT) && a.out_scale != 1.0f;
       const bool has_kv = (kEpi & E_KV) && a.kv_world > 0;
       // statistics: the 16 rows of a warp lie in ONE image (gemm_prepare checks it); the warp's first row has the
@@ -265,7 +323,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
           if (has_act) { f0 = silu_f(f0); f1 = silu_f(f1); }
           if (has_scale) { f0 *= a.out_scale; f1 *= a.out_scale; }
           if (has_res) {  // plain load: the residual may alias the output (in-place add)
-            const float2 v = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(a.residual + static_cast<size_t>(rows[h]) * a.ld_res + col));
+            const float2 v = unpack_bf16x2(staged ? ld_shared_u32(stg_addr(j, h))
+                                                  : *reinterpret_cast<const uint32_t*>(a.residual + static_cast<size_t>(rows[h]) * a.ld_res + col));
             f0 += v.x; f1 += v.y;
           }
           const uint32_t o = pack_bf16x2(f0, f1);
@@ -281,6 +340,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             const size_t off = static_cast<size_t>(grow) * a.kv_ld + (col - a.kv_col0);
 #pragma unroll 1
             for (int rk = 0; rk < a.kv_world; ++rk) *reinterpret_cast<uint32_t*>(a.kv_dst[rk] + off) = o;
+          } else if (staged) {
+            st_shared_u32(stg_addr(j, h), o);
           } else {
             *reinterpret_cast<uint32_t*>(a.out + static_cast<size_t>(rows[h]) * a.ldo + col) = o;
           }
@@ -306,7 +367,18 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         }
       }
     }
+    if (staged) {
+      // the slab writes (generic proxy) become visible to the TMA store (async proxy); TMA clips rows >= M, columns >= N
+      fence_proxy_async_smem();
+      named_barrier_sync(1 + wg, 128);
+      if (wg_leader && stg_live) {
+        for (int s = 0; s < n_slabs; ++s) tma_store_2d(&tmap_c, stg + s * SLAB_BYTES, ocol0 + s * SLAB_COLS, orow0);
+        bulk_commit_group();
+      }
+    }
   }
+  // no bulk store may still be reading the shared memory of an exited CTA
+  if (staged && wg_leader) bulk_wait_group<0>();
 }
 
 }  // namespace
@@ -321,12 +393,14 @@ int gemm_prepare(const GemmDesc& d, GemmLaunch* L) {
   D4D_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   int bn = d.block_n;
   if (bn <= 0) {
-    // tile width 64, 128 or 256 (the last N tile may overhang; its extra columns are not stored): the widest one unless a
-    // narrower one wastes fewer SM-waves of the persistent grid (cost ~ waves * (block_n + fixed per-tile work))
+    // tile width 64, 128, 160, 192 or 256 (the last N tile may overhang; its extra columns are not stored): the one with
+    // the fewest SM-waves of the persistent grid, weighted by the tile's work (cost ~ waves * (block_n + fixed per-tile
+    // work)), ties to the wider.  GEGLU keeps to widths whose halves fill whole 32-column store slabs.
     const long long rows = d.conv ? static_cast<long long>(d.n_img) * d.H * d.W : d.M;
     const long long m_tiles_est = (rows + BLOCK_M - 1) / BLOCK_M;
     long long best_cost = -1;
-    for (int c = 64; c <= 256; c *= 2) {
+    for (int c : {64, 128, 160, 192, 256}) {
+      if (d.geglu && c % 64 != 0) continue;
       const long long tiles = m_tiles_est * ((d.N + c - 1) / c);
       const long long waves = (tiles + sms - 1) / sms;
       const long long cost = waves * (c + 64) + (static_cast<long long>((d.N + c - 1) / c) * c - d.N) / 4;
@@ -382,6 +456,17 @@ int gemm_prepare(const GemmDesc& d, GemmLaunch* L) {
       L->tmap_a2 = L->tmap_a;
     }
     if (int rc = make_tmap_2d(&L->tmap_b, d.Wt, d.N, K, K, BLOCK_K, bn, 128)) return rc;
+    // staged epilogue unless the K/V scatter writes elsewhere, a tile's columns do not fill whole slabs (narrow block_n:
+    // a slab would store into the next tile's columns) or an operand is not 16-byte aligned for TMA
+    const auto aligned16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+    a.staged = d.kv_world == 0 && (d.geglu ? bn % (2 * SLAB_COLS) : bn % SLAB_COLS) == 0 && aligned16(d.out) &&
+               (d.residual == nullptr || aligned16(d.residual));
+    L->tmap_c = L->tmap_r = L->tmap_a;
+    if (a.staged) {
+      if (int rc = make_tmap_2d(&L->tmap_c, d.out, d.M, d.geglu ? d.N / 2 : d.N, d.ldo, SLAB_COLS, 64, 64)) return rc;
+      if (d.residual && !d.geglu)
+        if (int rc = make_tmap_2d(&L->tmap_r, d.residual, d.M, d.N, d.ld_res, SLAB_COLS, 64, 64)) return rc;
+    }
   } else {
     D4D_REQUIRE(d.Cin % 8 == 0, "conv Cin must be a multiple of 8");
     D4D_REQUIRE(d.conv_kind >= 0 && d.conv_kind <= 3, "conv_kind");
@@ -430,7 +515,7 @@ int gemm_prepare(const GemmDesc& d, GemmLaunch* L) {
     a.m_tiles = a.tiles_per_phase * a.n_phases;
     a.M *= a.n_phases;  // output positions of the launch (FLOP count)
     if (int rc = make_tmap_nhwc(&L->tmap_a, d.A, d.n_img, d.H, d.W, d.Cin, BLOCK_K, bw, bh, bnimg, 128, a.in_stride)) return rc;
-    L->tmap_a2 = L->tmap_a;
+    L->tmap_a2 = L->tmap_c = L->tmap_r = L->tmap_a;
     const uint64_t kw = static_cast<uint64_t>(a.n_taps) * d.Cin;
     if (int rc = make_tmap_2d(&L->tmap_b, d.Wt, static_cast<uint64_t>(d.N) * a.n_phases, kw, kw, BLOCK_K, bn, 128)) return rc;
   }
@@ -441,7 +526,8 @@ int gemm_prepare(const GemmDesc& d, GemmLaunch* L) {
 
 namespace {
 
-using GemmKernelFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const GemmKernelArgs);
+using GemmKernelFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
+                              const CUtensorMap, const GemmKernelArgs);
 struct GemmVariant {
   int bn;
   bool geglu, conv;
@@ -449,28 +535,32 @@ struct GemmVariant {
   GemmKernelFn fn;
   int smem;
 };
-#define D4D_GV(BN, G, C, E) {BN, G, C, E, gemm_wgmma_kernel<BN, G, C, E>, GemmCfg<BN>::SMEM}
-#define D4D_GV_SET(BN)                                                                                                \
+#define D4D_GV(BN, G, C, E) {BN, G, C, E, gemm_wgmma_kernel<BN, G, C, E>, GemmCfg<BN, gemm_staged(C, E)>::SMEM}
+#define D4D_GV_PLAIN(BN)                                                                                              \
   /* plain GEMM: qkv | proj_in, shortcut | attn out, ff2 | proj_out, conv_in */                                       \
   D4D_GV(BN, false, false, 0), D4D_GV(BN, false, false, E_BIAS), D4D_GV(BN, false, false, E_BIAS | E_RES),           \
-  D4D_GV(BN, false, false, E_BIAS | E_RES | E_STATS), D4D_GV(BN, false, false, E_ALL),                                \
+  D4D_GV(BN, false, false, E_BIAS | E_RES | E_STATS), D4D_GV(BN, false, false, E_ALL)
+#define D4D_GV_CONV(BN)                                                                                               \
   /* 3x3 convs: resnet conv1 | conv2 | down / up sampling */                                                          \
   D4D_GV(BN, false, true, E_BIAS | E_ROWVEC | E_STATS), D4D_GV(BN, false, true, E_BIAS | E_RES | E_STATS),           \
-  D4D_GV(BN, false, true, E_BIAS | E_STATS), D4D_GV(BN, false, true, E_ALL),                                          \
-  /* GEGLU projection (only the bias bit matters) */                                                                  \
-  D4D_GV(BN, true, false, E_BIAS)
-// the feature sets the UNet plan launches (csrc/unet.cu) at the tile widths it picks, plus E_ALL kernels for the rest
+  D4D_GV(BN, false, true, E_BIAS | E_STATS), D4D_GV(BN, false, true, E_ALL)
+// the feature sets the UNet plan launches (csrc/unet.cu) at the tile widths it picks, plus E_ALL kernels for the rest.
+// GEGLU (only the bias bit matters) runs at widths whose output halves fill whole store slabs; no conv picks 192.
 const GemmVariant kGemmVariants[] = {
-    D4D_GV_SET(128), D4D_GV_SET(256),
+    D4D_GV_PLAIN(128), D4D_GV_CONV(128), D4D_GV(128, true, false, E_BIAS),
+    D4D_GV_PLAIN(160), D4D_GV_CONV(160),
+    D4D_GV_PLAIN(192),
+    D4D_GV_PLAIN(256), D4D_GV_CONV(256), D4D_GV(256, true, false, E_BIAS),
     D4D_GV(64, false, false, E_ALL), D4D_GV(64, false, true, E_ALL), D4D_GV(64, true, false, E_BIAS),
 };
-#undef D4D_GV_SET
+#undef D4D_GV_CONV
+#undef D4D_GV_PLAIN
 #undef D4D_GV
 constexpr int kNumGemmVariants = sizeof(kGemmVariants) / sizeof(kGemmVariants[0]);
 
-int gemm_variant_of(const GemmKernelArgs& a) {
+// the instantiation of kernel width bn whose feature bits equal the launch's, else the E_ALL one (-1: none)
+int gemm_variant_at(const GemmKernelArgs& a, int bn) {
   const bool conv = a.mode != 0, geglu = a.geglu != 0;
-  const int bn = a.block_n <= 64 ? 64 : a.block_n <= 128 ? 128 : 256;  // narrower tiles run on a wider kernel, masked
   int need = 0;
   if (a.bias) need |= E_BIAS;
   if (!geglu) {
@@ -490,6 +580,17 @@ int gemm_variant_of(const GemmKernelArgs& a) {
   return generic;
 }
 
+// The instantiation that runs a launch: the narrowest kernel width >= block_n that has the launch's feature set (a narrower
+// block_n runs on a wider kernel with the extra columns masked).
+int gemm_variant_of(const GemmKernelArgs& a) {
+  for (int bn : {64, 128, 160, 192, 256}) {
+    if (bn < a.block_n) continue;
+    const int vi = gemm_variant_at(a, bn);
+    if (vi >= 0) return vi;
+  }
+  return -1;
+}
+
 }  // namespace
 
 int gemm_run(const GemmLaunch& L, cudaStream_t stream) {
@@ -498,7 +599,8 @@ int gemm_run(const GemmLaunch& L, cudaStream_t stream) {
   D4D_REQUIRE(vi >= 0, "no GEMM kernel instantiation covers this launch");
   const GemmVariant& v = kGemmVariants[vi];
   if (int rc = ensure_dyn_smem(v.fn, v.smem, attr_once[vi])) return rc;
-  D4D_CUDA_OK(launch_pdl(v.fn, dim3(L.grid), dim3(NUM_THREADS), v.smem, stream, L.tmap_a, L.tmap_a2, L.tmap_b, L.args));
+  D4D_CUDA_OK(launch_pdl(v.fn, dim3(L.grid), dim3(NUM_THREADS), v.smem, stream, L.tmap_a, L.tmap_a2, L.tmap_b, L.tmap_c, L.tmap_r,
+                         L.args));
   D4D_CUDA_OK(cudaGetLastError());
   return 0;
 }

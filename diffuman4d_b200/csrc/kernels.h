@@ -38,6 +38,9 @@ struct GemmKernelArgs {
   int ld_res;
   bf16* out;
   int ldo;
+  // plain GEMM: the MMA warpgroups stage the output tile in shared memory and TMA stores it (tmap_c); the residual tile
+  // arrives by TMA into the same buffer (tmap_r).  0: stores from registers (conv, K/V scatter, narrow block_n)
+  int staged;
   int geglu;
   int act;          // 0 none, 1 SiLU applied to (acc + bias + rowvec) before scale/residual
   float out_scale;  // multiplies (acc + bias + rowvec) after the activation
@@ -71,7 +74,7 @@ struct GemmDesc {
   int geglu = 0;
   int act = 0;
   float out_scale = 1.0f;
-  int block_n = 0;  // 0 = auto (64, 128 or 256; the last N tile may overhang)
+  int block_n = 0;  // 0 = auto (64, 128, 160, 192 or 256; the last N tile may overhang)
   // GroupNorm statistics of the output (see GemmKernelArgs::stats); plain GEMM: stats_rows = rows per image
   long long* stats = nullptr;
   int stats_rows = 0;
@@ -90,7 +93,7 @@ struct GemmDesc {
 };
 
 struct GemmLaunch {
-  CUtensorMap tmap_a, tmap_a2, tmap_b;
+  CUtensorMap tmap_a, tmap_a2, tmap_b, tmap_c, tmap_r;  // tmap_c / tmap_r: output / residual of a staged epilogue
   GemmKernelArgs args;
   int grid;
 };

@@ -85,9 +85,4 @@ int make_tmap_nhwc(CUtensorMap* out, const void* base, uint64_t n, uint64_t h, u
   return 0;
 }
 
-int make_tmap_nhwc_store(CUtensorMap* out, void* base, uint64_t n, uint64_t h, uint64_t w, uint64_t c, uint32_t box_w,
-                         uint32_t box_h, uint32_t box_n) {
-  return make_tmap_nhwc(out, base, n, h, w, c, 32, box_w, box_h, box_n, 64, 1);
-}
-
 }  // namespace d4d

@@ -1,0 +1,263 @@
+"""Per-shape timing of the GEMM / conv launches of one W16@64² UNet forward (SD-2.1 layout, 32 images, CFG).
+
+    python tools/gemm_shapes.py [--reps 20] [--json OUT]
+
+Every distinct launch shape of the plan (csrc/unet.cu: PlanBuilder::resnet, transformer, self_attention, the down /
+up-sampling convs, conv_in, the pose encoder's GEMM-kernel layers and the time embedding) runs with the epilogue features
+the plan gives it, through the C ABI on pre-allocated buffers, captured `reps` times into a CUDA graph and timed with CUDA
+events after warm-up.  Per shape: launches per forward, the tile width gemm_prepare picks, µs per launch, TFLOP/s
+(executed FLOPs: the upsampling convs run 4 taps per phase), compulsory HBM bytes and GB/s, and the least time the card
+could take: the larger of FLOPs / tensor peak and bytes / 3.35 TB/s, naming which bounds the shape.  The tensor peak is
+4096 dense BF16 FLOP/clk/SM at the card's maximum SM clock; a power-limited card runs below it under load.
+The count-weighted totals are the `gemm` and `conv3x3` kinds of bench.py's roofline.by_kind_ms.
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+import torch  # noqa: E402
+
+HBM_BPS = 3.35e12
+C = (320, 640, 1280, 1280)
+HW = (64, 32, 16, 8)
+B, F = 32, 16
+
+
+def plan_shapes():
+    """(kind, name, count, spec) for one forward.  spec: plain {M, N, K1, K2, feats} / conv {n, H, W, Cin, Cout, mode, feats}."""
+    shapes = {}
+
+    def add(kind, name, **spec):
+        key = (kind, tuple(sorted(spec.items())))
+        if key in shapes:
+            shapes[key][2] += 1
+        else:
+            shapes[key] = [kind, name, 1, spec]
+
+    def resnet(lvl, cin, cout, cskip=0):
+        n, s = B, HW[lvl]
+        add("conv", f"L{lvl + 1} conv1", n=n, H=s, W=s, Cin=cin + cskip, Cout=cout, mode="s1", feats=("bias", "rowvec", "stats"))
+        if cin + cskip != cout:
+            add("gemm", f"L{lvl + 1} shortcut", M=n * s * s, N=cout, K1=cin, K2=cskip, feats=("bias", "two_source") if cskip else ("bias",))
+        add("conv", f"L{lvl + 1} conv2", n=n, H=s, W=s, Cin=cout, Cout=cout, mode="s1", feats=("bias", "residual", "stats"))
+
+    def transformer(lvl, name="L"):
+        c, M = C[lvl], B * HW[lvl] ** 2
+        tag = f"{name}{lvl + 1}" if name == "L" else name
+        add("gemm", f"{tag} proj_in", M=M, N=c, K1=c, K2=0, feats=("bias",))
+        add("gemm", f"{tag} qkv", M=M, N=3 * c, K1=c, K2=0, feats=())
+        add("gemm", f"{tag} out-proj", M=M, N=c, K1=c, K2=0, feats=("bias", "residual"))
+        add("gemm", f"{tag} ff1 geglu", M=M, N=8 * c, K1=c, K2=0, feats=("bias", "geglu"))
+        add("gemm", f"{tag} ff2", M=M, N=c, K1=4 * c, K2=0, feats=("bias", "residual"))
+        add("gemm", f"{tag} proj_out", M=M, N=c, K1=c, K2=0, feats=("bias", "residual", "stats"))
+
+    TE = 4 * C[0]
+    ldt = sum([320, 320, 640, 640, 1280, 1280, 1280, 1280] + [1280, 1280] + [1280] * 6 + [640] * 3 + [320] * 3)
+    add("gemm", "time1 / tem1", M=B, N=TE, K1=C[0], K2=0, feats=("bias", "act"))
+    add("gemm", "time1 / tem1", M=B, N=TE, K1=C[0], K2=0, feats=("bias", "act"))
+    add("gemm", "time2", M=B, N=TE, K1=TE, K2=0, feats=("bias",))
+    add("gemm", "tem2", M=B, N=TE, K1=TE, K2=0, feats=("bias", "residual"))
+    add("gemm", "temb_all", M=B, N=ldt, K1=TE, K2=0, feats=("bias",))
+    # pose encoder (the 2F-image batch of bench.py's by_kind forward): layer 5 as a GEMM over im2col, 6 and 7 as convs
+    PB, s0 = 2 * F, HW[0]
+    add("gemm", "pose l5", M=PB * s0 * s0, N=64, K1=512, K2=0, feats=("bias", "act"))
+    add("conv", "pose l6", n=PB, H=s0, W=s0, Cin=64, Cout=64, mode="s1", feats=("bias", "act"))
+    add("conv", "pose l7", n=PB, H=s0, W=s0, Cin=64, Cout=128, mode="s1", feats=("bias", "act"))
+    add("gemm", "pose proj", M=PB * s0 * s0, N=C[0], K1=128, K2=0, feats=("bias", "scale"))
+    add("gemm", "conv_in", M=B * s0 * s0, N=C[0], K1=192, K2=0, feats=("bias", "residual", "stats"))
+    # down
+    x = C[0]
+    skips = [C[0]]
+    for i in range(4):
+        for _ in range(2):
+            resnet(i, x, C[i])
+            x = C[i]
+            if i < 3:
+                transformer(i)
+            skips.append(x)
+        if i < 3:
+            add("conv", f"L{i + 1} downsample", n=B, H=HW[i], W=HW[i], Cin=x, Cout=x, mode="s2", feats=("bias", "stats"))
+            skips.append(x)
+    # mid
+    resnet(3, x, x)
+    transformer(3, "mid")
+    resnet(3, x, x)
+    # up
+    for i in range(4):
+        lvl = 3 - i
+        for _ in range(3):
+            sk = skips.pop()
+            resnet(lvl, x, C[lvl], sk)
+            x = C[lvl]
+            if i > 0:
+                transformer(lvl)
+        if i < 3:
+            add("conv", f"L{lvl + 1} upsample", n=B, H=HW[lvl], W=HW[lvl], Cin=x, Cout=x, mode="up", feats=("bias", "stats"))
+    add("conv", "conv_out", n=B, H=s0, W=s0, Cin=C[0], Cout=16, mode="s1", feats=("bias",))
+    return list(shapes.values())
+
+
+def auto_block_n(rows, N, geglu, sms):
+    """Mirror of gemm_prepare's automatic tile width (csrc/gemm_wgmma.cu)."""
+    best = None
+    for c in (64, 128, 160, 192, 256):
+        if geglu and c % 64:
+            continue
+        n_tiles = -(-N // c)
+        waves = -(-(-(-rows // 128) * n_tiles) // sms)
+        cost = waves * (c + 64) + (n_tiles * c - N) // 4
+        if best is None or cost <= best[0]:
+            best = (cost, c)
+    return best[1]
+
+
+def card():
+    name = torch.cuda.get_device_name(0)
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader,nounits", "-i", "0"],
+                           capture_output=True, text=True, timeout=30).stdout.strip().split(",")
+        return name, float(q[0]), float(q[1])
+    except Exception:  # noqa: BLE001 - the tool may be missing; the numbers are then reported as unknown
+        return name, float("nan"), float("nan")
+
+
+def make_launch(kind, spec, dev):
+    """A zero-argument callable that enqueues the launch, plus its executed FLOPs and compulsory bytes."""
+    from diffuman4d_b200._lib import check, lib
+    from diffuman4d_b200 import ops
+    g = torch.Generator(device="cpu").manual_seed(0)
+    r = lambda *s: (torch.randn(*s, generator=g) * 0.5).to(torch.bfloat16).to(dev)
+    stream = lambda: torch.cuda.current_stream().cuda_stream
+    f = set(spec["feats"])
+    if kind == "gemm":
+        M, N, K1, K2 = spec["M"], spec["N"], spec["K1"], spec["K2"]
+        geglu = "geglu" in f
+        a, a2 = r(M, K1), (r(M, K2) if K2 else None)
+        w = r(N, K1 + K2) * (K1 + K2) ** -0.5
+        bias = torch.randn(N, generator=g).to(dev) if "bias" in f else None
+        nout = N // 2 if geglu else N
+        out = torch.empty(M, nout, device=dev, dtype=torch.bfloat16)
+        res = r(M, N) if "residual" in f else None
+        stats_rows = M // B if "stats" in f else 0  # rows per image
+        stats = torch.zeros(B * N * 2, device=dev, dtype=torch.int64) if "stats" in f else None
+        act = 1 if "act" in f else 0
+        scale = 2.0 if "scale" in f else 1.0
+        p = lambda t: None if t is None else t.data_ptr()
+
+        def run():
+            check(lib().d4d_op_gemm(a.data_ptr(), K1, K1, p(a2), K2, K2, w.data_ptr(), M, N, p(bias), None, 0, 0, p(res),
+                                    N if res is not None else 0, out.data_ptr(), nout, int(geglu), act, scale, 0,
+                                    p(stats), stats_rows, stream()), "d4d_op_gemm")
+        K = K1 + K2
+        flops = 2.0 * M * N * K
+        byts = 2.0 * (M * K + N * K + M * nout + (M * N if res is not None else 0))
+        return run, flops, byts, auto_block_n(M, N, geglu, torch.cuda.get_device_properties(0).multi_processor_count)
+    n, H, W, Cin, Cout, mode = spec["n"], spec["H"], spec["W"], spec["Cin"], spec["Cout"], spec["mode"]
+    x = r(n, H, W, Cin)
+    bias = torch.randn(Cout, generator=g).to(dev) if "bias" in f else None
+    stats = torch.zeros(n * Cout * 2, device=dev, dtype=torch.int64) if "stats" in f else None
+    # pointers are taken inside run(), so that its closure keeps every tensor alive for as long as the launch is replayed
+    p = lambda t: None if t is None else t.data_ptr()
+    if mode == "up":
+        taps, Mo = 4, n * 4 * H * W
+        wp = torch.stack(ops.upsample_phase_weights(r(Cout, Cin, 3, 3) * (9 * Cin) ** -0.5)).contiguous()
+        out = torch.empty(n, 2 * H, 2 * W, Cout, device=dev, dtype=torch.bfloat16)
+
+        def run():
+            check(lib().d4d_op_conv_resample(x.data_ptr(), n, H, W, Cin, wp.data_ptr(), Cout, p(bias), 3, 0, 0, out.data_ptr(),
+                                             p(stats), stream()), "d4d_op_conv_resample")
+        rows = n * H * W
+    elif mode == "s2":
+        taps, Mo = 9, n * (H // 2) * (W // 2)
+        wt = r(Cout, 9, Cin) * (9 * Cin) ** -0.5
+        out = torch.empty(n, H // 2, W // 2, Cout, device=dev, dtype=torch.bfloat16)
+
+        def run():
+            check(lib().d4d_op_conv_resample(x.data_ptr(), n, H, W, Cin, wt.data_ptr(), Cout, p(bias), 1, 0, 0, out.data_ptr(),
+                                             p(stats), stream()), "d4d_op_conv_resample")
+        rows = n * H * W  # gemm_prepare sizes the tile width on the input grid
+    else:
+        taps, Mo = 9, n * H * W
+        wt = r(Cout, 9, Cin) * (9 * Cin) ** -0.5
+        out = torch.empty(n, H, W, Cout, device=dev, dtype=torch.bfloat16)
+        rowvec = r(n, Cout) if "rowvec" in f else None
+        res = r(n, H, W, Cout) if "residual" in f else None
+        act = 1 if "act" in f else 0
+
+        def run():
+            check(lib().d4d_op_conv3x3(x.data_ptr(), n, H, W, Cin, wt.data_ptr(), Cout, p(bias), p(rowvec), Cout, p(res), act,
+                                       out.data_ptr(), 0, p(stats), stream()),
+                  "d4d_op_conv3x3")
+        rows = Mo
+    flops = 2.0 * Mo * Cout * taps * Cin
+    byts = 2.0 * (x.numel() + taps * Cin * Cout + Mo * Cout * (2 if "residual" in f else 1))
+    return run, flops, byts, auto_block_n(rows, Cout, False, torch.cuda.get_device_properties(0).multi_processor_count)
+
+
+def time_launch(run, reps):
+    for _ in range(3):
+        run()
+    torch.cuda.synchronize()
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        for _ in range(reps):
+            run()
+    graph.replay()
+    torch.cuda.synchronize()
+    t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    t0.record()
+    graph.replay()
+    t1.record()
+    t1.synchronize()
+    return t0.elapsed_time(t1) * 1e3 / reps
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--reps", type=int, default=20, help="launches per timed graph replay")
+    ap.add_argument("--json", default=None, help="also write the table as JSON here")
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("gemm_shapes.py needs a CUDA device")
+    dev = torch.device("cuda:0")
+    name, power_w, max_mhz = card()
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    peak = 4096.0 * sms * max_mhz * 1e6
+    print(f"# {name}, power limit {power_w:.0f} W, max SM clock {max_mhz:.0f} MHz, {sms} SMs; "
+          f"tensor peak {peak / 1e12:.0f} TFLOP/s (4096 FLOP/clk/SM at max clock), HBM 3.35 TB/s")
+    hdr = f"{'kind':5} {'shape':58} {'cnt':>3} {'bn':>4} {'us':>9} {'TFLOP/s':>8} {'MB':>8} {'GB/s':>7} {'min us':>8} {'bound':>6} {'eff':>5}"
+    print(hdr)
+    rows, tot = [], {"gemm": 0.0, "conv": 0.0}
+    for kind, nm, cnt, spec in plan_shapes():
+        run, flops, byts, bn = make_launch(kind, spec, dev)
+        us = time_launch(run, args.reps)
+        t_f, t_b = flops / peak * 1e6, byts / HBM_BPS * 1e6
+        bound = "tensor" if t_f >= t_b else "HBM"
+        tmin = max(t_f, t_b)
+        dims = (f"M{spec['M']} N{spec['N']} K{spec['K1']}" + (f"+{spec['K2']}" if spec["K2"] else "")) if kind == "gemm" else \
+            f"{spec['n']}x{spec['H']}x{spec['W']} {spec['Cin']}->{spec['Cout']} {spec['mode']}"
+        label = f"{nm}: {dims} [{','.join(spec['feats']) or '-'}]"
+        print(f"{kind:5} {label:58} {cnt:3d} {bn:4d} {us:9.1f} {flops / us / 1e6:8.1f} {byts / 1e6:8.1f} "
+              f"{byts / us / 1e3:7.0f} {tmin:8.1f} {bound:>6} {tmin / us:5.2f}")
+        tot[kind] += cnt * us
+        rows.append({"kind": kind, "name": nm, "spec": {k: (list(v) if isinstance(v, tuple) else v) for k, v in spec.items()},
+                     "count": cnt, "block_n": bn, "us": us, "tflops": flops / us / 1e6, "bytes": byts,
+                     "gbps": byts / us / 1e3, "min_us": tmin, "bound": bound})
+        del run
+        torch.cuda.empty_cache()
+    print(f"# count-weighted per forward: gemm {tot['gemm'] / 1e3:.2f} ms, conv3x3 {tot['conv'] / 1e3:.2f} ms")
+    if args.json:
+        with open(args.json, "w") as fh:
+            json.dump({"card": name, "power_limit_w": power_w, "max_sm_mhz": max_mhz, "rows": rows,
+                       "total_ms": {k: v / 1e3 for k, v in tot.items()}}, fh, indent=1)
+
+
+if __name__ == "__main__":
+    main()
