@@ -12,7 +12,8 @@ LIB_PATH = os.path.join(_HERE, "libd4d.so")
 EXPORTS = [
     "d4d_last_error", "d4d_version", "d4d_create", "d4d_destroy", "d4d_load_weight", "d4d_finalize_weights",
     "d4d_num_weights", "d4d_weight_key", "d4d_unet_forward", "d4d_profile_forward", "d4d_workspace_bytes", "d4d_forward_launches",
-    "d4d_denoise_window", "d4d_assemble_input", "d4d_cfg_ddim_step", "d4d_op_gemm", "d4d_op_conv3x3",
+    "d4d_denoise_window", "d4d_denoise_window_dpm", "d4d_assemble_input", "d4d_cfg_ddim_step", "d4d_cfg_dpm_step",
+    "d4d_op_gemm", "d4d_op_conv3x3",
     "d4d_op_attention", "d4d_op_groupnorm", "d4d_op_conv3x3_groupnorm", "d4d_op_conv_resample", "d4d_op_layernorm", "d4d_op_pose_conv0", "d4d_op_pose_conv", "d4d_debug_tap", "d4d_exchange_alloc",
     "d4d_exchange_open", "d4d_unet_forward_sharded", "d4d_denoise_window_sharded",
 ]
@@ -33,6 +34,13 @@ class D4DSched(C.Structure):
         ("timesteps_table", C.c_void_p), ("alphas_cumprod", C.c_void_p), ("n_steps", C.c_int32),
         ("num_train_timesteps", C.c_int32), ("final_alpha_cumprod", C.c_float), ("prediction_type", C.c_int32),
         ("clip_sample", C.c_int32), ("clip_sample_range", C.c_float), ("emulate_bf16", C.c_int32),
+    ]
+
+
+class D4DDpmSched(C.Structure):
+    _fields_ = [
+        ("timesteps_table", C.c_void_p), ("coefs", C.c_void_p), ("n_steps", C.c_int32), ("prediction_type", C.c_int32),
+        ("solver_order", C.c_int32), ("final_first_order", C.c_int32), ("emulate_bf16", C.c_int32),
     ]
 
 
@@ -75,8 +83,11 @@ def _load(path: str) -> C.CDLL:
     l.d4d_workspace_bytes.argtypes = [vp, i32, i32, i32, i32, i32, C.POINTER(C.c_size_t)]
     l.d4d_forward_launches.argtypes = [vp, i32, i32, i32, i32, i32, C.POINTER(C.c_int)]
     l.d4d_denoise_window.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.POINTER(D4DSched), f32, i32, i32, i32, i32, i32, vp]
+    l.d4d_denoise_window_dpm.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.POINTER(D4DDpmSched), f32, i32, i32, i32, i32, i32,
+                                         vp, vp, vp]
     l.d4d_assemble_input.argtypes = [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]
     l.d4d_cfg_ddim_step.argtypes = [vp, vp, vp, vp, vp, C.POINTER(D4DSched), f32, i32, i32, i32, i32, vp, vp]
+    l.d4d_cfg_dpm_step.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, C.POINTER(D4DDpmSched), f32, i32, i32, i32, i32, vp, vp]
     l.d4d_op_gemm.argtypes = [vp, i32, i32, vp, i32, i32, vp, i32, i32, f32p, vp, i32, i32, vp, i32, vp, i32, i32,
                               i32, f32, i32, vp, i32, vp]
     l.d4d_op_conv3x3.argtypes = [vp, i32, i32, i32, i32, vp, i32, f32p, vp, i32, vp, i32, vp, i32, vp, vp]
@@ -99,8 +110,8 @@ def _load(path: str) -> C.CDLL:
         fn = getattr(l, name)
         if fn.restype is C.c_int or name.startswith("d4d_op_") or name in (
                 "d4d_create", "d4d_load_weight", "d4d_finalize_weights", "d4d_unet_forward", "d4d_denoise_window",
-                "d4d_exchange_alloc", "d4d_exchange_open", "d4d_unet_forward_sharded", "d4d_denoise_window_sharded",
-                "d4d_debug_tap"):
+                "d4d_denoise_window_dpm", "d4d_exchange_alloc", "d4d_exchange_open", "d4d_unet_forward_sharded",
+                "d4d_denoise_window_sharded", "d4d_debug_tap"):
             fn.restype = C.c_int
     return l
 

@@ -121,3 +121,21 @@ class SchedulerConfig:
     timestep_spacing: str = "leading"
     clip_sample: bool = False
     clip_sample_range: float = 1.0
+
+
+@dataclass
+class DPMSolverConfig:
+    """DPM-Solver++ scheduler knobs (upstream diffusers==0.33.1 ``DPMSolverMultistepScheduler`` defaults) that the fused
+    step implements: algorithm_type "dpmsolver++", solver_type "midpoint", solver_order 1 or 2, no thresholding, sigmas
+    straight from the beta schedule."""
+    num_train_timesteps: int = 1000
+    beta_start: float = 0.0001
+    beta_end: float = 0.02
+    beta_schedule: str = "linear"         # or "scaled_linear"
+    solver_order: int = 2                 # 1 or 2
+    prediction_type: str = "epsilon"      # or "v_prediction", "sample"
+    lower_order_final: bool = True
+    euler_at_final: bool = False
+    final_sigmas_type: str = "zero"       # or "sigma_min"
+    timestep_spacing: str = "linspace"    # or "leading", "trailing"
+    steps_offset: int = 0

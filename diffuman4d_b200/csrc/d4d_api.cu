@@ -45,7 +45,7 @@ struct DeviceGuard {
 extern "C" {
 
 const char* d4d_last_error(void) { return d4d::g_last_error.c_str(); }
-int d4d_version(void) { return 102; }
+int d4d_version(void) { return 103; }
 
 int d4d_create(const d4d_config* cfg, int device, d4d_handle** out) {
   D4D_API_BEGIN
@@ -166,6 +166,21 @@ int d4d_denoise_window(d4d_handle* h, void* latents, const void* pixel_latents, 
   D4D_API_END
 }
 
+int d4d_denoise_window_dpm(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                           const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                           const d4d_dpm_sched* sched, float guidance_scale, int domain, int F, int height, int width,
+                           int num_steps, void* x0_prev, int32_t* lower_order_nums, void* stream) {
+  D4D_API_BEGIN
+  D4D_REQUIRE(h != nullptr && sched != nullptr, "null argument");
+  DeviceGuard g(h->model->device());
+  return h->model->denoise_window_dpm(static_cast<bf16*>(latents), static_cast<const bf16*>(pixel_latents),
+                                      static_cast<const bf16*>(plucker), static_cast<const bf16*>(skeletons),
+                                      static_cast<const bf16*>(cond_mask), reinterpret_cast<long long*>(timestep_indices),
+                                      *sched, guidance_scale, domain, F, height, width, num_steps,
+                                      static_cast<bf16*>(x0_prev), lower_order_nums, static_cast<cudaStream_t>(stream));
+  D4D_API_END
+}
+
 int d4d_assemble_input(void* latents, const void* pixel_latents, const void* plucker, const void* skel_latents,
                        const void* cond_mask, const int64_t* timestep_indices, const int64_t* timesteps_table,
                        int n_steps, int F, int height, int width, int cfg, void* sample_out, int64_t* timestep_out,
@@ -207,6 +222,29 @@ int d4d_cfg_ddim_step(const void* noise, const void* latents, const void* cond_m
   d.prediction_type = sched->prediction_type; d.clip_sample = sched->clip_sample; d.clip_range = sched->clip_sample_range;
   d.emulate_bf16 = sched->emulate_bf16; d.out = static_cast<bf16*>(latents_out);
   return d4d::cfg_ddim_step_run(d, reinterpret_cast<long long*>(timestep_indices_out), static_cast<cudaStream_t>(stream));
+  D4D_API_END
+}
+
+int d4d_cfg_dpm_step(const void* noise, const void* latents, const void* cond_mask, const int64_t* timestep_indices,
+                     int64_t* timestep_indices_out, void* x0_prev, const int32_t* lower_order_nums,
+                     int32_t* lower_order_nums_out, const d4d_dpm_sched* sched, float guidance_scale, int cfg, int F,
+                     int height, int width, void* latents_out, void* stream) {
+  D4D_API_BEGIN
+  D4D_REQUIRE(noise && latents && cond_mask && timestep_indices && timestep_indices_out && x0_prev && lower_order_nums &&
+                  lower_order_nums_out && sched && sched->timesteps_table && sched->coefs && latents_out,
+              "null argument");
+  d4d::DpmArgs d;
+  const int hw = height * width;
+  d.noise = static_cast<const bf16*>(noise); d.latents = static_cast<const bf16*>(latents);
+  d.mask = static_cast<const bf16*>(cond_mask);
+  d.timestep_indices = reinterpret_cast<const long long*>(timestep_indices);
+  d.coefs = sched->coefs; d.n_steps = sched->n_steps;
+  d.F = F; d.chw = 4 * hw; d.hw = hw; d.cfg = cfg; d.guidance = guidance_scale;
+  d.prediction_type = sched->prediction_type; d.solver_order = sched->solver_order;
+  d.final_first_order = sched->final_first_order; d.emulate_bf16 = sched->emulate_bf16;
+  d.x0_prev = static_cast<bf16*>(x0_prev); d.lower_order_nums = lower_order_nums;
+  d.lower_order_nums_out = lower_order_nums_out; d.out = static_cast<bf16*>(latents_out);
+  return d4d::cfg_dpm_step_run(d, reinterpret_cast<long long*>(timestep_indices_out), static_cast<cudaStream_t>(stream));
   D4D_API_END
 }
 

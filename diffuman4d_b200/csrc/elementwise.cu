@@ -373,6 +373,63 @@ __global__ void cfg_ddim_kernel(const DdimArgs a, long long* ts_out) {
 }
 
 // ---------------------------------------------------------------------------------------------
+// CFG combine + per-frame DPM-Solver++ step (upstream DPMSolverMultistepScheduler.step, dpmsolver++ / midpoint, order
+// <= 2).  Every frame carries its own history (x0_prev, lower_order_nums); its step index is its timestep index.
+// ---------------------------------------------------------------------------------------------
+// fp32 a - b without contraction into an FMA with a preceding product (the reference evaluates each op separately)
+template <bool EMU>
+__device__ __forceinline__ float sub_nc(float a, float b) { return EMU ? __fsub_rn(a, b) : a - b; }
+template <bool EMU>
+__device__ __forceinline__ float mul_nc(float a, float b) { return EMU ? __fmul_rn(a, b) : a * b; }
+
+template <bool EMU>
+__global__ void cfg_dpm_kernel(const DpmArgs a, long long* ts_out) {
+  const int f = blockIdx.y;
+  const bool is_cond = __bfloat162float(a.mask[static_cast<size_t>(f) * a.hw]) == 0.f;
+  long long idx = a.timestep_indices[f];
+  const int lon = a.lower_order_nums[f];
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    ts_out[f] = is_cond ? 0 : idx + 1;
+    a.lower_order_nums_out[f] = is_cond ? lon : min(lon + 1, a.solver_order);
+  }
+  const size_t base = static_cast<size_t>(f) * a.chw;
+  if (is_cond) {  // never stepped: latents pass through, history untouched
+    if (a.out != a.latents)
+      for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.chw; i += gridDim.x * blockDim.x)
+        a.out[base + i] = a.latents[base + i];
+    return;
+  }
+  idx = idx < 0 ? 0 : (idx >= a.n_steps ? a.n_steps - 1 : idx);
+  const float* k = a.coefs + idx * kDpmCoefs;
+  const float alpha_s = k[0], sigma_s = k[1], ratio = k[2], c = k[3], half_c = k[4], inv_r0 = k[5];
+  const bool first = a.solver_order == 1 || lon < 1 || (a.final_first_order && idx == a.n_steps - 1);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.chw; i += gridDim.x * blockDim.x) {
+    float m;
+    if (a.cfg) {
+      const float u = __bfloat162float(a.noise[base + i]);
+      const float cn = __bfloat162float(a.noise[static_cast<size_t>(a.F) * a.chw + base + i]);
+      m = rnd<EMU>(u + rnd<EMU>(a.guidance * rnd<EMU>(cn - u)));   // u + g * (c - u), as in cfg_ddim_kernel
+    } else {
+      m = __bfloat162float(a.noise[base + i]);
+    }
+    const float x = __bfloat162float(a.latents[base + i]);
+    float x0;  // convert_model_output: runs in the model output's dtype
+    if (a.prediction_type == 0) x0 = rnd<EMU>(rnd<EMU>(x - rnd<EMU>(sigma_s * m)) / alpha_s);
+    else if (a.prediction_type == 1) x0 = rnd<EMU>(rnd<EMU>(alpha_s * x) - rnd<EMU>(sigma_s * m));
+    else x0 = m;
+    const float m1 = __bfloat162float(a.x0_prev[base + i]);
+    a.x0_prev[base + i] = __float2bfloat16_rn(x0);
+    // sample is upcast to fp32: (sigma_t / sigma_s) * sample stays fp32, each coef * (bf16 tensor) rounds to bf16
+    float prev = sub_nc<EMU>(mul_nc<EMU>(ratio, x), rnd<EMU>(c * x0));
+    if (!first) {
+      const float d1 = rnd<EMU>(inv_r0 * rnd<EMU>(x0 - m1));
+      prev = sub_nc<EMU>(prev, rnd<EMU>(half_c * d1));
+    }
+    a.out[base + i] = __float2bfloat16_rn(prev);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
 // frame-sharded window: K/V arrival flags in peer memory
 // ---------------------------------------------------------------------------------------------
 __global__ void kv_signal_kernel(const KvFlagArgs a) {
@@ -526,6 +583,19 @@ int cfg_ddim_step_run(const DdimArgs& a, long long* ts_out, cudaStream_t stream)
   dim3 grid(min(64, blocks_for(a.chw, 256)), a.F);
   if (a.emulate_bf16) cfg_ddim_kernel<true><<<grid, 256, 0, stream>>>(a, ts_out);
   else cfg_ddim_kernel<false><<<grid, 256, 0, stream>>>(a, ts_out);
+  D4D_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int cfg_dpm_step_run(const DpmArgs& a, long long* ts_out, cudaStream_t stream) {
+  D4D_REQUIRE(a.n_steps > 0 && a.F > 0 && a.coefs && a.x0_prev && a.lower_order_nums && a.lower_order_nums_out, "dpm args");
+  D4D_REQUIRE(a.solver_order == 1 || a.solver_order == 2, "solver_order must be 1 or 2");
+  D4D_REQUIRE(a.prediction_type >= 0 && a.prediction_type <= 2, "prediction_type");
+  D4D_REQUIRE(a.lower_order_nums != a.lower_order_nums_out && ts_out != a.timestep_indices,
+              "the timestep index and order count outputs may not alias their inputs");
+  dim3 grid(min(64, blocks_for(a.chw, 256)), a.F);
+  if (a.emulate_bf16) cfg_dpm_kernel<true><<<grid, 256, 0, stream>>>(a, ts_out);
+  else cfg_dpm_kernel<false><<<grid, 256, 0, stream>>>(a, ts_out);
   D4D_CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -200,6 +200,32 @@ struct DdimArgs {
 // ts_out[F]: updated timestep indices (targets +1, cond 0); may not alias a.timestep_indices
 int cfg_ddim_step_run(const DdimArgs& a, long long* ts_out, cudaStream_t stream);
 
+// CFG combine + per-frame DPM-Solver++ step (upstream DPMSolverMultistepScheduler, dpmsolver++ / midpoint, order <= 2).
+// Per-step coefficients row i of `coefs` (fp32, built on the host like the upstream scheduler builds them from its sigma
+// table): alpha_s, sigma_s (alpha_t / sigma_t of sigma_i), sigma_t(i+1) / sigma_t(i), c = alpha_t(i+1) * (exp(-h) - 1),
+// 0.5 * c, 1 / r0 (0 in row 0).
+constexpr int kDpmCoefs = 6;
+struct DpmArgs {
+  const bf16* noise;        // [(cfg?2:1)*F,4,h,w]
+  const bf16* latents;      // [F,4,h,w]
+  const bf16* mask;         // [F,1,h,w]  (cond frame <=> mask[f,0,0,0]==0; never stepped, state untouched)
+  const long long* timestep_indices;  // [F] = the step index of each frame
+  const float* coefs;       // [n_steps][kDpmCoefs]
+  int n_steps;
+  int F, chw, hw, cfg;
+  float guidance;
+  int prediction_type;      // 0 epsilon, 1 v_prediction, 2 sample
+  int solver_order;         // 1 or 2
+  int final_first_order;    // 1: step n_steps-1 is first order
+  int emulate_bf16;
+  bf16* x0_prev;            // [F,4,h,w] in/out: each frame's previous data prediction
+  const int* lower_order_nums;        // [F]
+  int* lower_order_nums_out;          // [F] (may not alias lower_order_nums)
+  bf16* out;                // [F,4,h,w] (may alias latents)
+};
+// ts_out[F]: updated timestep indices (targets +1, cond 0); may not alias a.timestep_indices
+int cfg_dpm_step_run(const DpmArgs& a, long long* ts_out, cudaStream_t stream);
+
 // cross-rank K/V arrival flags (frame-sharded window): signal = system-scope release of `epoch` into slot `my_rank` of
 // every rank's flag array; wait = acquire-spin until all `world` slots of the local array reach `epoch`
 struct KvFlagArgs {

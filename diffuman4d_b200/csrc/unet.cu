@@ -74,6 +74,7 @@ WindowBufs::~WindowBufs() {
   cudaFree(noise);
   cudaFree(latents_tmp);
   cudaFree(ts_tmp);
+  cudaFree(order_tmp);
 }
 
 // =================================================================================================
@@ -1246,6 +1247,53 @@ int Model::denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker,
                           int num_steps, cudaStream_t stream, int F_total) {
   D4D_REQUIRE(latents && pixel && plucker && mask && ts_idx, "null argument");
   D4D_REQUIRE(sched.timesteps_table && sched.alphas_cumprod && sched.n_steps > 0, "scheduler tables");
+  const bool cfg_on = guidance > 1.0f;
+  const int hw = h * w;
+  return run_window(latents, pixel, plucker, skeletons, mask, ts_idx,
+                    reinterpret_cast<const long long*>(sched.timesteps_table), sched.n_steps, guidance, domain, F, h, w,
+                    num_steps, stream, F_total, [&](WindowBufs& wb, cudaStream_t s) -> int {
+    DdimArgs d;
+    d.noise = wb.noise; d.latents = latents; d.mask = mask; d.timestep_indices = ts_idx;
+    d.timesteps_table = reinterpret_cast<const long long*>(sched.timesteps_table); d.alphas_cumprod = sched.alphas_cumprod;
+    d.n_steps = sched.n_steps; d.T = sched.num_train_timesteps; d.final_alpha_cumprod = sched.final_alpha_cumprod;
+    d.F = F; d.chw = 4 * hw; d.hw = hw; d.cfg = cfg_on ? 1 : 0; d.guidance = guidance;
+    d.prediction_type = sched.prediction_type; d.clip_sample = sched.clip_sample; d.clip_range = sched.clip_sample_range;
+    d.emulate_bf16 = sched.emulate_bf16; d.out = wb.latents_tmp;
+    if (int rc = cfg_ddim_step_run(d, wb.ts_tmp, s)) return rc;
+    D4D_CUDA_OK(cudaMemcpyAsync(latents, wb.latents_tmp, sizeof(bf16) * F * 4 * hw, cudaMemcpyDeviceToDevice, s));
+    D4D_CUDA_OK(cudaMemcpyAsync(ts_idx, wb.ts_tmp, sizeof(long long) * F, cudaMemcpyDeviceToDevice, s));
+    return 0;
+  });
+}
+
+int Model::denoise_window_dpm(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
+                              long long* ts_idx, const d4d_dpm_sched& sched, float guidance, int domain, int F, int h, int w,
+                              int num_steps, bf16* x0_prev, int* lower_order_nums, cudaStream_t stream) {
+  D4D_REQUIRE(latents && pixel && plucker && mask && ts_idx && x0_prev && lower_order_nums, "null argument");
+  D4D_REQUIRE(sched.timesteps_table && sched.coefs && sched.n_steps > 0, "scheduler tables");
+  const bool cfg_on = guidance > 1.0f;
+  const int hw = h * w;
+  return run_window(latents, pixel, plucker, skeletons, mask, ts_idx,
+                    reinterpret_cast<const long long*>(sched.timesteps_table), sched.n_steps, guidance, domain, F, h, w,
+                    num_steps, stream, 0, [&](WindowBufs& wb, cudaStream_t s) -> int {
+    if (!wb.order_tmp) D4D_CUDA_OK(cudaMalloc(&wb.order_tmp, sizeof(int) * F));
+    DpmArgs d;
+    d.noise = wb.noise; d.latents = latents; d.mask = mask; d.timestep_indices = ts_idx; d.coefs = sched.coefs;
+    d.n_steps = sched.n_steps; d.F = F; d.chw = 4 * hw; d.hw = hw; d.cfg = cfg_on ? 1 : 0; d.guidance = guidance;
+    d.prediction_type = sched.prediction_type; d.solver_order = sched.solver_order;
+    d.final_first_order = sched.final_first_order; d.emulate_bf16 = sched.emulate_bf16;
+    d.x0_prev = x0_prev; d.lower_order_nums = lower_order_nums; d.lower_order_nums_out = wb.order_tmp;
+    d.out = latents;  // each element is read and written by the same thread
+    if (int rc = cfg_dpm_step_run(d, wb.ts_tmp, s)) return rc;
+    D4D_CUDA_OK(cudaMemcpyAsync(ts_idx, wb.ts_tmp, sizeof(long long) * F, cudaMemcpyDeviceToDevice, s));
+    D4D_CUDA_OK(cudaMemcpyAsync(lower_order_nums, wb.order_tmp, sizeof(int) * F, cudaMemcpyDeviceToDevice, s));
+    return 0;
+  });
+}
+
+int Model::run_window(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
+                      long long* ts_idx, const long long* timesteps_table, int n_steps, float guidance, int domain, int F,
+                      int h, int w, int num_steps, cudaStream_t stream, int F_total, const WindowStep& step) {
   D4D_REQUIRE(domain == 0 || domain == 1, "Invalid domain");
   const bool cfg_on = guidance > 1.0f;
   const int B = cfg_on ? 2 * F : F;
@@ -1273,11 +1321,11 @@ int Model::denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker,
   WindowBufs& wb = *it->second;
   const int doms[2] = {domain, domain};
   const int hw = h * w;
-  for (int step = 0; step < num_steps; ++step) {
+  for (int s = 0; s < num_steps; ++s) {
     AssembleArgs a;
     a.latents = latents; a.pixel = pixel; a.plucker = plucker; a.skel_latents = pose ? nullptr : skeletons; a.mask = mask;
-    a.timestep_indices = ts_idx; a.timesteps_table = reinterpret_cast<const long long*>(sched.timesteps_table);
-    a.n_steps = sched.n_steps; a.F = F; a.h = h; a.w = w; a.cfg = cfg_on ? 1 : 0;
+    a.timestep_indices = ts_idx; a.timesteps_table = timesteps_table;
+    a.n_steps = n_steps; a.F = F; a.h = h; a.w = w; a.cfg = cfg_on ? 1 : 0;
     a.sample = wb.sample; a.timestep_out = wb.timestep;
     if (int rc = assemble_input_run(a, stream)) return rc;
     const bf16* skel_in = nullptr;
@@ -1291,16 +1339,7 @@ int Model::denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker,
       }
     }
     if (int rc = forward(wb.sample, wb.timestep, skel_in, doms, cfg_on ? 2 : 1, B, F, h, w, wb.noise, stream, F_total, pose && cfg_on)) return rc;
-    DdimArgs d;
-    d.noise = wb.noise; d.latents = latents; d.mask = mask; d.timestep_indices = ts_idx;
-    d.timesteps_table = reinterpret_cast<const long long*>(sched.timesteps_table); d.alphas_cumprod = sched.alphas_cumprod;
-    d.n_steps = sched.n_steps; d.T = sched.num_train_timesteps; d.final_alpha_cumprod = sched.final_alpha_cumprod;
-    d.F = F; d.chw = 4 * hw; d.hw = hw; d.cfg = cfg_on ? 1 : 0; d.guidance = guidance;
-    d.prediction_type = sched.prediction_type; d.clip_sample = sched.clip_sample; d.clip_range = sched.clip_sample_range;
-    d.emulate_bf16 = sched.emulate_bf16; d.out = wb.latents_tmp;
-    if (int rc = cfg_ddim_step_run(d, wb.ts_tmp, stream)) return rc;
-    D4D_CUDA_OK(cudaMemcpyAsync(latents, wb.latents_tmp, sizeof(bf16) * F * 4 * hw, cudaMemcpyDeviceToDevice, stream));
-    D4D_CUDA_OK(cudaMemcpyAsync(ts_idx, wb.ts_tmp, sizeof(long long) * F, cudaMemcpyDeviceToDevice, stream));
+    if (int rc = step(wb, stream)) return rc;
   }
   return 0;
 }

@@ -75,6 +75,7 @@ struct WindowBufs {  // scratch of d4d_denoise_window for one (F, h, w, cfg)
   bf16* noise = nullptr;
   bf16* latents_tmp = nullptr;
   long long* ts_tmp = nullptr;
+  int* order_tmp = nullptr;  // DPM-Solver++ only (allocated on first use)
   ~WindowBufs();
 };
 
@@ -104,6 +105,10 @@ class Model {
   int denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
                      long long* ts_idx, const d4d_sched& sched, float guidance, int domain, int F, int h, int w,
                      int num_steps, cudaStream_t stream, int F_total = 0);
+  // the same window step with the DPM-Solver++ step; x0_prev [F,4,h,w] and lower_order_nums [F] are updated in place
+  int denoise_window_dpm(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
+                         long long* ts_idx, const d4d_dpm_sched& sched, float guidance, int domain, int F, int h, int w,
+                         int num_steps, bf16* x0_prev, int* lower_order_nums, cudaStream_t stream);
   // per-kind device time (ms) of one forward, measured with CUDA events around every op
   int profile(const bf16* sample, const long long* timestep, const bf16* skeletons, const int* domain_ids, int n_domains,
               int B, int F, int h, int w, bf16* out, cudaStream_t stream, float* ms_by_kind, int* launches_by_kind,
@@ -149,6 +154,11 @@ class Model {
 
   void need(const std::string& key, std::vector<int64_t> shape);
   void declare_keys();
+  // num_steps x (assemble -> UNet -> step(noise, bufs, stream)); step writes the new latents and timestep indices
+  using WindowStep = std::function<int(WindowBufs&, cudaStream_t)>;
+  int run_window(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
+                 long long* ts_idx, const long long* timesteps_table, int n_steps, float guidance, int domain, int F, int h,
+                 int w, int num_steps, cudaStream_t stream, int F_total, const WindowStep& step);
   int cin_pad() const { return 16; }
   int kp_in() const { return 192; }
 };

@@ -12,13 +12,14 @@ from __future__ import annotations
 
 import importlib
 import json
+import math
 import os
 import warnings
 from typing import Callable, List, Optional, Union
 
 import torch
 
-from .config import SchedulerConfig, UNetConfig
+from .config import DPMSolverConfig, SchedulerConfig, UNetConfig
 from .pipeline import B200Diffuman4DPipeline
 from .unet import B200MultiviewUNet
 
@@ -59,11 +60,56 @@ def unet_config_from_json(d: dict) -> UNetConfig:
         center_input_sample=d.get("center_input_sample", False))
 
 
-def scheduler_config_from_json(d: dict) -> SchedulerConfig:
+def dpm_solver_config_from_json(d: dict) -> DPMSolverConfig:
+    """Map a diffusers ``DPMSolverMultistepScheduler`` config; every knob the fused step does not implement raises
+    ``NotImplementedError`` naming the key."""
+    def refuse(key, why):
+        raise NotImplementedError(f"DPMSolverMultistepScheduler {key}={d.get(key)!r} is not supported by the CUDA path "
+                                  f"({why})")
+
+    def want(key, allowed, default):
+        v = d.get(key, default)
+        if v not in allowed:
+            refuse(key, f"supported: {allowed}")
+        return v
+
+    if d.get("thresholding", False):
+        refuse("thresholding", "dynamic thresholding is not implemented")
+    for key in ("use_karras_sigmas", "use_exponential_sigmas", "use_beta_sigmas", "use_lu_lambdas", "use_flow_sigmas"):
+        if d.get(key, False):
+            refuse(key, "sigmas come straight from the beta schedule")
+    if d.get("rescale_betas_zero_snr", False):
+        refuse("rescale_betas_zero_snr", "zero-SNR rescaling is not implemented")
+    lmc = d.get("lambda_min_clipped", -math.inf)
+    if lmc is not None and math.isfinite(float(lmc)):
+        refuse("lambda_min_clipped", "only -inf (no clipping)")
+    if d.get("variance_type") is not None:
+        refuse("variance_type", "only None")
+    want("algorithm_type", ("dpmsolver++",), "dpmsolver++")
+    want("solver_type", ("midpoint",), "midpoint")
+    want("solver_order", (1, 2), 2)
+    want("beta_schedule", ("linear", "scaled_linear"), "linear")
+    want("prediction_type", ("epsilon", "v_prediction", "sample"), "epsilon")
+    want("final_sigmas_type", ("zero", "sigma_min"), "zero")
+    want("timestep_spacing", ("linspace", "leading", "trailing"), "linspace")
+    if d.get("trained_betas") is not None:
+        refuse("trained_betas", "betas come from beta_schedule")
+    return DPMSolverConfig(
+        num_train_timesteps=d.get("num_train_timesteps", 1000), beta_start=d.get("beta_start", 0.0001),
+        beta_end=d.get("beta_end", 0.02), beta_schedule=d.get("beta_schedule", "linear"),
+        solver_order=d.get("solver_order", 2), prediction_type=d.get("prediction_type", "epsilon"),
+        lower_order_final=d.get("lower_order_final", True), euler_at_final=d.get("euler_at_final", False),
+        final_sigmas_type=d.get("final_sigmas_type", "zero"), timestep_spacing=d.get("timestep_spacing", "linspace"),
+        steps_offset=d.get("steps_offset", 0))
+
+
+def scheduler_config_from_json(d: dict) -> Union[SchedulerConfig, DPMSolverConfig]:
     cls = d.get("_class_name", "DDIMScheduler")
+    if cls == "DPMSolverMultistepScheduler":
+        return dpm_solver_config_from_json(d)
     if cls != "DDIMScheduler":
         raise NotImplementedError(
-            f"scheduler {cls} is not fused on the CUDA path (DDIM epsilon / v_prediction / sample only); "
+            f"scheduler {cls} is not fused on the CUDA path (DDIMScheduler and DPMSolverMultistepScheduler only); "
             "run the reference's Python scheduler loop for other classes")
     if d.get("thresholding", False):
         raise NotImplementedError("dynamic thresholding is not supported")

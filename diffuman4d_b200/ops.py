@@ -2,6 +2,7 @@
 and the current stream; all arithmetic happens in libd4d.so."""
 from __future__ import annotations
 
+import ctypes as C
 from typing import Optional
 
 import torch
@@ -257,3 +258,25 @@ def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: flo
     check(lib().d4d_op_layernorm(_p(x), rows, C, float(eps), _p(gamma), _p(beta), _p(out), _stream()),
           "d4d_op_layernorm")
     return out
+
+
+def cfg_dpm_step(noise: torch.Tensor, latents: torch.Tensor, cond_mask: torch.Tensor, timestep_indices: torch.Tensor,
+                 x0_prev: torch.Tensor, lower_order_nums: torch.Tensor, sched, guidance_scale: float, cfg: bool):
+    """One CFG + DPM-Solver++ step of F frames (``sched``: a ``d4d_dpm_sched`` from ``DPMSolverTables.c_struct``).
+    ``noise`` [(cfg?2:1)*F,4,h,w]; ``x0_prev`` [F,4,h,w] bf16 is updated in place.  Returns (new latents, advanced
+    timestep indices, advanced ``lower_order_nums``)."""
+    _bf16c(noise, "noise"), _bf16c(latents, "latents"), _bf16c(cond_mask, "cond_mask"), _bf16c(x0_prev, "x0_prev")
+    F, _, h, w = latents.shape
+    if x0_prev.shape != latents.shape:
+        raise ValueError("x0_prev must have the shape of latents")
+    if lower_order_nums.dtype != torch.int32 or not lower_order_nums.is_cuda or lower_order_nums.numel() != F:
+        raise ValueError("lower_order_nums must be a CUDA int32 [F] tensor")
+    if timestep_indices.dtype != torch.int64 or not timestep_indices.is_cuda or timestep_indices.numel() != F:
+        raise ValueError("timestep_indices must be a CUDA int64 [F] tensor")
+    out = torch.empty_like(latents)
+    ti_out = torch.empty_like(timestep_indices)
+    lon_out = torch.empty_like(lower_order_nums)
+    check(lib().d4d_cfg_dpm_step(_p(noise), _p(latents), _p(cond_mask), _p(timestep_indices), _p(ti_out), _p(x0_prev),
+                                 _p(lower_order_nums), _p(lon_out), C.byref(sched), float(guidance_scale), int(cfg), F, h, w,
+                                 _p(out), _stream()), "d4d_cfg_dpm_step")
+    return out, ti_out, lon_out

@@ -3,7 +3,9 @@
 Seams (SURVEY.md section 8b):
   B-3  ``denoise_window``  == ``Diffuman4DPipeline.__call__`` with latents given
        (reference src/diffusers/pipelines/diffuman4d/pipeline_diffuman4d.py:345-425): input assembly, UNet, CFG
-       combine and the F per-frame scheduler steps run as ONE C-ABI call (no per-frame host sync).
+       combine and the F per-frame scheduler steps run as ONE C-ABI call (no per-frame host sync).  The scheduler is DDIM
+       (``SchedulerConfig``) or DPM-Solver++ (``DPMSolverConfig``); the latter keeps a per-frame history on the device
+       (``DPMSolverState``) in place of the reference's per-frame scheduler copies.
   B-4  ``sliding_iterative_denoise`` == PIPE:439-559: same arguments, same ValueErrors, same returned dict.  The VAE
        (stock AutoencoderKL, out of scope per SURVEY section 8f) is pluggable: pass ``vae`` with ``encode_latents(x)`` /
        ``decode_latents(z)`` callables, or feed latents directly (``pixel_values_latents=...``).
@@ -14,13 +16,13 @@ libd4d.so.
 from __future__ import annotations
 
 import ctypes as C
-from typing import Callable, List, Optional
+from typing import Callable, List, Optional, Union
 
 import torch
 
 from ._lib import check, lib
-from .config import SchedulerConfig
-from .scheduler import DDIMTables
+from .config import DPMSolverConfig, SchedulerConfig
+from .scheduler import DDIMTables, DPMSolverFrame, DPMSolverState, DPMSolverTables
 from .unet import B200MultiviewUNet
 
 _DOMAIN_IDS = {"spatial": 0, "temporal": 1}
@@ -56,13 +58,16 @@ def resize_conditions(plucker_embeds: torch.Tensor, cond_masks: torch.Tensor, h:
 
 
 class B200Diffuman4DPipeline:
-    def __init__(self, unet: B200MultiviewUNet, scheduler_config: Optional[SchedulerConfig] = None, vae=None,
-                 emulate_bf16_scheduler: bool = False):
+    def __init__(self, unet: B200MultiviewUNet, scheduler_config: Union[SchedulerConfig, DPMSolverConfig, None] = None,
+                 vae=None, emulate_bf16_scheduler: bool = False):
         self.unet = unet
         self.vae = vae
         self.device = unet.device
         self.dtype = torch.bfloat16
-        self.scheduler = DDIMTables(scheduler_config, device=self.device)
+        if isinstance(scheduler_config, DPMSolverConfig):
+            self.scheduler = DPMSolverTables(scheduler_config, device=self.device)
+        else:
+            self.scheduler = DDIMTables(scheduler_config, device=self.device)
         self.emulate_bf16_scheduler = emulate_bf16_scheduler
         self._guidance_scale = 1.0
 
@@ -81,18 +86,26 @@ class B200Diffuman4DPipeline:
     def do_classifier_free_guidance(self):
         return self._guidance_scale > 1 and self.unet.config.time_cond_proj_dim is None
 
+    @property
+    def _multistep(self) -> bool:
+        return isinstance(self.scheduler, DPMSolverTables)
+
     def parepare_schedulers(self, num_inference_steps: int, num_frames: int):
         """PIPE:265-271.  The per-frame deep copies exist in the reference only because scheduler objects are
-        stateful; DDIM is stateless, so one table serves all frames."""
+        stateful; DDIM is stateless, so one table serves all frames.  DPM-Solver++ gets a fresh (zeroed) device state for
+        the frames, and one ``DPMSolverFrame`` handle per frame in place of each copy."""
         ts = self.scheduler.set_timesteps(num_inference_steps)
+        if self._multistep:
+            return DPMSolverState(num_frames, self.device).frames(), ts
         return [self.scheduler] * num_frames, ts
 
     # B-3 -----------------------------------------------------------------------------------------------
     def denoise_window(self, *, latents, pixel_values_latents, plucker_embeds_latents, skeletons_latents,
                        cond_masks_latents, timestep_indices, domain: str, guidance_scale: float,
-                       num_inference_steps: int = 1):
-        """One window: ``num_inference_steps`` x (assemble -> UNet -> CFG -> per-frame DDIM).  ``latents`` [F,4,h,w] and
-        ``timestep_indices`` [F] (int64, device) are updated IN PLACE and returned."""
+                       num_inference_steps: int = 1, solver_state: Optional[DPMSolverState] = None):
+        """One window: ``num_inference_steps`` x (assemble -> UNet -> CFG -> per-frame scheduler step).  ``latents``
+        [F,4,h,w] and ``timestep_indices`` [F] (int64, device) are updated IN PLACE and returned.  With DPM-Solver++,
+        ``solver_state`` is the window frames' ``DPMSolverState`` (``DPMSolverState.take``), also updated in place."""
         if domain not in _DOMAIN_IDS:
             raise ValueError(f"Invalid domain for temporal embedding: {domain}")
         F_, _, h, w = latents.shape
@@ -115,6 +128,23 @@ class B200Diffuman4DPipeline:
         sched = self.scheduler.c_struct(self.emulate_bf16_scheduler)
         self._guidance_scale = guidance_scale
         g = guidance_scale if self.do_classifier_free_guidance else 1.0
+        if self._multistep:
+            st = solver_state
+            if st is None:
+                raise ValueError("the DPM-Solver++ scheduler needs the window frames' solver_state")
+            if not (st.x0_prev is not None and st.x0_prev.is_cuda and st.x0_prev.dtype == torch.bfloat16
+                    and st.x0_prev.is_contiguous() and st.x0_prev.shape == latents.shape):
+                raise ValueError("solver_state.x0_prev must be a contiguous CUDA bfloat16 tensor shaped like latents")
+            lon = st.lower_order_nums
+            if not (lon.is_cuda and lon.dtype == torch.int32 and lon.is_contiguous() and lon.numel() == F_):
+                raise ValueError("solver_state.lower_order_nums must be a contiguous CUDA int32 [F] tensor")
+            with torch.cuda.device(dev):
+                check(lib().d4d_denoise_window_dpm(
+                    self.unet._h, latents.data_ptr(), pix.data_ptr(), plk.data_ptr(), skl.data_ptr(), msk.data_ptr(),
+                    timestep_indices.data_ptr(), C.byref(sched), float(g), _DOMAIN_IDS[domain], F_, h, w,
+                    int(num_inference_steps), st.x0_prev.data_ptr(), lon.data_ptr(),
+                    torch.cuda.current_stream().cuda_stream), "d4d_denoise_window_dpm")
+            return latents, timestep_indices
         with torch.cuda.device(dev):
             check(lib().d4d_denoise_window(self.unet._h, latents.data_ptr(), pix.data_ptr(), plk.data_ptr(),
                                            skl.data_ptr(), msk.data_ptr(), timestep_indices.data_ptr(), C.byref(sched),
@@ -134,17 +164,29 @@ class B200Diffuman4DPipeline:
             raise ValueError("domains must be a one-element list, e.g. ['spatial']")
         F_ = pixel_values_latents.shape[0]
         if schedulers is None:
-            self.parepare_schedulers(num_inference_steps, F_)
+            schedulers, _ = self.parepare_schedulers(num_inference_steps, F_)
             timestep_indices = torch.zeros(F_)
         if latents is None:        # PIPE:172-183 prepare_latents: draw the initial noise
             latents = torch.randn(tuple(pixel_values_latents.shape), generator=unused.get("generator"), device=self.device,
                                   dtype=torch.bfloat16)
         lat = (latents * self.scheduler.init_noise_sigma).to(device=self.device, dtype=torch.bfloat16).contiguous().clone()
         ti = timestep_indices.to(device=self.device, dtype=torch.int64).contiguous().clone()
+        task, frames, window_state = None, None, None
+        if self._multistep:   # the frames' solver history travels with the `schedulers` handles
+            if len(schedulers) != F_ or not all(isinstance(s, DPMSolverFrame) for s in schedulers):
+                raise ValueError("schedulers must be the per-frame handles of parepare_schedulers, one per frame")
+            task = schedulers[0].state
+            if any(s.state is not task for s in schedulers):
+                raise ValueError("schedulers must all come from one parepare_schedulers call")
+            frames = torch.tensor([s.index for s in schedulers], dtype=torch.int64)
+            window_state = task.take(frames, *lat.shape[2:])
         self.denoise_window(latents=lat, pixel_values_latents=pixel_values_latents,
                             plucker_embeds_latents=plucker_embeds_latents, skeletons_latents=skeletons_latents,
                             cond_masks_latents=cond_masks_latents, timestep_indices=ti, domain=domains[0],
-                            guidance_scale=guidance_scale, num_inference_steps=num_inference_steps)
+                            guidance_scale=guidance_scale, num_inference_steps=num_inference_steps,
+                            solver_state=window_state)
+        if task is not None:
+            task.put(frames, window_state)
         return lat
 
     # B-4 -------------------------------------------------------------------------------------------------
@@ -200,7 +242,8 @@ class B200Diffuman4DPipeline:
             latents = torch.randn(n, 4, h, w, generator=generator, device=dev, dtype=torch.bfloat16)
         latents = (latents.to(dev, torch.bfloat16) * self.scheduler.init_noise_sigma).contiguous().clone()
 
-        self.parepare_schedulers(num_inference_steps, n)
+        schedulers, _ = self.parepare_schedulers(num_inference_steps, n)   # a fresh solver state per task (PIPE:501)
+        task = schedulers[0].state if self._multistep else None
         target_windows, input_windows = build_windows(target_indices, input_indices, domain, window_size,
                                                       sliding_stride, sliding_shift, bidirectional)
         it = zip(target_windows, input_windows)
@@ -210,10 +253,13 @@ class B200Diffuman4DPipeline:
             window = torch.cat([iw, tw])
             lw = latents[window].contiguous()
             tiw = timestep_indices[window].contiguous()
+            sw = task.take(window, h, w) if task is not None else None
             self.denoise_window(latents=lw, pixel_values_latents=pixel_values_latents[window],
                                 plucker_embeds_latents=plk[window], skeletons_latents=skl[window],
                                 cond_masks_latents=msk[window], timestep_indices=tiw, domain=domain,
-                                guidance_scale=guidance_scale, num_inference_steps=num_denoising_steps)
+                                guidance_scale=guidance_scale, num_inference_steps=num_denoising_steps, solver_state=sw)
+            if task is not None:
+                task.put(window, sw)
             timestep_indices[tw] += num_denoising_steps
             latents[window] = lw
 

@@ -1,9 +1,13 @@
-"""Host-side DDIM tables for the fused CFG+DDIM kernel.
+"""Host-side scheduler tables for the fused CFG + scheduler-step kernels: DDIM and DPM-Solver++.
 
 Mirrors what the reference obtains from ``self.scheduler.set_timesteps(n)`` + per-frame deep copies
 (pipeline_diffuman4d.py:265-271) for upstream diffusers==0.33.1 ``DDIMScheduler``: the ``timesteps`` vector and
 ``alphas_cumprod`` / ``final_alpha_cumprod``.  Only table construction lives here (numpy, host); the update itself
 runs on the GPU (csrc/elementwise.cu ``cfg_ddim_kernel``).
+
+``DPMSolverTables`` does the same for ``DPMSolverMultistepScheduler`` (dpmsolver++ / midpoint, order 1 or 2): the timesteps,
+the sigma table and the per-step solver coefficients (``cfg_dpm_kernel``).  That scheduler is stateful, which is why the
+reference deep-copies it per frame; here the state of every frame of a task is a ``DPMSolverState`` on the device.
 """
 from __future__ import annotations
 
@@ -12,8 +16,8 @@ import ctypes as C
 import numpy as np
 import torch
 
-from ._lib import D4DSched
-from .config import SchedulerConfig
+from ._lib import D4DDpmSched, D4DSched
+from .config import DPMSolverConfig, SchedulerConfig
 
 _PRED = {"epsilon": 0, "v_prediction": 1, "sample": 2}
 
@@ -78,3 +82,156 @@ class DDIMTables:
         s.clip_sample_range = float(c.clip_sample_range)
         s.emulate_bf16 = int(emulate_bf16)
         return s
+
+
+def _betas(c) -> torch.Tensor:
+    T = c.num_train_timesteps
+    if c.beta_schedule == "scaled_linear":
+        return torch.linspace(c.beta_start ** 0.5, c.beta_end ** 0.5, T, dtype=torch.float32) ** 2
+    if c.beta_schedule == "linear":
+        return torch.linspace(c.beta_start, c.beta_end, T, dtype=torch.float32)
+    raise ValueError(f"{c.beta_schedule} is not implemented")
+
+
+def dpm_timesteps(c: DPMSolverConfig, n: int) -> np.ndarray:
+    """``DPMSolverMultistepScheduler.set_timesteps(n)`` timesteps (lambda_min_clipped = -inf); duplicates are refused,
+    so that a frame's step index is always its timestep index."""
+    T = c.num_train_timesteps
+    if n > T:
+        raise ValueError(f"`num_inference_steps`: {n} cannot be larger than `self.config.train_timesteps`: {T}")
+    if c.timestep_spacing == "linspace":
+        ts = np.linspace(0, T - 1, n + 1).round()[::-1][:-1].copy().astype(np.int64)
+    elif c.timestep_spacing == "leading":
+        ts = (np.arange(0, n + 1) * (T // (n + 1))).round()[::-1][:-1].copy().astype(np.int64) + c.steps_offset
+    elif c.timestep_spacing == "trailing":
+        ts = np.arange(T, 0, -T / n).round().copy().astype(np.int64) - 1
+    else:
+        raise ValueError(f"{c.timestep_spacing} is not supported")
+    if len(np.unique(ts)) != len(ts):
+        raise ValueError(f"{c.timestep_spacing} spacing gives duplicate timesteps for {n} steps of {T}: {ts.tolist()}")
+    return ts
+
+
+def dpm_step_coefficients(sigmas: torch.Tensor) -> torch.Tensor:
+    """[n, 6] fp32 coefficients of the n steps over ``sigmas`` [n+1] (layout in include/d4d.h ``d4d_dpm_sched``), each
+    evaluated on 0-dim fp32 tensors in the order ``DPMSolverMultistepScheduler``'s ``convert_model_output`` /
+    ``dpm_solver_first_order_update`` / ``multistep_dpm_solver_second_order_update`` evaluate them."""
+    def alpha_sigma(sigma):
+        alpha_t = 1 / ((sigma ** 2 + 1) ** 0.5)
+        return alpha_t, sigma * alpha_t
+
+    def lam(sigma):
+        a, s = alpha_sigma(sigma)
+        return torch.log(a) - torch.log(s)
+
+    n = sigmas.numel() - 1
+    out = torch.zeros(n, 6, dtype=torch.float32)
+    for i in range(n):
+        alpha_s, sigma_s = alpha_sigma(sigmas[i])
+        alpha_t, sigma_t = alpha_sigma(sigmas[i + 1])
+        h = lam(sigmas[i + 1]) - lam(sigmas[i])
+        c = alpha_t * (torch.exp(-h) - 1.0)
+        inv_r0 = 1.0 / ((lam(sigmas[i]) - lam(sigmas[i - 1])) / h) if i > 0 else torch.tensor(0.0)
+        out[i] = torch.stack([alpha_s, sigma_s, sigma_t / sigma_s, c, 0.5 * c, inv_r0])
+    return out
+
+
+class DPMSolverTables:
+    """Timesteps, sigmas and step coefficients of ``DPMSolverMultistepScheduler`` (diffusers 0.33.1) for
+    ``cfg_dpm_kernel``."""
+    init_noise_sigma = 1.0  # upstream: init_noise_sigma 1, scale_model_input is the identity
+
+    def __init__(self, cfg: DPMSolverConfig = None, device="cuda:0"):
+        self.config = cfg or DPMSolverConfig()
+        c = self.config
+        if c.prediction_type not in _PRED:
+            raise ValueError(f"prediction_type given as {c.prediction_type} must be one of {list(_PRED)}")
+        if c.solver_order not in (1, 2):
+            raise NotImplementedError(f"solver_order={c.solver_order}: the fused step implements orders 1 and 2")
+        if c.final_sigmas_type not in ("zero", "sigma_min"):
+            raise ValueError(f"final_sigmas_type {c.final_sigmas_type!r} must be 'zero' or 'sigma_min'")
+        self.alphas_cumprod = torch.cumprod(1.0 - _betas(c), dim=0)
+        self.all_sigmas = ((1 - self.alphas_cumprod) / self.alphas_cumprod) ** 0.5   # fp32 [T]
+        self.device = torch.device(device)
+        self.num_inference_steps = None
+        self.timesteps = None          # host int64 [n]
+        self.sigmas = None             # host fp32 [n+1]
+        self.coefs = None              # host fp32 [n, 6]
+        self._dev = None
+
+    def set_timesteps(self, n: int, device=None):
+        c = self.config
+        ts = dpm_timesteps(c, n)
+        last = 0.0 if c.final_sigmas_type == "zero" else float(self.all_sigmas[0])
+        self.num_inference_steps = n
+        self.timesteps = torch.from_numpy(ts)
+        self.sigmas = torch.cat([self.all_sigmas[self.timesteps], torch.tensor([last], dtype=torch.float32)])
+        self.coefs = dpm_step_coefficients(self.sigmas)
+        self._dev = None
+        return self.timesteps
+
+    @property
+    def final_first_order(self) -> bool:
+        """The last step falls back to first order (upstream ``lower_order_final`` in ``step``)."""
+        c = self.config
+        return bool(c.euler_at_final or (c.lower_order_final and self.num_inference_steps < 15)
+                    or c.final_sigmas_type == "zero")
+
+    def c_struct(self, emulate_bf16: bool = False) -> D4DDpmSched:
+        if self.timesteps is None:
+            raise ValueError("call set_timesteps first")
+        if self._dev is None:
+            self._dev = (self.timesteps.to(self.device), self.coefs.to(self.device).contiguous())
+        c = self.config
+        s = D4DDpmSched()
+        s.timesteps_table = self._dev[0].data_ptr()
+        s.coefs = self._dev[1].data_ptr()
+        s.n_steps = int(self.num_inference_steps)
+        s.prediction_type = _PRED[c.prediction_type]
+        s.solver_order = int(c.solver_order)
+        s.final_first_order = int(self.final_first_order)
+        s.emulate_bf16 = int(emulate_bf16)
+        return s
+
+
+class DPMSolverState:
+    """The DPM-Solver++ history of every frame of one task, on the device: ``x0_prev`` [F,4,h,w] bf16 (each frame's
+    previous data prediction) and ``lower_order_nums`` [F] int32.  A new task starts from zeros, which is the state of a
+    freshly deep-copied upstream scheduler.  ``take`` / ``put`` gather and scatter the frames of one window."""
+
+    def __init__(self, num_frames: int, device, x0_prev: torch.Tensor = None, lower_order_nums: torch.Tensor = None):
+        self.num_frames = num_frames
+        self.device = torch.device(device)
+        self.x0_prev = x0_prev         # allocated (zeroed) when the latent size is first known
+        self.lower_order_nums = (torch.zeros(num_frames, dtype=torch.int32, device=self.device)
+                                 if lower_order_nums is None else lower_order_nums)
+
+    def frames(self) -> list:
+        """One handle per frame: what ``parepare_schedulers`` hands out in place of the per-frame scheduler copies."""
+        return [DPMSolverFrame(self, i) for i in range(self.num_frames)]
+
+    def _ensure(self, h: int, w: int):
+        if self.x0_prev is None:
+            self.x0_prev = torch.zeros(self.num_frames, 4, h, w, dtype=torch.bfloat16, device=self.device)
+        elif tuple(self.x0_prev.shape[2:]) != (h, w):
+            raise ValueError(f"solver state holds {tuple(self.x0_prev.shape[2:])} latents, got {(h, w)}")
+
+    def take(self, index: torch.Tensor, h: int, w: int) -> "DPMSolverState":
+        """The state of frames ``index`` as a new (contiguous) state, for one window."""
+        self._ensure(h, w)
+        index = index.to(self.device)
+        return DPMSolverState(len(index), self.device, self.x0_prev[index].contiguous(),
+                              self.lower_order_nums[index].contiguous())
+
+    def put(self, index: torch.Tensor, window: "DPMSolverState"):
+        index = index.to(self.device)
+        self.x0_prev[index] = window.x0_prev
+        self.lower_order_nums[index] = window.lower_order_nums
+
+
+class DPMSolverFrame:
+    """Frame ``index`` of a task's ``DPMSolverState`` (the per-frame scheduler object of the reference's lists)."""
+    __slots__ = ("state", "index")
+
+    def __init__(self, state: DPMSolverState, index: int):
+        self.state, self.index = state, index

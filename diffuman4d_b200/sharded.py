@@ -15,6 +15,7 @@ import torch.distributed as dist
 
 from ._lib import check, lib
 from .pipeline import B200Diffuman4DPipeline, _DOMAIN_IDS
+from .scheduler import DDIMTables
 from .sharding import frame_shard
 
 
@@ -103,6 +104,8 @@ class FrameShardedPipeline:
                        timestep_indices, domain: str, guidance_scale: float, F_total: int, num_inference_steps: int = 1):
         """B-3 on this rank's frames (all tensors hold the LOCAL frames; updated in place like the single-GPU call)."""
         pipe = self.pipe
+        if not isinstance(pipe.scheduler, DDIMTables):
+            raise NotImplementedError("the frame-sharded window runs the DDIM step only")
         if domain not in _DOMAIN_IDS:
             raise ValueError(f"Invalid domain for temporal embedding: {domain}")
         self._inplace(latents, "latents", torch.bfloat16)

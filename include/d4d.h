@@ -63,6 +63,26 @@ typedef struct d4d_sched {
   int32_t emulate_bf16;             /* 1: round after every arithmetic op like the reference's bf16 eager maths */
 } d4d_sched;
 
+/* DPM-Solver++ constants for the fused step (upstream diffusers DPMSolverMultistepScheduler with algorithm_type
+ * "dpmsolver++", solver_type "midpoint", solver_order 1 or 2).  The solver's history is per frame and lives on the device
+ * (x0_prev / lower_order_nums of d4d_denoise_window_dpm); a frame's step index is its timestep index, so schedules with
+ * duplicate timesteps are not accepted by the host tables.
+ * coefs row i (fp32), computed on the host from the sigma table in the upstream scheduler's own fp32 order of operations
+ * (so the device evaluates no log / exp and the bf16-emulating step is bit-exact against a CPU evaluation):
+ *   [0] alpha_s = 1 / sqrt(sigma_i^2 + 1)   [1] sigma_s = sigma_i * alpha_s   [2] sigma_t(i+1) / sigma_s
+ *   [3] c = alpha_t(i+1) * (exp(-h) - 1), h = lambda_(i+1) - lambda_i        [4] 0.5 * c
+ *   [5] 1 / r0, r0 = (lambda_i - lambda_(i-1)) / h   (0 in row 0) */
+typedef struct d4d_dpm_sched {
+  const int64_t* timesteps_table;   /* device, [n_steps]  (scheduler.timesteps after set_timesteps) */
+  const float* coefs;               /* device, [n_steps][6], see above */
+  int32_t n_steps;
+  int32_t prediction_type;          /* 0 epsilon, 1 v_prediction, 2 sample */
+  int32_t solver_order;             /* 1 or 2 */
+  int32_t final_first_order;        /* 1: the last step is first order (euler_at_final, lower_order_final with fewer
+                                       than 15 steps, or final_sigmas_type "zero") */
+  int32_t emulate_bf16;             /* 1: round like the reference's bf16 eager maths (history and x0 in bf16) */
+} d4d_dpm_sched;
+
 const char* d4d_last_error(void);
 int d4d_version(void);
 
@@ -110,6 +130,15 @@ int d4d_denoise_window(d4d_handle* h, void* latents, const void* pixel_latents, 
                        const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
                        const d4d_sched* sched, float guidance_scale, int domain, int F, int height, int width,
                        int num_steps, void* stream);
+/* The same window step with a DPM-Solver++ scheduler.  Arguments as d4d_denoise_window, plus the window frames' solver
+ * state, read and updated in place (conditioning frames keep theirs):
+ *   x0_prev           device bf16 [F,4,h,w]: each frame's data prediction of its previous step (zeros for a new task)
+ *   lower_order_nums  device int32 [F]: steps each frame has taken, capped at solver_order (zeros for a new task)
+ * A caller carries both across the windows of one task, gathered and scattered with the frames like the latents. */
+int d4d_denoise_window_dpm(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                           const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                           const d4d_dpm_sched* sched, float guidance_scale, int domain, int F, int height, int width,
+                           int num_steps, void* x0_prev, int32_t* lower_order_nums, void* stream);
 
 /* ---- building blocks of B-3, exported for parity tests ------------------------------------------------ */
 int d4d_assemble_input(void* latents, const void* pixel_latents, const void* plucker, const void* skel_latents,
@@ -119,6 +148,13 @@ int d4d_assemble_input(void* latents, const void* pixel_latents, const void* plu
 int d4d_cfg_ddim_step(const void* noise, const void* latents, const void* cond_mask, const int64_t* timestep_indices,
                       int64_t* timestep_indices_out, const d4d_sched* sched, float guidance_scale, int cfg, int F,
                       int height, int width, void* latents_out, void* stream);
+/* One CFG + DPM-Solver++ step of the frames (cfg: noise holds [uncond F | cond F]).  x0_prev [F,4,h,w] is updated in
+ * place; lower_order_nums_out and timestep_indices_out receive the advanced counters (they may not alias the inputs);
+ * latents_out may alias latents. */
+int d4d_cfg_dpm_step(const void* noise, const void* latents, const void* cond_mask, const int64_t* timestep_indices,
+                     int64_t* timestep_indices_out, void* x0_prev, const int32_t* lower_order_nums,
+                     int32_t* lower_order_nums_out, const d4d_dpm_sched* sched, float guidance_scale, int cfg, int F,
+                     int height, int width, void* latents_out, void* stream);
 
 /* ---- op-level entry points (each is one hot-path kernel; used by tests/ and bench.py) ------------------
  * d4d_op_gemm:   out[M,N] = act((A|A2)[M,K1+K2] . W[N,K]^T + bias + rowvec[row/rows_per_image]) * scale + residual

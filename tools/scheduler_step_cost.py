@@ -1,0 +1,132 @@
+"""What the DPM-Solver++ step costs against DDIM in the window step of bench.py's workload (W16 @ 64x64 latents, CFG 2.0,
+SD-2.1 channel layout, random weights), on one GPU in one process.
+
+Both pipelines share one UNet; rounds alternate DDIM and DPM-Solver++ so that clock drift hits both alike.  Each step
+restores its inputs (latents, timestep indices and, for DPM-Solver++, the frames' solver state) from device copies and
+then makes ONE public ``denoise_window`` call; the DPM-Solver++ frames start with a history, so the timed step is the
+second-order one.  Also times the two fused step kernels alone.  Prints one JSON line (and writes it to --out) with the
+card's name, power limit and max SM clock beside the numbers.
+
+    python tools/scheduler_step_cost.py --rounds 8 --steps 10 --out /tmp/scheduler_step_cost.json
+"""
+from __future__ import annotations
+
+import argparse
+import ctypes as C
+import json
+import os
+import statistics
+import sys
+
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--rounds", type=int, default=8)
+    ap.add_argument("--steps", type=int, default=10, help="window steps per round and scheduler")
+    ap.add_argument("--kernel-iters", type=int, default=200)
+    ap.add_argument("--out", default=None)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("needs an H100: there is no CPU fallback")
+
+    from bench import WORKLOAD, gpu_identity, synth_inputs
+    from diffuman4d_b200 import ops
+    from diffuman4d_b200._lib import check, lib
+    from diffuman4d_b200.config import DPMSolverConfig, SchedulerConfig, UNetConfig
+    from diffuman4d_b200.pipeline import B200Diffuman4DPipeline
+    from diffuman4d_b200.scheduler import DPMSolverState
+    from diffuman4d_b200.unet import B200MultiviewUNet
+    from diffuman4d_b200.weights import random_state_dict
+
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    wl = WORKLOAD
+    F, h, w, n_cond = wl["F"], wl["h"], wl["w"], wl["n_cond"]
+    cfg = UNetConfig.sd21()
+    unet = B200MultiviewUNet(cfg, 0).load_state_dict(random_state_dict(cfg, seed=1))
+    ddim = B200Diffuman4DPipeline(unet, SchedulerConfig())
+    dpm = B200Diffuman4DPipeline(unet, DPMSolverConfig())
+    ddim.parepare_schedulers(wl["n_steps"], F)
+    dpm.parepare_schedulers(wl["n_steps"], F)
+
+    inp = {k: (v.to(torch.bfloat16) if v.dtype.is_floating_point else v).to(dev)
+           for k, v in synth_inputs(F, n_cond, h, w).items()}
+    lat, ts = inp["latents"].clone(), inp["ts"].clone()
+    g = torch.Generator(device=dev).manual_seed(0)
+    x0_init = torch.randn(F, 4, h, w, device=dev, generator=g).to(torch.bfloat16)
+    lon_init = torch.full((F,), 1, dtype=torch.int32, device=dev)          # every frame has a history: second order
+    state = DPMSolverState(F, dev).take(torch.arange(F), h, w)
+
+    def window(p, solver_state=None):
+        def step():
+            lat.copy_(inp["latents"])
+            ts.copy_(inp["ts"])
+            if solver_state is not None:
+                solver_state.x0_prev.copy_(x0_init)
+                solver_state.lower_order_nums.copy_(lon_init)
+            p.denoise_window(latents=lat, pixel_values_latents=inp["pixel"], plucker_embeds_latents=inp["plucker"],
+                             skeletons_latents=inp["skel"], cond_masks_latents=inp["mask"], timestep_indices=ts,
+                             domain=wl["domain"], guidance_scale=wl["guidance"], solver_state=solver_state)
+        return step
+
+    # the two fused step kernels alone, on the window's shapes (CFG noise [2F,4,h,w])
+    noise = torch.randn(2 * F, 4, h, w, device=dev, generator=g).to(torch.bfloat16)
+    ddim_s, dpm_s = ddim.scheduler.c_struct(), dpm.scheduler.c_struct()
+    out = torch.empty_like(lat)
+    ts_out = torch.empty_like(ts)
+    x0_k, lon_k = x0_init.clone(), lon_init.clone()
+    stream = lambda: torch.cuda.current_stream().cuda_stream
+
+    def ddim_kernel():
+        check(lib().d4d_cfg_ddim_step(noise.data_ptr(), lat.data_ptr(), inp["mask"].data_ptr(), ts.data_ptr(),
+                                      ts_out.data_ptr(), C.byref(ddim_s), wl["guidance"], 1, F, h, w, out.data_ptr(),
+                                      stream()))
+
+    def dpm_kernel():
+        ops.cfg_dpm_step(noise, lat, inp["mask"], ts, x0_k, lon_k, dpm_s, wl["guidance"], True)
+
+    def timed(fn, n):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(n):
+            fn()
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / n
+
+    arms = {"ddim": window(ddim), "dpm_solver++": window(dpm, state)}
+    for fn in arms.values():                                             # warm-up: plans, buffers, clocks
+        for _ in range(3):
+            fn()
+    torch.cuda.synchronize()
+    per_round = {k: [] for k in arms}
+    kernel = {"ddim": [], "dpm_solver++": []}
+    for _ in range(args.rounds):
+        for k, fn in arms.items():
+            per_round[k].append(timed(fn, args.steps))
+        kernel["ddim"].append(timed(ddim_kernel, args.kernel_iters))
+        kernel["dpm_solver++"].append(timed(dpm_kernel, args.kernel_iters))
+    med = {k: statistics.median(v) for k, v in per_round.items()}
+    kmed = {k: statistics.median(v) for k, v in kernel.items()}
+    res = {"workload": wl["name"], "gpu": gpu_identity(0), "rounds": args.rounds, "steps_per_round": args.steps,
+           "window_step_ms_median": med, "window_step_ms_rounds": per_round,
+           "dpm_minus_ddim_ms": med["dpm_solver++"] - med["ddim"],
+           "dpm_over_ddim": med["dpm_solver++"] / med["ddim"],
+           "step_kernel_us_median": {k: 1e3 * v for k, v in kmed.items()},
+           "note": "DPM-Solver++ step timed in its second-order branch (every frame has a history); the kernel-only "
+                   "DPM time includes the op wrapper's output allocations"}
+    line = json.dumps(res)
+    print(line)
+    if args.out:
+        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+        with open(args.out, "w") as f:
+            f.write(line + "\n")
+
+
+if __name__ == "__main__":
+    main()
