@@ -589,6 +589,10 @@ class PlanBuilder {
   void tap(const std::string& name, const Act& a) {
     if (!dry_) p_.taps.push_back({name, a.p, a.C, a.H, a.W, p_.ops.size()});
   }
+  // module taps, named after the diffusers module path whose output `a` is; numbered after the block taps (end of build)
+  void module_tap(const std::string& name, const Act& a) {
+    if (!dry_) module_taps_.push_back({name, a.p, a.C, a.H, a.W, p_.ops.size()});
+  }
   void gemm(const GemmDesc& d) {
     if (dry_) { p_.launches += 1; return; }
     GemmLaunch L;
@@ -870,6 +874,7 @@ class PlanBuilder {
       release(emb);
       emb = emb2;
     }
+    module_tap("time_embedding", Act{emb, TE, 1, 1});
     op([=](cudaStream_t s) { return silu_run(emb, static_cast<long long>(B) * TE, e1, s); });
     const int ldt = m.temb_total_;
     bf16* temb_all = alloc(static_cast<size_t>(B) * ldt);
@@ -960,10 +965,13 @@ class PlanBuilder {
     skips.push_back(x);
     for (int i = 0; i < 4; ++i) {
       const int nf = (4 - i - 1) < cfg.num_3d_attn_blocks ? F : 1;
+      const std::string blk = "down_blocks." + std::to_string(i);
       for (int j = 0; j < L; ++j) {
         Act y = resnet(m.down_res_[i][j], x, nullptr, temb_all, ldt);
+        module_tap(blk + ".resnets." + std::to_string(j), y);
         if (i < 3) {
           Act z = transformer(m.down_xf_[i][j], y, nf);
+          module_tap(blk + ".attentions." + std::to_string(j), z);
           release(y.p);
           y = z;
         }
@@ -977,17 +985,21 @@ class PlanBuilder {
         d.conv = 1; d.conv_kind = 1; d.A = x.p; d.n_img = B; d.H = x.H; d.W = x.W; d.Cin = x.C;
         d.Wt = m.down_ds_[i].w; d.N = x.C; d.bias = m.down_ds_[i].b; d.out = y.p; d.ldo = x.C;
         gemm_stats(d, y, B, Ho, Wo);
+        module_tap(blk + ".downsamplers.0", y);
         x = y;
         skips.push_back(x);
       }
-      tap("down_blocks." + std::to_string(i), x);
+      tap(blk, x);
     }
     // ---- 4. mid: UNET:568-572 ----
     {
       Act y = resnet(m.mid_res_[0], x, nullptr, temb_all, ldt);  // x is a skip: keep it
+      module_tap("mid_block.resnets.0", y);
       Act z = transformer(m.mid_xf_, y, F);
+      module_tap("mid_block.attentions.0", z);
       release(y.p);
       Act u = resnet(m.mid_res_[1], z, nullptr, temb_all, ldt);
+      module_tap("mid_block.resnets.1", u);
       release(z.p);
       x = u;
     }
@@ -995,14 +1007,17 @@ class PlanBuilder {
     // ---- 5. up: UNET:575-587 ----
     for (int i = 0; i < 4; ++i) {
       const int nf = i < cfg.num_3d_attn_blocks ? F : 1;
+      const std::string blk = "up_blocks." + std::to_string(i);
       for (int j = 0; j <= L; ++j) {
         const Act sk = skips.back();
         skips.pop_back();
         Act y = resnet(m.up_res_[i][j], x, &sk, temb_all, ldt);
+        module_tap(blk + ".resnets." + std::to_string(j), y);
         release(x.p);
         release(sk.p);
         if (i > 0) {
           Act z = transformer(m.up_xf_[i][j], y, nf);
+          module_tap(blk + ".attentions." + std::to_string(j), z);
           release(y.p);
           y = z;
         }
@@ -1018,10 +1033,11 @@ class PlanBuilder {
           d.Wt = m.up_us_[i].w; d.N = x.C; d.bias = m.up_us_[i].b; d.out = y.p; d.ldo = x.C;
           gemm_stats(d, y, B, x.H, x.W);  // (tiles walk the low-resolution grid)
         }
+        module_tap(blk + ".upsamplers.0", y);
         release(x.p);
         x = y;
       }
-      tap("up_blocks." + std::to_string(i), x);
+      tap(blk, x);
     }
     // ---- 6. out: UNET:590-593 ----
     {
@@ -1037,6 +1053,7 @@ class PlanBuilder {
       release(y.p);
     }
     release(temb_all);
+    p_.taps.insert(p_.taps.end(), module_taps_.begin(), module_taps_.end());
     return rc_;
   }
 
@@ -1051,6 +1068,7 @@ class PlanBuilder {
   long long* stats_pool_ = nullptr;
   size_t stats_used_ = 0;
   int rc_ = 0;
+  std::vector<Plan::Tap> module_taps_;
 };
 
 Plan* Model::find_plan(int n_domains, int B, int F, int h, int w) {

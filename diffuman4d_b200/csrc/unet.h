@@ -56,8 +56,9 @@ struct Plan {
   std::vector<int> op_kind;       // 0 gemm, 1 conv3x3, 2 attention, 3 groupnorm, 4 layernorm, 5 other
   std::vector<double> op_flops;   // executed FLOPs (incl. tile/head padding) of tensor-core ops
   std::vector<cudaEvent_t> events; // lazily created by profile()
-  // debug taps (per-level drift report, tests/test_gpu_fullsize.py): a named intermediate activation [B*H*W, C] (NHWC) that is
-  // complete once ops[0 .. n_ops) have run; the arena may reuse its storage afterwards
+  // debug taps (per-level drift report, tests/test_gpu_fullsize.py; per-module checks, tests/test_gpu_unet_modules.py): a
+  // named intermediate activation [B*H*W, C] (NHWC) that is complete once ops[0 .. n_ops) have run; the arena may reuse its
+  // storage afterwards.  The ten block taps come first, then the module taps in forward order (include/d4d.h).
   struct Tap { std::string name; const bf16* p; int C, H, W; size_t n_ops; };
   std::vector<Tap> taps;
   // per-call externals, set by Model::forward before running the ops

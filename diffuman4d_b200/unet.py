@@ -18,6 +18,7 @@ from .config import UNetConfig
 
 _DOMAIN_IDS = {"spatial": 0, "temporal": 1}
 _DTYPE_CODE = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
+_BLOCK_TAPS = 10   # d4d_debug_tap indices 0-9: conv_in, down_blocks.0-3, mid_block, up_blocks.0-3; module taps follow
 
 
 class UNetMultiviewConditionOutput(SimpleNamespace):
@@ -158,8 +159,11 @@ class B200MultiviewUNet:
 
     __call__ = forward
 
-    def debug_taps(self, sample, timestep, skeletons=None, domains=None, num_frames: int = 1) -> Dict[str, torch.Tensor]:
+    def debug_taps(self, sample, timestep, skeletons=None, domains=None, num_frames: int = 1,
+                   modules: bool = False) -> Dict[str, torch.Tensor]:
         """Intermediate activations for drift reports: {"conv_in", "down_blocks.i", "mid_block", "up_blocks.i"} -> NCHW bf16.
+        ``modules=True`` adds the output of every module, named by its diffusers path ("time_embedding" [B, 4*C0, 1, 1]
+        before the SiLU, "down_blocks.0.resnets.0", "mid_block.attentions.0", "up_blocks.2.upsamplers.0", ...; include/d4d.h).
         One (prefix of a) forward is run per tap (``d4d_debug_tap``); same argument checks as ``forward``."""
         cfg = self.config
         B, _, H, W = sample.shape
@@ -174,8 +178,9 @@ class B200MultiviewUNet:
         with torch.cuda.device(self._device):
             stream = torch.cuda.current_stream().cuda_stream
             tap = 0
-            while lib().d4d_debug_tap(self._h, sample.data_ptr(), timestep.data_ptr(), sk_ptr, dom, len(domains), B,
-                                      num_frames, H, W, tap, None, name, dims, stream) == 0:
+            while (modules or tap < _BLOCK_TAPS) and lib().d4d_debug_tap(
+                    self._h, sample.data_ptr(), timestep.data_ptr(), sk_ptr, dom, len(domains), B, num_frames, H, W, tap,
+                    None, name, dims, stream) == 0:
                 t = torch.empty(B, dims[0], dims[1], dims[2], device=self._device, dtype=torch.bfloat16)
                 check(lib().d4d_debug_tap(self._h, sample.data_ptr(), timestep.data_ptr(), sk_ptr, dom, len(domains), B,
                                           num_frames, H, W, tap, t.data_ptr(), name, dims, stream), "d4d_debug_tap")

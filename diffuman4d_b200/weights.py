@@ -107,27 +107,30 @@ def state_dict_spec(cfg: UNetConfig) -> "OrderedDict[str, Tuple[int, ...]]":
     return spec
 
 
-def random_state_dict(cfg: UNetConfig, seed: int = 1, dtype=torch.bfloat16) -> Dict[str, torch.Tensor]:
+def random_state_dict(cfg: UNetConfig, seed: int = 1, dtype=torch.bfloat16, device="cpu") -> Dict[str, torch.Tensor]:
     """Seeded random weights (no network for the real checkpoint).  Fan-in-scaled normal weights, small biases,
     randomised norm affines and NON-zero values for the reference's zero-initialised branches
-    (pose_encoder.final_proj, temporal_pos_embed.linear_2) so those paths carry signal."""
-    g = torch.Generator().manual_seed(seed)
+    (pose_encoder.final_proj, temporal_pos_embed.linear_2) so those paths carry signal.  The values depend on the seed
+    and on the device whose generator draws them; a CUDA draw of the full-width UNet takes a fraction of the host's
+    seconds."""
+    g = torch.Generator(device=device).manual_seed(seed)
+    randn = lambda shape: torch.randn(shape, generator=g, device=device)
     sd: Dict[str, torch.Tensor] = {}
     for key, shape in state_dict_spec(cfg).items():
         if key.endswith("scale"):
-            t = torch.full(shape, 2.0)
+            t = torch.full(shape, 2.0, device=device)
         else:
             is_norm = ".norm" in key or key.startswith("conv_norm_out")
             if is_norm and key.endswith("weight"):
-                t = 1.0 + 0.2 * torch.randn(shape, generator=g)
+                t = 1.0 + 0.2 * randn(shape)
             elif is_norm and key.endswith("bias"):
-                t = 0.1 * torch.randn(shape, generator=g)
+                t = 0.1 * randn(shape)
             elif key.endswith("bias"):
-                t = 0.05 * torch.randn(shape, generator=g)
+                t = 0.05 * randn(shape)
             else:
                 fan_in = 1
                 for s in shape[1:]:
                     fan_in *= s
-                t = torch.randn(shape, generator=g) / math.sqrt(fan_in)
+                t = randn(shape) / math.sqrt(fan_in)
         sd[key] = t.to(dtype)
     return sd

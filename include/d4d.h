@@ -210,10 +210,16 @@ int d4d_op_pose_conv0(const void* x_nchw, int n, int H, int W, const void* Wt, c
  * for arithmetic, and for Cin 4 the weights of channel 3 must be 0.  bias fp32 [Cout]. */
 int d4d_op_pose_conv(const void* x_nhwc, int n, int Cin, int H, int W, const void* Wt, const float* bias, int Cout,
                      int ksize, int stride, void* out, void* stream);
-/* Debug tap (per-level drift reports in tests/): runs the forward of d4d_unet_forward up to intermediate activation
- * `tap` (0 = conv_in(+pose), then down_blocks.0-3, mid_block, up_blocks.0-3) and copies it out as NCHW bf16
- * [B, C, H, W].  name64 (64 bytes) / dims3 (C, H, W) are filled when non-NULL; out == NULL only queries them.
- * Returns 1 when `tap` is out of range. */
+/* Debug tap (per-level drift reports and per-module checks in tests/): runs the forward of d4d_unet_forward up to
+ * intermediate activation `tap` and copies it out as NCHW bf16 [B, C, H, W].  name64 (64 bytes) / dims3 (C, H, W) are
+ * filled when non-NULL; out == NULL only queries them.  Returns 1 when `tap` is out of range.
+ *   0-9   block outputs: conv_in (+ pose encoder), down_blocks.0-3, mid_block, up_blocks.0-3
+ *   10-   module outputs, named after the diffusers module paths (d4d_version() 104 and later), in forward order:
+ *         time_embedding (time embedding + frame-index embedding, before the SiLU; C = 4 * block_out_channels[0],
+ *         H = W = 1), down_blocks.i.resnets.j, down_blocks.i.attentions.j and down_blocks.i.downsamplers.0 (i < 3),
+ *         mid_block.resnets.0, mid_block.attentions.0, mid_block.resnets.1, up_blocks.i.resnets.j,
+ *         up_blocks.i.attentions.j (i > 0) and up_blocks.i.upsamplers.0 (i < 3).
+ * Taps add no launch: a forward enqueues the same kernels whether or not they are read. */
 int d4d_debug_tap(d4d_handle* h, const void* sample, const int64_t* timestep, const void* skeletons,
                   const int32_t* domain_ids, int n_domains, int B, int F, int height, int width, int tap, void* out,
                   char* name64, int32_t* dims3, void* stream);
