@@ -13,7 +13,7 @@ EXPORTS = [
     "d4d_last_error", "d4d_version", "d4d_create", "d4d_destroy", "d4d_load_weight", "d4d_finalize_weights",
     "d4d_num_weights", "d4d_weight_key", "d4d_unet_forward", "d4d_profile_forward", "d4d_workspace_bytes", "d4d_forward_launches",
     "d4d_denoise_window", "d4d_denoise_window_dpm", "d4d_assemble_input", "d4d_cfg_ddim_step", "d4d_cfg_dpm_step",
-    "d4d_op_gemm", "d4d_op_conv3x3",
+    "d4d_op_gemm", "d4d_op_gemm_kv_scatter", "d4d_op_conv3x3",
     "d4d_op_attention", "d4d_op_groupnorm", "d4d_op_conv3x3_groupnorm", "d4d_op_conv_resample", "d4d_op_layernorm", "d4d_op_pose_conv0", "d4d_op_pose_conv", "d4d_debug_tap", "d4d_exchange_alloc",
     "d4d_exchange_open", "d4d_unet_forward_sharded", "d4d_denoise_window_sharded",
 ]
@@ -90,6 +90,8 @@ def _load(path: str) -> C.CDLL:
     l.d4d_cfg_dpm_step.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, C.POINTER(D4DDpmSched), f32, i32, i32, i32, i32, vp, vp]
     l.d4d_op_gemm.argtypes = [vp, i32, i32, vp, i32, i32, vp, i32, i32, f32p, vp, i32, i32, vp, i32, vp, i32, i32,
                               i32, f32, i32, vp, i32, vp]
+    l.d4d_op_gemm_kv_scatter.argtypes = [vp, i32, i32, vp, i32, i32, vp, i32, i32, i32, C.c_int64, C.c_int64, C.c_int64,
+                                         i32, vp, i32, vp]
     l.d4d_op_conv3x3.argtypes = [vp, i32, i32, i32, i32, vp, i32, f32p, vp, i32, vp, i32, vp, i32, vp, vp]
     l.d4d_op_attention.argtypes = [vp, vp, vp, i32, vp, i32, i32, i32, i32, i32, f32, i32, i32, vp]
     l.d4d_op_groupnorm.argtypes = [vp, i32, vp, i32, i32, i32, i32, f32, f32p, f32p, i32, vp, vp, vp]

@@ -45,7 +45,7 @@ struct DeviceGuard {
 extern "C" {
 
 const char* d4d_last_error(void) { return d4d::g_last_error.c_str(); }
-int d4d_version(void) { return 104; }
+int d4d_version(void) { return 105; }
 
 int d4d_create(const d4d_config* cfg, int device, d4d_handle** out) {
   D4D_API_BEGIN
@@ -262,6 +262,26 @@ int d4d_op_gemm(const void* A, int lda, int K1, const void* A2, int lda2, int K2
   d.out = static_cast<bf16*>(out); d.ldo = ldo; d.geglu = geglu; d.act = act; d.out_scale = out_scale; d.block_n = block_n;
   d.stats = reinterpret_cast<long long*>(stats); d.stats_rows = stats_rows;
   D4D_REQUIRE(M > 0, "empty GEMM");
+  d4d::GemmLaunch L;
+  if (int rc = d4d::gemm_prepare(d, &L)) return rc;
+  return d4d::gemm_run(L, static_cast<cudaStream_t>(stream));
+  D4D_API_END
+}
+
+int d4d_op_gemm_kv_scatter(const void* A, int lda, int K, const void* W, int M, int N, void* out, int ldo, int kv_col0,
+                           int kv_ld, int64_t rows_local, int64_t rows_global, int64_t row_offset, int world,
+                           void* const* kv_dst, int block_n, void* stream) {
+  D4D_API_BEGIN
+  D4D_REQUIRE(M > 0, "empty GEMM");
+  D4D_REQUIRE(world >= 1 && world <= 8, "K/V scatter: world must be in [1, 8]");
+  D4D_REQUIRE(kv_dst != nullptr, "K/V scatter: null destination buffer");
+  // the descriptor of the frame-sharded QKV projection (PlanBuilder::sharded_qkv_attention, csrc/unet.cu)
+  d4d::GemmDesc d;
+  d.A = static_cast<const bf16*>(A); d.lda = lda; d.K1 = K; d.Wt = static_cast<const bf16*>(W); d.M = M; d.N = N;
+  d.out = static_cast<bf16*>(out); d.ldo = ldo; d.block_n = block_n;
+  d.kv_world = world; d.kv_col0 = kv_col0; d.kv_ld = kv_ld;
+  d.kv_rows_local = rows_local; d.kv_rows_global = rows_global; d.kv_row_offset = row_offset;
+  for (int r = 0; r < world; ++r) d.kv_dst[r] = static_cast<bf16*>(kv_dst[r]);
   d4d::GemmLaunch L;
   if (int rc = d4d::gemm_prepare(d, &L)) return rc;
   return d4d::gemm_run(L, static_cast<cudaStream_t>(stream));

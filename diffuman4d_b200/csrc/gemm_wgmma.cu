@@ -386,6 +386,17 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 int gemm_prepare(const GemmDesc& d, GemmLaunch* L) {
   D4D_REQUIRE(d.N % 16 == 0, "GEMM N must be a multiple of 16");
   D4D_REQUIRE(d.out != nullptr && d.A != nullptr && d.Wt != nullptr, "null operand");
+  // K/V scatter: every rank's buffer exists, and local row m of CFG half m / rows_local lands inside that half's
+  // [rows_global] rows of the gathered buffer (the kernel writes without bounds checks)
+  D4D_REQUIRE(d.kv_world >= 0 && d.kv_world <= 8, "K/V scatter: world must be in [1, 8]");
+  if (d.kv_world > 0) {
+    D4D_REQUIRE(!d.conv && !d.geglu && d.kv_col0 >= 0 && d.kv_col0 < d.N && d.kv_col0 % 16 == 0 && d.kv_ld % 8 == 0 &&
+                d.kv_ld >= d.N - d.kv_col0, "K/V scatter arguments");
+    for (int r = 0; r < d.kv_world; ++r) D4D_REQUIRE(d.kv_dst[r] != nullptr, "K/V scatter: null destination buffer");
+    D4D_REQUIRE(d.kv_rows_local > 0 && d.M % d.kv_rows_local == 0, "K/V scatter: M must be a multiple of rows_local");
+    D4D_REQUIRE(d.kv_row_offset >= 0 && d.kv_row_offset + d.kv_rows_local <= d.kv_rows_global,
+                "K/V scatter: row_offset + rows_local exceeds rows_global");
+  }
   GemmKernelArgs& a = L->args;
   memset(&a, 0, sizeof(a));
   int dev = 0, sms = 0;
@@ -435,7 +446,6 @@ int gemm_prepare(const GemmDesc& d, GemmLaunch* L) {
   a.kv_rows_global = d.kv_rows_global;
   a.kv_row_offset = d.kv_row_offset;
   for (int i = 0; i < 8; ++i) a.kv_dst[i] = d.kv_dst[i];
-  D4D_REQUIRE(d.kv_world >= 0 && d.kv_world <= 8 && (d.kv_world == 0 || (d.kv_col0 % 16 == 0 && d.kv_ld % 8 == 0 && !d.geglu)), "K/V scatter arguments");
   D4D_REQUIRE(d.ldo % 8 == 0 && (d.residual == nullptr || d.ld_res % 8 == 0) &&
               (d.rowvec == nullptr || d.ld_rowvec % 8 == 0), "leading dimensions must be multiples of 8");
 

@@ -725,7 +725,7 @@ class PlanBuilder {
     const int Cp = x.heads * x.dpad;
     bf16* qkv = alloc(static_cast<size_t>(M) * 3 * Cp);
     bf16* o = nullptr;
-    if (is3d && p_.world > 1) {
+    if (is3d && p_.F_total > 0) {
       o = alloc(static_cast<size_t>(M) * Cp);
       sharded_qkv_attention(a, x, normed, qkv, o, M, batch, seq);
     } else {
@@ -854,7 +854,7 @@ class PlanBuilder {
       if (!dry_) {
         std::vector<float> hp(B);
         for (int dmn = 0; dmn < p_.n_domains; ++dmn)
-          for (int f = 0; f < F; ++f) hp[dmn * F + f] = p_.domains[dmn] == 0 ? 0.f : static_cast<float>((p_.rank * F + f) % std::max(1, (p_.world > 1 ? p_.F_total : F) / 2));
+          for (int f = 0; f < F; ++f) hp[dmn * F + f] = p_.domains[dmn] == 0 ? 0.f : static_cast<float>((p_.rank * F + f) % std::max(1, (p_.F_total > 0 ? p_.F_total : F) / 2));
         if (cudaMemcpy(pos, hp.data(), sizeof(float) * B, cudaMemcpyHostToDevice) != cudaSuccess) rc_ = 2;
       }
       op([=](cudaStream_t s) { return sinusoid_run(pos, B, C0, 1, 0.f, tsin, s); });
@@ -1092,9 +1092,10 @@ int Model::get_plan(const int* domain_ids, int n_domains, int B, int F, int h, i
   }
   D4D_REQUIRE(h % 8 == 0 && w % 8 == 0 && h > 0 && w > 0, "latent height/width must be divisible by 8");
   for (int i = 0; i < n_domains; ++i) D4D_REQUIRE(domain_ids[i] == 0 || domain_ids[i] == 1, "Invalid domain for temporal embedding");
-  const bool sharded = F_total > F;
+  // every *_sharded call runs the sharded plan, also with world = 1 (rank 0 exchanging with itself)
+  const bool sharded = F_total > 0;
   if (sharded) {
-    D4D_REQUIRE(xch_.ready && xch_.world > 1, "frame-sharded forward needs d4d_exchange_open first");
+    D4D_REQUIRE(xch_.ready && xch_.world >= 1, "frame-sharded forward needs d4d_exchange_open first");
     D4D_REQUIRE(F * xch_.world == F_total, "F_total must equal world * local frames");
   }
   const std::string key = plan_key(domain_ids, n_domains, B, F, h, w) + (sharded ? "_sh" + std::to_string(F_total) : std::string()) + (pose_shared_neg ? "_pn" : "");

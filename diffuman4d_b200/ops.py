@@ -3,7 +3,7 @@ and the current stream; all arithmetic happens in libd4d.so."""
 from __future__ import annotations
 
 import ctypes as C
-from typing import Optional
+from typing import List, Optional
 
 import torch
 
@@ -59,6 +59,36 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, 
                             int(geglu), act, float(out_scale), block_n,
                             _stats_ws(stats, M // stats_rows if stats_rows > 0 else 0, N), stats_rows, _stream()),
           "d4d_op_gemm")
+    return out
+
+
+def gemm_kv_scatter(a: torch.Tensor, w: torch.Tensor, *, kv_col0: int, rows_local: int, rows_global: int, row_offset: int,
+                    dst: List[torch.Tensor], out: Optional[torch.Tensor] = None, block_n: int = 0) -> torch.Tensor:
+    """QKV projection of a frame-sharded 3-D attention layer: ``a @ w.T`` with its columns >= ``kv_col0`` (K|V) stored
+    into every buffer of ``dst`` (one per rank, 1 to 8) instead of ``out``.  Local row m of CFG half h = m // rows_local
+    lands at row h * rows_global + row_offset + m % rows_local of each [halves * rows_global, ld] buffer.  Returns ``out``
+    [M, N], whose columns < kv_col0 hold Q; its K|V columns are left as they were."""
+    _bf16c(a, "a"), _bf16c(w, "w")
+    M, K = a.shape
+    N = w.shape[0]
+    if w.shape[1] != K:
+        raise ValueError("w must be [N, K]")
+    if not 1 <= len(dst) <= 8:
+        raise ValueError("dst must hold 1 to 8 buffers (one per rank)")
+    ld = dst[0].stride(0)
+    for t in dst:
+        if t.dtype != torch.bfloat16 or not t.is_cuda or t.dim() != 2 or t.stride(1) != 1 or t.stride(0) != ld:
+            raise ValueError("dst buffers must be row-major CUDA bfloat16 [rows, ld] matrices with one leading dimension")
+        if t.shape[1] < N - kv_col0 or (rows_local > 0 and t.shape[0] < -(-M // rows_local) * rows_global):
+            raise ValueError(f"dst buffers need [{-(-M // max(rows_local, 1))} * {rows_global}, {N - kv_col0}] elements")
+    if out is None:
+        out = torch.empty(M, N, device=a.device, dtype=torch.bfloat16)
+    elif out.dtype != torch.bfloat16 or not out.is_cuda or out.shape != (M, N) or out.stride(1) != 1:
+        raise ValueError(f"out must be a row-major CUDA bfloat16 [{M}, {N}] matrix")
+    ptrs = (C.c_void_p * len(dst))(*[t.data_ptr() for t in dst])
+    check(lib().d4d_op_gemm_kv_scatter(_p(a), a.stride(0), K, _p(w), M, N, _p(out), out.stride(0), kv_col0, ld, rows_local,
+                                       rows_global, row_offset, len(dst), ptrs, block_n, _stream()),
+          "d4d_op_gemm_kv_scatter")
     return out
 
 

@@ -20,9 +20,12 @@ from .sharding import frame_shard
 
 
 def exchange_bytes(cfg, F_total: int, h: int, w: int, cfg_halves: int = 2) -> int:
-    """Size of one gathered K|V buffer: the largest 3-D attention layer (level 1)."""
+    """Size of one gathered K|V buffer: the largest 3-D attention layer.  The mid block (level 3) always runs one; level
+    L < 3 runs them (down_blocks.L, up_blocks.3-L) when 3 - L < num_3d_attn_blocks, so level 0 with 4."""
     best = 0
-    for lvl in (1, 2, 3):
+    for lvl in (0, 1, 2, 3):
+        if lvl < 3 and 3 - lvl >= cfg.num_3d_attn_blocks:
+            continue
         d = cfg.head_dim(lvl)
         dpad = 64 if d <= 64 else (128 if d <= 128 else 192)
         cp = cfg.heads(lvl) * dpad

@@ -168,6 +168,14 @@ int d4d_op_gemm(const void* A, int lda, int K1, const void* A2, int lda2, int K2
                 const float* bias, const void* rowvec, int ld_rowvec, int rows_per_image, const void* residual,
                 int ld_res, void* out, int ldo, int geglu, int act, float out_scale, int block_n, int64_t* stats,
                 int stats_rows, void* stream);
+/* The QKV projection of a frame-sharded 3-D attention layer (d4d_version() 105 and later): out = A[M,K] . W[N,K]^T, but
+ * only columns < kv_col0 (Q) are written to out [M, ldo]; columns >= kv_col0 (K|V) are NOT written to out and go instead to
+ * every kv_dst[r], r < world, a [halves * rows_global, kv_ld] matrix: local row m of CFG half h = m / rows_local lands at
+ * row h * rows_global + row_offset + m % rows_local, column - kv_col0.  Needs 1 <= world <= 8, kv_col0 % 16 == 0,
+ * kv_ld % 8 == 0, M % rows_local == 0 and row_offset + rows_local <= rows_global; returns 1 otherwise, before any launch. */
+int d4d_op_gemm_kv_scatter(const void* A, int lda, int K, const void* W, int M, int N, void* out, int ldo, int kv_col0,
+                           int kv_ld, int64_t rows_local, int64_t rows_global, int64_t row_offset, int world,
+                           void* const* kv_dst, int block_n, void* stream);
 int d4d_op_conv3x3(const void* x_nhwc, int n_img, int H, int W, int Cin, const void* Wt, int Cout, const float* bias,
                    const void* rowvec, int ld_rowvec, const void* residual, int act, void* out, int block_n,
                    int64_t* stats, void* stream);
@@ -232,8 +240,11 @@ int d4d_debug_tap(d4d_handle* h, const void* sample, const int64_t* timestep, co
  * alternate per layer so a rank may run one layer ahead of its peers.
  *   d4d_exchange_alloc  allocates this rank's two K/V buffers (kv_bytes each) + flag array and returns three 64-byte
  *                       cudaIpcMemHandle_t blobs (kv0, kv1, flags) to be all-gathered by the host (torch.distributed);
- *   d4d_exchange_open   maps the peers' buffers: all_handles = [world][3][64] bytes in rank order.
- * kv_bytes must cover 2 (CFG halves) * F_total * (h/2)*(w/2) tokens * 2*C_level1' bf16 (the largest 3-D layer). */
+ *   d4d_exchange_open   maps the peers' buffers: all_handles = [world][3][64] bytes in rank order.  world = 1 (rank 0 on
+ *                       its own buffers) runs the sharded plan on one GPU.
+ * kv_bytes must cover the largest 3-D attention layer: 2 (CFG halves) * F_total * (h >> L)*(w >> L) tokens * 2*C'_L bf16
+ * (C'_L = heads * padded head_dim) over the levels L that run 3-D attention: the mid block's (L = 3) always, and level
+ * L < 3 when 3 - L < num_3d_attn_blocks (level 0 with num_3d_attn_blocks = 4).  sharded.exchange_bytes computes it. */
 int d4d_exchange_alloc(d4d_handle* h, size_t kv_bytes, unsigned char* handles_out /* [3][64] */);
 int d4d_exchange_open(d4d_handle* h, int rank, int world, const unsigned char* all_handles /* [world][3][64] */);
 /* B-2 / B-3 on a frame shard: same contracts as d4d_unet_forward / d4d_denoise_window on the LOCAL frames; every rank

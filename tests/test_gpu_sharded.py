@@ -9,7 +9,7 @@ import torch
 pytestmark = pytest.mark.gpu
 
 
-def _worker(rank, world, port, q):
+def _worker(rank, world, port, q, n3d=3):
     import torch.distributed as dist
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     torch.cuda.set_device(rank)
@@ -20,7 +20,7 @@ def _worker(rank, world, port, q):
         from diffuman4d_b200.sharded import FrameShardedPipeline
         from diffuman4d_b200.unet import B200MultiviewUNet
         from diffuman4d_b200.weights import random_state_dict
-        cfg = UNetConfig.tiny()
+        cfg = UNetConfig.tiny(num_3d_attn_blocks=n3d)
         sd = random_state_dict(cfg, seed=1)
         F, h, w = 4, 16, 16
         g = torch.Generator().manual_seed(0)
@@ -73,14 +73,14 @@ def _worker(rank, world, port, q):
         dist.destroy_process_group()
 
 
-def test_two_rank_frame_sharded_window_is_bit_identical(cuda):
+def _run_two_ranks(n3d):
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs")
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = 29600 + (os.getpid() % 1000)
-    procs = [ctx.Process(target=_worker, args=(r, 2, port, q)) for r in range(2)]
+    port = 29600 + (os.getpid() % 1000) + 7 * n3d
+    procs = [ctx.Process(target=_worker, args=(r, 2, port, q, n3d)) for r in range(2)]
     for p in procs:
         p.start()
     items = [q.get(timeout=600) for _ in range(3)]
@@ -99,3 +99,13 @@ def test_two_rank_frame_sharded_window_is_bit_identical(cuda):
             idx = torch.cat([torch.arange(lo, hi), torch.arange(lo, hi) + F])
             assert torch.equal(y, ry[idx]), f"UNet output differs on frames {lo}:{hi} ({dom}): {(y - ry[idx]).abs().max()}"
             assert torch.equal(lat, rlat[lo:hi]) and torch.equal(ti, rti[lo:hi])
+
+
+def test_two_rank_frame_sharded_window_is_bit_identical(cuda):
+    _run_two_ranks(3)
+
+
+def test_two_rank_frame_sharded_window_with_level0_3d_attention(cuda):
+    """num_3d_attn_blocks = 4: down_blocks.0 and up_blocks.3 exchange full-resolution K/V, the largest layer of the
+    window (sharded.exchange_bytes)."""
+    _run_two_ranks(4)
