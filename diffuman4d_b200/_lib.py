@@ -15,7 +15,8 @@ EXPORTS = [
     "d4d_denoise_window", "d4d_denoise_window_dpm", "d4d_assemble_input", "d4d_cfg_ddim_step", "d4d_cfg_dpm_step",
     "d4d_op_gemm", "d4d_op_gemm_kv_scatter", "d4d_op_conv3x3",
     "d4d_op_attention", "d4d_op_groupnorm", "d4d_op_conv3x3_groupnorm", "d4d_op_conv_resample", "d4d_op_layernorm", "d4d_op_pose_conv0", "d4d_op_pose_conv", "d4d_debug_tap", "d4d_exchange_alloc",
-    "d4d_exchange_open", "d4d_unet_forward_sharded", "d4d_denoise_window_sharded",
+    "d4d_exchange_open", "d4d_unet_forward_sharded", "d4d_denoise_window_sharded", "d4d_denoise_window_dpm_sharded",
+    "d4d_window_exchange", "d4d_op_window_scatter",
 ]
 
 
@@ -108,12 +109,16 @@ def _load(path: str) -> C.CDLL:
     l.d4d_unet_forward_sharded.argtypes = [vp, vp, vp, vp, C.POINTER(C.c_int32), i32, i32, i32, i32, i32, i32, vp, vp]
     l.d4d_denoise_window_sharded.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.POINTER(D4DSched), f32, i32, i32, i32, i32,
                                              i32, i32, vp]
+    l.d4d_denoise_window_dpm_sharded.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.POINTER(D4DDpmSched), f32, i32, i32, i32,
+                                                 i32, i32, i32, vp, vp, vp]
+    l.d4d_window_exchange.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp]
+    l.d4d_op_window_scatter.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, C.c_size_t, vp]
     for name in EXPORTS:
         fn = getattr(l, name)
         if fn.restype is C.c_int or name.startswith("d4d_op_") or name in (
                 "d4d_create", "d4d_load_weight", "d4d_finalize_weights", "d4d_unet_forward", "d4d_denoise_window",
                 "d4d_denoise_window_dpm", "d4d_exchange_alloc", "d4d_exchange_open", "d4d_unet_forward_sharded",
-                "d4d_denoise_window_sharded", "d4d_debug_tap"):
+                "d4d_denoise_window_sharded", "d4d_denoise_window_dpm_sharded", "d4d_window_exchange", "d4d_debug_tap"):
             fn.restype = C.c_int
     return l
 

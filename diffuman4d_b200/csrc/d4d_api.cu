@@ -45,7 +45,7 @@ struct DeviceGuard {
 extern "C" {
 
 const char* d4d_last_error(void) { return d4d::g_last_error.c_str(); }
-int d4d_version(void) { return 105; }
+int d4d_version(void) { return 106; }
 
 int d4d_create(const d4d_config* cfg, int device, d4d_handle** out) {
   D4D_API_BEGIN
@@ -436,6 +436,55 @@ int d4d_denoise_window_sharded(d4d_handle* h, void* latents, const void* pixel_l
                                   static_cast<const bf16*>(cond_mask), reinterpret_cast<long long*>(timestep_indices),
                                   *sched, guidance_scale, domain, F_local, height, width, num_steps,
                                   static_cast<cudaStream_t>(stream), F_total);
+  D4D_API_END
+}
+
+int d4d_denoise_window_dpm_sharded(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                   const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                   const d4d_dpm_sched* sched, float guidance_scale, int domain, int F_local, int F_total,
+                                   int height, int width, int num_steps, void* x0_prev, int32_t* lower_order_nums,
+                                   void* stream) {
+  D4D_API_BEGIN
+  D4D_REQUIRE(h != nullptr && sched != nullptr, "null argument");
+  DeviceGuard g(h->model->device());
+  return h->model->denoise_window_dpm(static_cast<bf16*>(latents), static_cast<const bf16*>(pixel_latents),
+                                      static_cast<const bf16*>(plucker), static_cast<const bf16*>(skeletons),
+                                      static_cast<const bf16*>(cond_mask), reinterpret_cast<long long*>(timestep_indices),
+                                      *sched, guidance_scale, domain, F_local, height, width, num_steps,
+                                      static_cast<bf16*>(x0_prev), lower_order_nums, static_cast<cudaStream_t>(stream),
+                                      F_total);
+  D4D_API_END
+}
+
+int d4d_window_exchange(d4d_handle* h, const void* latents_local, const int64_t* timestep_indices_local,
+                        const void* x0_prev_local, const int32_t* lower_order_nums_local, int F_local, int F_total,
+                        int height, int width, void* latents_out, int64_t* timestep_indices_out, void* x0_prev_out,
+                        int32_t* lower_order_nums_out, void* stream) {
+  D4D_API_BEGIN
+  D4D_REQUIRE(h != nullptr, "null handle");
+  DeviceGuard g(h->model->device());
+  return h->model->window_exchange(static_cast<const bf16*>(latents_local),
+                                   reinterpret_cast<const long long*>(timestep_indices_local),
+                                   static_cast<const bf16*>(x0_prev_local), lower_order_nums_local, F_local, F_total, height,
+                                   width, static_cast<bf16*>(latents_out), reinterpret_cast<long long*>(timestep_indices_out),
+                                   static_cast<bf16*>(x0_prev_out), lower_order_nums_out, static_cast<cudaStream_t>(stream));
+  D4D_API_END
+}
+
+int d4d_op_window_scatter(const void* latents, const int64_t* timestep_indices, const void* x0_prev,
+                          const int32_t* lower_order_nums, int F_local, int F_total, int height, int width, int world,
+                          int rank, void* const* dst, size_t dst_bytes, void* stream) {
+  D4D_API_BEGIN
+  D4D_REQUIRE(world >= 1 && world <= 8, "window scatter: world must be in [1, 8]");
+  D4D_REQUIRE(dst != nullptr, "window scatter: null destination buffer");
+  D4D_REQUIRE(height > 0 && width > 0, "window scatter: latent height/width");
+  d4d::WindowScatterArgs a;
+  for (int r = 0; r < 8; ++r) a.dst[r] = r < world ? dst[r] : nullptr;
+  a.world = world; a.rank = rank; a.F_local = F_local; a.F_total = F_total;
+  a.chw = 4ll * height * width;
+  a.latents = static_cast<const bf16*>(latents); a.ts = reinterpret_cast<const long long*>(timestep_indices);
+  a.x0_prev = static_cast<const bf16*>(x0_prev); a.lower_order_nums = lower_order_nums;
+  return d4d::window_scatter_run(a, dst_bytes, static_cast<cudaStream_t>(stream));
   D4D_API_END
 }
 

@@ -455,6 +455,31 @@ __global__ void kv_wait_kernel(const KvFlagArgs a) {
   __threadfence_system();
 }
 
+// frame-sharded sliding loop: this rank's updated frames into every rank's gathered window (blockIdx.y = destination),
+// plain 16-byte stores through the peer pointers like the K/V scatter epilogue; the flag round follows in the stream
+__global__ void window_scatter_kernel(const WindowScatterArgs a, const WindowResultLayout L) {
+  char* d = static_cast<char*>(a.dst[blockIdx.y]);
+  const long long row0 = static_cast<long long>(a.rank) * a.F_local;
+  const long long n = a.F_local * a.chw / 8;
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  const uint4* lat = reinterpret_cast<const uint4*>(a.latents);
+  uint4* lat_d = reinterpret_cast<uint4*>(d) + row0 * a.chw / 8;
+  for (long long i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) lat_d[i] = lat[i];
+  if (a.x0_prev) {
+    const uint4* x0 = reinterpret_cast<const uint4*>(a.x0_prev);
+    uint4* x0_d = reinterpret_cast<uint4*>(d + L.x0) + row0 * a.chw / 8;
+    for (long long i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) x0_d[i] = x0[i];
+  }
+  if (blockIdx.x == 0) {
+    long long* ts_d = reinterpret_cast<long long*>(d + L.ts) + row0;
+    int* lon_d = reinterpret_cast<int*>(d + L.lon) + row0;
+    for (int f = threadIdx.x; f < a.F_local; f += blockDim.x) {
+      ts_d[f] = a.ts[f];
+      if (a.lower_order_nums) lon_d[f] = a.lower_order_nums[f];
+    }
+  }
+}
+
 inline int blocks_for(long long total, int threads) { return static_cast<int>((total + threads - 1) / threads); }
 
 }  // namespace
@@ -553,6 +578,34 @@ int kv_signal_run(const KvFlagArgs& a, cudaStream_t stream) {
 }
 int kv_wait_run(const KvFlagArgs& a, cudaStream_t stream) {
   kv_wait_kernel<<<1, 32, 0, stream>>>(a);
+  D4D_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int window_scatter_run(const WindowScatterArgs& a, size_t dst_bytes, cudaStream_t stream) {
+  D4D_REQUIRE(a.world >= 1 && a.world <= 8, "window scatter: world must be in [1, 8]");
+  D4D_REQUIRE(a.rank >= 0 && a.rank < a.world, "window scatter: rank must be in [0, world)");
+  D4D_REQUIRE(a.F_local >= 1 && static_cast<long long>(a.F_local) * a.world == a.F_total,
+              "window scatter: F_total must equal world * local frames");
+  D4D_REQUIRE(a.chw > 0 && a.chw % 8 == 0, "window scatter: 4*h*w must be a positive multiple of 8");
+  D4D_REQUIRE(a.latents != nullptr && a.ts != nullptr, "window scatter: null source");
+  D4D_REQUIRE((a.x0_prev == nullptr) == (a.lower_order_nums == nullptr),
+              "window scatter: x0_prev and lower_order_nums are given together or not at all");
+  for (int r = 0; r < a.world; ++r) {
+    D4D_REQUIRE(a.dst[r] != nullptr, "window scatter: null destination buffer");
+    D4D_REQUIRE(reinterpret_cast<uintptr_t>(a.dst[r]) % 16 == 0, "window scatter: destinations must be 16-byte aligned");
+  }
+  D4D_REQUIRE(reinterpret_cast<uintptr_t>(a.latents) % 16 == 0 && reinterpret_cast<uintptr_t>(a.x0_prev) % 16 == 0,
+              "window scatter: latents and x0_prev must be 16-byte aligned");
+  const WindowResultLayout L = window_result_layout(a.F_total, a.chw, a.x0_prev != nullptr);
+  if (L.bytes > dst_bytes) {
+    set_error("window scatter: the window result (" + std::to_string(L.bytes) + " bytes) does not fit the " +
+              std::to_string(dst_bytes) + "-byte exchange buffer (d4d_exchange_alloc)");
+    return 1;
+  }
+  const long long n = a.F_local * a.chw / 8;
+  dim3 grid(static_cast<unsigned>(std::min<long long>(132, blocks_for(n, 256))), a.world);
+  window_scatter_kernel<<<grid, 256, 0, stream>>>(a, L);
   D4D_CUDA_OK(cudaGetLastError());
   return 0;
 }

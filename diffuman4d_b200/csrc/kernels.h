@@ -237,6 +237,34 @@ struct KvFlagArgs {
 int kv_signal_run(const KvFlagArgs& a, cudaStream_t stream);
 int kv_wait_run(const KvFlagArgs& a, cudaStream_t stream);
 
+// frame-sharded sliding loop: the updated frames of a window, gathered in every rank's exchange buffer.  Layout of the
+// gathered window (F_total frames in window order, chw = 4*h*w): latents [F_total][chw] bf16 | x0_prev [F_total][chw] bf16
+// (DPM-Solver++ only) | timestep indices [F_total] int64 | lower_order_nums [F_total] int32 (DPM-Solver++ only).
+struct WindowResultLayout {
+  size_t x0, ts, lon, bytes;  // byte offsets of the regions after the latents (at 0), and the total size
+};
+inline WindowResultLayout window_result_layout(long long F_total, long long chw, bool dpm) {
+  WindowResultLayout L;
+  const size_t rows = static_cast<size_t>(F_total) * static_cast<size_t>(chw) * 2;
+  L.x0 = rows;
+  L.ts = dpm ? 2 * rows : rows;
+  L.lon = L.ts + static_cast<size_t>(F_total) * 8;
+  L.bytes = L.lon + (dpm ? static_cast<size_t>(F_total) * 4 : 0);
+  return L;
+}
+struct WindowScatterArgs {
+  void* dst[8];              // dst[r] = rank r's gathered window (peer mapped); r < world
+  int world, rank, F_local, F_total;
+  long long chw;
+  const bf16* latents;       // [F_local][chw], 16-byte aligned
+  const long long* ts;       // [F_local]
+  const bf16* x0_prev;       // [F_local][chw] or nullptr (DDIM), 16-byte aligned
+  const int* lower_order_nums;  // [F_local] or nullptr, with x0_prev
+};
+// Stores this rank's F_local frames at rows [rank*F_local, (rank+1)*F_local) of every dst[r].  Returns 1 before any launch
+// for arguments that would store outside a dst_bytes destination.
+int window_scatter_run(const WindowScatterArgs& a, size_t dst_bytes, cudaStream_t stream);
+
 // per-device "opt in to large dynamic smem" helper.  `once` holds one flag per device ordinal; the reference drives one
 // pipeline per GPU from its own thread (sampling_runner.py:36-43), so the first launches may race: std::call_once.
 struct PerDeviceOnce {

@@ -1287,14 +1287,14 @@ int Model::denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker,
 
 int Model::denoise_window_dpm(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
                               long long* ts_idx, const d4d_dpm_sched& sched, float guidance, int domain, int F, int h, int w,
-                              int num_steps, bf16* x0_prev, int* lower_order_nums, cudaStream_t stream) {
+                              int num_steps, bf16* x0_prev, int* lower_order_nums, cudaStream_t stream, int F_total) {
   D4D_REQUIRE(latents && pixel && plucker && mask && ts_idx && x0_prev && lower_order_nums, "null argument");
   D4D_REQUIRE(sched.timesteps_table && sched.coefs && sched.n_steps > 0, "scheduler tables");
   const bool cfg_on = guidance > 1.0f;
   const int hw = h * w;
   return run_window(latents, pixel, plucker, skeletons, mask, ts_idx,
                     reinterpret_cast<const long long*>(sched.timesteps_table), sched.n_steps, guidance, domain, F, h, w,
-                    num_steps, stream, 0, [&](WindowBufs& wb, cudaStream_t s) -> int {
+                    num_steps, stream, F_total, [&](WindowBufs& wb, cudaStream_t s) -> int {
     if (!wb.order_tmp) D4D_CUDA_OK(cudaMalloc(&wb.order_tmp, sizeof(int) * F));
     DpmArgs d;
     d.noise = wb.noise; d.latents = latents; d.mask = mask; d.timestep_indices = ts_idx; d.coefs = sched.coefs;
@@ -1308,6 +1308,45 @@ int Model::denoise_window_dpm(bf16* latents, const bf16* pixel, const bf16* pluc
     D4D_CUDA_OK(cudaMemcpyAsync(lower_order_nums, wb.order_tmp, sizeof(int) * F, cudaMemcpyDeviceToDevice, s));
     return 0;
   });
+}
+
+// One more exchange of the global epoch sequence (DESIGN.md section 7): counter e = epoch_base stores into parity e & 1 of
+// every rank's K/V buffers, signals epoch e + 1 in flag slot e & 1, and reads the gathered window back after the wait.  The
+// next write to parity e & 1 by any rank is exchange e + 2, which needs this rank's signal of exchange e + 1, enqueued after
+// the copies below: a rank one exchange ahead cannot overwrite the rows a peer is still reading.
+int Model::window_exchange(const bf16* latents, const long long* ts_idx, const bf16* x0_prev, const int* lower_order_nums,
+                           int F, int F_total, int h, int w, bf16* latents_out, long long* ts_out, bf16* x0_out,
+                           int* lon_out, cudaStream_t stream) {
+  D4D_REQUIRE(xch_.ready, "window exchange needs d4d_exchange_open first");
+  D4D_REQUIRE(h > 0 && w > 0, "latent height/width");
+  D4D_REQUIRE(latents_out && ts_out, "null argument");
+  const bool dpm = x0_prev != nullptr;
+  D4D_REQUIRE((x0_out != nullptr) == dpm && (lon_out != nullptr) == dpm,
+              "x0_prev, lower_order_nums and their outputs are given together or not at all");
+  D4D_CUDA_OK(cudaSetDevice(device_));
+  const unsigned int counter = xch_.epoch_base;
+  const int par = counter & 1;
+  WindowScatterArgs a;
+  for (int r = 0; r < 8; ++r) a.dst[r] = r < xch_.world ? xch_.peer_kv[par][r] : nullptr;
+  a.world = xch_.world; a.rank = xch_.rank; a.F_local = F; a.F_total = F_total;
+  a.chw = 4ll * h * w;
+  a.latents = latents; a.ts = ts_idx; a.x0_prev = x0_prev; a.lower_order_nums = lower_order_nums;
+  if (int rc = window_scatter_run(a, xch_.kv_bytes, stream)) return rc;
+  KvFlagArgs f;
+  for (int r = 0; r < 8; ++r) f.flags[r] = r < xch_.world ? xch_.peer_flags[r] : nullptr;
+  f.rank = xch_.rank; f.world = xch_.world; f.epoch = counter + 1; f.slot = par;
+  xch_.epoch_base += 1;  // the stores are enqueued: every rank counts this exchange, whatever happens below
+  if (int rc = kv_signal_run(f, stream)) return rc;
+  if (int rc = kv_wait_run(f, stream)) return rc;
+  const char* g = static_cast<const char*>(xch_.kv[par]);
+  const WindowResultLayout L = window_result_layout(F_total, a.chw, dpm);
+  D4D_CUDA_OK(cudaMemcpyAsync(latents_out, g, L.x0, cudaMemcpyDeviceToDevice, stream));
+  D4D_CUDA_OK(cudaMemcpyAsync(ts_out, g + L.ts, sizeof(long long) * F_total, cudaMemcpyDeviceToDevice, stream));
+  if (dpm) {
+    D4D_CUDA_OK(cudaMemcpyAsync(x0_out, g + L.x0, L.x0, cudaMemcpyDeviceToDevice, stream));
+    D4D_CUDA_OK(cudaMemcpyAsync(lon_out, g + L.lon, sizeof(int) * F_total, cudaMemcpyDeviceToDevice, stream));
+  }
+  return 0;
 }
 
 int Model::run_window(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,

@@ -109,7 +109,12 @@ class Model {
   // the same window step with the DPM-Solver++ step; x0_prev [F,4,h,w] and lower_order_nums [F] are updated in place
   int denoise_window_dpm(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
                          long long* ts_idx, const d4d_dpm_sched& sched, float guidance, int domain, int F, int h, int w,
-                         int num_steps, bf16* x0_prev, int* lower_order_nums, cudaStream_t stream);
+                         int num_steps, bf16* x0_prev, int* lower_order_nums, cudaStream_t stream, int F_total = 0);
+  // frame-sharded sliding loop: this rank's F updated frames (+ DPM-Solver++ state when x0_prev != nullptr) to every rank,
+  // one flag round (one more exchange of the epoch sequence), then the gathered F_total frames to the *_out buffers
+  int window_exchange(const bf16* latents, const long long* ts_idx, const bf16* x0_prev, const int* lower_order_nums, int F,
+                      int F_total, int h, int w, bf16* latents_out, long long* ts_out, bf16* x0_out, int* lon_out,
+                      cudaStream_t stream);
   // per-kind device time (ms) of one forward, measured with CUDA events around every op
   int profile(const bf16* sample, const long long* timestep, const bf16* skeletons, const int* domain_ids, int n_domains,
               int B, int F, int h, int w, bf16* out, cudaStream_t stream, float* ms_by_kind, int* launches_by_kind,

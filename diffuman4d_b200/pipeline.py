@@ -197,6 +197,29 @@ class B200Diffuman4DPipeline:
                                   num_denoising_steps: int = 1, alternation_rounds: int = 3, guidance_scale: float = 2.0,
                                   tqdm: Callable = None, pixel_values_latents=None, skeletons_latents=None,
                                   generator=None):
+        return self._sliding(self._task_window, pixel_values=pixel_values, plucker_embeds=plucker_embeds,
+                             skeletons=skeletons, cond_masks=cond_masks, latents=latents, domain=domain,
+                             timestep_indices=timestep_indices, window_size=window_size, sliding_stride=sliding_stride,
+                             sliding_shift=sliding_shift, bidirectional=bidirectional,
+                             num_denoising_steps=num_denoising_steps, alternation_rounds=alternation_rounds,
+                             guidance_scale=guidance_scale, tqdm=tqdm, pixel_values_latents=pixel_values_latents,
+                             skeletons_latents=skeletons_latents, generator=generator)
+
+    def _task_window(self, window, lw, tiw, sw, conds, **kw):
+        """One window of the sliding loop: ``lw`` / ``tiw`` / ``sw`` (the window frames' latents, timestep indices and
+        solver state) are updated in place; ``conds`` are the task's conditioning tensors, indexed by ``window``."""
+        pix, plk, skl, msk = (t[window] for t in conds)
+        self.denoise_window(latents=lw, pixel_values_latents=pix, plucker_embeds_latents=plk, skeletons_latents=skl,
+                            cond_masks_latents=msk, timestep_indices=tiw, solver_state=sw, **kw)
+        return lw, sw
+
+    def _sliding(self, window_step: Callable, *, pixel_values, plucker_embeds, skeletons, cond_masks, latents, domain,
+                 timestep_indices, window_size, sliding_stride, sliding_shift, bidirectional, num_denoising_steps,
+                 alternation_rounds, guidance_scale, tqdm, pixel_values_latents, skeletons_latents, generator,
+                 share_noise: Optional[Callable] = None):
+        """The B-4 loop around ``window_step(window, lw, tiw, sw, conds, ...) -> (lw, sw)``, which returns the window's
+        updated latents and solver state (``FrameShardedPipeline`` runs it on a frame shard).  ``share_noise`` is applied
+        to freshly drawn initial noise."""
         dev = self.device
         if (window_size * num_denoising_steps) % sliding_stride != 0:
             raise ValueError(
@@ -240,6 +263,8 @@ class B200Diffuman4DPipeline:
             skl = self.vae.encode_latents(skeletons.to(dev, torch.bfloat16))
         if latents is None:
             latents = torch.randn(n, 4, h, w, generator=generator, device=dev, dtype=torch.bfloat16)
+            if share_noise is not None:
+                share_noise(latents)
         latents = (latents.to(dev, torch.bfloat16) * self.scheduler.init_noise_sigma).contiguous().clone()
 
         schedulers, _ = self.parepare_schedulers(num_inference_steps, n)   # a fresh solver state per task (PIPE:501)
@@ -249,15 +274,14 @@ class B200Diffuman4DPipeline:
         it = zip(target_windows, input_windows)
         if tqdm is not None:
             it = tqdm(it, total=len(target_windows))
+        conds = (pixel_values_latents, plk, skl, msk)
         for tw, iw in it:
             window = torch.cat([iw, tw])
             lw = latents[window].contiguous()
             tiw = timestep_indices[window].contiguous()
             sw = task.take(window, h, w) if task is not None else None
-            self.denoise_window(latents=lw, pixel_values_latents=pixel_values_latents[window],
-                                plucker_embeds_latents=plk[window], skeletons_latents=skl[window],
-                                cond_masks_latents=msk[window], timestep_indices=tiw, domain=domain,
-                                guidance_scale=guidance_scale, num_inference_steps=num_denoising_steps, solver_state=sw)
+            lw, sw = window_step(window, lw, tiw, sw, conds, domain=domain, guidance_scale=guidance_scale,
+                                 num_inference_steps=num_denoising_steps)
             if task is not None:
                 task.put(window, sw)
             timestep_indices[tw] += num_denoising_steps

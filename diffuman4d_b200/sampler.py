@@ -14,7 +14,9 @@ Multi-GPU (one process per GPU, SURVEY 8e row 1): the tasks of a round are indep
 ``sharding.shard_tasks(len(tasks), r, world)`` and the ranks exchange the updated cells with one all-gather per round
 (``sharding.exchange_grid_updates``) instead of the reference's shared dict + lock + thread-per-GPU queue
 (src/samplers/sampling_runner.py:26-43).  Pinned against the reference sampler run end to end on stubs
-(tests/golden/gen_golden.py::gen_sampler -> tests/test_sampler.py).
+(tests/golden/gen_golden.py::gen_sampler -> tests/test_sampler.py).  Alternatively (``execute_tasks(frame_sharded=True)``
+with a ``sharded.FrameShardedPipeline``) every rank runs every task with each window split over the ranks by frames, which
+keeps all GPUs busy when a round has fewer tasks than GPUs (DESIGN.md section 7).
 
 The dataset object supplies ``scene_label`` and ``get_item(scene_label, spa_labels, tem_labels, input_spa_labels)`` exactly
 like the reference's ``SpaTemDataset`` (src/data/spatem_dataset.py:76-212); pipelines supply
@@ -228,10 +230,22 @@ class B200SlidingIterativeSampler:
             self.save_fn(sample, self.output_dir)
         return sample
 
-    def execute_tasks(self, rank: int = 0, world: int = 1, group=None, pipe_idx: int = 0):
+    def execute_tasks(self, rank: int = 0, world: int = 1, group=None, pipe_idx: int = 0, frame_sharded: bool = False):
         """All rounds.  ``world > 1`` (inside an initialised ``torch.distributed`` job): this rank runs its share of every
-        round, then the ranks all-gather the cells they updated (the round barrier of RUN:53-55)."""
-        saver = _AsyncSaver(self.save_fn, self.output_dir) if (self.async_save and self.save_fn is not None) else None
+        round, then the ranks all-gather the cells they updated (the round barrier of RUN:53-55).
+
+        ``frame_sharded=True``: ``pipelines[pipe_idx]`` is a ``FrameShardedPipeline`` and every rank of its process group
+        runs every task, each window split over the ranks by frames.  Every rank's grid ends up identical, so there is no
+        per-round exchange; ``rank`` / ``world`` / ``group`` are not used (the pipeline's group defines the ranks), and
+        ``save_fn`` runs on the pipeline's rank 0 only."""
+        save_fn = self.save_fn
+        if frame_sharded:
+            from .sharded import FrameShardedPipeline
+            pipe = self.pipelines[pipe_idx]
+            if not isinstance(pipe, FrameShardedPipeline):
+                raise ValueError("frame_sharded=True needs a FrameShardedPipeline in pipelines[pipe_idx]")
+            rank, world, save_fn = 0, 1, (save_fn if pipe.rank == 0 else None)
+        saver = _AsyncSaver(save_fn, self.output_dir) if (self.async_save and save_fn is not None) else None
         try:
             for tasks in self.all_tasks:
                 mine = list(shard_tasks(len(tasks), rank, world) if world > 1 else range(len(tasks)))
@@ -242,8 +256,8 @@ class B200SlidingIterativeSampler:
                     sample = self.denoise(self._attach_grid(raw), pipe_idx=pipe_idx)
                     if saver is not None:
                         saver.submit(sample)
-                    elif self.save_fn is not None:
-                        self.save_fn(sample, self.output_dir)
+                    elif save_fn is not None:
+                        save_fn(sample, self.output_dir)
                     if world > 1:
                         vi, ti = sample["_cells"]
                         keys += list(zip(vi.tolist(), ti.tolist()))

@@ -256,6 +256,36 @@ int d4d_denoise_window_sharded(d4d_handle* h, void* latents, const void* pixel_l
                                const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
                                const d4d_sched* sched, float guidance_scale, int domain, int F_local, int F_total,
                                int height, int width, int num_steps, void* stream);
+/* d4d_denoise_window_dpm on a frame shard (d4d_version() 106 and later): x0_prev [F_local,4,h,w] and lower_order_nums
+ * [F_local] hold the LOCAL frames' solver state. */
+int d4d_denoise_window_dpm_sharded(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                   const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                   const d4d_dpm_sched* sched, float guidance_scale, int domain, int F_local, int F_total,
+                                   int height, int width, int num_steps, void* x0_prev, int32_t* lower_order_nums,
+                                   void* stream);
+/* Window-result exchange of the frame-sharded sliding loop (d4d_version() 106 and later): after a window step every rank
+ * passes its F_local updated frames -- latents [F_local,4,h,w], timestep indices int64 [F_local] and, with DPM-Solver++,
+ * x0_prev [F_local,4,h,w] and lower_order_nums int32 [F_local] (both NULL for DDIM) -- and receives the whole window,
+ * F_total = world * F_local frames in window order, in latents_out / timestep_indices_out / x0_prev_out /
+ * lower_order_nums_out (NULL exactly when the inputs are).  The frames are stored into every rank's exchange buffer at
+ * row rank * F_local (d4d_op_window_scatter), one flag round publishes them, and each rank copies the gathered window out.
+ * It is one exchange of the same epoch sequence as the 3-D attention layers, so every rank must call it in the same
+ * order as its sharded window steps (SPMD).  The gathered window needs F_total * (4*h*w * 2 * (1 + dpm) + 8 + 4 * dpm)
+ * bytes of the exchange buffer; a larger window returns 1 before any launch.  Latent pointers must be 16-byte aligned. */
+int d4d_window_exchange(d4d_handle* h, const void* latents_local, const int64_t* timestep_indices_local,
+                        const void* x0_prev_local, const int32_t* lower_order_nums_local, int F_local, int F_total,
+                        int height, int width, void* latents_out, int64_t* timestep_indices_out, void* x0_prev_out,
+                        int32_t* lower_order_nums_out, void* stream);
+/* The store kernel of d4d_window_exchange alone, with explicit destinations (d4d_version() 106 and later): writes this
+ * rank's frames into every dst[r], r < world, each a gathered window of dst_bytes bytes laid out as
+ *   latents [F_total][4*h*w] bf16 | x0_prev [F_total][4*h*w] bf16 (DPM only) | timestep indices [F_total] int64 |
+ *   lower_order_nums [F_total] int32 (DPM only),
+ * at frame rows [rank * F_local, (rank + 1) * F_local); nothing else of dst is written.  Returns 1 before any launch for a
+ * null destination, world outside [1, 8], rank outside [0, world), F_local * world != F_total, x0_prev without
+ * lower_order_nums (or the reverse), unaligned pointers, or a window larger than dst_bytes. */
+int d4d_op_window_scatter(const void* latents, const int64_t* timestep_indices, const void* x0_prev,
+                          const int32_t* lower_order_nums, int F_local, int F_total, int height, int width, int world,
+                          int rank, void* const* dst, size_t dst_bytes, void* stream);
 
 #ifdef __cplusplus
 }

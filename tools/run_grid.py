@@ -6,6 +6,7 @@ with the reference's get_item contract and a pooling stand-in for the VAE (the V
 
     python tools/run_grid.py [--latent 64] [--cams 48] [--frames 16] [--out grid.json]
     torchrun --nproc-per-node N tools/run_grid.py ...     # replicas: tasks of a round sharded over the ranks
+    torchrun --nproc-per-node N tools/run_grid.py --frame-sharded ...   # every task on all ranks, windows split by frames
 
 Prints one JSON line (and writes it to --out when given): window steps executed (W16 spatial / W24 temporal), device time inside denoise_window, wall time of execute_tasks.
 """
@@ -29,6 +30,9 @@ def main():
     ap.add_argument("--frames", type=int, default=16)
     ap.add_argument("--out", default=None, help="also write the JSON result to this file")
     ap.add_argument("--prefetch", action="store_true", help="load the next task's dataset item on a helper thread")
+    ap.add_argument("--frame-sharded", action="store_true",
+                    help="run every task on all ranks with each window split by frames (windows of 16 spatial / 24 temporal "
+                         "frames need a rank count that divides 8)")
     args = ap.parse_args()
 
     rank, world = int(os.environ.get("RANK", "0")), int(os.environ.get("WORLD_SIZE", "1"))
@@ -51,7 +55,16 @@ def main():
     pipe = B200Diffuman4DPipeline(unet, SchedulerConfig(), vae=PoolVAE())
     ds = SyntheticSpaTemDataset(args.cams, h=args.latent, w=args.latent)
     inputs = [1, 13, 25, 37] if args.cams >= 48 else sorted({(args.cams * k) // 4 + 1 for k in range(4)})
-    sampler = B200SlidingIterativeSampler(ds, [pipe], output_dir=None, spa_label_range=[0, args.cams, 1],
+    driver = pipe
+    if args.frame_sharded:
+        if world == 1:   # one rank exchanging with itself
+            import tempfile
+            import torch.distributed as dist
+            store = os.path.join(tempfile.mkdtemp(prefix="d4d-grid-"), "store")
+            dist.init_process_group("gloo", init_method=f"file://{store}", rank=0, world_size=1)
+        from diffuman4d_b200.sharded import FrameShardedPipeline
+        driver = FrameShardedPipeline(pipe, max_frames=max(len(inputs) + 12, 24), h=args.latent, w=args.latent)
+    sampler = B200SlidingIterativeSampler(ds, [driver], output_dir=None, spa_label_range=[0, args.cams, 1],
                                           tem_label_range=[0, args.frames, 1], input_spa_labels=inputs, window_size=12,
                                           sliding_stride=1, bidirectional=False, alternation_rounds=3, guidance_scale=2.0,
                                           prefetch=args.prefetch)
@@ -59,7 +72,7 @@ def main():
     # count window steps and their device time (CUDA events around every denoise_window call)
     stats = {"spatial": [0, 0.0], "temporal": [0, 0.0]}
     events = []
-    inner = pipe.denoise_window
+    inner = driver.denoise_window   # frame-sharded: the local frames of each window step
 
     def counted(**kw):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -69,10 +82,10 @@ def main():
         events.append((kw["domain"], int(kw["latents"].shape[0]), e0, e1))
         return out
 
-    pipe.denoise_window = counted
+    driver.denoise_window = counted
     torch.cuda.synchronize()
     t0 = time.time()
-    sampler.execute_tasks(rank, world)
+    sampler.execute_tasks(rank, world, frame_sharded=args.frame_sharded)
     torch.cuda.synchronize()
     wall = time.time() - t0
     frames = {}
@@ -86,7 +99,7 @@ def main():
         "workload": f"demo_4d_tiny-shaped grid: {args.cams} cameras x {args.frames} frames @ {args.latent}x{args.latent} latents, "
                     "window 12 (+4 / +12 cond), stride 1, 3 alternation rounds, CFG 2.0, SD-2.1 UNet layout, random weights, "
                     "synthetic dataset, pooling stand-in for the VAE",
-        "n_gpus": world, "rank": rank, "prefetch": bool(args.prefetch),
+        "n_gpus": world, "rank": rank, "prefetch": bool(args.prefetch), "frame_sharded": bool(args.frame_sharded),
         "window_steps": {d: stats[d][0] for d in stats}, "frames_per_window": {d: sorted(frames.get(d, [])) for d in stats},
         "device_ms_in_denoise_window": {d: round(stats[d][1], 1) for d in stats},
         "ms_per_window_step": {d: round(stats[d][1] / max(1, stats[d][0]), 2) for d in stats},
@@ -100,11 +113,16 @@ def main():
         allr = [None] * world
         dist.all_gather_object(allr, res)
         if rank == 0:
+            # frame-sharded: every rank steps (its shard of) every window, so the windows are rank 0's
+            steps = {d: (allr[0]["window_steps"][d] if args.frame_sharded else sum(r["window_steps"][d] for r in allr))
+                     for d in stats}
             res = {"ranks": allr, "wall_s_execute_tasks": max(r["wall_s_execute_tasks"] for r in allr),
-                   "window_steps_total": {d: sum(r["window_steps"][d] for r in allr) for d in stats}, "n_gpus": world,
+                   "window_steps_total": steps, "n_gpus": world, "frame_sharded": bool(args.frame_sharded),
                    "workload": res["workload"]}
             tot = sum(res["window_steps_total"].values())
             res["window_steps_per_s_wall"] = round(tot / res["wall_s_execute_tasks"], 2)
+    if world > 1 or args.frame_sharded:
+        import torch.distributed as dist
         dist.destroy_process_group()
     if rank == 0:
         if args.out:
