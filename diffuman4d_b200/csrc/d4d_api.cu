@@ -40,6 +40,36 @@ struct DeviceGuard {
     if (prev >= 0) cudaSetDevice(prev);
   }
 };
+
+// d4d_unet_forward and d4d_unet_forward_sharded; F_total = 0 runs the single-GPU plan
+int unet_forward(d4d_handle* h, const void* sample, const int64_t* timestep, const void* skeletons,
+                 const int32_t* domain_ids, int n_domains, int B, int F, int F_total, int height, int width, void* out,
+                 void* stream) {
+  D4D_API_BEGIN
+  D4D_REQUIRE(h != nullptr, "null handle");
+  DeviceGuard g(h->model->device());
+  return h->model->forward(static_cast<const bf16*>(sample), reinterpret_cast<const long long*>(timestep),
+                           static_cast<const bf16*>(skeletons), domain_ids, n_domains, B, F, height, width,
+                           static_cast<bf16*>(out), static_cast<cudaStream_t>(stream), F_total);
+  D4D_API_END
+}
+
+// the four d4d_denoise_window* entry points: the DDIM (ddim) or the DPM-Solver++ (dpm, with x0_prev and
+// lower_order_nums) scheduler, the other one null; F_total = 0 runs the single-GPU plan
+int denoise_window(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker, const void* skeletons,
+                   const void* cond_mask, int64_t* timestep_indices, const d4d_sched* ddim, const d4d_dpm_sched* dpm,
+                   float guidance_scale, int domain, int F, int F_total, int height, int width, int num_steps,
+                   void* x0_prev, int32_t* lower_order_nums, void* stream) {
+  D4D_API_BEGIN
+  D4D_REQUIRE(h != nullptr && (ddim != nullptr || dpm != nullptr), "null argument");
+  DeviceGuard g(h->model->device());
+  return h->model->denoise_window(static_cast<bf16*>(latents), static_cast<const bf16*>(pixel_latents),
+                                  static_cast<const bf16*>(plucker), static_cast<const bf16*>(skeletons),
+                                  static_cast<const bf16*>(cond_mask), reinterpret_cast<long long*>(timestep_indices),
+                                  ddim, dpm, static_cast<bf16*>(x0_prev), lower_order_nums, guidance_scale, domain, F,
+                                  height, width, num_steps, static_cast<cudaStream_t>(stream), F_total);
+  D4D_API_END
+}
 }  // namespace
 
 extern "C" {
@@ -112,13 +142,7 @@ const char* d4d_weight_key(d4d_handle* h, int i) {
 int d4d_unet_forward(d4d_handle* h, const void* sample, const int64_t* timestep, const void* skeletons,
                      const int32_t* domain_ids, int n_domains, int B, int F, int height, int width, void* out,
                      void* stream) {
-  D4D_API_BEGIN
-  D4D_REQUIRE(h != nullptr, "null handle");
-  DeviceGuard g(h->model->device());
-  return h->model->forward(static_cast<const bf16*>(sample), reinterpret_cast<const long long*>(timestep),
-                           static_cast<const bf16*>(skeletons), domain_ids, n_domains, B, F, height, width,
-                           static_cast<bf16*>(out), static_cast<cudaStream_t>(stream));
-  D4D_API_END
+  return unet_forward(h, sample, timestep, skeletons, domain_ids, n_domains, B, F, 0, height, width, out, stream);
 }
 
 int d4d_profile_forward(d4d_handle* h, const void* sample, const int64_t* timestep, const void* skeletons,
@@ -155,30 +179,16 @@ int d4d_forward_launches(d4d_handle* h, int n_domains, int B, int F, int height,
 int d4d_denoise_window(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
                        const void* skeletons, const void* cond_mask, int64_t* timestep_indices, const d4d_sched* sched,
                        float guidance_scale, int domain, int F, int height, int width, int num_steps, void* stream) {
-  D4D_API_BEGIN
-  D4D_REQUIRE(h != nullptr && sched != nullptr, "null argument");
-  DeviceGuard g(h->model->device());
-  return h->model->denoise_window(static_cast<bf16*>(latents), static_cast<const bf16*>(pixel_latents),
-                                  static_cast<const bf16*>(plucker), static_cast<const bf16*>(skeletons),
-                                  static_cast<const bf16*>(cond_mask), reinterpret_cast<long long*>(timestep_indices),
-                                  *sched, guidance_scale, domain, F, height, width, num_steps,
-                                  static_cast<cudaStream_t>(stream));
-  D4D_API_END
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, sched, nullptr,
+                        guidance_scale, domain, F, 0, height, width, num_steps, nullptr, nullptr, stream);
 }
 
 int d4d_denoise_window_dpm(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
                            const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
                            const d4d_dpm_sched* sched, float guidance_scale, int domain, int F, int height, int width,
                            int num_steps, void* x0_prev, int32_t* lower_order_nums, void* stream) {
-  D4D_API_BEGIN
-  D4D_REQUIRE(h != nullptr && sched != nullptr, "null argument");
-  DeviceGuard g(h->model->device());
-  return h->model->denoise_window_dpm(static_cast<bf16*>(latents), static_cast<const bf16*>(pixel_latents),
-                                      static_cast<const bf16*>(plucker), static_cast<const bf16*>(skeletons),
-                                      static_cast<const bf16*>(cond_mask), reinterpret_cast<long long*>(timestep_indices),
-                                      *sched, guidance_scale, domain, F, height, width, num_steps,
-                                      static_cast<bf16*>(x0_prev), lower_order_nums, static_cast<cudaStream_t>(stream));
-  D4D_API_END
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, nullptr, sched,
+                        guidance_scale, domain, F, 0, height, width, num_steps, x0_prev, lower_order_nums, stream);
 }
 
 int d4d_assemble_input(void* latents, const void* pixel_latents, const void* plucker, const void* skel_latents,
@@ -415,28 +425,16 @@ int d4d_debug_tap(d4d_handle* h, const void* sample, const int64_t* timestep, co
 int d4d_unet_forward_sharded(d4d_handle* h, const void* sample, const int64_t* timestep, const void* skeletons,
                              const int32_t* domain_ids, int n_domains, int B_local, int F_local, int F_total, int height,
                              int width, void* out, void* stream) {
-  D4D_API_BEGIN
-  D4D_REQUIRE(h != nullptr, "null handle");
-  DeviceGuard g(h->model->device());
-  return h->model->forward(static_cast<const bf16*>(sample), reinterpret_cast<const long long*>(timestep),
-                           static_cast<const bf16*>(skeletons), domain_ids, n_domains, B_local, F_local, height, width,
-                           static_cast<bf16*>(out), static_cast<cudaStream_t>(stream), F_total);
-  D4D_API_END
+  return unet_forward(h, sample, timestep, skeletons, domain_ids, n_domains, B_local, F_local, F_total, height, width,
+                      out, stream);
 }
 
 int d4d_denoise_window_sharded(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
                                const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
                                const d4d_sched* sched, float guidance_scale, int domain, int F_local, int F_total,
                                int height, int width, int num_steps, void* stream) {
-  D4D_API_BEGIN
-  D4D_REQUIRE(h != nullptr && sched != nullptr, "null argument");
-  DeviceGuard g(h->model->device());
-  return h->model->denoise_window(static_cast<bf16*>(latents), static_cast<const bf16*>(pixel_latents),
-                                  static_cast<const bf16*>(plucker), static_cast<const bf16*>(skeletons),
-                                  static_cast<const bf16*>(cond_mask), reinterpret_cast<long long*>(timestep_indices),
-                                  *sched, guidance_scale, domain, F_local, height, width, num_steps,
-                                  static_cast<cudaStream_t>(stream), F_total);
-  D4D_API_END
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, sched, nullptr,
+                        guidance_scale, domain, F_local, F_total, height, width, num_steps, nullptr, nullptr, stream);
 }
 
 int d4d_denoise_window_dpm_sharded(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
@@ -444,16 +442,9 @@ int d4d_denoise_window_dpm_sharded(d4d_handle* h, void* latents, const void* pix
                                    const d4d_dpm_sched* sched, float guidance_scale, int domain, int F_local, int F_total,
                                    int height, int width, int num_steps, void* x0_prev, int32_t* lower_order_nums,
                                    void* stream) {
-  D4D_API_BEGIN
-  D4D_REQUIRE(h != nullptr && sched != nullptr, "null argument");
-  DeviceGuard g(h->model->device());
-  return h->model->denoise_window_dpm(static_cast<bf16*>(latents), static_cast<const bf16*>(pixel_latents),
-                                      static_cast<const bf16*>(plucker), static_cast<const bf16*>(skeletons),
-                                      static_cast<const bf16*>(cond_mask), reinterpret_cast<long long*>(timestep_indices),
-                                      *sched, guidance_scale, domain, F_local, height, width, num_steps,
-                                      static_cast<bf16*>(x0_prev), lower_order_nums, static_cast<cudaStream_t>(stream),
-                                      F_total);
-  D4D_API_END
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, nullptr, sched,
+                        guidance_scale, domain, F_local, F_total, height, width, num_steps, x0_prev, lower_order_nums,
+                        stream);
 }
 
 int d4d_window_exchange(d4d_handle* h, const void* latents_local, const int64_t* timestep_indices_local,

@@ -1147,7 +1147,6 @@ int Model::forward(const bf16* sample, const long long* timestep, const bf16* sk
   p->epoch0 = xch_.epoch_base;  // global, monotonic exchange counter: every rank runs the same forwards in the same order
   for (auto& f : p->ops)
     if (int rc = f(stream)) return rc;
-  p->run_index++;
   xch_.epoch_base += static_cast<unsigned int>(p->n3d);
   return 0;
 }
@@ -1262,52 +1261,86 @@ int Model::profile(const bf16* sample, const long long* timestep, const bf16* sk
 }
 
 int Model::denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
-                          long long* ts_idx, const d4d_sched& sched, float guidance, int domain, int F, int h, int w,
-                          int num_steps, cudaStream_t stream, int F_total) {
-  D4D_REQUIRE(latents && pixel && plucker && mask && ts_idx, "null argument");
-  D4D_REQUIRE(sched.timesteps_table && sched.alphas_cumprod && sched.n_steps > 0, "scheduler tables");
+                          long long* ts_idx, const d4d_sched* ddim, const d4d_dpm_sched* dpm, bf16* x0_prev,
+                          int* lower_order_nums, float guidance, int domain, int F, int h, int w, int num_steps,
+                          cudaStream_t stream, int F_total) {
+  D4D_REQUIRE(latents && pixel && plucker && mask && ts_idx && (ddim || (dpm && x0_prev && lower_order_nums)),
+              "null argument");
+  D4D_REQUIRE(dpm ? dpm->timesteps_table && dpm->coefs && dpm->n_steps > 0
+                  : ddim->timesteps_table && ddim->alphas_cumprod && ddim->n_steps > 0, "scheduler tables");
+  D4D_REQUIRE(domain == 0 || domain == 1, "Invalid domain");
+  const long long* timesteps_table = reinterpret_cast<const long long*>(dpm ? dpm->timesteps_table : ddim->timesteps_table);
+  const int n_steps = dpm ? dpm->n_steps : ddim->n_steps;
   const bool cfg_on = guidance > 1.0f;
+  const int B = cfg_on ? 2 * F : F;
+  const bool pose = cfg_.enable_pose_encoder != 0;
+  const int Cin = 4 + 6 + (pose ? 0 : 4) + 1;
+  D4D_REQUIRE(Cin == cfg_.in_channels, "in_channels does not match the latent/plucker/skeleton/mask channel layout");
+  D4D_REQUIRE(skeletons != nullptr, "skeletons required");
+  D4D_CUDA_OK(cudaSetDevice(device_));
+  const std::string key = std::to_string(B) + "_" + std::to_string(F) + "_" + std::to_string(h) + "_" + std::to_string(w);
+  auto it = wbufs_.find(key);
+  if (it == wbufs_.end()) {
+    std::unique_ptr<WindowBufs> wb(new WindowBufs());
+    const size_t hw = static_cast<size_t>(h) * w;
+    D4D_CUDA_OK(cudaMalloc(&wb->sample, sizeof(bf16) * B * Cin * hw));
+    D4D_CUDA_OK(cudaMalloc(&wb->timestep, sizeof(long long) * B));
+    if (pose) {
+      D4D_CUDA_OK(cudaMalloc(&wb->skel, sizeof(bf16) * (F + 1) * 3 * 64 * hw));
+      if (int rc = fill_bf16_run(wb->skel, static_cast<long long>(3) * 64 * hw, -1.0f, stream)) return rc;  // constant negative image
+    }
+    D4D_CUDA_OK(cudaMalloc(&wb->noise, sizeof(bf16) * B * cfg_.out_channels * hw));
+    D4D_CUDA_OK(cudaMalloc(&wb->latents_tmp, sizeof(bf16) * F * 4 * hw));
+    D4D_CUDA_OK(cudaMalloc(&wb->ts_tmp, sizeof(long long) * F));
+    it = wbufs_.emplace(key, std::move(wb)).first;
+  }
+  WindowBufs& wb = *it->second;
+  if (dpm && !wb.order_tmp) D4D_CUDA_OK(cudaMalloc(&wb.order_tmp, sizeof(int) * F));
+  const int doms[2] = {domain, domain};
   const int hw = h * w;
-  return run_window(latents, pixel, plucker, skeletons, mask, ts_idx,
-                    reinterpret_cast<const long long*>(sched.timesteps_table), sched.n_steps, guidance, domain, F, h, w,
-                    num_steps, stream, F_total, [&](WindowBufs& wb, cudaStream_t s) -> int {
-    DdimArgs d;
-    d.noise = wb.noise; d.latents = latents; d.mask = mask; d.timestep_indices = ts_idx;
-    d.timesteps_table = reinterpret_cast<const long long*>(sched.timesteps_table); d.alphas_cumprod = sched.alphas_cumprod;
-    d.n_steps = sched.n_steps; d.T = sched.num_train_timesteps; d.final_alpha_cumprod = sched.final_alpha_cumprod;
-    d.F = F; d.chw = 4 * hw; d.hw = hw; d.cfg = cfg_on ? 1 : 0; d.guidance = guidance;
-    d.prediction_type = sched.prediction_type; d.clip_sample = sched.clip_sample; d.clip_range = sched.clip_sample_range;
-    d.emulate_bf16 = sched.emulate_bf16; d.out = wb.latents_tmp;
-    if (int rc = cfg_ddim_step_run(d, wb.ts_tmp, s)) return rc;
-    D4D_CUDA_OK(cudaMemcpyAsync(latents, wb.latents_tmp, sizeof(bf16) * F * 4 * hw, cudaMemcpyDeviceToDevice, s));
-    D4D_CUDA_OK(cudaMemcpyAsync(ts_idx, wb.ts_tmp, sizeof(long long) * F, cudaMemcpyDeviceToDevice, s));
-    return 0;
-  });
-}
-
-int Model::denoise_window_dpm(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
-                              long long* ts_idx, const d4d_dpm_sched& sched, float guidance, int domain, int F, int h, int w,
-                              int num_steps, bf16* x0_prev, int* lower_order_nums, cudaStream_t stream, int F_total) {
-  D4D_REQUIRE(latents && pixel && plucker && mask && ts_idx && x0_prev && lower_order_nums, "null argument");
-  D4D_REQUIRE(sched.timesteps_table && sched.coefs && sched.n_steps > 0, "scheduler tables");
-  const bool cfg_on = guidance > 1.0f;
-  const int hw = h * w;
-  return run_window(latents, pixel, plucker, skeletons, mask, ts_idx,
-                    reinterpret_cast<const long long*>(sched.timesteps_table), sched.n_steps, guidance, domain, F, h, w,
-                    num_steps, stream, F_total, [&](WindowBufs& wb, cudaStream_t s) -> int {
-    if (!wb.order_tmp) D4D_CUDA_OK(cudaMalloc(&wb.order_tmp, sizeof(int) * F));
-    DpmArgs d;
-    d.noise = wb.noise; d.latents = latents; d.mask = mask; d.timestep_indices = ts_idx; d.coefs = sched.coefs;
-    d.n_steps = sched.n_steps; d.F = F; d.chw = 4 * hw; d.hw = hw; d.cfg = cfg_on ? 1 : 0; d.guidance = guidance;
-    d.prediction_type = sched.prediction_type; d.solver_order = sched.solver_order;
-    d.final_first_order = sched.final_first_order; d.emulate_bf16 = sched.emulate_bf16;
-    d.x0_prev = x0_prev; d.lower_order_nums = lower_order_nums; d.lower_order_nums_out = wb.order_tmp;
-    d.out = latents;  // each element is read and written by the same thread
-    if (int rc = cfg_dpm_step_run(d, wb.ts_tmp, s)) return rc;
-    D4D_CUDA_OK(cudaMemcpyAsync(ts_idx, wb.ts_tmp, sizeof(long long) * F, cudaMemcpyDeviceToDevice, s));
-    D4D_CUDA_OK(cudaMemcpyAsync(lower_order_nums, wb.order_tmp, sizeof(int) * F, cudaMemcpyDeviceToDevice, s));
-    return 0;
-  });
+  for (int s = 0; s < num_steps; ++s) {
+    AssembleArgs a;
+    a.latents = latents; a.pixel = pixel; a.plucker = plucker; a.skel_latents = pose ? nullptr : skeletons; a.mask = mask;
+    a.timestep_indices = ts_idx; a.timesteps_table = timesteps_table;
+    a.n_steps = n_steps; a.F = F; a.h = h; a.w = w; a.cfg = cfg_on ? 1 : 0;
+    a.sample = wb.sample; a.timestep_out = wb.timestep;
+    if (int rc = assemble_input_run(a, stream)) return rc;
+    const bf16* skel_in = nullptr;
+    if (pose) {
+      if (cfg_on) {  // [negative (filled once) | F positive images]
+        D4D_CUDA_OK(cudaMemcpyAsync(wb.skel + static_cast<size_t>(3) * 64 * hw, skeletons, sizeof(bf16) * F * 3 * 64 * hw,
+                                    cudaMemcpyDeviceToDevice, stream));
+        skel_in = wb.skel;
+      } else {
+        skel_in = skeletons;
+      }
+    }
+    if (int rc = forward(wb.sample, wb.timestep, skel_in, doms, cfg_on ? 2 : 1, B, F, h, w, wb.noise, stream, F_total, pose && cfg_on)) return rc;
+    // the scheduler step writes the new latents and timestep indices (and DPM-Solver++ state) of the frames
+    if (dpm) {
+      DpmArgs d;
+      d.noise = wb.noise; d.latents = latents; d.mask = mask; d.timestep_indices = ts_idx; d.coefs = dpm->coefs;
+      d.n_steps = dpm->n_steps; d.F = F; d.chw = 4 * hw; d.hw = hw; d.cfg = cfg_on ? 1 : 0; d.guidance = guidance;
+      d.prediction_type = dpm->prediction_type; d.solver_order = dpm->solver_order;
+      d.final_first_order = dpm->final_first_order; d.emulate_bf16 = dpm->emulate_bf16;
+      d.x0_prev = x0_prev; d.lower_order_nums = lower_order_nums; d.lower_order_nums_out = wb.order_tmp;
+      d.out = latents;  // each element is read and written by the same thread
+      if (int rc = cfg_dpm_step_run(d, wb.ts_tmp, stream)) return rc;
+      D4D_CUDA_OK(cudaMemcpyAsync(lower_order_nums, wb.order_tmp, sizeof(int) * F, cudaMemcpyDeviceToDevice, stream));
+    } else {
+      DdimArgs d;
+      d.noise = wb.noise; d.latents = latents; d.mask = mask; d.timestep_indices = ts_idx;
+      d.timesteps_table = timesteps_table; d.alphas_cumprod = ddim->alphas_cumprod;
+      d.n_steps = ddim->n_steps; d.T = ddim->num_train_timesteps; d.final_alpha_cumprod = ddim->final_alpha_cumprod;
+      d.F = F; d.chw = 4 * hw; d.hw = hw; d.cfg = cfg_on ? 1 : 0; d.guidance = guidance;
+      d.prediction_type = ddim->prediction_type; d.clip_sample = ddim->clip_sample; d.clip_range = ddim->clip_sample_range;
+      d.emulate_bf16 = ddim->emulate_bf16; d.out = wb.latents_tmp;
+      if (int rc = cfg_ddim_step_run(d, wb.ts_tmp, stream)) return rc;
+      D4D_CUDA_OK(cudaMemcpyAsync(latents, wb.latents_tmp, sizeof(bf16) * F * 4 * hw, cudaMemcpyDeviceToDevice, stream));
+    }
+    D4D_CUDA_OK(cudaMemcpyAsync(ts_idx, wb.ts_tmp, sizeof(long long) * F, cudaMemcpyDeviceToDevice, stream));
+  }
+  return 0;
 }
 
 // One more exchange of the global epoch sequence (DESIGN.md section 7): counter e = epoch_base stores into parity e & 1 of
@@ -1345,59 +1378,6 @@ int Model::window_exchange(const bf16* latents, const long long* ts_idx, const b
   if (dpm) {
     D4D_CUDA_OK(cudaMemcpyAsync(x0_out, g + L.x0, L.x0, cudaMemcpyDeviceToDevice, stream));
     D4D_CUDA_OK(cudaMemcpyAsync(lon_out, g + L.lon, sizeof(int) * F_total, cudaMemcpyDeviceToDevice, stream));
-  }
-  return 0;
-}
-
-int Model::run_window(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
-                      long long* ts_idx, const long long* timesteps_table, int n_steps, float guidance, int domain, int F,
-                      int h, int w, int num_steps, cudaStream_t stream, int F_total, const WindowStep& step) {
-  D4D_REQUIRE(domain == 0 || domain == 1, "Invalid domain");
-  const bool cfg_on = guidance > 1.0f;
-  const int B = cfg_on ? 2 * F : F;
-  const bool pose = cfg_.enable_pose_encoder != 0;
-  const int Cin = 4 + 6 + (pose ? 0 : 4) + 1;
-  D4D_REQUIRE(Cin == cfg_.in_channels, "in_channels does not match the latent/plucker/skeleton/mask channel layout");
-  D4D_REQUIRE(skeletons != nullptr, "skeletons required");
-  D4D_CUDA_OK(cudaSetDevice(device_));
-  const std::string key = std::to_string(B) + "_" + std::to_string(F) + "_" + std::to_string(h) + "_" + std::to_string(w);
-  auto it = wbufs_.find(key);
-  if (it == wbufs_.end()) {
-    std::unique_ptr<WindowBufs> wb(new WindowBufs());
-    const size_t hw = static_cast<size_t>(h) * w;
-    D4D_CUDA_OK(cudaMalloc(&wb->sample, sizeof(bf16) * B * Cin * hw));
-    D4D_CUDA_OK(cudaMalloc(&wb->timestep, sizeof(long long) * B));
-    if (pose) {
-      D4D_CUDA_OK(cudaMalloc(&wb->skel, sizeof(bf16) * (F + 1) * 3 * 64 * hw));
-      if (int rc = fill_bf16_run(wb->skel, static_cast<long long>(3) * 64 * hw, -1.0f, stream)) return rc;  // constant negative image
-    }
-    D4D_CUDA_OK(cudaMalloc(&wb->noise, sizeof(bf16) * B * cfg_.out_channels * hw));
-    D4D_CUDA_OK(cudaMalloc(&wb->latents_tmp, sizeof(bf16) * F * 4 * hw));
-    D4D_CUDA_OK(cudaMalloc(&wb->ts_tmp, sizeof(long long) * F));
-    it = wbufs_.emplace(key, std::move(wb)).first;
-  }
-  WindowBufs& wb = *it->second;
-  const int doms[2] = {domain, domain};
-  const int hw = h * w;
-  for (int s = 0; s < num_steps; ++s) {
-    AssembleArgs a;
-    a.latents = latents; a.pixel = pixel; a.plucker = plucker; a.skel_latents = pose ? nullptr : skeletons; a.mask = mask;
-    a.timestep_indices = ts_idx; a.timesteps_table = timesteps_table;
-    a.n_steps = n_steps; a.F = F; a.h = h; a.w = w; a.cfg = cfg_on ? 1 : 0;
-    a.sample = wb.sample; a.timestep_out = wb.timestep;
-    if (int rc = assemble_input_run(a, stream)) return rc;
-    const bf16* skel_in = nullptr;
-    if (pose) {
-      if (cfg_on) {  // [negative (filled once) | F positive images]
-        D4D_CUDA_OK(cudaMemcpyAsync(wb.skel + static_cast<size_t>(3) * 64 * hw, skeletons, sizeof(bf16) * F * 3 * 64 * hw,
-                                    cudaMemcpyDeviceToDevice, stream));
-        skel_in = wb.skel;
-      } else {
-        skel_in = skeletons;
-      }
-    }
-    if (int rc = forward(wb.sample, wb.timestep, skel_in, doms, cfg_on ? 2 : 1, B, F, h, w, wb.noise, stream, F_total, pose && cfg_on)) return rc;
-    if (int rc = step(wb, stream)) return rc;
   }
   return 0;
 }

@@ -50,7 +50,6 @@ struct Plan {
   bool pose_shared_neg = false;  // skeleton batch = [1 CFG-negative image | F positive images] (window step)
   size_t stats_words = 0;      // GroupNorm statistics pool: 64-bit fixed-point per-(image, channel) sums of every tensor a GroupNorm reads
   int n3d = 0;                 // number of 3-D attention layers (K/V exchanges) per forward
-  unsigned int run_index = 0;  // forwards executed on this plan
   unsigned int epoch0 = 0;     // exchange counter at the start of the current forward (epoch / buffer parity per layer)
   std::vector<std::function<int(cudaStream_t)>> ops;
   std::vector<int> op_kind;       // 0 gemm, 1 conv3x3, 2 attention, 3 groupnorm, 4 layernorm, 5 other
@@ -103,13 +102,13 @@ class Model {
               bool pose_shared_neg = false);
   int exchange_alloc(size_t kv_bytes, unsigned char* handles_out /* 3 x 64 bytes */);
   int exchange_open(int rank, int world, const unsigned char* all_handles /* world x 3 x 64 bytes */);
+  // num_steps x (assemble -> UNet -> CFG + scheduler step) on the window's F frames; latents and ts_idx are updated in
+  // place.  The scheduler is DDIM (ddim) or DPM-Solver++ (dpm, the other one null); with DPM-Solver++ x0_prev [F,4,h,w]
+  // and lower_order_nums [F] are the frames' solver state, also updated in place.
   int denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
-                     long long* ts_idx, const d4d_sched& sched, float guidance, int domain, int F, int h, int w,
-                     int num_steps, cudaStream_t stream, int F_total = 0);
-  // the same window step with the DPM-Solver++ step; x0_prev [F,4,h,w] and lower_order_nums [F] are updated in place
-  int denoise_window_dpm(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
-                         long long* ts_idx, const d4d_dpm_sched& sched, float guidance, int domain, int F, int h, int w,
-                         int num_steps, bf16* x0_prev, int* lower_order_nums, cudaStream_t stream, int F_total = 0);
+                     long long* ts_idx, const d4d_sched* ddim, const d4d_dpm_sched* dpm, bf16* x0_prev,
+                     int* lower_order_nums, float guidance, int domain, int F, int h, int w, int num_steps,
+                     cudaStream_t stream, int F_total);
   // frame-sharded sliding loop: this rank's F updated frames (+ DPM-Solver++ state when x0_prev != nullptr) to every rank,
   // one flag round (one more exchange of the epoch sequence), then the gathered F_total frames to the *_out buffers
   int window_exchange(const bf16* latents, const long long* ts_idx, const bf16* x0_prev, const int* lower_order_nums, int F,
@@ -160,11 +159,6 @@ class Model {
 
   void need(const std::string& key, std::vector<int64_t> shape);
   void declare_keys();
-  // num_steps x (assemble -> UNet -> step(noise, bufs, stream)); step writes the new latents and timestep indices
-  using WindowStep = std::function<int(WindowBufs&, cudaStream_t)>;
-  int run_window(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
-                 long long* ts_idx, const long long* timesteps_table, int n_steps, float guidance, int domain, int F, int h,
-                 int w, int num_steps, cudaStream_t stream, int F_total, const WindowStep& step);
   int cin_pad() const { return 16; }
   int kp_in() const { return 192; }
 };

@@ -23,9 +23,14 @@ import torch
 from ._lib import check, lib
 from .config import DPMSolverConfig, SchedulerConfig
 from .scheduler import DDIMTables, DPMSolverFrame, DPMSolverState, DPMSolverTables
-from .unet import B200MultiviewUNet
+from .unet import _DOMAIN_IDS, B200MultiviewUNet
 
-_DOMAIN_IDS = {"spatial": 0, "temporal": 1}
+
+def _check_inplace(t, name: str, dtype: torch.dtype):
+    """Raw pointers of tensors the library updates in place cross the C ABI: they must be contiguous CUDA tensors of
+    ``dtype`` (a copy would not receive the update)."""
+    if not (torch.is_tensor(t) and t.is_cuda and t.dtype == dtype and t.is_contiguous()):
+        raise ValueError(f"{name} must be a contiguous CUDA {str(dtype).replace('torch.', '')} tensor (updated in place)")
 
 
 def build_windows(target_indices: torch.Tensor, input_indices: torch.Tensor, domain: str, window_size: int,
@@ -106,9 +111,20 @@ class B200Diffuman4DPipeline:
         """One window: ``num_inference_steps`` x (assemble -> UNet -> CFG -> per-frame scheduler step).  ``latents``
         [F,4,h,w] and ``timestep_indices`` [F] (int64, device) are updated IN PLACE and returned.  With DPM-Solver++,
         ``solver_state`` is the window frames' ``DPMSolverState`` (``DPMSolverState.take``), also updated in place."""
+        return self._window_step(latents=latents, pixel_values_latents=pixel_values_latents,
+                                 plucker_embeds_latents=plucker_embeds_latents, skeletons_latents=skeletons_latents,
+                                 cond_masks_latents=cond_masks_latents, timestep_indices=timestep_indices, domain=domain,
+                                 guidance_scale=guidance_scale, num_inference_steps=num_inference_steps,
+                                 solver_state=solver_state)
+
+    def _window_step(self, *, latents, pixel_values_latents, plucker_embeds_latents, skeletons_latents,
+                     cond_masks_latents, timestep_indices, domain: str, guidance_scale: float,
+                     num_inference_steps: int = 1, solver_state: Optional[DPMSolverState] = None,
+                     F_total: Optional[int] = None):
+        """``denoise_window``'s checks and library call.  ``F_total`` given: the tensors hold this rank's frames of a
+        frame-sharded window of ``F_total`` frames (``FrameShardedPipeline.denoise_window``)."""
         if domain not in _DOMAIN_IDS:
             raise ValueError(f"Invalid domain for temporal embedding: {domain}")
-        F_, _, h, w = latents.shape
         dev = self.device
 
         def prep(t, name):
@@ -117,10 +133,9 @@ class B200Diffuman4DPipeline:
             t = t.to(device=dev, dtype=torch.bfloat16)
             return t if t.is_contiguous() else t.contiguous()
 
-        if not (latents.is_cuda and latents.dtype == torch.bfloat16 and latents.is_contiguous()):
-            raise ValueError("latents must be a contiguous CUDA bfloat16 tensor (updated in place)")
-        if not (timestep_indices.is_cuda and timestep_indices.dtype == torch.int64 and timestep_indices.is_contiguous()):
-            raise ValueError("timestep_indices must be a contiguous CUDA int64 tensor (updated in place)")
+        _check_inplace(latents, "latents", torch.bfloat16)
+        _check_inplace(timestep_indices, "timestep_indices", torch.int64)
+        F_, _, h, w = latents.shape
         pix = prep(pixel_values_latents, "pixel_values_latents")
         plk = prep(plucker_embeds_latents, "plucker_embeds_latents")
         skl = prep(skeletons_latents, "skeletons")
@@ -128,6 +143,10 @@ class B200Diffuman4DPipeline:
         sched = self.scheduler.c_struct(self.emulate_bf16_scheduler)
         self._guidance_scale = guidance_scale
         g = guidance_scale if self.do_classifier_free_guidance else 1.0
+        frames = (F_,) if F_total is None else (F_, F_total)
+        args = [self.unet._h, latents.data_ptr(), pix.data_ptr(), plk.data_ptr(), skl.data_ptr(), msk.data_ptr(),
+                timestep_indices.data_ptr(), C.byref(sched), float(g), _DOMAIN_IDS[domain], *frames, h, w,
+                int(num_inference_steps)]
         if self._multistep:
             st = solver_state
             if st is None:
@@ -138,18 +157,12 @@ class B200Diffuman4DPipeline:
             lon = st.lower_order_nums
             if not (lon.is_cuda and lon.dtype == torch.int32 and lon.is_contiguous() and lon.numel() == F_):
                 raise ValueError("solver_state.lower_order_nums must be a contiguous CUDA int32 [F] tensor")
-            with torch.cuda.device(dev):
-                check(lib().d4d_denoise_window_dpm(
-                    self.unet._h, latents.data_ptr(), pix.data_ptr(), plk.data_ptr(), skl.data_ptr(), msk.data_ptr(),
-                    timestep_indices.data_ptr(), C.byref(sched), float(g), _DOMAIN_IDS[domain], F_, h, w,
-                    int(num_inference_steps), st.x0_prev.data_ptr(), lon.data_ptr(),
-                    torch.cuda.current_stream().cuda_stream), "d4d_denoise_window_dpm")
-            return latents, timestep_indices
+            args += [st.x0_prev.data_ptr(), lon.data_ptr()]
+            name = "d4d_denoise_window_dpm" if F_total is None else "d4d_denoise_window_dpm_sharded"
+        else:
+            name = "d4d_denoise_window" if F_total is None else "d4d_denoise_window_sharded"
         with torch.cuda.device(dev):
-            check(lib().d4d_denoise_window(self.unet._h, latents.data_ptr(), pix.data_ptr(), plk.data_ptr(),
-                                           skl.data_ptr(), msk.data_ptr(), timestep_indices.data_ptr(), C.byref(sched),
-                                           float(g), _DOMAIN_IDS[domain], F_, h, w, int(num_inference_steps),
-                                           torch.cuda.current_stream().cuda_stream), "d4d_denoise_window")
+            check(getattr(lib(), name)(*args, torch.cuda.current_stream().cuda_stream), name)
         return latents, timestep_indices
 
     # Diffuman4DPipeline.__call__ with latents given (PIPE:289-437) ----------------------------------------

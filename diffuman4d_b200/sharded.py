@@ -19,8 +19,8 @@ import torch
 import torch.distributed as dist
 
 from ._lib import check, lib
-from .pipeline import B200Diffuman4DPipeline, _DOMAIN_IDS, build_windows
-from .scheduler import DDIMTables, DPMSolverState
+from .pipeline import B200Diffuman4DPipeline, _check_inplace, build_windows
+from .scheduler import DPMSolverState
 from .sharding import frame_shard
 
 
@@ -70,104 +70,30 @@ class FrameShardedPipeline:
     def frames(self, F_total: int):
         return frame_shard(F_total, self.rank, self.world)
 
-    def _bf16(self, t, name):
-        """Same argument contract as the single-GPU path (pipeline.py ``denoise_window``): raw pointers cross the C ABI, so a
-        CPU / strided / wrongly typed tensor must be rejected here instead of surfacing as a peer K/V-flag timeout."""
-        if t is None:
-            raise ValueError(f"{name} is required")
-        t = t.to(device=self.pipe.device, dtype=torch.bfloat16)
-        return t if t.is_contiguous() else t.contiguous()
-
-    @staticmethod
-    def _inplace(t, name, dtype):
-        if not (torch.is_tensor(t) and t.is_cuda and t.dtype == dtype and t.is_contiguous()):
-            raise ValueError(f"{name} must be a contiguous CUDA {str(dtype).replace('torch.', '')} tensor (updated in place)")
+    def _check_world(self, F_local: int, F_total: int):
+        if F_local * self.world != F_total:
+            raise ValueError(f"F_total ({F_total}) must equal world ({self.world}) * local frames ({F_local})")
 
     def unet_forward(self, sample, timestep, skeletons, domains: List[str], F_local: int, F_total: int):
-        """B-2 on this rank's frames: sample [len(domains)*F_local, Cin, h, w] (CFG-major like the reference batch)."""
-        unet = self.pipe.unet
-        sample = self._bf16(sample, "sample")
-        if sample.dim() != 4 or sample.shape[1] != unet.config.in_channels:
-            raise ValueError(f"sample must be [B, {unet.config.in_channels}, h, w]")
-        B, _, H, W = sample.shape
-        if len(domains) * F_local != B:
-            raise ValueError(f"num_frames: {F_local} * len(domains): {len(domains)} != len(emb): {B}")
-        if F_local * self.world != F_total:
-            raise ValueError(f"F_total ({F_total}) must equal world ({self.world}) * local frames ({F_local})")
-        for d in domains:
-            if d not in _DOMAIN_IDS:
-                raise ValueError(f"Invalid domain for temporal embedding: {d}")
-        timestep = timestep.to(device=unet.device, dtype=torch.int64).reshape(-1).contiguous()
-        if timestep.numel() != B:
-            raise ValueError("timestep must have one entry per image")
-        if unet.config.enable_pose_encoder:
-            skeletons = self._bf16(skeletons, "skeletons")
-            if tuple(skeletons.shape) != (B, 3, 8 * H, 8 * W):
-                raise ValueError(f"skeletons must be [B, 3, 8H, 8W], got {tuple(skeletons.shape)}")
-        else:
-            skeletons = None
-        dom = (C.c_int32 * len(domains))(*[_DOMAIN_IDS[d] for d in domains])
-        out = torch.empty(B, unet.config.out_channels, H, W, device=unet.device, dtype=torch.bfloat16)
-        with torch.cuda.device(unet.device):
-            check(lib().d4d_unet_forward_sharded(unet._h, sample.data_ptr(), timestep.data_ptr(),
-                                                 None if skeletons is None else skeletons.data_ptr(), dom, len(domains), B,
-                                                 F_local, F_total, H, W, out.data_ptr(),
-                                                 torch.cuda.current_stream().cuda_stream), "d4d_unet_forward_sharded")
-        return out
+        """B-2 on this rank's frames: sample [len(domains)*F_local, Cin, h, w] (CFG-major like the reference batch);
+        otherwise the arguments and checks of ``B200MultiviewUNet.forward``."""
+        self._check_world(F_local, F_total)
+        return self.pipe.unet._forward(sample, timestep, skeletons, domains, F_local, F_total)
 
-    def denoise_window(self, *, latents, pixel_values_latents, plucker_embeds_latents, skeletons_latents, cond_masks_latents,
-                       timestep_indices, domain: str, guidance_scale: float, F_total: int, num_inference_steps: int = 1,
-                       solver_state: Optional[DPMSolverState] = None):
-        """B-3 on this rank's frames (all tensors hold the LOCAL frames; updated in place like the single-GPU call).  With
-        DPM-Solver++, ``solver_state`` is the local frames' ``DPMSolverState``, also updated in place."""
-        pipe = self.pipe
-        if domain not in _DOMAIN_IDS:
-            raise ValueError(f"Invalid domain for temporal embedding: {domain}")
-        self._inplace(latents, "latents", torch.bfloat16)
-        self._inplace(timestep_indices, "timestep_indices", torch.int64)
-        F_local, _, h, w = latents.shape
-        if F_local * self.world != F_total:
-            raise ValueError(f"F_total ({F_total}) must equal world ({self.world}) * local frames ({F_local})")
-        pixel_values_latents = self._bf16(pixel_values_latents, "pixel_values_latents")
-        plucker_embeds_latents = self._bf16(plucker_embeds_latents, "plucker_embeds_latents")
-        skeletons_latents = self._bf16(skeletons_latents, "skeletons")
-        cond_masks_latents = self._bf16(cond_masks_latents, "cond_masks_latents")
-        sched = pipe.scheduler.c_struct(pipe.emulate_bf16_scheduler)
-        stream = torch.cuda.current_stream(pipe.device).cuda_stream
-        if isinstance(pipe.scheduler, DDIMTables):
-            with torch.cuda.device(pipe.device):
-                check(lib().d4d_denoise_window_sharded(
-                    pipe.unet._h, latents.data_ptr(), pixel_values_latents.data_ptr(), plucker_embeds_latents.data_ptr(),
-                    skeletons_latents.data_ptr(), cond_masks_latents.data_ptr(), timestep_indices.data_ptr(),
-                    C.byref(sched), float(guidance_scale), _DOMAIN_IDS[domain], F_local, F_total, h, w,
-                    int(num_inference_steps), stream), "d4d_denoise_window_sharded")
-            return latents, timestep_indices
-        # DPM-Solver++: the checks and the guidance of B200Diffuman4DPipeline.denoise_window
-        pipe._guidance_scale = guidance_scale
-        g = guidance_scale if pipe.do_classifier_free_guidance else 1.0
-        st = solver_state
-        if st is None:
-            raise ValueError("the DPM-Solver++ scheduler needs the window frames' solver_state")
-        if not (st.x0_prev is not None and st.x0_prev.is_cuda and st.x0_prev.dtype == torch.bfloat16
-                and st.x0_prev.is_contiguous() and st.x0_prev.shape == latents.shape):
-            raise ValueError("solver_state.x0_prev must be a contiguous CUDA bfloat16 tensor shaped like latents")
-        lon = st.lower_order_nums
-        if not (lon.is_cuda and lon.dtype == torch.int32 and lon.is_contiguous() and lon.numel() == F_local):
-            raise ValueError("solver_state.lower_order_nums must be a contiguous CUDA int32 [F] tensor")
-        with torch.cuda.device(pipe.device):
-            check(lib().d4d_denoise_window_dpm_sharded(
-                pipe.unet._h, latents.data_ptr(), pixel_values_latents.data_ptr(), plucker_embeds_latents.data_ptr(),
-                skeletons_latents.data_ptr(), cond_masks_latents.data_ptr(), timestep_indices.data_ptr(), C.byref(sched),
-                float(g), _DOMAIN_IDS[domain], F_local, F_total, h, w, int(num_inference_steps), st.x0_prev.data_ptr(),
-                lon.data_ptr(), stream), "d4d_denoise_window_dpm_sharded")
-        return latents, timestep_indices
+    def denoise_window(self, *, latents, F_total: int, **kw):
+        """B-3 on this rank's frames: every tensor, ``latents`` [F_local,4,h,w] and with DPM-Solver++ ``solver_state``
+        included, holds the LOCAL frames and is updated in place; otherwise the arguments and checks of
+        ``B200Diffuman4DPipeline.denoise_window``."""
+        if torch.is_tensor(latents):   # anything else is refused with the single-GPU message
+            self._check_world(latents.shape[0], F_total)
+        return self.pipe._window_step(latents=latents, F_total=F_total, **kw)
 
     def window_exchange(self, latents, timestep_indices, solver_state: Optional[DPMSolverState], F_total: int):
         """Every rank's updated frames to every rank: the LOCAL ``latents`` [F_local,4,h,w], ``timestep_indices`` and
         (DPM-Solver++) ``solver_state`` in, the whole window's (F_total frames, window order) out as new tensors
         ``(latents, timestep_indices, solver_state or None)``.  SPMD: every rank calls it after the same window step."""
-        self._inplace(latents, "latents", torch.bfloat16)
-        self._inplace(timestep_indices, "timestep_indices", torch.int64)
+        _check_inplace(latents, "latents", torch.bfloat16)
+        _check_inplace(timestep_indices, "timestep_indices", torch.int64)
         F_local, c, h, w = latents.shape
         dev = latents.device
         lat = torch.empty(F_total, c, h, w, dtype=torch.bfloat16, device=dev)
@@ -175,8 +101,8 @@ class FrameShardedPipeline:
         out = None
         ptrs = [None] * 4
         if solver_state is not None:
-            self._inplace(solver_state.x0_prev, "solver_state.x0_prev", torch.bfloat16)
-            self._inplace(solver_state.lower_order_nums, "solver_state.lower_order_nums", torch.int32)
+            _check_inplace(solver_state.x0_prev, "solver_state.x0_prev", torch.bfloat16)
+            _check_inplace(solver_state.lower_order_nums, "solver_state.lower_order_nums", torch.int32)
             out = DPMSolverState(F_total, dev, torch.empty_like(lat), torch.empty(F_total, dtype=torch.int32, device=dev))
             ptrs = [solver_state.x0_prev.data_ptr(), solver_state.lower_order_nums.data_ptr(), out.x0_prev.data_ptr(),
                     out.lower_order_nums.data_ptr()]

@@ -118,8 +118,16 @@ class B200MultiviewUNet:
     def forward(self, sample: torch.Tensor, timestep: Union[torch.Tensor, float, int],
                 skeletons: Optional[torch.Tensor] = None, domains: List[str] = None, num_frames: int = 1,
                 return_dict: bool = True):
+        out = self._forward(sample, timestep, skeletons, domains, num_frames)
+        return UNetMultiviewConditionOutput(sample=out) if return_dict else (out,)
+
+    __call__ = forward
+
+    def _forward(self, sample, timestep, skeletons, domains, num_frames: int, F_total: Optional[int] = None):
+        """``forward``'s checks and library call.  ``F_total`` given: ``num_frames`` are this rank's frames of a
+        frame-sharded window of ``F_total`` frames (``FrameShardedPipeline.unet_forward``)."""
         cfg = self.config
-        if sample.dim() != 4:
+        if not torch.is_tensor(sample) or sample.dim() != 4:
             raise ValueError("sample must be [B, C, H, W]")
         B, Cin, H, W = sample.shape
         if Cin != cfg.in_channels:
@@ -139,6 +147,8 @@ class B200MultiviewUNet:
         timestep = timestep.to(device=self._device, dtype=torch.int64).reshape(-1)
         if timestep.numel() == 1:
             timestep = timestep.expand(B)
+        if timestep.numel() != B:
+            raise ValueError("timestep must have one entry per image")
         timestep = timestep.contiguous()
         sample = sample.to(device=self._device, dtype=torch.bfloat16).contiguous()
         if cfg.enable_pose_encoder:
@@ -147,17 +157,18 @@ class B200MultiviewUNet:
             skeletons = skeletons.to(device=self._device, dtype=torch.bfloat16).contiguous()
             if tuple(skeletons.shape) != (B, 3, 8 * H, 8 * W):
                 raise ValueError(f"skeletons must be [B, 3, 8H, 8W], got {tuple(skeletons.shape)}")
+        sk = skeletons.data_ptr() if cfg.enable_pose_encoder else None
         out = torch.empty(B, cfg.out_channels, H, W, device=self._device, dtype=torch.bfloat16)
         with torch.cuda.device(self._device):
             stream = torch.cuda.current_stream().cuda_stream
-            check(lib().d4d_unet_forward(self._h, sample.data_ptr(), timestep.data_ptr(),
-                                         skeletons.data_ptr() if cfg.enable_pose_encoder else None, dom, len(domains),
-                                         B, num_frames, H, W, out.data_ptr(), stream), "d4d_unet_forward")
-        if not return_dict:
-            return (out,)
-        return UNetMultiviewConditionOutput(sample=out)
-
-    __call__ = forward
+            if F_total is None:
+                check(lib().d4d_unet_forward(self._h, sample.data_ptr(), timestep.data_ptr(), sk, dom, len(domains), B,
+                                             num_frames, H, W, out.data_ptr(), stream), "d4d_unet_forward")
+            else:
+                check(lib().d4d_unet_forward_sharded(self._h, sample.data_ptr(), timestep.data_ptr(), sk, dom,
+                                                     len(domains), B, num_frames, F_total, H, W, out.data_ptr(), stream),
+                      "d4d_unet_forward_sharded")
+        return out
 
     def debug_taps(self, sample, timestep, skeletons=None, domains=None, num_frames: int = 1,
                    modules: bool = False) -> Dict[str, torch.Tensor]:

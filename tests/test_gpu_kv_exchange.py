@@ -373,15 +373,62 @@ def test_loopback_denoise_window_is_bit_identical(cuda, gloo_world1, name):
                 f"{dom} guidance {gs}: max diff {(l_sh.float() - l_ref.float()).abs().max().item()}"
 
 
+@pytest.mark.gpu
+@pytest.mark.parametrize("dpm", [False, True], ids=["ddim", "dpm"])
+def test_loopback_refusals_match_the_single_gpu_calls(cuda, gloo_world1, dpm):
+    """The sharded window step and forward refuse what denoise_window and forward refuse, with the same message."""
+    from diffuman4d_b200.config import DPMSolverConfig
+    from diffuman4d_b200.pipeline import B200Diffuman4DPipeline
+    from diffuman4d_b200.scheduler import DPMSolverState
+    from diffuman4d_b200.sharded import FrameShardedPipeline
+    from diffuman4d_b200.unet import B200MultiviewUNet
+    from diffuman4d_b200.weights import random_state_dict
+    cfg = LOOP_CONFIGS["tiny_pose_tem_linear"]
+    F, h, w = 4, 16, 16
+    pipe = B200Diffuman4DPipeline(B200MultiviewUNet(cfg, 0).load_state_dict(random_state_dict(cfg, seed=1)),
+                                  DPMSolverConfig() if dpm else SchedulerConfig())
+    sh = FrameShardedPipeline(pipe, max_frames=F, h=h, w=w)
+    pipe.parepare_schedulers(18, F)
+    g = torch.Generator().manual_seed(3)
+    lat, pix, plk = (torch.randn(F, c, h, w, generator=g).to(torch.bfloat16).cuda() for c in (4, 4, 6))
+    skel = (torch.rand(F, 3, 8 * h, 8 * w, generator=g) * 2 - 1).to(torch.bfloat16).cuda()
+    ti = torch.zeros(F, dtype=torch.int64, device="cuda")
+    state = lambda **k: DPMSolverState(F, "cuda", **{"x0_prev": torch.zeros_like(lat), **k})
+    ok = dict(latents=lat, pixel_values_latents=pix, plucker_embeds_latents=plk, skeletons_latents=skel,
+              cond_masks_latents=torch.ones(F, 1, h, w, dtype=torch.bfloat16, device="cuda"), timestep_indices=ti,
+              domain="spatial", guidance_scale=2.0, solver_state=state() if dpm else None)
+    refused = [(dict(latents=lat.float()), "latents must be"),
+               (dict(latents=lat.transpose(2, 3)), "latents must be"),
+               (dict(timestep_indices=ti.int()), "timestep_indices must be"),
+               (dict(timestep_indices=torch.zeros(2 * F, dtype=torch.int64, device="cuda")[::2]), "timestep_indices must be")]
+    if dpm:
+        refused += [(dict(solver_state=None), "needs the window frames' solver_state"),
+                    (dict(solver_state=state(x0_prev=torch.zeros_like(lat[:, :, : h // 2]))), "solver_state.x0_prev must be"),
+                    (dict(solver_state=state(lower_order_nums=ti.clone())), "solver_state.lower_order_nums must be")]
+    for change, msg in refused:
+        kw = {**ok, **change}
+        with pytest.raises(ValueError, match=msg) as single:
+            pipe.denoise_window(**kw)
+        with pytest.raises(ValueError) as sharded:
+            sh.denoise_window(F_total=F, **kw)
+        assert str(sharded.value) == str(single.value)
+
+    x, t, sk = _inputs(cfg, F, h, w)
+    doms = ["spatial", "spatial"]
+    refused = [((x, t, sk, ["spatial"]), "num_frames"), ((x, t, sk, ["diagonal", "spatial"]), "Invalid domain"),
+               ((x[:, :5], t, sk, doms), "channels"), ((x, t[:3], sk, doms), "one entry per image"),
+               ((x, t, None, doms), "skeletons are required"), ((x, t, sk[..., : 4 * w], doms), "skeletons must be")]
+    for args, msg in refused:
+        with pytest.raises(ValueError, match=msg) as single:
+            pipe.unet(*args, F)
+        with pytest.raises(ValueError) as sharded:
+            sh.unet_forward(*args, F, F)
+        assert str(sharded.value) == str(single.value)
+
+
 def _sharded_forward(unet, x, t, sk, doms, F):
-    from diffuman4d_b200._lib import check, lib
-    from diffuman4d_b200.unet import _DOMAIN_IDS
-    dom = (C.c_int32 * len(doms))(*[_DOMAIN_IDS[d] for d in doms])
-    out = torch.empty(x.shape[0], unet.config.out_channels, *x.shape[2:], device="cuda", dtype=torch.bfloat16)
-    check(lib().d4d_unet_forward_sharded(unet._h, x.data_ptr(), t.data_ptr(), None if sk is None else sk.data_ptr(), dom,
-                                         len(doms), x.shape[0], F, F, x.shape[2], x.shape[3], out.data_ptr(),
-                                         torch.cuda.current_stream().cuda_stream), "d4d_unet_forward_sharded")
-    return out
+    """The sharded forward of a handle whose exchange was opened by hand (no FrameShardedPipeline)."""
+    return unet._forward(x, t, sk, doms, F, F_total=F)
 
 
 @pytest.mark.gpu

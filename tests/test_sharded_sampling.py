@@ -230,6 +230,35 @@ def test_indivisible_window_is_refused_before_any_window(monkeypatch):
         sh.sliding_iterative_denoise(**kw, window_size=6, sliding_stride=1, bidirectional=False, alternation_rounds=1)
 
 
+WINDOW_REFUSALS = [  # (case, F_total, message); the frame-sharded step runs on rank 0 of 2 with 2 local frames
+    ("invalid-domain", 4, "Invalid domain for temporal embedding: diagonal"),
+    ("cpu-latents", 4, "latents must be a contiguous CUDA bfloat16 tensor (updated in place)"),
+    ("F_total-mismatch", 6, "F_total (6) must equal world (2) * local frames (2)"),
+]
+
+
+@pytest.mark.parametrize("dpm", [False, True], ids=["ddim", "dpm"])
+@pytest.mark.parametrize("case,F_total,msg", WINDOW_REFUSALS, ids=[r[0] for r in WINDOW_REFUSALS])
+def test_sharded_window_refusals_before_any_library_call(monkeypatch, case, F_total, msg, dpm):
+    """The frame-sharded window step refuses these inputs with the single-GPU step's message (the F_total mismatch has no
+    single-GPU counterpart), before the library is loaded."""
+    import diffuman4d_b200.pipeline as pipeline_mod
+    monkeypatch.setattr(pipeline_mod, "lib", lambda: pytest.fail("the library was called"))
+    pipe = _pipe(dpm)
+    sh = _sharded(pipe, 0, 2)
+    r = lambda c: torch.zeros(2, c, H, W, dtype=torch.bfloat16)
+    kw = dict(latents=r(4), pixel_values_latents=r(4), plucker_embeds_latents=r(6), skeletons_latents=r(4),
+              cond_masks_latents=r(1), timestep_indices=torch.zeros(2, dtype=torch.int64),
+              domain="diagonal" if case == "invalid-domain" else "spatial", guidance_scale=2.0)
+    calls = [lambda: sh.denoise_window(F_total=F_total, **kw)]
+    if case != "F_total-mismatch":
+        calls.append(lambda: pipe.denoise_window(**kw))
+    for call in calls:
+        with pytest.raises(ValueError) as e:
+            call()
+        assert str(e.value) == msg
+
+
 def test_sampler_frame_sharded_needs_a_sharded_pipeline():
     from diffuman4d_b200.sampler import B200SlidingIterativeSampler
     ds = types.SimpleNamespace(scene_label="s")
