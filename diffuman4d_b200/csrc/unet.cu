@@ -55,6 +55,13 @@ inline float h2f(uint16_t h) {  // IEEE half -> float
 
 inline int pad_head_dim(int d) { return d <= 64 ? 64 : (d <= 128 ? 128 : (d <= 192 ? 192 : 0)); }
 
+// the pose encoder's convolutions: module path, Cin, Cout, kernel
+const struct { const char* path; int cin, cout, k; } kPoseLayers[8] = {
+    {"pose_encoder.conv_layers.0", 3, 3, 3},    {"pose_encoder.conv_layers.2", 3, 16, 4},
+    {"pose_encoder.conv_layers.4", 16, 16, 3},  {"pose_encoder.conv_layers.6", 16, 32, 4},
+    {"pose_encoder.conv_layers.8", 32, 32, 3},  {"pose_encoder.conv_layers.10", 32, 64, 4},
+    {"pose_encoder.conv_layers.12", 64, 64, 3}, {"pose_encoder.conv_layers.14", 64, 128, 3}};
+
 std::string plan_key(const int* dom, int nd, int B, int F, int h, int w) {
   std::string k = std::to_string(B) + "_" + std::to_string(F) + "_" + std::to_string(h) + "_" + std::to_string(w) + "_";
   for (int i = 0; i < nd; ++i) k += dom[i] ? 't' : 's';
@@ -80,23 +87,11 @@ WindowBufs::~WindowBufs() {
 // =================================================================================================
 // weights
 // =================================================================================================
-Model::Model(const d4d_config& cfg, int device) : cfg_(cfg), device_(device) { declare_keys(); }
-
-Model::~Model() {
-  cudaSetDevice(device_);
-  plans_.clear();
-  wbufs_.clear();
-  for (void* p : dev_allocs_) cudaFree(p);
-}
-
-void Model::need(const std::string& key, std::vector<int64_t> shape) {
-  expected_[key] = std::move(shape);
-  key_order_.push_back(key);
-}
-
-void Model::declare_keys() {
+// The module tree: every module's path and shapes, and its weight keys in state_dict order (weights.state_dict_spec).
+Model::Model(const d4d_config& cfg, int device) : cfg_(cfg), device_(device) {
   const int* ch = cfg_.block_out_channels;
   const int C0 = ch[0], TE = 4 * C0, L = cfg_.layers_per_block;
+  temb_all_.in = TE;
   auto lin = [&](const std::string& p, int out, int in, bool bias = true) {
     need(p + ".weight", {out, in});
     if (bias) need(p + ".bias", {out});
@@ -110,14 +105,31 @@ void Model::declare_keys() {
     need(p + ".bias", {c});
   };
   auto resnet = [&](const std::string& p, int cin, int cout) {
+    ResnetW r;
+    r.path = p;
+    r.cin = cin;
+    r.cout = cout;
+    r.temb_off = temb_all_.out;
+    temb_all_.out += cout;
     norm(p + ".norm1", cin);
     conv(p + ".conv1", cout, cin, 3);
     lin(p + ".time_emb_proj", cout, TE);
     norm(p + ".norm2", cout);
     conv(p + ".conv2", cout, cout, 3);
     if (cin != cout) conv(p + ".conv_shortcut", cout, cin, 1);
+    return r;
   };
-  auto xf = [&](const std::string& p, int C, bool attn2) {
+  // transformer at channel level c; attn1 is 3-D at the num_3d_attn_blocks deepest levels and in the mid block
+  auto xf = [&](const std::string& p, int c, bool mid = false) {
+    XfW x;
+    x.path = p;
+    x.C = ch[c];
+    x.heads = cfg_.num_heads[c];
+    x.d = x.C / x.heads;
+    x.dpad = pad_head_dim(x.d);
+    x.has2 = cfg_.has_attn2[c] != 0;
+    x.is3d = mid || 3 - c < cfg_.num_3d_attn_blocks;
+    const int C = x.C;
     norm(p + ".norm", C);
     lin(p + ".proj_in", C, C);
     const std::string b = p + ".transformer_blocks.0";
@@ -126,7 +138,7 @@ void Model::declare_keys() {
     lin(b + ".attn1.to_k", C, C, false);
     lin(b + ".attn1.to_v", C, C, false);
     lin(b + ".attn1.to_out.0", C, C);
-    if (attn2) {
+    if (x.has2) {
       norm(b + ".norm2", C);
       lin(b + ".attn2.to_q", C, C, false);
       lin(b + ".attn2.to_k", C, C, false);
@@ -137,6 +149,11 @@ void Model::declare_keys() {
     lin(b + ".ff.net.0.proj", 8 * C, C);
     lin(b + ".ff.net.2", C, 4 * C);
     lin(p + ".proj_out", C, C);
+    return x;
+  };
+  auto sampler = [&](LevelW& lv, const char* name) {
+    lv.sampler = lv.path + name;
+    conv(lv.sampler + ".conv", lv.C, lv.C, 3);
   };
   conv("conv_in", C0, cfg_.in_channels, 3);
   lin("time_embedding.linear_1", TE, C0);
@@ -146,8 +163,7 @@ void Model::declare_keys() {
     lin("temporal_pos_embed.linear_2", TE, TE);
   }
   if (cfg_.enable_pose_encoder) {
-    static const int spec[8][3] = {{3, 3, 3}, {3, 16, 4}, {16, 16, 3}, {16, 32, 4}, {32, 32, 3}, {32, 64, 4}, {64, 64, 3}, {64, 128, 3}};
-    for (int i = 0; i < 8; ++i) conv("pose_encoder.conv_layers." + std::to_string(2 * i), spec[i][1], spec[i][0], spec[i][2]);
+    for (const auto& l : kPoseLayers) conv(l.path, l.cout, l.cin, l.k);
     conv("pose_encoder.final_proj", C0, 128, 1);
     need("pose_encoder.scale", {1});
   }
@@ -155,32 +171,48 @@ void Model::declare_keys() {
   for (int i = 0; i < 4; ++i) {
     const int cin = cout;
     cout = ch[i];
-    const std::string p = "down_blocks." + std::to_string(i);
+    LevelW& lv = down_[i];
+    lv.path = "down_blocks." + std::to_string(i);
+    lv.C = cout;
     for (int j = 0; j < L; ++j) {
-      resnet(p + ".resnets." + std::to_string(j), j == 0 ? cin : cout, cout);
-      if (i < 3) xf(p + ".attentions." + std::to_string(j), cout, cfg_.has_attn2[i] != 0);
+      lv.res.push_back(resnet(lv.path + ".resnets." + std::to_string(j), j == 0 ? cin : cout, cout));
+      if (i < 3) lv.xf.push_back(xf(lv.path + ".attentions." + std::to_string(j), i));
     }
-    if (i < 3) conv(p + ".downsamplers.0.conv", cout, cout, 3);
+    if (i < 3) sampler(lv, ".downsamplers.0");
   }
-  resnet("mid_block.resnets.0", ch[3], ch[3]);
-  xf("mid_block.attentions.0", ch[3], cfg_.has_attn2[3] != 0);
-  resnet("mid_block.resnets.1", ch[3], ch[3]);
+  mid_res_[0] = resnet("mid_block.resnets.0", ch[3], ch[3]);
+  mid_xf_ = xf("mid_block.attentions.0", 3, true);
+  mid_res_[1] = resnet("mid_block.resnets.1", ch[3], ch[3]);
   cout = ch[3];
   for (int i = 0; i < 4; ++i) {
     const int cprev = cout;
     cout = ch[3 - i];
     const int cin = ch[3 - std::min(i + 1, 3)];
-    const std::string p = "up_blocks." + std::to_string(i);
+    LevelW& lv = up_[i];
+    lv.path = "up_blocks." + std::to_string(i);
+    lv.C = cout;
     for (int j = 0; j <= L; ++j) {
       const int skip = j == L ? cin : cout;
       const int rin = j == 0 ? cprev : cout;
-      resnet(p + ".resnets." + std::to_string(j), rin + skip, cout);
-      if (i > 0) xf(p + ".attentions." + std::to_string(j), cout, cfg_.has_attn2[3 - i] != 0);
+      lv.res.push_back(resnet(lv.path + ".resnets." + std::to_string(j), rin + skip, cout));
+      if (i > 0) lv.xf.push_back(xf(lv.path + ".attentions." + std::to_string(j), 3 - i));
     }
-    if (i < 3) conv(p + ".upsamplers.0.conv", cout, cout, 3);
+    if (i < 3) sampler(lv, ".upsamplers.0");
   }
   norm("conv_norm_out", C0);
   conv("conv_out", cfg_.out_channels, C0, 3);
+}
+
+Model::~Model() {
+  cudaSetDevice(device_);
+  plans_.clear();
+  wbufs_.clear();
+  for (void* p : dev_allocs_) cudaFree(p);
+}
+
+void Model::need(const std::string& key, std::vector<int64_t> shape) {
+  expected_[key] = std::move(shape);
+  key_order_.push_back(key);
 }
 
 int Model::load_weight(const char* key, const void* data, const int64_t* shape, int ndim, int dtype) {
@@ -258,20 +290,10 @@ int Model::finalize() {
     return static_cast<float*>(p);
   };
   auto T = [&](const std::string& k) -> const std::vector<float>& { return staged_.at(k).v; };
-  auto normw = [&](const std::string& p, int c) {
-    NormW n;
-    n.g = up_f32(T(p + ".weight"));
-    n.b = up_f32(T(p + ".bias"));
-    n.c = c;
-    return n;
-  };
-  auto linw = [&](const std::string& p, int out, int in, bool bias = true) {
-    LinW l;
-    l.w = up_bf16(T(p + ".weight"));
-    l.b = bias ? up_f32(T(p + ".bias")) : nullptr;
-    l.in = in;
-    l.out = out;
-    return l;
+  auto normw = [&](const std::string& p) { return NormW{up_f32(T(p + ".weight")), up_f32(T(p + ".bias"))}; };
+  auto linw = [&](const std::string& p) {  // Linear / 1x1 conv [out][in]
+    const std::vector<int64_t>& s = expected_.at(p + ".weight");
+    return LinW{up_bf16(T(p + ".weight")), up_f32(T(p + ".bias")), static_cast<int>(s[1]), static_cast<int>(s[0])};
   };
   // OIHW [Cout,Cin,k,k] -> [Cout][tap][Cin]
   auto conv_gemm_layout = [&](const std::vector<float>& w, int cout, int cin, int k, int cout_pad = 0) {
@@ -283,37 +305,28 @@ int Model::finalize() {
           o[(static_cast<size_t>(co) * k * k + t) * cin + ci] = w[(static_cast<size_t>(co) * cin + ci) * k * k + t];
     return o;
   };
-  auto convw = [&](const std::string& p, int cout, int cin) {
-    LinW l;
-    l.w = up_bf16(conv_gemm_layout(T(p + ".weight"), cout, cin, 3));
-    l.b = up_f32(T(p + ".bias"));
-    l.in = cin;
-    l.out = cout;
-    return l;
+  auto convw = [&](const std::string& p) {  // conv3x3
+    const std::vector<int64_t>& s = expected_.at(p + ".weight");
+    const int cout = static_cast<int>(s[0]), cin = static_cast<int>(s[1]);
+    return LinW{up_bf16(conv_gemm_layout(T(p + ".weight"), cout, cin, 3)), up_f32(T(p + ".bias")), cin, cout};
   };
-  const int* ch = cfg_.block_out_channels;
-  const int C0 = ch[0], TE = 4 * C0, L = cfg_.layers_per_block;
+  const int C0 = cfg_.block_out_channels[0], TE = temb_all_.in;
 
-  std::vector<float> temb_w, temb_b;
-  auto resnetw = [&](const std::string& p, int cin, int cout) {
-    ResnetW r;
-    r.cin = cin;
-    r.cout = cout;
-    r.n1 = normw(p + ".norm1", cin);
-    r.c1 = convw(p + ".conv1", cout, cin);
-    r.n2 = normw(p + ".norm2", cout);
-    r.c2 = convw(p + ".conv2", cout, cout);
-    if (cin != cout) r.sc = linw(p + ".conv_shortcut", cout, cin);
-    r.temb_off = static_cast<int>(temb_b.size());
-    const auto& tw = T(p + ".time_emb_proj.weight");
-    const auto& tb = T(p + ".time_emb_proj.bias");
-    temb_w.insert(temb_w.end(), tw.begin(), tw.end());
-    temb_b.insert(temb_b.end(), tb.begin(), tb.end());
-    return r;
+  // every time_emb_proj at its block's rows of one [sum Cout][TE] projection
+  std::vector<float> temb_w(static_cast<size_t>(temb_all_.out) * TE), temb_b(temb_all_.out);
+  auto resnetw = [&](ResnetW& r) {
+    r.n1 = normw(r.path + ".norm1");
+    r.c1 = convw(r.path + ".conv1");
+    r.n2 = normw(r.path + ".norm2");
+    r.c2 = convw(r.path + ".conv2");
+    if (r.cin != r.cout) r.sc = linw(r.path + ".conv_shortcut");
+    const auto& tw = T(r.path + ".time_emb_proj.weight");
+    const auto& tb = T(r.path + ".time_emb_proj.bias");
+    std::copy(tw.begin(), tw.end(), temb_w.begin() + static_cast<size_t>(r.temb_off) * TE);
+    std::copy(tb.begin(), tb.end(), temb_b.begin() + r.temb_off);
   };
-  auto attnw = [&](const std::string& p, int C, int heads, int d, int dpad) {
-    AttnW a;
-    const int Cp = heads * dpad;
+  auto attnw = [&](const std::string& p, const XfW& x) {
+    const int C = x.C, heads = x.heads, d = x.d, dpad = x.dpad, Cp = heads * dpad;
     std::vector<float> qkv(static_cast<size_t>(3) * Cp * C, 0.f);
     const char* names[3] = {".to_q.weight", ".to_k.weight", ".to_v.weight"};
     for (int s = 0; s < 3; ++s) {
@@ -323,39 +336,26 @@ int Model::finalize() {
           memcpy(&qkv[(static_cast<size_t>(s) * Cp + hh * dpad + j) * C], &w[static_cast<size_t>(hh * d + j) * C],
                  sizeof(float) * C);
     }
-    a.qkv.w = up_bf16(qkv);
-    a.qkv.b = nullptr;
-    a.qkv.in = C;
-    a.qkv.out = 3 * Cp;
     const auto& wo = T(p + ".to_out.0.weight");
     std::vector<float> o(static_cast<size_t>(C) * Cp, 0.f);
     for (int r = 0; r < C; ++r)
       for (int hh = 0; hh < heads; ++hh)
         for (int j = 0; j < d; ++j) o[static_cast<size_t>(r) * Cp + hh * dpad + j] = wo[static_cast<size_t>(r) * C + hh * d + j];
-    a.out.w = up_bf16(o);
-    a.out.b = up_f32(T(p + ".to_out.0.bias"));
-    a.out.in = Cp;
-    a.out.out = C;
-    return a;
+    return AttnW{LinW{up_bf16(qkv), nullptr, C, 3 * Cp}, LinW{up_bf16(o), up_f32(T(p + ".to_out.0.bias")), Cp, C}};
   };
-  auto xfw = [&](const std::string& p, int C, int heads, bool attn2) {
-    XfW x;
-    x.C = C;
-    x.heads = heads;
-    x.d = C / heads;
-    x.dpad = pad_head_dim(x.d);
-    x.has2 = attn2;
-    x.gn = normw(p + ".norm", C);
-    x.pin = linw(p + ".proj_in", C, C);
-    x.pout = linw(p + ".proj_out", C, C);
-    const std::string b = p + ".transformer_blocks.0";
-    x.ln1 = normw(b + ".norm1", C);
-    x.a1 = attnw(b + ".attn1", C, heads, x.d, x.dpad);
-    if (attn2) {
-      x.ln2 = normw(b + ".norm2", C);
-      x.a2 = attnw(b + ".attn2", C, heads, x.d, x.dpad);
+  auto xfw = [&](XfW& x) {
+    const int C = x.C;
+    const std::string b = x.path + ".transformer_blocks.0";
+    x.gn = normw(x.path + ".norm");
+    x.pin = linw(x.path + ".proj_in");
+    x.pout = linw(x.path + ".proj_out");
+    x.ln1 = normw(b + ".norm1");
+    x.a1 = attnw(b + ".attn1", x);
+    if (x.has2) {
+      x.ln2 = normw(b + ".norm2");
+      x.a2 = attnw(b + ".attn2", x);
     }
-    x.ln3 = normw(b + ".norm3", C);
+    x.ln3 = normw(b + ".norm3");
     // GEGLU interleave in groups of 8 rows: rows 16p .. 16p+7 = a[8p .. 8p+7], rows 16p+8 .. 16p+15 = g[8p .. 8p+7]
     const int N = 8 * C;
     const auto& w = T(b + ".ff.net.0.proj.weight");
@@ -367,12 +367,28 @@ int Model::finalize() {
       memcpy(&wi[static_cast<size_t>(r) * C], &w[static_cast<size_t>(src) * C], sizeof(float) * C);
       bi[r] = bb[src];
     }
-    x.ff1.w = up_bf16(wi);
-    x.ff1.b = up_f32(bi);
-    x.ff1.in = C;
-    x.ff1.out = N;
-    x.ff2 = linw(b + ".ff.net.2", C, 4 * C);
-    return x;
+    x.ff1 = LinW{up_bf16(wi), up_f32(bi), C, N};
+    x.ff2 = linw(b + ".ff.net.2");
+  };
+  // Upsample2D = nearest x2 followed by a 3x3 conv: every output pixel (2y + a, 2x + b) only ever sees a 2x2 patch of
+  // the LOW-resolution input, so the layer is computed as four sub-pixel phases with pre-summed weights
+  // (rows {-1, 0} weigh {w0, w1 + w2} for a = 0 and rows {0, +1} weigh {w0 + w1, w2} for a = 1; same for columns):
+  // 4/9 of the multiply-adds and no materialised upsampled tensor.  Layout per phase: [Cout][ty*2 + tx][Cin].
+  auto upsamplew = [&](const std::string& p, int C) {
+    const auto& w = T(p + ".weight");
+    std::vector<float> o(static_cast<size_t>(4) * C * 4 * C, 0.f);  // [phase = a*2+b][Cout][ty*2+tx][Cin]
+    for (int a = 0; a < 2; ++a)
+      for (int b = 0; b < 2; ++b)
+        for (int co = 0; co < C; ++co)
+          for (int ci = 0; ci < C; ++ci)
+            for (int ky = 0; ky < 3; ++ky)
+              for (int kx = 0; kx < 3; ++kx) {
+                const int ty = a == 0 ? (ky == 0 ? 0 : 1) : (ky == 2 ? 1 : 0);
+                const int tx = b == 0 ? (kx == 0 ? 0 : 1) : (kx == 2 ? 1 : 0);
+                o[((static_cast<size_t>(a * 2 + b) * C + co) * 4 + ty * 2 + tx) * C + ci] +=
+                    w[(static_cast<size_t>(co) * C + ci) * 9 + ky * 3 + kx];
+              }
+    return LinW{up_bf16(o), up_f32(T(p + ".bias")), C, C};
   };
 
   {  // conv_in -> [C0][KP] with k = tap*16 + c
@@ -382,27 +398,20 @@ int Model::finalize() {
     for (int co = 0; co < C0; ++co)
       for (int ci = 0; ci < Cin; ++ci)
         for (int t = 0; t < 9; ++t) o[static_cast<size_t>(co) * KP + t * cp + ci] = w[(static_cast<size_t>(co) * Cin + ci) * 9 + t];
-    conv_in_.w = up_bf16(o);
-    conv_in_.b = up_f32(T("conv_in.bias"));
-    conv_in_.in = KP;
-    conv_in_.out = C0;
+    conv_in_ = LinW{up_bf16(o), up_f32(T("conv_in.bias")), KP, C0};
   }
-  time1_ = linw("time_embedding.linear_1", TE, C0);
-  time2_ = linw("time_embedding.linear_2", TE, TE);
+  time1_ = linw("time_embedding.linear_1");
+  time2_ = linw("time_embedding.linear_2");
   if (cfg_.enable_tem_embeds) {
-    tem1_ = linw("temporal_pos_embed.linear_1", TE, C0);
-    tem2_ = linw("temporal_pos_embed.linear_2", TE, TE);
+    tem1_ = linw("temporal_pos_embed.linear_1");
+    tem2_ = linw("temporal_pos_embed.linear_2");
   }
   if (cfg_.enable_pose_encoder) {
-    static const int spec[8][3] = {{3, 3, 3}, {3, 16, 4}, {16, 16, 3}, {16, 32, 4}, {32, 32, 3}, {32, 64, 4}, {64, 64, 3}, {64, 128, 3}};
     for (int i = 0; i < 8; ++i) {
-      const std::string p = "pose_encoder.conv_layers." + std::to_string(2 * i);
-      const int cin = spec[i][0], cout = spec[i][1], k = spec[i][2];
+      const std::string p = kPoseLayers[i].path;
+      const int cin = kPoseLayers[i].cin, cout = kPoseLayers[i].cout, k = kPoseLayers[i].k;
       const auto& w = T(p + ".weight");
-      LinW l;
-      l.in = cin;
-      l.out = cout;
-      l.b = up_f32(T(p + ".bias"));
+      LinW l{nullptr, up_f32(T(p + ".bias")), cin, cout};
       if (i == 0) {  // FMA kernel: [k*k][Cin][Cout]
         std::vector<float> o(w.size());
         for (int co = 0; co < cout; ++co)
@@ -419,77 +428,35 @@ int Model::finalize() {
         l.in = cp;
       } else {
         l.w = up_bf16(conv_gemm_layout(w, cout, cin, k));
+        if (i == 5) l.in = k * k * cin;  // GEMM over the im2col columns
       }
       pose_.conv[i] = l;
     }
-    pose_.proj = linw("pose_encoder.final_proj", C0, 128);
+    pose_.proj = linw("pose_encoder.final_proj");
     pose_.scale = T("pose_encoder.scale")[0];
   }
-  int cout = C0;
-  for (int i = 0; i < 4; ++i) {
-    const int cin = cout;
-    cout = ch[i];
-    const std::string p = "down_blocks." + std::to_string(i);
-    for (int j = 0; j < L; ++j) {
-      down_res_[i].push_back(resnetw(p + ".resnets." + std::to_string(j), j == 0 ? cin : cout, cout));
-      if (i < 3) down_xf_[i].push_back(xfw(p + ".attentions." + std::to_string(j), cout, cfg_.num_heads[i], cfg_.has_attn2[i] != 0));
-    }
-    if (i < 3) down_ds_[i] = convw(p + ".downsamplers.0.conv", cout, cout);
+  for (LevelW& lv : down_) {
+    for (ResnetW& r : lv.res) resnetw(r);
+    for (XfW& x : lv.xf) xfw(x);
+    if (!lv.sampler.empty()) lv.conv = convw(lv.sampler + ".conv");
   }
-  mid_res_[0] = resnetw("mid_block.resnets.0", ch[3], ch[3]);
-  mid_xf_ = xfw("mid_block.attentions.0", ch[3], cfg_.num_heads[3], cfg_.has_attn2[3] != 0);
-  mid_res_[1] = resnetw("mid_block.resnets.1", ch[3], ch[3]);
-  cout = ch[3];
-  for (int i = 0; i < 4; ++i) {
-    const int cprev = cout;
-    cout = ch[3 - i];
-    const int cin = ch[3 - std::min(i + 1, 3)];
-    const std::string p = "up_blocks." + std::to_string(i);
-    for (int j = 0; j <= L; ++j) {
-      const int skip = j == L ? cin : cout;
-      const int rin = j == 0 ? cprev : cout;
-      up_res_[i].push_back(resnetw(p + ".resnets." + std::to_string(j), rin + skip, cout));
-      if (i > 0) up_xf_[i].push_back(xfw(p + ".attentions." + std::to_string(j), cout, cfg_.num_heads[3 - i], cfg_.has_attn2[3 - i] != 0));
-    }
-    if (i < 3) {
-      // Upsample2D = nearest x2 followed by a 3x3 conv: every output pixel (2y + a, 2x + b) only ever sees a 2x2 patch of
-      // the LOW-resolution input, so the layer is computed as four sub-pixel phases with pre-summed weights
-      // (rows {-1, 0} weigh {w0, w1 + w2} for a = 0 and rows {0, +1} weigh {w0 + w1, w2} for a = 1; same for columns):
-      // 4/9 of the multiply-adds and no materialised upsampled tensor.  Layout per phase: [Cout][ty*2 + tx][Cin].
-      const auto& w = T(p + ".upsamplers.0.conv.weight");
-      std::vector<float> o(static_cast<size_t>(4) * cout * 4 * cout, 0.f);  // [phase = a*2+b][Cout][ty*2+tx][Cin]
-      for (int a = 0; a < 2; ++a)
-        for (int b = 0; b < 2; ++b)
-          for (int co = 0; co < cout; ++co)
-            for (int ci = 0; ci < cout; ++ci)
-              for (int ky = 0; ky < 3; ++ky)
-                for (int kx = 0; kx < 3; ++kx) {
-                  const int ty = a == 0 ? (ky == 0 ? 0 : 1) : (ky == 2 ? 1 : 0);
-                  const int tx = b == 0 ? (kx == 0 ? 0 : 1) : (kx == 2 ? 1 : 0);
-                  o[((static_cast<size_t>(a * 2 + b) * cout + co) * 4 + ty * 2 + tx) * cout + ci] +=
-                      w[(static_cast<size_t>(co) * cout + ci) * 9 + ky * 3 + kx];
-                }
-      up_us_[i].w = up_bf16(o);
-      up_us_[i].b = up_f32(T(p + ".upsamplers.0.conv.bias"));
-      up_us_[i].in = cout;
-      up_us_[i].out = cout;
-    }
+  resnetw(mid_res_[0]);
+  xfw(mid_xf_);
+  resnetw(mid_res_[1]);
+  for (LevelW& lv : up_) {
+    for (ResnetW& r : lv.res) resnetw(r);
+    for (XfW& x : lv.xf) xfw(x);
+    if (!lv.sampler.empty()) lv.conv = upsamplew(lv.sampler + ".conv", lv.C);
   }
-  norm_out_ = normw("conv_norm_out", C0);
-  {
-    conv_out_.w = up_bf16(conv_gemm_layout(T("conv_out.weight"), cfg_.out_channels, C0, 3, 16));
+  norm_out_ = normw("conv_norm_out");
+  {  // conv_out, zero-padded to 16 output channels
     std::vector<float> b(16, 0.f);
     const auto& bo = T("conv_out.bias");
-    for (int i = 0; i < cfg_.out_channels; ++i) b[i] = bo[i];
-    conv_out_.b = up_f32(b);
-    conv_out_.in = C0;
-    conv_out_.out = 16;
+    std::copy(bo.begin(), bo.end(), b.begin());
+    conv_out_ = LinW{up_bf16(conv_gemm_layout(T("conv_out.weight"), cfg_.out_channels, C0, 3, 16)), up_f32(b), C0, 16};
   }
-  temb_total_ = static_cast<int>(temb_b.size());
   temb_all_.w = up_bf16(temb_w);
   temb_all_.b = up_f32(temb_b);
-  temb_all_.in = TE;
-  temb_all_.out = temb_total_;
   if (failed) {
     set_error(std::string("device allocation/upload failed while finalizing weights: ") + cudaGetErrorString(cudaGetLastError()));
     return 2;
@@ -616,6 +583,19 @@ class PlanBuilder {
   void layernorm(const bf16* x, int rows, int C, const NormW& n, bf16* out) {
     op([=](cudaStream_t s) { return layernorm_run(x, rows, C, 1e-5f, n.g, n.b, out, s); }, 1, 4);
   }
+  // GEMM descriptors of a weight: out[M, w.out] = A[M, w.in] * w^T + bias, and the conv (conv_kind `kind`) of n_img NHWC
+  // images [H, W, w.in]; call sites set what differs
+  static GemmDesc linear(const LinW& w, const bf16* A, int M, bf16* out) {
+    GemmDesc d;
+    d.A = A; d.lda = w.in; d.K1 = w.in; d.Wt = w.w; d.M = M; d.N = w.out; d.bias = w.b; d.out = out; d.ldo = w.out;
+    return d;
+  }
+  static GemmDesc conv(const LinW& w, const bf16* A, int n_img, int H, int W, bf16* out, int kind = 0) {
+    GemmDesc d;
+    d.conv = 1; d.conv_kind = kind; d.A = A; d.n_img = n_img; d.H = H; d.W = W; d.Cin = w.in;
+    d.Wt = w.w; d.N = w.out; d.bias = w.b; d.out = out; d.ldo = w.out;
+    return d;
+  }
 
   // ResnetBlock2D on (xa | xb) -> new buffer   (reference semantics: SURVEY R-1)
   Act resnet(const ResnetW& r, Act xa, const Act* xb, const bf16* temb_all, int ld_temb) {
@@ -626,11 +606,8 @@ class PlanBuilder {
     groupnorm(xa, xb, B, m_.cfg_.norm_eps, r.n1, 1, h0);
     Act h1{alloc(static_cast<size_t>(M) * r.cout), r.cout, xa.H, xa.W, stats_alloc(B, r.cout)};
     {
-      GemmDesc d;
-      d.conv = 1; d.A = h0; d.n_img = B; d.H = xa.H; d.W = xa.W; d.Cin = Cin;
-      d.Wt = r.c1.w; d.N = r.cout; d.bias = r.c1.b;
+      GemmDesc d = conv(r.c1, h0, B, xa.H, xa.W, h1.p);
       d.rowvec = temb_all + r.temb_off; d.ld_rowvec = ld_temb;
-      d.out = h1.p; d.ldo = r.cout;
       gemm_stats(d, h1, B, xa.H, xa.W);
     }
     release(h0);
@@ -641,20 +618,16 @@ class PlanBuilder {
     bf16* sc = nullptr;
     if (r.sc.w) {
       sc = alloc(static_cast<size_t>(M) * r.cout);
-      GemmDesc d;
-      d.A = xa.p; d.lda = xa.C; d.K1 = xa.C;
+      GemmDesc d = linear(r.sc, xa.p, M, sc);
+      d.lda = xa.C; d.K1 = xa.C;
       if (xb) { d.A2 = xb->p; d.lda2 = Cb; d.K2 = Cb; }
-      d.Wt = r.sc.w; d.M = M; d.N = r.cout; d.bias = r.sc.b; d.out = sc; d.ldo = r.cout;
       gemm(d);
       res = sc;
     }
     Act out{alloc(static_cast<size_t>(M) * r.cout), r.cout, xa.H, xa.W, stats_alloc(B, r.cout)};
     {
-      GemmDesc d;
-      d.conv = 1; d.A = h2; d.n_img = B; d.H = xa.H; d.W = xa.W; d.Cin = r.cout;
-      d.Wt = r.c2.w; d.N = r.cout; d.bias = r.c2.b;
+      GemmDesc d = conv(r.c2, h2, B, xa.H, xa.W, out.p);
       d.residual = res; d.ld_res = r.cout;
-      d.out = out.p; d.ldo = r.cout;
       gemm_stats(d, out, B, xa.H, xa.W);
     }
     release(h2);
@@ -680,8 +653,7 @@ class PlanBuilder {
     GemmLaunch G[2];
     AttnLaunch A[2];
     for (int par = 0; par < 2; ++par) {
-      GemmDesc d;
-      d.A = normed; d.lda = x.C; d.K1 = x.C; d.Wt = a.qkv.w; d.M = M; d.N = 3 * Cp; d.out = qkv; d.ldo = 3 * Cp;
+      GemmDesc d = linear(a.qkv, normed, M, qkv);
       d.kv_world = X.world; d.kv_col0 = Cp; d.kv_ld = 2 * Cp;
       d.kv_rows_local = rows_local; d.kv_rows_global = rows_global; d.kv_row_offset = static_cast<long long>(X.rank) * rows_local;
       for (int r = 0; r < X.world; ++r) d.kv_dst[r] = static_cast<bf16*>(X.peer_kv[par][r]);
@@ -729,11 +701,7 @@ class PlanBuilder {
       o = alloc(static_cast<size_t>(M) * Cp);
       sharded_qkv_attention(a, x, normed, qkv, o, M, batch, seq);
     } else {
-      {
-        GemmDesc d;
-        d.A = normed; d.lda = x.C; d.K1 = x.C; d.Wt = a.qkv.w; d.M = M; d.N = 3 * Cp; d.out = qkv; d.ldo = 3 * Cp;
-        gemm(d);
-      }
+      gemm(linear(a.qkv, normed, M, qkv));
       o = alloc(static_cast<size_t>(M) * Cp);
       AttnDesc d;
       d.q = qkv; d.k = qkv + Cp; d.v = qkv + 2 * Cp; d.ld_qkv = 3 * Cp;
@@ -743,25 +711,20 @@ class PlanBuilder {
     }
     release(qkv);
     {
-      GemmDesc d;
-      d.A = o; d.lda = Cp; d.K1 = Cp; d.Wt = a.out.w; d.M = M; d.N = x.C; d.bias = a.out.b;
-      d.residual = resid; d.ld_res = x.C; d.out = out; d.ldo = x.C;
+      GemmDesc d = linear(a.out, o, M, out);
+      d.residual = resid; d.ld_res = x.C;
       gemm(d);
     }
     release(o);
   }
 
   // TransformerMultiviewModel (+ its single MultiviewTransformerBlock): x -> new buffer
-  Act transformer(const XfW& x, Act in, int num_frames) {
-    const int B = p_.B, hw = in.H * in.W, M = B * hw, C = x.C;
+  Act transformer(const XfW& x, Act in) {
+    const int B = p_.B, hw = in.H * in.W, M = B * hw, C = x.C, num_frames = x.is3d ? p_.F : 1;
     bf16* n = alloc(static_cast<size_t>(M) * C);
     groupnorm(in, nullptr, B, 1e-6f, x.gn, 0, n);
     bf16* t = alloc(static_cast<size_t>(M) * C);
-    {
-      GemmDesc d;
-      d.A = n; d.lda = C; d.K1 = C; d.Wt = x.pin.w; d.M = M; d.N = C; d.bias = x.pin.b; d.out = t; d.ldo = C;
-      gemm(d);
-    }
+    gemm(linear(x.pin, n, M, t));
     // attn1 (3-D when num_frames > 1: batch = B / num_frames sequences of num_frames*hw tokens)
     layernorm(t, M, C, x.ln1, n);
     bf16* t1 = alloc(static_cast<size_t>(M) * C);
@@ -777,27 +740,23 @@ class PlanBuilder {
     layernorm(t1, M, C, x.ln3, n);
     bf16* g = alloc(static_cast<size_t>(M) * 4 * C);
     {
-      GemmDesc d;
-      d.A = n; d.lda = C; d.K1 = C; d.Wt = x.ff1.w; d.M = M; d.N = 8 * C; d.bias = x.ff1.b; d.out = g; d.ldo = 4 * C;
-      d.geglu = 1;
+      GemmDesc d = linear(x.ff1, n, M, g);
+      d.geglu = 1; d.ldo = 4 * C;
       gemm(d);
     }
     release(n);
     bf16* t3 = alloc(static_cast<size_t>(M) * C);
     {
-      GemmDesc d;
-      d.A = g; d.lda = 4 * C; d.K1 = 4 * C; d.Wt = x.ff2.w; d.M = M; d.N = C; d.bias = x.ff2.b;
-      d.residual = t1; d.ld_res = C; d.out = t3; d.ldo = C;
+      GemmDesc d = linear(x.ff2, g, M, t3);
+      d.residual = t1; d.ld_res = C;
       gemm(d);
     }
     release(g);
     release(t1);
     Act out{alloc(static_cast<size_t>(M) * C), C, in.H, in.W, stats_alloc(B, C)};
     {
-      GemmDesc d;
-      d.A = t3; d.lda = C; d.K1 = C; d.Wt = x.pout.w; d.M = M; d.N = C; d.bias = x.pout.b;
-      d.residual = in.p; d.ld_res = C; d.out = out.p; d.ldo = C;
-      d.stats_rows = hw;
+      GemmDesc d = linear(x.pout, t3, M, out.p);
+      d.residual = in.p; d.ld_res = C; d.stats_rows = hw;
       gemm_stats(d, out, B, in.H, in.W);
     }
     release(t3);
@@ -808,9 +767,8 @@ class PlanBuilder {
     if (n_img <= 0) n_img = p_.B;
     const int M = n_img * in.H * in.W;
     Act out{alloc(static_cast<size_t>(M) * w.out), w.out, in.H, in.W};
-    GemmDesc d;
-    d.conv = 1; d.A = in.p; d.n_img = n_img; d.H = in.H; d.W = in.W; d.Cin = in.C;
-    d.Wt = w.w; d.N = w.out; d.bias = w.b; d.out = out.p; d.ldo = w.out; d.act = act;
+    GemmDesc d = conv(w, in.p, n_img, in.H, in.W, out.p);
+    d.act = act;
     gemm(d);
     return out;
   }
@@ -839,16 +797,12 @@ class PlanBuilder {
     op([=](cudaStream_t s) { return sinusoid_i64_run(pl->timestep, B, C0, cfg.flip_sin_to_cos, cfg.freq_shift, tsin, s); });
     bf16* e1 = alloc(static_cast<size_t>(B) * TE);
     {
-      GemmDesc d;
-      d.A = tsin; d.lda = C0; d.K1 = C0; d.Wt = m.time1_.w; d.M = B; d.N = TE; d.bias = m.time1_.b; d.act = 1; d.out = e1; d.ldo = TE;
+      GemmDesc d = linear(m.time1_, tsin, B, e1);
+      d.act = 1;
       gemm(d);
     }
     bf16* emb = alloc(static_cast<size_t>(B) * TE);
-    {
-      GemmDesc d;
-      d.A = e1; d.lda = TE; d.K1 = TE; d.Wt = m.time2_.w; d.M = B; d.N = TE; d.bias = m.time2_.b; d.out = emb; d.ldo = TE;
-      gemm(d);
-    }
+    gemm(linear(m.time2_, e1, B, emb));
     if (cfg.enable_tem_embeds) {
       float* pos = reinterpret_cast<float*>(alloc(static_cast<size_t>(B) * 2));
       if (!dry_) {
@@ -859,15 +813,14 @@ class PlanBuilder {
       }
       op([=](cudaStream_t s) { return sinusoid_run(pos, B, C0, 1, 0.f, tsin, s); });
       {
-        GemmDesc d;
-        d.A = tsin; d.lda = C0; d.K1 = C0; d.Wt = m.tem1_.w; d.M = B; d.N = TE; d.bias = m.tem1_.b; d.act = 1; d.out = e1; d.ldo = TE;
+        GemmDesc d = linear(m.tem1_, tsin, B, e1);
+        d.act = 1;
         gemm(d);
       }
       bf16* emb2 = alloc(static_cast<size_t>(B) * TE);
       {
-        GemmDesc d;
-        d.A = e1; d.lda = TE; d.K1 = TE; d.Wt = m.tem2_.w; d.M = B; d.N = TE; d.bias = m.tem2_.b;
-        d.residual = emb; d.ld_res = TE; d.out = emb2; d.ldo = TE;
+        GemmDesc d = linear(m.tem2_, e1, B, emb2);
+        d.residual = emb; d.ld_res = TE;
         gemm(d);
       }
       // pos stays allocated for the lifetime of the plan (it is read on every forward)
@@ -876,13 +829,9 @@ class PlanBuilder {
     }
     module_tap("time_embedding", Act{emb, TE, 1, 1});
     op([=](cudaStream_t s) { return silu_run(emb, static_cast<long long>(B) * TE, e1, s); });
-    const int ldt = m.temb_total_;
+    const int ldt = m.temb_all_.out;
     bf16* temb_all = alloc(static_cast<size_t>(B) * ldt);
-    {
-      GemmDesc d;
-      d.A = e1; d.lda = TE; d.K1 = TE; d.Wt = m.temb_all_.w; d.M = B; d.N = ldt; d.bias = m.temb_all_.b; d.out = temb_all; d.ldo = ldt;
-      gemm(d);
-    }
+    gemm(linear(m.temb_all_, e1, B, temb_all));
     release(tsin);
     release(e1);
     release(emb);
@@ -916,8 +865,8 @@ class PlanBuilder {
       release(a4);
       bf16* a5 = alloc(static_cast<size_t>(PM0) * 64);
       {
-        GemmDesc d;
-        d.A = col; d.lda = 512; d.K1 = 512; d.Wt = pw.conv[5].w; d.M = PM0; d.N = 64; d.bias = pw.conv[5].b; d.act = 1; d.out = a5; d.ldo = 64;
+        GemmDesc d = linear(pw.conv[5], col, PM0, a5);
+        d.act = 1;
         gemm(d);
       }
       release(col);
@@ -928,9 +877,8 @@ class PlanBuilder {
       release(x6.p);
       pose_emb = alloc(static_cast<size_t>(PM0) * C0);
       {
-        GemmDesc d;
-        d.A = x7.p; d.lda = 128; d.K1 = 128; d.Wt = pw.proj.w; d.M = PM0; d.N = C0; d.bias = pw.proj.b; d.out_scale = pw.scale;
-        d.out = pose_emb; d.ldo = C0;
+        GemmDesc d = linear(pw.proj, x7.p, PM0, pose_emb);
+        d.out_scale = pw.scale;
         gemm(d);
       }
       release(x7.p);
@@ -949,10 +897,8 @@ class PlanBuilder {
       bf16* col = alloc(static_cast<size_t>(M0) * KP);
       op([=](cudaStream_t s) { return im2col_nchw_run(pl->sample, B, Cin, h, w, cp, KP, col, s); });
       x = {alloc(static_cast<size_t>(M0) * C0), C0, h, w, stats_alloc(B, C0)};
-      GemmDesc d;
-      d.A = col; d.lda = KP; d.K1 = KP; d.Wt = m.conv_in_.w; d.M = M0; d.N = C0; d.bias = m.conv_in_.b;
+      GemmDesc d = linear(m.conv_in_, col, M0, x.p);
       if (pose_emb) { d.residual = pose_emb; d.ld_res = C0; }
-      d.out = x.p; d.ldo = C0;
       d.stats_rows = h * w;
       gemm_stats(d, x, B, h, w);
       release(col);
@@ -964,14 +910,13 @@ class PlanBuilder {
     std::vector<Act> skips;
     skips.push_back(x);
     for (int i = 0; i < 4; ++i) {
-      const int nf = (4 - i - 1) < cfg.num_3d_attn_blocks ? F : 1;
-      const std::string blk = "down_blocks." + std::to_string(i);
+      const LevelW& lv = m.down_[i];
       for (int j = 0; j < L; ++j) {
-        Act y = resnet(m.down_res_[i][j], x, nullptr, temb_all, ldt);
-        module_tap(blk + ".resnets." + std::to_string(j), y);
+        Act y = resnet(lv.res[j], x, nullptr, temb_all, ldt);
+        module_tap(lv.res[j].path, y);
         if (i < 3) {
-          Act z = transformer(m.down_xf_[i][j], y, nf);
-          module_tap(blk + ".attentions." + std::to_string(j), z);
+          Act z = transformer(lv.xf[j], y);
+          module_tap(lv.xf[j].path, z);
           release(y.p);
           y = z;
         }
@@ -981,43 +926,39 @@ class PlanBuilder {
       if (i < 3) {  // Downsample2D: 3x3 stride-2 pad-1 conv, read in place through a strided tensor map
         const int Ho = x.H / 2, Wo = x.W / 2, Mo = B * Ho * Wo;
         const Act y{alloc(static_cast<size_t>(Mo) * x.C), x.C, Ho, Wo, stats_alloc(B, x.C)};
-        GemmDesc d;
-        d.conv = 1; d.conv_kind = 1; d.A = x.p; d.n_img = B; d.H = x.H; d.W = x.W; d.Cin = x.C;
-        d.Wt = m.down_ds_[i].w; d.N = x.C; d.bias = m.down_ds_[i].b; d.out = y.p; d.ldo = x.C;
-        gemm_stats(d, y, B, Ho, Wo);
-        module_tap(blk + ".downsamplers.0", y);
+        gemm_stats(conv(lv.conv, x.p, B, x.H, x.W, y.p, 1), y, B, Ho, Wo);
+        module_tap(lv.sampler, y);
         x = y;
         skips.push_back(x);
       }
-      tap(blk, x);
+      tap(lv.path, x);
     }
     // ---- 4. mid: UNET:568-572 ----
     {
       Act y = resnet(m.mid_res_[0], x, nullptr, temb_all, ldt);  // x is a skip: keep it
-      module_tap("mid_block.resnets.0", y);
-      Act z = transformer(m.mid_xf_, y, F);
-      module_tap("mid_block.attentions.0", z);
+      module_tap(m.mid_res_[0].path, y);
+      Act z = transformer(m.mid_xf_, y);
+      module_tap(m.mid_xf_.path, z);
       release(y.p);
       Act u = resnet(m.mid_res_[1], z, nullptr, temb_all, ldt);
-      module_tap("mid_block.resnets.1", u);
+      module_tap(m.mid_res_[1].path, u);
       release(z.p);
       x = u;
     }
     tap("mid_block", x);
     // ---- 5. up: UNET:575-587 ----
     for (int i = 0; i < 4; ++i) {
-      const int nf = i < cfg.num_3d_attn_blocks ? F : 1;
-      const std::string blk = "up_blocks." + std::to_string(i);
+      const LevelW& lv = m.up_[i];
       for (int j = 0; j <= L; ++j) {
         const Act sk = skips.back();
         skips.pop_back();
-        Act y = resnet(m.up_res_[i][j], x, &sk, temb_all, ldt);
-        module_tap(blk + ".resnets." + std::to_string(j), y);
+        Act y = resnet(lv.res[j], x, &sk, temb_all, ldt);
+        module_tap(lv.res[j].path, y);
         release(x.p);
         release(sk.p);
         if (i > 0) {
-          Act z = transformer(m.up_xf_[i][j], y, nf);
-          module_tap(blk + ".attentions." + std::to_string(j), z);
+          Act z = transformer(lv.xf[j], y);
+          module_tap(lv.xf[j].path, z);
           release(y.p);
           y = z;
         }
@@ -1026,18 +967,12 @@ class PlanBuilder {
       if (i < 3) {  // Upsample2D (nearest x2, then 3x3 conv) as four sub-pixel phases on the low-resolution tensor
         const int H2 = 2 * x.H, W2 = 2 * x.W;
         Act y{alloc(static_cast<size_t>(B) * H2 * W2 * x.C), x.C, H2, W2, stats_alloc(B, x.C)};
-        {
-          GemmDesc d;
-          d.conv = 1; d.conv_kind = 3;
-          d.A = x.p; d.n_img = B; d.H = x.H; d.W = x.W; d.Cin = x.C;
-          d.Wt = m.up_us_[i].w; d.N = x.C; d.bias = m.up_us_[i].b; d.out = y.p; d.ldo = x.C;
-          gemm_stats(d, y, B, x.H, x.W);  // (tiles walk the low-resolution grid)
-        }
-        module_tap(blk + ".upsamplers.0", y);
+        gemm_stats(conv(lv.conv, x.p, B, x.H, x.W, y.p, 3), y, B, x.H, x.W);  // (tiles walk the low-resolution grid)
+        module_tap(lv.sampler, y);
         release(x.p);
         x = y;
       }
-      tap(blk, x);
+      tap(lv.path, x);
     }
     // ---- 6. out: UNET:590-593 ----
     {

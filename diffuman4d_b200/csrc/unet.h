@@ -16,25 +16,38 @@ struct HostTensor {
   std::vector<int64_t> shape;
 };
 
-struct NormW { float* g = nullptr; float* b = nullptr; int c = 0; };
+// Module structs: the Model constructor sets the diffusers module path (also the module's debug tap name) and the shapes;
+// finalize() uploads the weights of the keys path + ".conv1.weight" etc.
+struct NormW { float* g = nullptr; float* b = nullptr; };
 struct LinW { bf16* w = nullptr; float* b = nullptr; int in = 0, out = 0; };
 struct ResnetW {
+  std::string path;
   NormW n1, n2;
   LinW c1, c2;   // conv3x3 weights [Cout][9][Cin]; in = Cin, out = Cout
   LinW sc;       // 1x1 shortcut (w == nullptr when Cin == Cout)
-  int temb_off = 0;
+  int temb_off = 0;  // first row of this block's time_emb_proj in the concatenated projection
   int cin = 0, cout = 0;
 };
 struct AttnW { LinW qkv, out; };
 struct XfW {
+  std::string path;
   NormW gn, ln1, ln2, ln3;
   LinW pin, pout, ff1, ff2;
   AttnW a1, a2;
   bool has2 = false;
+  bool is3d = false;  // attn1 attends over all frames of a sequence (num_3d_attn_blocks deepest levels, mid block)
   int C = 0, heads = 0, d = 0, dpad = 0;
 };
+struct LevelW {  // down_blocks.i / up_blocks.i
+  std::string path;
+  std::vector<ResnetW> res;
+  std::vector<XfW> xf;   // empty where the level has no transformers
+  std::string sampler;   // module path of the Downsample2D / Upsample2D (empty on the last level)
+  int C = 0;             // output channels (also the sampler's)
+  LinW conv;             // Downsample2D [C][9][C]; Upsample2D as four sub-pixel phase kernels [phase = a*2+b][C][4][C] (unet.cu)
+};
 struct PoseW {
-  LinW conv[8];   // layers 0..5 direct layout [k*k][Cin][Cout]; 5 -> GEMM layout [Cout][16*Cin]; 6,7 conv3x3 layout
+  LinW conv[8];   // layers 0..5 direct layout [k*k][Cin][Cout]; 5 -> GEMM layout [Cout][16*Cin], in = 16*Cin; 6,7 conv3x3 layout
   LinW proj;      // [C0][128]
   float scale = 1.f;
 };
@@ -141,24 +154,19 @@ class Model {
   // device weights
   LinW conv_in_;          // [C0][KP_IN]
   LinW time1_, time2_, tem1_, tem2_;
-  LinW temb_all_;         // concatenated time_emb_proj [sum Cout][1280]
+  LinW temb_all_;         // every resnet's time_emb_proj, concatenated: [sum Cout][TE] (in / out set by the constructor)
   PoseW pose_;
-  std::vector<ResnetW> down_res_[4], up_res_[4];
-  std::vector<XfW> down_xf_[4], up_xf_[4];
-  LinW down_ds_[4];
-  LinW up_us_[4];         // Upsample2D convs as four sub-pixel phase kernels: [phase = a*2+b][Cout][4][Cin] (unet.cu)
+  LevelW down_[4], up_[4];
   ResnetW mid_res_[2];
   XfW mid_xf_;
   NormW norm_out_;
   LinW conv_out_;         // [16][9][C0]
-  int temb_total_ = 0;
 
   std::map<std::string, std::unique_ptr<Plan>> plans_;
   std::map<std::string, std::unique_ptr<WindowBufs>> wbufs_;
   Exchange xch_;
 
   void need(const std::string& key, std::vector<int64_t> shape);
-  void declare_keys();
   int cin_pad() const { return 16; }
   int kp_in() const { return 192; }
 };

@@ -1,7 +1,7 @@
 """Weight-key contract of the UNet (diffusers layout, SURVEY.md section 8b) and seeded random weights.
 
 ``state_dict_spec`` lists every parameter of ``unet/diffusion_pytorch_model.safetensors`` for a given config with its
-diffusers shape; the C++ loader (csrc/unet.cu ``declare_keys``) and the CPU oracle must agree with it (tested).
+diffusers shape; the C++ loader (the ``Model`` constructor in csrc/unet.cu) and the CPU oracle must agree with it (tested).
 """
 from __future__ import annotations
 

@@ -9,6 +9,7 @@ than 1e-3 (SURVEY.md section 7).  The bar used here is the reference's own preci
 we require e_ours <= 1.5 * e_eager + 2e-3 and e_ours <= 4e-2 absolute.  Both numbers are printed.
 """
 import math
+import re
 
 import pytest
 import torch
@@ -96,6 +97,28 @@ def test_unet_forward_interface_errors(cuda):
     with pytest.raises(RuntimeError):
         from diffuman4d_b200.unet import B200MultiviewUNet
         B200MultiviewUNet(cfg, 0).load_state_dict({"conv_in.weight": torch.zeros(64, 11, 3, 3)})
+
+
+@pytest.mark.parametrize("name", [*CONFIGS, "tiny_3d0", "tiny_3d1", "tiny_3d4"])
+def test_weight_keys_and_load_refusals(cuda, name):
+    """The library's weight keys are state_dict_spec's, in order; a transposed tensor (right element count) and an
+    unknown key are refused, naming the key."""
+    import ctypes as C
+    from diffuman4d_b200._lib import check, lib
+    from diffuman4d_b200.unet import B200MultiviewUNet
+    from diffuman4d_b200.weights import state_dict_spec
+    cfg = CONFIGS[name] if name in CONFIGS else UNetConfig.tiny(num_3d_attn_blocks=int(name[-1]))
+    unet = B200MultiviewUNet(cfg, 0)
+    assert unet.expected_keys() == list(state_dict_spec(cfg))
+    sd = random_state_dict(cfg, seed=1, device="cuda")
+    for key in ("time_embedding.linear_1.weight", "conv_in.weight", "up_blocks.1.resnets.2.conv_shortcut.weight"):
+        with pytest.raises(ValueError, match=f"shape mismatch for {re.escape(key)}"):
+            unet.load_state_dict({**sd, key: sd[key].transpose(0, 1).contiguous()})
+    with pytest.raises(RuntimeError, match="unexpected"):
+        unet.load_state_dict({**sd, "down_blocks.0.bogus.weight": torch.zeros(4)})
+    t = torch.zeros(4)
+    with pytest.raises(ValueError, match="unknown weight key: down_blocks.0.bogus.weight"):
+        check(lib().d4d_load_weight(unet._h, b"down_blocks.0.bogus.weight", t.data_ptr(), (C.c_int64 * 1)(4), 1, 0))
 
 
 def _sched_pair(pred="epsilon", emulate=False):
