@@ -139,3 +139,25 @@ class DPMSolverConfig:
     final_sigmas_type: str = "zero"       # or "sigma_min"
     timestep_spacing: str = "linspace"    # or "leading", "trailing"
     steps_offset: int = 0
+
+
+@dataclass
+class UniPCConfig:
+    """UniPC scheduler knobs (upstream diffusers==0.33.1 ``UniPCMultistepScheduler`` defaults) that the fused step
+    implements: predict_x0, solver_type "bh1" or "bh2", solver_order 1 or 2, no solver_p, no thresholding, sigmas straight
+    from the beta schedule."""
+    num_train_timesteps: int = 1000
+    beta_start: float = 0.0001
+    beta_end: float = 0.02
+    beta_schedule: str = "linear"         # or "scaled_linear"
+    solver_order: int = 2                 # 1 or 2
+    prediction_type: str = "epsilon"      # or "v_prediction", "sample"
+    solver_type: str = "bh2"              # or "bh1"
+    lower_order_final: bool = True
+    disable_corrector: Tuple[int, ...] = ()   # step indices whose result is not corrected by the next step
+    final_sigmas_type: str = "zero"       # or "sigma_min"
+    timestep_spacing: str = "linspace"    # or "leading", "trailing"
+    steps_offset: int = 0
+
+    def __post_init__(self):
+        self.disable_corrector = tuple(int(i) for i in self.disable_corrector)

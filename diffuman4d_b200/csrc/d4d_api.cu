@@ -54,28 +54,39 @@ int unet_forward(d4d_handle* h, const void* sample, const int64_t* timestep, con
   D4D_API_END
 }
 
-// the four d4d_denoise_window* entry points: the DDIM (ddim) or the DPM-Solver++ (dpm, with x0_prev and
-// lower_order_nums) scheduler, the other one null; F_total = 0 runs the single-GPU plan
+// every d4d_denoise_window* entry point: `step` names the scheduler table and the frames' solver state; F_total = 0 runs
+// the single-GPU plan
 int denoise_window(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker, const void* skeletons,
-                   const void* cond_mask, int64_t* timestep_indices, const d4d_sched* ddim, const d4d_dpm_sched* dpm,
-                   float guidance_scale, int domain, int F, int F_total, int height, int width, int num_steps,
-                   void* x0_prev, int32_t* lower_order_nums, void* stream) {
+                   const void* cond_mask, int64_t* timestep_indices, const d4d::WindowStep& step, float guidance_scale,
+                   int domain, int F, int F_total, int height, int width, int num_steps, void* stream) {
   D4D_API_BEGIN
-  D4D_REQUIRE(h != nullptr && (ddim != nullptr || dpm != nullptr), "null argument");
+  D4D_REQUIRE(h != nullptr && (step.ddim != nullptr || step.dpm != nullptr || step.unipc != nullptr), "null argument");
   DeviceGuard g(h->model->device());
   return h->model->denoise_window(static_cast<bf16*>(latents), static_cast<const bf16*>(pixel_latents),
                                   static_cast<const bf16*>(plucker), static_cast<const bf16*>(skeletons),
                                   static_cast<const bf16*>(cond_mask), reinterpret_cast<long long*>(timestep_indices),
-                                  ddim, dpm, static_cast<bf16*>(x0_prev), lower_order_nums, guidance_scale, domain, F,
-                                  height, width, num_steps, static_cast<cudaStream_t>(stream), F_total);
+                                  step, guidance_scale, domain, F, height, width, num_steps,
+                                  static_cast<cudaStream_t>(stream), F_total);
   D4D_API_END
+}
+
+d4d::WindowStep ddim_step(const d4d_sched* sched) {
+  d4d::WindowStep s;
+  s.ddim = sched;
+  return s;
+}
+
+d4d::WindowStep dpm_step(const d4d_dpm_sched* sched, void* x0_prev, int32_t* lower_order_nums) {
+  d4d::WindowStep s;
+  s.dpm = sched; s.x0_prev = static_cast<bf16*>(x0_prev); s.lower_order_nums = lower_order_nums;
+  return s;
 }
 }  // namespace
 
 extern "C" {
 
 const char* d4d_last_error(void) { return d4d::g_last_error.c_str(); }
-int d4d_version(void) { return 106; }
+int d4d_version(void) { return 107; }
 
 int d4d_create(const d4d_config* cfg, int device, d4d_handle** out) {
   D4D_API_BEGIN
@@ -179,16 +190,29 @@ int d4d_forward_launches(d4d_handle* h, int n_domains, int B, int F, int height,
 int d4d_denoise_window(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
                        const void* skeletons, const void* cond_mask, int64_t* timestep_indices, const d4d_sched* sched,
                        float guidance_scale, int domain, int F, int height, int width, int num_steps, void* stream) {
-  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, sched, nullptr,
-                        guidance_scale, domain, F, 0, height, width, num_steps, nullptr, nullptr, stream);
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, ddim_step(sched),
+                        guidance_scale, domain, F, 0, height, width, num_steps, stream);
 }
 
 int d4d_denoise_window_dpm(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
                            const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
                            const d4d_dpm_sched* sched, float guidance_scale, int domain, int F, int height, int width,
                            int num_steps, void* x0_prev, int32_t* lower_order_nums, void* stream) {
-  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, nullptr, sched,
-                        guidance_scale, domain, F, 0, height, width, num_steps, x0_prev, lower_order_nums, stream);
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
+                        dpm_step(sched, x0_prev, lower_order_nums), guidance_scale, domain, F, 0, height, width, num_steps,
+                        stream);
+}
+
+int d4d_denoise_window_unipc(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                             const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                             const d4d_unipc_sched* sched, float guidance_scale, int domain, int F, int height, int width,
+                             int num_steps, void* x0_prev, void* x0_prev2, void* last_sample, int32_t* lower_order_nums,
+                             void* stream) {
+  d4d::WindowStep s;
+  s.unipc = sched; s.x0_prev = static_cast<bf16*>(x0_prev); s.x0_prev2 = static_cast<bf16*>(x0_prev2);
+  s.last_sample = static_cast<bf16*>(last_sample); s.lower_order_nums = lower_order_nums;
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, s, guidance_scale,
+                        domain, F, 0, height, width, num_steps, stream);
 }
 
 int d4d_assemble_input(void* latents, const void* pixel_latents, const void* plucker, const void* skel_latents,
@@ -255,6 +279,29 @@ int d4d_cfg_dpm_step(const void* noise, const void* latents, const void* cond_ma
   d.x0_prev = static_cast<bf16*>(x0_prev); d.lower_order_nums = lower_order_nums;
   d.lower_order_nums_out = lower_order_nums_out; d.out = static_cast<bf16*>(latents_out);
   return d4d::cfg_dpm_step_run(d, reinterpret_cast<long long*>(timestep_indices_out), static_cast<cudaStream_t>(stream));
+  D4D_API_END
+}
+
+int d4d_cfg_unipc_step(const void* noise, const void* latents, const void* cond_mask, const int64_t* timestep_indices,
+                       int64_t* timestep_indices_out, void* x0_prev, void* x0_prev2, void* last_sample,
+                       const int32_t* lower_order_nums, int32_t* lower_order_nums_out, const d4d_unipc_sched* sched,
+                       float guidance_scale, int cfg, int F, int height, int width, void* latents_out, void* stream) {
+  D4D_API_BEGIN
+  D4D_REQUIRE(noise && latents && cond_mask && timestep_indices && timestep_indices_out && x0_prev && last_sample &&
+                  lower_order_nums && lower_order_nums_out && sched && sched->timesteps_table && sched->coefs && latents_out,
+              "null argument");
+  d4d::UniPCArgs d;
+  const int hw = height * width;
+  d.noise = static_cast<const bf16*>(noise); d.latents = static_cast<const bf16*>(latents);
+  d.mask = static_cast<const bf16*>(cond_mask);
+  d.timestep_indices = reinterpret_cast<const long long*>(timestep_indices);
+  d.coefs = sched->coefs; d.n_steps = sched->n_steps;
+  d.F = F; d.chw = 4 * hw; d.hw = hw; d.cfg = cfg; d.guidance = guidance_scale;
+  d.prediction_type = sched->prediction_type; d.solver_order = sched->solver_order; d.emulate_bf16 = sched->emulate_bf16;
+  d.x0_prev = static_cast<bf16*>(x0_prev); d.x0_prev2 = static_cast<bf16*>(x0_prev2);
+  d.last_sample = static_cast<bf16*>(last_sample); d.lower_order_nums = lower_order_nums;
+  d.lower_order_nums_out = lower_order_nums_out; d.out = static_cast<bf16*>(latents_out);
+  return d4d::cfg_unipc_step_run(d, reinterpret_cast<long long*>(timestep_indices_out), static_cast<cudaStream_t>(stream));
   D4D_API_END
 }
 
@@ -433,8 +480,8 @@ int d4d_denoise_window_sharded(d4d_handle* h, void* latents, const void* pixel_l
                                const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
                                const d4d_sched* sched, float guidance_scale, int domain, int F_local, int F_total,
                                int height, int width, int num_steps, void* stream) {
-  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, sched, nullptr,
-                        guidance_scale, domain, F_local, F_total, height, width, num_steps, nullptr, nullptr, stream);
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, ddim_step(sched),
+                        guidance_scale, domain, F_local, F_total, height, width, num_steps, stream);
 }
 
 int d4d_denoise_window_dpm_sharded(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
@@ -442,9 +489,9 @@ int d4d_denoise_window_dpm_sharded(d4d_handle* h, void* latents, const void* pix
                                    const d4d_dpm_sched* sched, float guidance_scale, int domain, int F_local, int F_total,
                                    int height, int width, int num_steps, void* x0_prev, int32_t* lower_order_nums,
                                    void* stream) {
-  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, nullptr, sched,
-                        guidance_scale, domain, F_local, F_total, height, width, num_steps, x0_prev, lower_order_nums,
-                        stream);
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
+                        dpm_step(sched, x0_prev, lower_order_nums), guidance_scale, domain, F_local, F_total, height,
+                        width, num_steps, stream);
 }
 
 int d4d_window_exchange(d4d_handle* h, const void* latents_local, const int64_t* timestep_indices_local,

@@ -430,6 +430,83 @@ __global__ void cfg_dpm_kernel(const DpmArgs a, long long* ts_out) {
 }
 
 // ---------------------------------------------------------------------------------------------
+// CFG combine + per-frame UniPC step (upstream UniPCMultistepScheduler.step, predict_x0, bh1 / bh2, order <= 2).  Every
+// frame carries its own history (x0_prev, x0_prev2, last_sample, lower_order_nums); its step index is its timestep index.
+// Unlike DPM-Solver++, upstream does not upcast the sample: every product and difference rounds to bf16 in EMU mode.
+// ---------------------------------------------------------------------------------------------
+template <bool EMU>
+__global__ void cfg_unipc_kernel(const UniPCArgs a, long long* ts_out) {
+  const int f = blockIdx.y;
+  const bool is_cond = __bfloat162float(a.mask[static_cast<size_t>(f) * a.hw]) == 0.f;
+  long long idx = a.timestep_indices[f];
+  const int lon = a.lower_order_nums[f];
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    ts_out[f] = is_cond ? 0 : idx + 1;
+    a.lower_order_nums_out[f] = is_cond ? lon : min(lon + 1, a.solver_order);
+  }
+  const size_t base = static_cast<size_t>(f) * a.chw;
+  if (is_cond) {  // never stepped: latents pass through, history untouched
+    if (a.out != a.latents)
+      for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.chw; i += gridDim.x * blockDim.x)
+        a.out[base + i] = a.latents[base + i];
+    return;
+  }
+  idx = idx < 0 ? 0 : (idx >= a.n_steps ? a.n_steps - 1 : idx);
+  const float* k = a.coefs + idx * kUniPCCoefs;
+  const float alpha_s = k[0], sigma_s = k[1];
+  const float p_ratio = k[2], p_cphi = k[3], p_cB = k[4], p_rk = k[5];
+  const float c_ratio = k[6], c_cphi = k[7], c_cB = k[8], c_rk = k[9];
+  const float rho0 = rnd<EMU>(k[10]), rho1 = rnd<EMU>(k[11]);   // upstream casts the solved rhos to the sample dtype
+  // the corrector runs at the previous step's order, which is lon; the predictor's order is capped by the row
+  const bool correct = lon >= 1 && k[12] != 0.f;
+  const int c_order = min(lon, a.solver_order);
+  const int p_order = min(static_cast<int>(k[13]), lon + 1);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.chw; i += gridDim.x * blockDim.x) {
+    float m;
+    if (a.cfg) {
+      const float u = __bfloat162float(a.noise[base + i]);
+      const float cn = __bfloat162float(a.noise[static_cast<size_t>(a.F) * a.chw + base + i]);
+      m = rnd<EMU>(u + rnd<EMU>(a.guidance * rnd<EMU>(cn - u)));   // u + g * (c - u), as in cfg_ddim_kernel
+    } else {
+      m = __bfloat162float(a.noise[base + i]);
+    }
+    float x = __bfloat162float(a.latents[base + i]);
+    float x0;  // convert_model_output: runs in the model output's dtype
+    if (a.prediction_type == 0) x0 = rnd<EMU>(rnd<EMU>(x - rnd<EMU>(sigma_s * m)) / alpha_s);
+    else if (a.prediction_type == 1) x0 = rnd<EMU>(rnd<EMU>(alpha_s * x) - rnd<EMU>(sigma_s * m));
+    else x0 = m;
+    const float m0 = __bfloat162float(a.x0_prev[base + i]);
+    const float m1 = a.x0_prev2 ? __bfloat162float(a.x0_prev2[base + i]) : 0.f;
+    if (correct) {  // UniC: recompute the sample from last_sample with this step's data prediction
+      const float last = __bfloat162float(a.last_sample[base + i]);
+      const float xt = rnd<EMU>(sub_nc<EMU>(rnd<EMU>(c_ratio * last), rnd<EMU>(c_cphi * m0)));
+      const float d1t = rnd<EMU>(x0 - m0);
+      float inner;
+      if (c_order == 1) {
+        inner = rnd<EMU>(0.f + rnd<EMU>(0.5f * d1t));   // upstream: 0 + rhos_c[-1] * D1_t
+      } else {
+        const float d1 = rnd<EMU>(rnd<EMU>(m1 - m0) / c_rk);
+        inner = rnd<EMU>(rnd<EMU>(rho0 * d1) + rnd<EMU>(rho1 * d1t));
+      }
+      x = rnd<EMU>(sub_nc<EMU>(xt, rnd<EMU>(c_cB * inner)));
+    }
+    if (a.x0_prev2) a.x0_prev2[base + i] = __float2bfloat16_rn(m0);
+    a.x0_prev[base + i] = __float2bfloat16_rn(x0);
+    a.last_sample[base + i] = __float2bfloat16_rn(x);
+    // UniP from the (corrected) sample
+    const float xt = rnd<EMU>(sub_nc<EMU>(rnd<EMU>(p_ratio * x), rnd<EMU>(p_cphi * x0)));
+    float prev;
+    if (p_order == 1) {
+      prev = sub_nc<EMU>(xt, mul_nc<EMU>(p_cB, 0.f));   // upstream: x_t_ - alpha_t * B_h * 0 (a signed zero)
+    } else {
+      const float d1 = rnd<EMU>(rnd<EMU>(m0 - x0) / p_rk);
+      prev = rnd<EMU>(sub_nc<EMU>(xt, rnd<EMU>(p_cB * rnd<EMU>(0.5f * d1))));
+    }
+    a.out[base + i] = __float2bfloat16_rn(prev);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
 // frame-sharded window: K/V arrival flags in peer memory
 // ---------------------------------------------------------------------------------------------
 __global__ void kv_signal_kernel(const KvFlagArgs a) {
@@ -649,6 +726,21 @@ int cfg_dpm_step_run(const DpmArgs& a, long long* ts_out, cudaStream_t stream) {
   dim3 grid(min(64, blocks_for(a.chw, 256)), a.F);
   if (a.emulate_bf16) cfg_dpm_kernel<true><<<grid, 256, 0, stream>>>(a, ts_out);
   else cfg_dpm_kernel<false><<<grid, 256, 0, stream>>>(a, ts_out);
+  D4D_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int cfg_unipc_step_run(const UniPCArgs& a, long long* ts_out, cudaStream_t stream) {
+  D4D_REQUIRE(a.n_steps > 0 && a.F > 0 && a.coefs && a.x0_prev && a.last_sample && a.lower_order_nums &&
+                  a.lower_order_nums_out, "unipc args");
+  D4D_REQUIRE(a.solver_order == 1 || a.solver_order == 2, "solver_order must be 1 or 2");
+  D4D_REQUIRE((a.x0_prev2 != nullptr) == (a.solver_order == 2), "x0_prev2 is given exactly when solver_order is 2");
+  D4D_REQUIRE(a.prediction_type >= 0 && a.prediction_type <= 2, "prediction_type");
+  D4D_REQUIRE(a.lower_order_nums != a.lower_order_nums_out && ts_out != a.timestep_indices,
+              "the timestep index and order count outputs may not alias their inputs");
+  dim3 grid(min(64, blocks_for(a.chw, 256)), a.F);
+  if (a.emulate_bf16) cfg_unipc_kernel<true><<<grid, 256, 0, stream>>>(a, ts_out);
+  else cfg_unipc_kernel<false><<<grid, 256, 0, stream>>>(a, ts_out);
   D4D_CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -226,6 +226,32 @@ struct DpmArgs {
 // ts_out[F]: updated timestep indices (targets +1, cond 0); may not alias a.timestep_indices
 int cfg_dpm_step_run(const DpmArgs& a, long long* ts_out, cudaStream_t stream);
 
+// CFG combine + per-frame UniPC step (upstream UniPCMultistepScheduler, predict_x0, bh1 / bh2, order <= 2): the UniC
+// corrector of the frame's previous step, then the UniP predictor.  Coefficient row i of `coefs` (fp32, built on the host
+// in the upstream order of operations, layout in include/d4d.h d4d_unipc_sched).
+constexpr int kUniPCCoefs = 14;
+struct UniPCArgs {
+  const bf16* noise;        // [(cfg?2:1)*F,4,h,w]
+  const bf16* latents;      // [F,4,h,w]
+  const bf16* mask;         // [F,1,h,w]  (cond frame <=> mask[f,0,0,0]==0; never stepped, state untouched)
+  const long long* timestep_indices;  // [F] = the step index of each frame
+  const float* coefs;       // [n_steps][kUniPCCoefs]
+  int n_steps;
+  int F, chw, hw, cfg;
+  float guidance;
+  int prediction_type;      // 0 epsilon, 1 v_prediction, 2 sample
+  int solver_order;         // 1 or 2
+  int emulate_bf16;
+  bf16* x0_prev;            // [F,4,h,w] in/out: each frame's previous data prediction
+  bf16* x0_prev2;           // [F,4,h,w] in/out: the one before (solver_order 2; nullptr for order 1)
+  bf16* last_sample;        // [F,4,h,w] in/out: the sample each frame's last predictor started from
+  const int* lower_order_nums;        // [F]
+  int* lower_order_nums_out;          // [F] (may not alias lower_order_nums)
+  bf16* out;                // [F,4,h,w] (may alias latents)
+};
+// ts_out[F]: updated timestep indices (targets +1, cond 0); may not alias a.timestep_indices
+int cfg_unipc_step_run(const UniPCArgs& a, long long* ts_out, cudaStream_t stream);
+
 // cross-rank K/V arrival flags (frame-sharded window): signal = system-scope release of `epoch` into slot `my_rank` of
 // every rank's flag array; wait = acquire-spin until all `world` slots of the local array reach `epoch`
 struct KvFlagArgs {

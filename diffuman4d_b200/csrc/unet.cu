@@ -1195,17 +1195,71 @@ int Model::profile(const bf16* sample, const long long* timestep, const bf16* sk
   return 0;
 }
 
+// The scheduler step of one window step: writes the frames' new latents and solver state, and their advanced timestep
+// indices into ts_out (copied back by the caller).
+static int scheduler_step(const WindowStep& st, WindowBufs& wb, bf16* latents, const bf16* mask, const long long* ts_idx,
+                          int F, int hw, bool cfg_on, float guidance, cudaStream_t stream) {
+  if (const d4d_sched* ddim = st.ddim) {
+    DdimArgs d;
+    d.noise = wb.noise; d.latents = latents; d.mask = mask; d.timestep_indices = ts_idx;
+    d.timesteps_table = reinterpret_cast<const long long*>(ddim->timesteps_table); d.alphas_cumprod = ddim->alphas_cumprod;
+    d.n_steps = ddim->n_steps; d.T = ddim->num_train_timesteps; d.final_alpha_cumprod = ddim->final_alpha_cumprod;
+    d.F = F; d.chw = 4 * hw; d.hw = hw; d.cfg = cfg_on ? 1 : 0; d.guidance = guidance;
+    d.prediction_type = ddim->prediction_type; d.clip_sample = ddim->clip_sample; d.clip_range = ddim->clip_sample_range;
+    d.emulate_bf16 = ddim->emulate_bf16; d.out = wb.latents_tmp;
+    if (int rc = cfg_ddim_step_run(d, wb.ts_tmp, stream)) return rc;
+    D4D_CUDA_OK(cudaMemcpyAsync(latents, wb.latents_tmp, sizeof(bf16) * F * 4 * hw, cudaMemcpyDeviceToDevice, stream));
+    return 0;
+  }
+  if (const d4d_dpm_sched* dpm = st.dpm) {
+    DpmArgs d;
+    d.noise = wb.noise; d.latents = latents; d.mask = mask; d.timestep_indices = ts_idx; d.coefs = dpm->coefs;
+    d.n_steps = dpm->n_steps; d.F = F; d.chw = 4 * hw; d.hw = hw; d.cfg = cfg_on ? 1 : 0; d.guidance = guidance;
+    d.prediction_type = dpm->prediction_type; d.solver_order = dpm->solver_order;
+    d.final_first_order = dpm->final_first_order; d.emulate_bf16 = dpm->emulate_bf16;
+    d.x0_prev = st.x0_prev; d.lower_order_nums = st.lower_order_nums; d.lower_order_nums_out = wb.order_tmp;
+    d.out = latents;  // each element is read and written by the same thread
+    if (int rc = cfg_dpm_step_run(d, wb.ts_tmp, stream)) return rc;
+  } else {
+    const d4d_unipc_sched* u = st.unipc;
+    UniPCArgs d;
+    d.noise = wb.noise; d.latents = latents; d.mask = mask; d.timestep_indices = ts_idx; d.coefs = u->coefs;
+    d.n_steps = u->n_steps; d.F = F; d.chw = 4 * hw; d.hw = hw; d.cfg = cfg_on ? 1 : 0; d.guidance = guidance;
+    d.prediction_type = u->prediction_type; d.solver_order = u->solver_order; d.emulate_bf16 = u->emulate_bf16;
+    d.x0_prev = st.x0_prev; d.x0_prev2 = st.x0_prev2; d.last_sample = st.last_sample;
+    d.lower_order_nums = st.lower_order_nums; d.lower_order_nums_out = wb.order_tmp;
+    d.out = latents;  // each element is read and written by the same thread
+    if (int rc = cfg_unipc_step_run(d, wb.ts_tmp, stream)) return rc;
+  }
+  D4D_CUDA_OK(cudaMemcpyAsync(st.lower_order_nums, wb.order_tmp, sizeof(int) * F, cudaMemcpyDeviceToDevice, stream));
+  return 0;
+}
+
 int Model::denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
-                          long long* ts_idx, const d4d_sched* ddim, const d4d_dpm_sched* dpm, bf16* x0_prev,
-                          int* lower_order_nums, float guidance, int domain, int F, int h, int w, int num_steps,
-                          cudaStream_t stream, int F_total) {
-  D4D_REQUIRE(latents && pixel && plucker && mask && ts_idx && (ddim || (dpm && x0_prev && lower_order_nums)),
+                          long long* ts_idx, const WindowStep& step, float guidance, int domain, int F, int h, int w,
+                          int num_steps, cudaStream_t stream, int F_total) {
+  const bool multistep = step.dpm || step.unipc;
+  D4D_REQUIRE(latents && pixel && plucker && mask && ts_idx &&
+                  (step.ddim != nullptr) + (step.dpm != nullptr) + (step.unipc != nullptr) == 1 &&
+                  (!multistep || (step.x0_prev && step.lower_order_nums)) && (!step.unipc || step.last_sample),
               "null argument");
-  D4D_REQUIRE(dpm ? dpm->timesteps_table && dpm->coefs && dpm->n_steps > 0
-                  : ddim->timesteps_table && ddim->alphas_cumprod && ddim->n_steps > 0, "scheduler tables");
+  const void* table = nullptr;
+  int n_steps = 0;
+  if (step.ddim) {
+    D4D_REQUIRE(step.ddim->timesteps_table && step.ddim->alphas_cumprod, "scheduler tables");
+    table = step.ddim->timesteps_table; n_steps = step.ddim->n_steps;
+  } else if (step.dpm) {
+    D4D_REQUIRE(step.dpm->timesteps_table && step.dpm->coefs, "scheduler tables");
+    table = step.dpm->timesteps_table; n_steps = step.dpm->n_steps;
+  } else {
+    D4D_REQUIRE(step.unipc->timesteps_table && step.unipc->coefs, "scheduler tables");
+    D4D_REQUIRE((step.x0_prev2 != nullptr) == (step.unipc->solver_order == 2),
+                "x0_prev2 is given exactly when solver_order is 2");
+    table = step.unipc->timesteps_table; n_steps = step.unipc->n_steps;
+  }
+  D4D_REQUIRE(n_steps > 0, "scheduler tables");
   D4D_REQUIRE(domain == 0 || domain == 1, "Invalid domain");
-  const long long* timesteps_table = reinterpret_cast<const long long*>(dpm ? dpm->timesteps_table : ddim->timesteps_table);
-  const int n_steps = dpm ? dpm->n_steps : ddim->n_steps;
+  const long long* timesteps_table = static_cast<const long long*>(table);
   const bool cfg_on = guidance > 1.0f;
   const int B = cfg_on ? 2 * F : F;
   const bool pose = cfg_.enable_pose_encoder != 0;
@@ -1230,7 +1284,7 @@ int Model::denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker,
     it = wbufs_.emplace(key, std::move(wb)).first;
   }
   WindowBufs& wb = *it->second;
-  if (dpm && !wb.order_tmp) D4D_CUDA_OK(cudaMalloc(&wb.order_tmp, sizeof(int) * F));
+  if (multistep && !wb.order_tmp) D4D_CUDA_OK(cudaMalloc(&wb.order_tmp, sizeof(int) * F));
   const int doms[2] = {domain, domain};
   const int hw = h * w;
   for (int s = 0; s < num_steps; ++s) {
@@ -1251,28 +1305,7 @@ int Model::denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker,
       }
     }
     if (int rc = forward(wb.sample, wb.timestep, skel_in, doms, cfg_on ? 2 : 1, B, F, h, w, wb.noise, stream, F_total, pose && cfg_on)) return rc;
-    // the scheduler step writes the new latents and timestep indices (and DPM-Solver++ state) of the frames
-    if (dpm) {
-      DpmArgs d;
-      d.noise = wb.noise; d.latents = latents; d.mask = mask; d.timestep_indices = ts_idx; d.coefs = dpm->coefs;
-      d.n_steps = dpm->n_steps; d.F = F; d.chw = 4 * hw; d.hw = hw; d.cfg = cfg_on ? 1 : 0; d.guidance = guidance;
-      d.prediction_type = dpm->prediction_type; d.solver_order = dpm->solver_order;
-      d.final_first_order = dpm->final_first_order; d.emulate_bf16 = dpm->emulate_bf16;
-      d.x0_prev = x0_prev; d.lower_order_nums = lower_order_nums; d.lower_order_nums_out = wb.order_tmp;
-      d.out = latents;  // each element is read and written by the same thread
-      if (int rc = cfg_dpm_step_run(d, wb.ts_tmp, stream)) return rc;
-      D4D_CUDA_OK(cudaMemcpyAsync(lower_order_nums, wb.order_tmp, sizeof(int) * F, cudaMemcpyDeviceToDevice, stream));
-    } else {
-      DdimArgs d;
-      d.noise = wb.noise; d.latents = latents; d.mask = mask; d.timestep_indices = ts_idx;
-      d.timesteps_table = timesteps_table; d.alphas_cumprod = ddim->alphas_cumprod;
-      d.n_steps = ddim->n_steps; d.T = ddim->num_train_timesteps; d.final_alpha_cumprod = ddim->final_alpha_cumprod;
-      d.F = F; d.chw = 4 * hw; d.hw = hw; d.cfg = cfg_on ? 1 : 0; d.guidance = guidance;
-      d.prediction_type = ddim->prediction_type; d.clip_sample = ddim->clip_sample; d.clip_range = ddim->clip_sample_range;
-      d.emulate_bf16 = ddim->emulate_bf16; d.out = wb.latents_tmp;
-      if (int rc = cfg_ddim_step_run(d, wb.ts_tmp, stream)) return rc;
-      D4D_CUDA_OK(cudaMemcpyAsync(latents, wb.latents_tmp, sizeof(bf16) * F * 4 * hw, cudaMemcpyDeviceToDevice, stream));
-    }
+    if (int rc = scheduler_step(step, wb, latents, mask, ts_idx, F, hw, cfg_on, guidance, stream)) return rc;
     D4D_CUDA_OK(cudaMemcpyAsync(ts_idx, wb.ts_tmp, sizeof(long long) * F, cudaMemcpyDeviceToDevice, stream));
   }
   return 0;

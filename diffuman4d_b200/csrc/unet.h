@@ -88,8 +88,21 @@ struct WindowBufs {  // scratch of d4d_denoise_window for one (F, h, w, cfg)
   bf16* noise = nullptr;
   bf16* latents_tmp = nullptr;
   long long* ts_tmp = nullptr;
-  int* order_tmp = nullptr;  // DPM-Solver++ only (allocated on first use)
+  int* order_tmp = nullptr;  // multistep schedulers only (allocated on first use)
   ~WindowBufs();
+};
+
+// The scheduler of a window step: exactly one of the tables is set.  The multistep schedulers (DPM-Solver++, UniPC) also
+// get the window frames' solver state, read and updated in place: x0_prev [F,4,h,w] and lower_order_nums [F] for both,
+// and for UniPC last_sample [F,4,h,w] and, at solver_order 2, x0_prev2 [F,4,h,w].  Unused members are null.
+struct WindowStep {
+  const d4d_sched* ddim = nullptr;
+  const d4d_dpm_sched* dpm = nullptr;
+  const d4d_unipc_sched* unipc = nullptr;
+  bf16* x0_prev = nullptr;
+  bf16* x0_prev2 = nullptr;
+  bf16* last_sample = nullptr;
+  int* lower_order_nums = nullptr;
 };
 
 struct Exchange {  // K/V exchange buffers in peer memory (cudaIpc), two parities
@@ -115,13 +128,11 @@ class Model {
               bool pose_shared_neg = false);
   int exchange_alloc(size_t kv_bytes, unsigned char* handles_out /* 3 x 64 bytes */);
   int exchange_open(int rank, int world, const unsigned char* all_handles /* world x 3 x 64 bytes */);
-  // num_steps x (assemble -> UNet -> CFG + scheduler step) on the window's F frames; latents and ts_idx are updated in
-  // place.  The scheduler is DDIM (ddim) or DPM-Solver++ (dpm, the other one null); with DPM-Solver++ x0_prev [F,4,h,w]
-  // and lower_order_nums [F] are the frames' solver state, also updated in place.
+  // num_steps x (assemble -> UNet -> CFG + scheduler step) on the window's F frames; latents, ts_idx and the solver state
+  // of `step` are updated in place.
   int denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
-                     long long* ts_idx, const d4d_sched* ddim, const d4d_dpm_sched* dpm, bf16* x0_prev,
-                     int* lower_order_nums, float guidance, int domain, int F, int h, int w, int num_steps,
-                     cudaStream_t stream, int F_total);
+                     long long* ts_idx, const WindowStep& step, float guidance, int domain, int F, int h, int w,
+                     int num_steps, cudaStream_t stream, int F_total);
   // frame-sharded sliding loop: this rank's F updated frames (+ DPM-Solver++ state when x0_prev != nullptr) to every rank,
   // one flag round (one more exchange of the epoch sequence), then the gathered F_total frames to the *_out buffers
   int window_exchange(const bf16* latents, const long long* ts_idx, const bf16* x0_prev, const int* lower_order_nums, int F,

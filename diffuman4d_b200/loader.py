@@ -19,7 +19,7 @@ from typing import Callable, List, Optional, Union
 
 import torch
 
-from .config import DPMSolverConfig, SchedulerConfig, UNetConfig
+from .config import DPMSolverConfig, SchedulerConfig, UNetConfig, UniPCConfig
 from .pipeline import B200Diffuman4DPipeline
 from .unet import B200MultiviewUNet
 
@@ -103,14 +103,63 @@ def dpm_solver_config_from_json(d: dict) -> DPMSolverConfig:
         steps_offset=d.get("steps_offset", 0))
 
 
-def scheduler_config_from_json(d: dict) -> Union[SchedulerConfig, DPMSolverConfig]:
+def unipc_config_from_json(d: dict) -> UniPCConfig:
+    """Map a diffusers ``UniPCMultistepScheduler`` config; every knob the fused step does not implement raises
+    ``NotImplementedError`` naming the key."""
+    def refuse(key, why):
+        raise NotImplementedError(f"UniPCMultistepScheduler {key}={d.get(key)!r} is not supported by the CUDA path "
+                                  f"({why})")
+
+    def want(key, allowed, default):
+        v = d.get(key, default)
+        if v not in allowed:
+            refuse(key, f"supported: {allowed}")
+        return v
+
+    if not d.get("predict_x0", True):
+        refuse("predict_x0", "only the data-prediction (predict_x0=True) form is implemented")
+    if d.get("solver_p") is not None:
+        refuse("solver_p", "only UniPC's own predictor")
+    if d.get("thresholding", False):
+        refuse("thresholding", "dynamic thresholding is not implemented")
+    for key in ("use_karras_sigmas", "use_exponential_sigmas", "use_beta_sigmas", "use_flow_sigmas"):
+        if d.get(key, False):
+            refuse(key, "sigmas come straight from the beta schedule")
+    if d.get("rescale_betas_zero_snr", False):
+        refuse("rescale_betas_zero_snr", "zero-SNR rescaling is not implemented")
+    if d.get("trained_betas") is not None:
+        refuse("trained_betas", "betas come from beta_schedule")
+    order = want("solver_order", (1, 2), 2)
+    solver_type = want("solver_type", ("bh1", "bh2"), "bh2")
+    want("beta_schedule", ("linear", "scaled_linear"), "linear")
+    want("prediction_type", ("epsilon", "v_prediction", "sample"), "epsilon")
+    final = want("final_sigmas_type", ("zero", "sigma_min"), "zero")
+    want("timestep_spacing", ("linspace", "leading", "trailing"), "linspace")
+    lower_order_final = d.get("lower_order_final", True)
+    if final == "zero" and order == 2 and not lower_order_final:
+        refuse("final_sigmas_type", "'zero' with lower_order_final=False at solver_order 2: the last step's "
+                                    "second-order term divides by an infinite h")
+    if final == "zero" and solver_type == "bh1":
+        refuse("final_sigmas_type", "'zero' with solver_type='bh1': the last step's B(h) = -h is infinite")
+    return UniPCConfig(
+        num_train_timesteps=d.get("num_train_timesteps", 1000), beta_start=d.get("beta_start", 0.0001),
+        beta_end=d.get("beta_end", 0.02), beta_schedule=d.get("beta_schedule", "linear"), solver_order=order,
+        prediction_type=d.get("prediction_type", "epsilon"), solver_type=solver_type,
+        lower_order_final=lower_order_final, disable_corrector=tuple(d.get("disable_corrector") or ()),
+        final_sigmas_type=final, timestep_spacing=d.get("timestep_spacing", "linspace"),
+        steps_offset=d.get("steps_offset", 0))
+
+
+def scheduler_config_from_json(d: dict) -> Union[SchedulerConfig, DPMSolverConfig, UniPCConfig]:
     cls = d.get("_class_name", "DDIMScheduler")
     if cls == "DPMSolverMultistepScheduler":
         return dpm_solver_config_from_json(d)
+    if cls == "UniPCMultistepScheduler":
+        return unipc_config_from_json(d)
     if cls != "DDIMScheduler":
         raise NotImplementedError(
-            f"scheduler {cls} is not fused on the CUDA path (DDIMScheduler and DPMSolverMultistepScheduler only); "
-            "run the reference's Python scheduler loop for other classes")
+            f"scheduler {cls} is not fused on the CUDA path (DDIMScheduler, DPMSolverMultistepScheduler and "
+            "UniPCMultistepScheduler only); run the reference's Python scheduler loop for other classes")
     if d.get("thresholding", False):
         raise NotImplementedError("dynamic thresholding is not supported")
     return SchedulerConfig(

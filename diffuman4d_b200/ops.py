@@ -310,3 +310,29 @@ def cfg_dpm_step(noise: torch.Tensor, latents: torch.Tensor, cond_mask: torch.Te
                                  _p(lower_order_nums), _p(lon_out), C.byref(sched), float(guidance_scale), int(cfg), F, h, w,
                                  _p(out), _stream()), "d4d_cfg_dpm_step")
     return out, ti_out, lon_out
+
+
+def cfg_unipc_step(noise: torch.Tensor, latents: torch.Tensor, cond_mask: torch.Tensor, timestep_indices: torch.Tensor,
+                   x0_prev: torch.Tensor, x0_prev2: Optional[torch.Tensor], last_sample: torch.Tensor,
+                   lower_order_nums: torch.Tensor, sched, guidance_scale: float, cfg: bool):
+    """One CFG + UniPC step of F frames (``sched``: a ``d4d_unipc_sched`` from ``UniPCTables.c_struct``).  ``noise``
+    [(cfg?2:1)*F,4,h,w]; ``x0_prev``, ``x0_prev2`` (None at solver_order 1) and ``last_sample`` [F,4,h,w] bf16 are updated
+    in place.  Returns (new latents, advanced timestep indices, advanced ``lower_order_nums``)."""
+    _bf16c(noise, "noise"), _bf16c(latents, "latents"), _bf16c(cond_mask, "cond_mask")
+    F, _, h, w = latents.shape
+    for name, t in (("x0_prev", x0_prev), ("x0_prev2", x0_prev2), ("last_sample", last_sample)):
+        if t is not None:
+            _bf16c(t, name)
+            if t.shape != latents.shape:
+                raise ValueError(f"{name} must have the shape of latents")
+    if lower_order_nums.dtype != torch.int32 or not lower_order_nums.is_cuda or lower_order_nums.numel() != F:
+        raise ValueError("lower_order_nums must be a CUDA int32 [F] tensor")
+    if timestep_indices.dtype != torch.int64 or not timestep_indices.is_cuda or timestep_indices.numel() != F:
+        raise ValueError("timestep_indices must be a CUDA int64 [F] tensor")
+    out = torch.empty_like(latents)
+    ti_out = torch.empty_like(timestep_indices)
+    lon_out = torch.empty_like(lower_order_nums)
+    check(lib().d4d_cfg_unipc_step(_p(noise), _p(latents), _p(cond_mask), _p(timestep_indices), _p(ti_out), _p(x0_prev),
+                                   _p(x0_prev2), _p(last_sample), _p(lower_order_nums), _p(lon_out), C.byref(sched),
+                                   float(guidance_scale), int(cfg), F, h, w, _p(out), _stream()), "d4d_cfg_unipc_step")
+    return out, ti_out, lon_out

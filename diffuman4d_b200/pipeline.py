@@ -4,8 +4,9 @@ Seams (SURVEY.md section 8b):
   B-3  ``denoise_window``  == ``Diffuman4DPipeline.__call__`` with latents given
        (reference src/diffusers/pipelines/diffuman4d/pipeline_diffuman4d.py:345-425): input assembly, UNet, CFG
        combine and the F per-frame scheduler steps run as ONE C-ABI call (no per-frame host sync).  The scheduler is DDIM
-       (``SchedulerConfig``) or DPM-Solver++ (``DPMSolverConfig``); the latter keeps a per-frame history on the device
-       (``DPMSolverState``) in place of the reference's per-frame scheduler copies.
+       (``SchedulerConfig``), DPM-Solver++ (``DPMSolverConfig``) or UniPC (``UniPCConfig``); the multistep ones keep a
+       per-frame history on the device (``DPMSolverState`` / ``UniPCState``) in place of the reference's per-frame
+       scheduler copies.
   B-4  ``sliding_iterative_denoise`` == PIPE:439-559: same arguments, same ValueErrors, same returned dict.  The VAE
        (stock AutoencoderKL, out of scope per SURVEY section 8f) is pluggable: pass ``vae`` with ``encode_latents(x)`` /
        ``decode_latents(z)`` callables, or feed latents directly (``pixel_values_latents=...``).
@@ -21,8 +22,8 @@ from typing import Callable, List, Optional, Union
 import torch
 
 from ._lib import check, lib
-from .config import DPMSolverConfig, SchedulerConfig
-from .scheduler import DDIMTables, DPMSolverFrame, DPMSolverState, DPMSolverTables
+from .config import DPMSolverConfig, SchedulerConfig, UniPCConfig
+from .scheduler import DDIMTables, DPMSolverFrame, DPMSolverState, DPMSolverTables, UniPCState, UniPCTables
 from .unet import _DOMAIN_IDS, B200MultiviewUNet
 
 
@@ -63,7 +64,8 @@ def resize_conditions(plucker_embeds: torch.Tensor, cond_masks: torch.Tensor, h:
 
 
 class B200Diffuman4DPipeline:
-    def __init__(self, unet: B200MultiviewUNet, scheduler_config: Union[SchedulerConfig, DPMSolverConfig, None] = None,
+    def __init__(self, unet: B200MultiviewUNet,
+                 scheduler_config: Union[SchedulerConfig, DPMSolverConfig, UniPCConfig, None] = None,
                  vae=None, emulate_bf16_scheduler: bool = False):
         self.unet = unet
         self.vae = vae
@@ -71,6 +73,8 @@ class B200Diffuman4DPipeline:
         self.dtype = torch.bfloat16
         if isinstance(scheduler_config, DPMSolverConfig):
             self.scheduler = DPMSolverTables(scheduler_config, device=self.device)
+        elif isinstance(scheduler_config, UniPCConfig):
+            self.scheduler = UniPCTables(scheduler_config, device=self.device)
         else:
             self.scheduler = DDIMTables(scheduler_config, device=self.device)
         self.emulate_bf16_scheduler = emulate_bf16_scheduler
@@ -93,15 +97,15 @@ class B200Diffuman4DPipeline:
 
     @property
     def _multistep(self) -> bool:
-        return isinstance(self.scheduler, DPMSolverTables)
+        return isinstance(self.scheduler, (DPMSolverTables, UniPCTables))
 
     def parepare_schedulers(self, num_inference_steps: int, num_frames: int):
         """PIPE:265-271.  The per-frame deep copies exist in the reference only because scheduler objects are
-        stateful; DDIM is stateless, so one table serves all frames.  DPM-Solver++ gets a fresh (zeroed) device state for
-        the frames, and one ``DPMSolverFrame`` handle per frame in place of each copy."""
+        stateful; DDIM is stateless, so one table serves all frames.  DPM-Solver++ and UniPC get a fresh (zeroed) device
+        state for the frames, and one ``DPMSolverFrame`` handle per frame in place of each copy."""
         ts = self.scheduler.set_timesteps(num_inference_steps)
         if self._multistep:
-            return DPMSolverState(num_frames, self.device).frames(), ts
+            return self.scheduler.new_state(num_frames).frames(), ts
         return [self.scheduler] * num_frames, ts
 
     # B-3 -----------------------------------------------------------------------------------------------
@@ -109,8 +113,9 @@ class B200Diffuman4DPipeline:
                        cond_masks_latents, timestep_indices, domain: str, guidance_scale: float,
                        num_inference_steps: int = 1, solver_state: Optional[DPMSolverState] = None):
         """One window: ``num_inference_steps`` x (assemble -> UNet -> CFG -> per-frame scheduler step).  ``latents``
-        [F,4,h,w] and ``timestep_indices`` [F] (int64, device) are updated IN PLACE and returned.  With DPM-Solver++,
-        ``solver_state`` is the window frames' ``DPMSolverState`` (``DPMSolverState.take``), also updated in place."""
+        [F,4,h,w] and ``timestep_indices`` [F] (int64, device) are updated IN PLACE and returned.  With DPM-Solver++ or
+        UniPC, ``solver_state`` is the window frames' ``DPMSolverState`` / ``UniPCState`` (``take``), also updated in
+        place."""
         return self._window_step(latents=latents, pixel_values_latents=pixel_values_latents,
                                  plucker_embeds_latents=plucker_embeds_latents, skeletons_latents=skeletons_latents,
                                  cond_masks_latents=cond_masks_latents, timestep_indices=timestep_indices, domain=domain,
@@ -123,6 +128,9 @@ class B200Diffuman4DPipeline:
                      F_total: Optional[int] = None):
         """``denoise_window``'s checks and library call.  ``F_total`` given: the tensors hold this rank's frames of a
         frame-sharded window of ``F_total`` frames (``FrameShardedPipeline.denoise_window``)."""
+        unipc = isinstance(self.scheduler, UniPCTables)
+        if unipc and F_total is not None:
+            raise NotImplementedError("the frame-sharded window does not run the UniPC scheduler")
         if domain not in _DOMAIN_IDS:
             raise ValueError(f"Invalid domain for temporal embedding: {domain}")
         dev = self.device
@@ -150,15 +158,27 @@ class B200Diffuman4DPipeline:
         if self._multistep:
             st = solver_state
             if st is None:
-                raise ValueError("the DPM-Solver++ scheduler needs the window frames' solver_state")
-            if not (st.x0_prev is not None and st.x0_prev.is_cuda and st.x0_prev.dtype == torch.bfloat16
-                    and st.x0_prev.is_contiguous() and st.x0_prev.shape == latents.shape):
-                raise ValueError("solver_state.x0_prev must be a contiguous CUDA bfloat16 tensor shaped like latents")
+                raise ValueError(f"the {'UniPC' if unipc else 'DPM-Solver++'} scheduler needs the window frames' "
+                                 "solver_state")
+
+            def state_tensor(name):
+                t = getattr(st, name, None)
+                if not (t is not None and t.is_cuda and t.dtype == torch.bfloat16 and t.is_contiguous()
+                        and t.shape == latents.shape):
+                    raise ValueError(f"solver_state.{name} must be a contiguous CUDA bfloat16 tensor shaped like latents")
+                return t.data_ptr()
+
+            x0_prev = state_tensor("x0_prev")
             lon = st.lower_order_nums
             if not (lon.is_cuda and lon.dtype == torch.int32 and lon.is_contiguous() and lon.numel() == F_):
                 raise ValueError("solver_state.lower_order_nums must be a contiguous CUDA int32 [F] tensor")
-            args += [st.x0_prev.data_ptr(), lon.data_ptr()]
-            name = "d4d_denoise_window_dpm" if F_total is None else "d4d_denoise_window_dpm_sharded"
+            if unipc:
+                x0_prev2 = state_tensor("x0_prev2") if self.scheduler.config.solver_order == 2 else None
+                args += [x0_prev, x0_prev2, state_tensor("last_sample"), lon.data_ptr()]
+                name = "d4d_denoise_window_unipc"
+            else:
+                args += [x0_prev, lon.data_ptr()]
+                name = "d4d_denoise_window_dpm" if F_total is None else "d4d_denoise_window_dpm_sharded"
         else:
             name = "d4d_denoise_window" if F_total is None else "d4d_denoise_window_sharded"
         with torch.cuda.device(dev):

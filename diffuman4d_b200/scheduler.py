@@ -1,4 +1,4 @@
-"""Host-side scheduler tables for the fused CFG + scheduler-step kernels: DDIM and DPM-Solver++.
+"""Host-side scheduler tables for the fused CFG + scheduler-step kernels: DDIM, DPM-Solver++ and UniPC.
 
 Mirrors what the reference obtains from ``self.scheduler.set_timesteps(n)`` + per-frame deep copies
 (pipeline_diffuman4d.py:265-271) for upstream diffusers==0.33.1 ``DDIMScheduler``: the ``timesteps`` vector and
@@ -8,6 +8,8 @@ runs on the GPU (csrc/elementwise.cu ``cfg_ddim_kernel``).
 ``DPMSolverTables`` does the same for ``DPMSolverMultistepScheduler`` (dpmsolver++ / midpoint, order 1 or 2): the timesteps,
 the sigma table and the per-step solver coefficients (``cfg_dpm_kernel``).  That scheduler is stateful, which is why the
 reference deep-copies it per frame; here the state of every frame of a task is a ``DPMSolverState`` on the device.
+``UniPCTables`` / ``UniPCState`` do the same for ``UniPCMultistepScheduler`` (``cfg_unipc_kernel``), whose corrector also
+needs each frame's previous sample and, at order 2, a second data prediction of history.
 """
 from __future__ import annotations
 
@@ -16,8 +18,8 @@ import ctypes as C
 import numpy as np
 import torch
 
-from ._lib import D4DDpmSched, D4DSched
-from .config import DPMSolverConfig, SchedulerConfig
+from ._lib import D4DDpmSched, D4DSched, D4DUniPCSched
+from .config import DPMSolverConfig, SchedulerConfig, UniPCConfig
 
 _PRED = {"epsilon": 0, "v_prediction": 1, "sample": 2}
 
@@ -177,6 +179,9 @@ class DPMSolverTables:
         return bool(c.euler_at_final or (c.lower_order_final and self.num_inference_steps < 15)
                     or c.final_sigmas_type == "zero")
 
+    def new_state(self, num_frames: int) -> "DPMSolverState":
+        return DPMSolverState(num_frames, self.device)
+
     def c_struct(self, emulate_bf16: bool = False) -> D4DDpmSched:
         if self.timesteps is None:
             raise ValueError("call set_timesteps first")
@@ -230,8 +235,157 @@ class DPMSolverState:
 
 
 class DPMSolverFrame:
-    """Frame ``index`` of a task's ``DPMSolverState`` (the per-frame scheduler object of the reference's lists)."""
+    """Frame ``index`` of a task's ``DPMSolverState`` or ``UniPCState`` (the per-frame scheduler object of the reference's
+    lists)."""
     __slots__ = ("state", "index")
 
     def __init__(self, state: DPMSolverState, index: int):
         self.state, self.index = state, index
+
+
+# ---- UniPC ------------------------------------------------------------------------------------------------------------
+UNIPC_COEFS = 14   # row layout in include/d4d.h ``d4d_unipc_sched``
+
+
+def unipc_step_coefficients(c: UniPCConfig, sigmas: torch.Tensor) -> torch.Tensor:
+    """[n, 14] fp32 coefficients of the n steps over ``sigmas`` [n+1] (layout in include/d4d.h ``d4d_unipc_sched``), each
+    evaluated on 0-dim fp32 tensors in the order ``UniPCMultistepScheduler``'s ``convert_model_output`` /
+    ``multistep_uni_p_bh_update`` / ``multistep_uni_c_bh_update`` / ``step`` evaluate them."""
+    def alpha_sigma(sigma):
+        alpha_t = 1 / ((sigma ** 2 + 1) ** 0.5)
+        return alpha_t, sigma * alpha_t
+
+    def lam(j):
+        a, s = alpha_sigma(sigmas[j])
+        return torch.log(a) - torch.log(s)
+
+    def bh(t, s0, si):
+        alpha_t, sigma_t = alpha_sigma(sigmas[t])
+        h = lam(t) - lam(s0)
+        rk = (lam(si) - lam(s0)) / h if si is not None else torch.tensor(0.0)
+        hh = -h
+        h_phi_1 = torch.expm1(hh)
+        B_h = hh if c.solver_type == "bh1" else torch.expm1(hh)
+        return sigma_t / alpha_sigma(sigmas[s0])[1], alpha_t * h_phi_1, alpha_t * B_h, rk, hh, h_phi_1, B_h
+
+    n = sigmas.numel() - 1
+    zero = torch.tensor(0.0)
+    out = torch.zeros(n, UNIPC_COEFS, dtype=torch.float32)
+    for i in range(n):
+        alpha_s, sigma_s = alpha_sigma(sigmas[i])
+        p_ratio, p_cphi, p_cB, p_rk = bh(i + 1, i, i - 1 if i > 0 else None)[:4]
+        c_ratio = c_cphi = c_cB = c_rk = rho0 = rho1 = zero
+        if i > 0:
+            c_ratio, c_cphi, c_cB, c_rk, hh, h_phi_1, B_h = bh(i, i - 1, i - 2 if i > 1 else None)
+            if i > 1:   # torch.linalg.solve(R, b) of the order-2 corrector
+                rks = torch.stack([c_rk, torch.ones(())])
+                h_phi_k = h_phi_1 / hh - 1
+                factorial_i = 1
+                R, b = [], []
+                for k in range(1, 3):
+                    R.append(torch.pow(rks, k - 1))
+                    b.append(h_phi_k * factorial_i / B_h)
+                    factorial_i *= k + 1
+                    h_phi_k = h_phi_k / hh - 1 / factorial_i
+                rho0, rho1 = torch.linalg.solve(torch.stack(R), torch.stack(b))
+        corrector = float(i > 0 and (i - 1) not in c.disable_corrector)
+        order_cap = float(min(c.solver_order, n - i) if c.lower_order_final else c.solver_order)
+        out[i] = torch.stack([alpha_s, sigma_s, p_ratio, p_cphi, p_cB, p_rk, c_ratio, c_cphi, c_cB, c_rk, rho0, rho1,
+                              torch.tensor(corrector), torch.tensor(order_cap)])
+    return out
+
+
+class UniPCTables:
+    """Timesteps, sigmas and step coefficients of ``UniPCMultistepScheduler`` (diffusers 0.33.1) for
+    ``cfg_unipc_kernel``."""
+    init_noise_sigma = 1.0  # upstream: init_noise_sigma 1, scale_model_input is the identity
+
+    def __init__(self, cfg: UniPCConfig = None, device="cuda:0"):
+        self.config = cfg or UniPCConfig()
+        c = self.config
+        if c.prediction_type not in _PRED:
+            raise ValueError(f"prediction_type given as {c.prediction_type} must be one of {list(_PRED)}")
+        if c.solver_order not in (1, 2):
+            raise NotImplementedError(f"solver_order={c.solver_order}: the fused step implements orders 1 and 2")
+        if c.solver_type not in ("bh1", "bh2"):
+            raise ValueError(f"solver_type {c.solver_type!r} must be 'bh1' or 'bh2'")
+        if c.final_sigmas_type not in ("zero", "sigma_min"):
+            raise ValueError(f"final_sigmas_type {c.final_sigmas_type!r} must be 'zero' or 'sigma_min'")
+        if c.final_sigmas_type == "zero" and c.solver_order == 2 and not c.lower_order_final:
+            raise NotImplementedError("final_sigmas_type='zero' with lower_order_final=False at solver_order 2: the last "
+                                      "step's second-order term divides by an infinite h")
+        if c.final_sigmas_type == "zero" and c.solver_type == "bh1":
+            raise NotImplementedError("final_sigmas_type='zero' with solver_type='bh1': the last step's B(h) = -h is "
+                                      "infinite and upstream returns NaN")
+        self.alphas_cumprod = torch.cumprod(1.0 - _betas(c), dim=0)
+        self.all_sigmas = ((1 - self.alphas_cumprod) / self.alphas_cumprod) ** 0.5   # fp32 [T]
+        self.device = torch.device(device)
+        self.num_inference_steps = None
+        self.timesteps = None          # host int64 [n]
+        self.sigmas = None             # host fp32 [n+1]
+        self.coefs = None              # host fp32 [n, 14]
+        self._dev = None
+
+    def set_timesteps(self, n: int, device=None):
+        c = self.config
+        ts = dpm_timesteps(c, n)       # UniPC spaces its timesteps like DPM-Solver++
+        last = 0.0 if c.final_sigmas_type == "zero" else float(self.all_sigmas[0])
+        self.num_inference_steps = n
+        self.timesteps = torch.from_numpy(ts)
+        self.sigmas = torch.cat([self.all_sigmas[self.timesteps], torch.tensor([last], dtype=torch.float32)])
+        self.coefs = unipc_step_coefficients(c, self.sigmas)
+        self._dev = None
+        return self.timesteps
+
+    def new_state(self, num_frames: int) -> "UniPCState":
+        return UniPCState(num_frames, self.device, self.config.solver_order)
+
+    def c_struct(self, emulate_bf16: bool = False) -> D4DUniPCSched:
+        if self.timesteps is None:
+            raise ValueError("call set_timesteps first")
+        if self._dev is None:
+            self._dev = (self.timesteps.to(self.device), self.coefs.to(self.device).contiguous())
+        c = self.config
+        s = D4DUniPCSched()
+        s.timesteps_table = self._dev[0].data_ptr()
+        s.coefs = self._dev[1].data_ptr()
+        s.n_steps = int(self.num_inference_steps)
+        s.prediction_type = _PRED[c.prediction_type]
+        s.solver_order = int(c.solver_order)
+        s.emulate_bf16 = int(emulate_bf16)
+        return s
+
+
+class UniPCState(DPMSolverState):
+    """The UniPC history of every frame of one task, on the device: ``DPMSolverState``'s ``x0_prev`` and
+    ``lower_order_nums``, plus ``x0_prev2`` [F,4,h,w] bf16 (the data prediction before ``x0_prev``; order 2 only, else
+    None) and ``last_sample`` [F,4,h,w] bf16 (the sample each frame's last predictor started from, after correction).  A
+    new task starts from zeros, the state of a freshly deep-copied upstream scheduler."""
+
+    def __init__(self, num_frames: int, device, solver_order: int = 2, x0_prev: torch.Tensor = None,
+                 lower_order_nums: torch.Tensor = None, x0_prev2: torch.Tensor = None, last_sample: torch.Tensor = None):
+        super().__init__(num_frames, device, x0_prev, lower_order_nums)
+        self.solver_order = solver_order
+        self.x0_prev2 = x0_prev2
+        self.last_sample = last_sample
+
+    def _ensure(self, h: int, w: int):
+        super()._ensure(h, w)
+        if self.last_sample is None:
+            self.last_sample = torch.zeros_like(self.x0_prev)
+        if self.solver_order == 2 and self.x0_prev2 is None:
+            self.x0_prev2 = torch.zeros_like(self.x0_prev)
+
+    def take(self, index: torch.Tensor, h: int, w: int) -> "UniPCState":
+        self._ensure(h, w)
+        index = index.to(self.device)
+        g = lambda t: None if t is None else t[index].contiguous()
+        return UniPCState(len(index), self.device, self.solver_order, g(self.x0_prev), g(self.lower_order_nums),
+                          g(self.x0_prev2), g(self.last_sample))
+
+    def put(self, index: torch.Tensor, window: "UniPCState"):
+        super().put(index, window)
+        index = index.to(self.device)
+        self.last_sample[index] = window.last_sample
+        if self.x0_prev2 is not None:
+            self.x0_prev2[index] = window.x0_prev2

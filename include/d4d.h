@@ -83,6 +83,32 @@ typedef struct d4d_dpm_sched {
   int32_t emulate_bf16;             /* 1: round like the reference's bf16 eager maths (history and x0 in bf16) */
 } d4d_dpm_sched;
 
+/* UniPC constants for the fused step (upstream diffusers UniPCMultistepScheduler with predict_x0, solver_type "bh1" or
+ * "bh2", solver_order 1 or 2, no solver_p; d4d_version() 107 and later).  The solver's history is per frame and lives on
+ * the device (x0_prev / x0_prev2 / last_sample / lower_order_nums of d4d_denoise_window_unipc); a frame's step index is
+ * its timestep index.  Step i runs the corrector (UniC) of the frame's previous step when lower_order_nums >= 1 and row
+ * i enables it, at order lower_order_nums, then the predictor (UniP) at order min(row i's cap, lower_order_nums + 1).
+ * coefs row i (fp32), computed on the host in the upstream scheduler's fp32 order of operations (the device evaluates no
+ * log / exp / solve), with alpha_j = 1 / sqrt(sigma_j^2 + 1), sigma'_j = sigma_j * alpha_j, lambda_j = log alpha_j -
+ * log sigma'_j, h_j = lambda_(j+1) - lambda_j, hphi1(h) = expm1(-h), B(h) = -h ("bh1") or expm1(-h) ("bh2"):
+ *   [0] alpha_i   [1] sigma'_i                                               (convert_model_output)
+ *   [2] sigma'_(i+1) / sigma'_i   [3] alpha_(i+1) * hphi1(h_i)   [4] alpha_(i+1) * B(h_i)
+ *   [5] rk = (lambda_(i-1) - lambda_i) / h_i (0 in row 0)                    (predictor)
+ *   [6] sigma'_i / sigma'_(i-1)   [7] alpha_i * hphi1(h_(i-1))   [8] alpha_i * B(h_(i-1))
+ *   [9] rk' = (lambda_(i-2) - lambda_(i-1)) / h_(i-1) (0 in rows 0, 1)       (corrector; all 0 in row 0)
+ *   [10] rho0  [11] rho1: solve(R, b) of the order-2 corrector in fp32 (0 in rows 0, 1; the bf16-emulating step rounds
+ *        them to bf16 like upstream's cast to the sample dtype)
+ *   [12] 1 if the corrector runs at step i (i > 0 and i - 1 not in disable_corrector), else 0
+ *   [13] the predictor's order cap: min(solver_order, n_steps - i) with lower_order_final, else solver_order */
+typedef struct d4d_unipc_sched {
+  const int64_t* timesteps_table;   /* device, [n_steps]  (scheduler.timesteps after set_timesteps) */
+  const float* coefs;               /* device, [n_steps][14], see above */
+  int32_t n_steps;
+  int32_t prediction_type;          /* 0 epsilon, 1 v_prediction, 2 sample */
+  int32_t solver_order;             /* 1 or 2 */
+  int32_t emulate_bf16;             /* 1: round like the reference's bf16 eager maths (history, x0 and every op in bf16) */
+} d4d_unipc_sched;
+
 const char* d4d_last_error(void);
 int d4d_version(void);
 
@@ -140,6 +166,19 @@ int d4d_denoise_window_dpm(d4d_handle* h, void* latents, const void* pixel_laten
                            const d4d_dpm_sched* sched, float guidance_scale, int domain, int F, int height, int width,
                            int num_steps, void* x0_prev, int32_t* lower_order_nums, void* stream);
 
+/* The same window step with a UniPC scheduler (d4d_version() 107 and later).  Arguments as d4d_denoise_window, plus the
+ * window frames' solver state, read and updated in place (conditioning frames keep theirs; zeros for a new task):
+ *   x0_prev           device bf16 [F,4,h,w]: each frame's data prediction of its previous step
+ *   x0_prev2          device bf16 [F,4,h,w]: the one before (solver_order 2; NULL exactly when solver_order is 1)
+ *   last_sample       device bf16 [F,4,h,w]: the sample each frame's last predictor started from, after correction
+ *   lower_order_nums  device int32 [F]: steps each frame has taken, capped at solver_order
+ * A caller carries them across the windows of one task, gathered and scattered with the frames like the latents. */
+int d4d_denoise_window_unipc(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                             const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                             const d4d_unipc_sched* sched, float guidance_scale, int domain, int F, int height, int width,
+                             int num_steps, void* x0_prev, void* x0_prev2, void* last_sample, int32_t* lower_order_nums,
+                             void* stream);
+
 /* ---- building blocks of B-3, exported for parity tests ------------------------------------------------ */
 int d4d_assemble_input(void* latents, const void* pixel_latents, const void* plucker, const void* skel_latents,
                        const void* cond_mask, const int64_t* timestep_indices, const int64_t* timesteps_table,
@@ -155,6 +194,13 @@ int d4d_cfg_dpm_step(const void* noise, const void* latents, const void* cond_ma
                      int64_t* timestep_indices_out, void* x0_prev, const int32_t* lower_order_nums,
                      int32_t* lower_order_nums_out, const d4d_dpm_sched* sched, float guidance_scale, int cfg, int F,
                      int height, int width, void* latents_out, void* stream);
+/* One CFG + UniPC step of the frames (d4d_version() 107 and later; state as d4d_denoise_window_unipc).  x0_prev, x0_prev2
+ * and last_sample are updated in place; lower_order_nums_out and timestep_indices_out receive the advanced counters (they
+ * may not alias the inputs); latents_out may alias latents. */
+int d4d_cfg_unipc_step(const void* noise, const void* latents, const void* cond_mask, const int64_t* timestep_indices,
+                       int64_t* timestep_indices_out, void* x0_prev, void* x0_prev2, void* last_sample,
+                       const int32_t* lower_order_nums, int32_t* lower_order_nums_out, const d4d_unipc_sched* sched,
+                       float guidance_scale, int cfg, int F, int height, int width, void* latents_out, void* stream);
 
 /* ---- op-level entry points (each is one hot-path kernel; used by tests/ and bench.py) ------------------
  * d4d_op_gemm:   out[M,N] = act((A|A2)[M,K1+K2] . W[N,K]^T + bias + rowvec[row/rows_per_image]) * scale + residual

@@ -1,10 +1,11 @@
-"""What the DPM-Solver++ step costs against DDIM in the window step of bench.py's workload (W16 @ 64x64 latents, CFG 2.0,
-SD-2.1 channel layout, random weights), on one GPU in one process.
+"""What the DPM-Solver++ and UniPC steps cost against DDIM in the window step of bench.py's workload (W16 @ 64x64 latents,
+CFG 2.0, SD-2.1 channel layout, random weights), on one GPU in one process.
 
-Both pipelines share one UNet; rounds alternate DDIM and DPM-Solver++ so that clock drift hits both alike.  Each step
-restores its inputs (latents, timestep indices and, for DPM-Solver++, the frames' solver state) from device copies and
-then makes ONE public ``denoise_window`` call; the DPM-Solver++ frames start with a history, so the timed step is the
-second-order one.  Also times the two fused step kernels alone.  Prints one JSON line (and writes it to --out) with the
+The three pipelines share one UNet; rounds alternate DDIM, DPM-Solver++ and UniPC so that clock drift hits all alike.  Each
+step restores its inputs (latents, timestep indices and, for the multistep schedulers, the frames' solver state) from
+device copies and then makes ONE public ``denoise_window`` call.  The multistep frames start with a full history, so the
+timed step is the second-order one; the UniPC target frames also sit two steps further into the schedule, so that both
+its corrector and its predictor run at order 2.  Also times the three fused step kernels alone.  Prints one JSON line (and writes it to --out) with the
 card's name, power limit and max SM clock beside the numbers.
 
     python tools/scheduler_step_cost.py --rounds 8 --steps 10 --out /tmp/scheduler_step_cost.json
@@ -37,9 +38,9 @@ def main():
     from bench import WORKLOAD, gpu_identity, synth_inputs
     from diffuman4d_b200 import ops
     from diffuman4d_b200._lib import check, lib
-    from diffuman4d_b200.config import DPMSolverConfig, SchedulerConfig, UNetConfig
+    from diffuman4d_b200.config import DPMSolverConfig, SchedulerConfig, UNetConfig, UniPCConfig
     from diffuman4d_b200.pipeline import B200Diffuman4DPipeline
-    from diffuman4d_b200.scheduler import DPMSolverState
+    from diffuman4d_b200.scheduler import DPMSolverState, UniPCState
     from diffuman4d_b200.unet import B200MultiviewUNet
     from diffuman4d_b200.weights import random_state_dict
 
@@ -51,8 +52,9 @@ def main():
     unet = B200MultiviewUNet(cfg, 0).load_state_dict(random_state_dict(cfg, seed=1))
     ddim = B200Diffuman4DPipeline(unet, SchedulerConfig())
     dpm = B200Diffuman4DPipeline(unet, DPMSolverConfig())
-    ddim.parepare_schedulers(wl["n_steps"], F)
-    dpm.parepare_schedulers(wl["n_steps"], F)
+    unipc = B200Diffuman4DPipeline(unet, UniPCConfig())
+    for p in (ddim, dpm, unipc):
+        p.parepare_schedulers(wl["n_steps"], F)
 
     inp = {k: (v.to(torch.bfloat16) if v.dtype.is_floating_point else v).to(dev)
            for k, v in synth_inputs(F, n_cond, h, w).items()}
@@ -61,12 +63,23 @@ def main():
     x0_init = torch.randn(F, 4, h, w, device=dev, generator=g).to(torch.bfloat16)
     lon_init = torch.full((F,), 1, dtype=torch.int32, device=dev)          # every frame has a history: second order
     state = DPMSolverState(F, dev).take(torch.arange(F), h, w)
+    ts_unipc = inp["ts"].clone()
+    ts_unipc[n_cond:] += 2                                                 # rows with an order-2 corrector
+    lon2_init = torch.full((F,), 2, dtype=torch.int32, device=dev)
+    x0_init2 = torch.randn(F, 4, h, w, device=dev, generator=g).to(torch.bfloat16)
+    last_init = torch.randn(F, 4, h, w, device=dev, generator=g).to(torch.bfloat16)
+    state_u = UniPCState(F, dev).take(torch.arange(F), h, w)
 
-    def window(p, solver_state=None):
+    def window(p, solver_state=None, ts_init=inp["ts"]):
         def step():
             lat.copy_(inp["latents"])
-            ts.copy_(inp["ts"])
-            if solver_state is not None:
+            ts.copy_(ts_init)
+            if isinstance(solver_state, UniPCState):
+                solver_state.x0_prev2.copy_(x0_init2)
+                solver_state.last_sample.copy_(last_init)
+                solver_state.x0_prev.copy_(x0_init)
+                solver_state.lower_order_nums.copy_(lon2_init)
+            elif solver_state is not None:
                 solver_state.x0_prev.copy_(x0_init)
                 solver_state.lower_order_nums.copy_(lon_init)
             p.denoise_window(latents=lat, pixel_values_latents=inp["pixel"], plucker_embeds_latents=inp["plucker"],
@@ -76,10 +89,12 @@ def main():
 
     # the two fused step kernels alone, on the window's shapes (CFG noise [2F,4,h,w])
     noise = torch.randn(2 * F, 4, h, w, device=dev, generator=g).to(torch.bfloat16)
-    ddim_s, dpm_s = ddim.scheduler.c_struct(), dpm.scheduler.c_struct()
+    ddim_s, dpm_s, unipc_s = ddim.scheduler.c_struct(), dpm.scheduler.c_struct(), unipc.scheduler.c_struct()
     out = torch.empty_like(lat)
     ts_out = torch.empty_like(ts)
     x0_k, lon_k = x0_init.clone(), lon_init.clone()
+    x0_u, x02_u, last_u, lon_u = x0_init.clone(), x0_init2.clone(), last_init.clone(), lon2_init.clone()
+    ts_u = ts_unipc.clone()
     stream = lambda: torch.cuda.current_stream().cuda_stream
 
     def ddim_kernel():
@@ -90,6 +105,9 @@ def main():
     def dpm_kernel():
         ops.cfg_dpm_step(noise, lat, inp["mask"], ts, x0_k, lon_k, dpm_s, wl["guidance"], True)
 
+    def unipc_kernel():
+        ops.cfg_unipc_step(noise, lat, inp["mask"], ts_u, x0_u, x02_u, last_u, lon_u, unipc_s, wl["guidance"], True)
+
     def timed(fn, n):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
@@ -99,27 +117,31 @@ def main():
         torch.cuda.synchronize()
         return e0.elapsed_time(e1) / n
 
-    arms = {"ddim": window(ddim), "dpm_solver++": window(dpm, state)}
+    arms = {"ddim": window(ddim), "dpm_solver++": window(dpm, state), "unipc": window(unipc, state_u, ts_unipc)}
     for fn in arms.values():                                             # warm-up: plans, buffers, clocks
         for _ in range(3):
             fn()
     torch.cuda.synchronize()
     per_round = {k: [] for k in arms}
-    kernel = {"ddim": [], "dpm_solver++": []}
+    kernel = {"ddim": [], "dpm_solver++": [], "unipc": []}
     for _ in range(args.rounds):
         for k, fn in arms.items():
             per_round[k].append(timed(fn, args.steps))
         kernel["ddim"].append(timed(ddim_kernel, args.kernel_iters))
         kernel["dpm_solver++"].append(timed(dpm_kernel, args.kernel_iters))
+        kernel["unipc"].append(timed(unipc_kernel, args.kernel_iters))
     med = {k: statistics.median(v) for k, v in per_round.items()}
     kmed = {k: statistics.median(v) for k, v in kernel.items()}
     res = {"workload": wl["name"], "gpu": gpu_identity(0), "rounds": args.rounds, "steps_per_round": args.steps,
            "window_step_ms_median": med, "window_step_ms_rounds": per_round,
            "dpm_minus_ddim_ms": med["dpm_solver++"] - med["ddim"],
            "dpm_over_ddim": med["dpm_solver++"] / med["ddim"],
+           "unipc_minus_ddim_ms": med["unipc"] - med["ddim"],
+           "unipc_minus_dpm_ms": med["unipc"] - med["dpm_solver++"],
            "step_kernel_us_median": {k: 1e3 * v for k, v in kmed.items()},
-           "note": "DPM-Solver++ step timed in its second-order branch (every frame has a history); the kernel-only "
-                   "DPM time includes the op wrapper's output allocations"}
+           "note": "DPM-Solver++ and UniPC steps timed in their second-order branches (every frame has a full history, "
+                   "UniPC corrects at order 2); the kernel-only DPM and UniPC times include the op wrappers' output "
+                   "allocations"}
     line = json.dumps(res)
     print(line)
     if args.out:
