@@ -86,7 +86,7 @@ d4d::WindowStep dpm_step(const d4d_dpm_sched* sched, void* x0_prev, int32_t* low
 extern "C" {
 
 const char* d4d_last_error(void) { return d4d::g_last_error.c_str(); }
-int d4d_version(void) { return 107; }
+int d4d_version(void) { return 108; }
 
 int d4d_create(const d4d_config* cfg, int device, d4d_handle** out) {
   D4D_API_BEGIN
@@ -360,6 +360,34 @@ int d4d_op_conv3x3(const void* x_nhwc, int n_img, int H, int W, int Cin, const v
   d4d::GemmLaunch L;
   if (int rc = d4d::gemm_prepare(d, &L)) return rc;
   return d4d::gemm_run(L, static_cast<cudaStream_t>(stream));
+  D4D_API_END
+}
+
+int d4d_op_conv_tiled(const void* x_nhwc, int n_img, int H, int W, int Cin, const void* Wt, int Cout, const float* bias,
+                      const void* rowvec, int ld_rowvec, const void* residual, int act, void* out, int kind, int block_m,
+                      int block_n, int64_t* stats, void* stream) {
+  D4D_API_BEGIN
+  D4D_REQUIRE(n_img > 0 && H > 0 && W > 0 && (kind == 0 || kind == 1 || kind == 3), "conv_tiled arguments");
+  d4d::GemmDesc d;
+  d.conv = 1; d.conv_kind = kind; d.A = static_cast<const bf16*>(x_nhwc); d.n_img = n_img; d.H = H; d.W = W; d.Cin = Cin;
+  d.Wt = static_cast<const bf16*>(Wt); d.N = Cout; d.bias = bias;
+  d.rowvec = static_cast<const bf16*>(rowvec); d.ld_rowvec = ld_rowvec;
+  d.residual = static_cast<const bf16*>(residual); d.ld_res = Cout;
+  d.out = static_cast<bf16*>(out); d.ldo = Cout; d.act = act; d.block_m = block_m; d.block_n = block_n;
+  d.stats = reinterpret_cast<long long*>(stats);
+  d4d::GemmLaunch L;
+  if (int rc = d4d::gemm_prepare(d, &L)) return rc;
+  return d4d::gemm_run(L, static_cast<cudaStream_t>(stream));
+  D4D_API_END
+}
+
+int d4d_conv_tile_choice(int n_img, int H, int W, int Cin, int Cout, int kind, int sms, int* block_m, int* block_n) {
+  D4D_API_BEGIN
+  D4D_REQUIRE(n_img > 0 && H > 0 && W > 0 && Cin > 0 && kind >= 0 && kind <= 3 && sms > 0 && block_m && block_n,
+              "conv_tile_choice arguments");
+  d4d::GemmDesc d;
+  d.conv = 1; d.conv_kind = kind; d.n_img = n_img; d.H = H; d.W = W; d.Cin = Cin; d.N = Cout;
+  return d4d::gemm_choose_tile(d, sms, block_m, block_n);
   D4D_API_END
 }
 

@@ -4,8 +4,10 @@
 //
 // * operands are bf16, K-major, staged by TMA into 128B-swizzled shared memory (mbarrier ring, as deep as fits)
 // * three warpgroups: warpgroup 0 is the TMA producer (one thread; it hands most of its registers to the others), and
-//   warpgroups 1 and 2 each own 64 rows of the 128-row tile and issue wgmma.m64nBNk16 with fp32 accumulators in
-//   registers.  The kernel is persistent (grid = #SMs) and walks tiles n-fastest, so CTAs that run concurrently share
+//   warpgroups 1 and 2 each own 64 MI rows of the 128 MI-row tile (MI = 1, or 2 for the larger convs) and issue MI
+//   wgmma.m64nBNk16 per k16 slice against one B descriptor, with fp32 accumulators in registers: at MI = 2 a weight tile
+//   feeds twice the rows, which cuts the operand bytes a CTA pulls from L2 per FLOP from 1/128 + 1/BN to 1/256 + 1/BN and
+//   halves the TMA issues and mbarrier round trips per FLOP.  The kernel is persistent (grid = #SMs) and walks tiles n-fastest, so CTAs that run concurrently share
 //   the same A rows through L2; the producer runs ahead into the next tile while the MMA warpgroups run the epilogue.
 // * plain GEMMs stage the epilogue in shared memory: each MMA warpgroup writes its finished 64 x BN bf16 rows into 32-column
 //   slabs (64B-swizzled, conflict-free), and one thread TMA-stores them and goes on into the next tile's MMAs while the
@@ -31,7 +33,7 @@ namespace {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;
-constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
+constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB per 128 rows; a stage holds MI of them
 constexpr int BAR_BYTES = 1024;                 // barrier block in front of the ring keeps the stages 1024-B aligned
 constexpr int NUM_THREADS = 384;                // warpgroup 0: TMA producer, warpgroups 1-2: MMA + epilogue
 constexpr int MAX_SMEM = 227 * 1024;
@@ -40,11 +42,11 @@ constexpr int MAX_SMEM = 227 * 1024;
 constexpr int SLAB_COLS = 32;
 constexpr int SLAB_BYTES = 64 * SLAB_COLS * 2;
 
-// Tile width BN (the wgmma N) is a template parameter; after the staging slabs of both warpgroups (plain GEMM only), the
-// ring takes as many stages as fit (at most 8).
-template <int BN, bool kStaged>
+// Tile width BN (the wgmma N) and the m64 blocks per warpgroup MI (tile rows = 128 MI) are template parameters; after the
+// staging slabs of both warpgroups (plain GEMM only), the ring takes as many stages as fit (at most 8).
+template <int BN, int MI, bool kStaged>
 struct GemmCfg {
-  static constexpr int STAGE_BYTES = A_BYTES + BN * BLOCK_K * 2;
+  static constexpr int STAGE_BYTES = MI * A_BYTES + BN * BLOCK_K * 2;
   static constexpr int STAGING_BYTES = kStaged ? 2 * 64 * BN * 2 : 0;
   static constexpr int STAGES_FIT = (MAX_SMEM - 1024 - BAR_BYTES - STAGING_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;
@@ -106,13 +108,14 @@ enum : int { E_BIAS = 1, E_ROWVEC = 2, E_ACT = 4, E_RES = 8, E_STATS = 16, E_KV 
 // range), and so do the E_KV kernels (they serve the K/V scatter and, as E_ALL, the rare feature sets no other kernel has).
 __host__ __device__ constexpr bool gemm_staged(bool conv, int epi) { return !conv && !(epi & E_KV); }
 
-template <int BN, bool kGeglu, bool kConv, int kEpi>
+template <int BN, int MI, bool kGeglu, bool kConv, int kEpi>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_a2,
                   const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ CUtensorMap tmap_c,
                   const __grid_constant__ CUtensorMap tmap_r, const GemmKernelArgs a) {
   constexpr bool kStaged = gemm_staged(kConv, kEpi);
-  using Cfg = GemmCfg<BN, kStaged>;
+  static_assert(MI == 1 || (kConv && MI == 2), "256-row tiles: conv mode only (a plain tile is 128 rows, as are its staging slabs)");
+  using Cfg = GemmCfg<BN, MI, kStaged>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment for the 128B swizzle atoms
@@ -146,7 +149,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     // ===================== TMA producer =====================
     setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
-      const uint32_t tx_bytes = A_BYTES + static_cast<uint32_t>(a.block_n) * BLOCK_K * 2;
+      const uint32_t tx_bytes = MI * A_BYTES + static_cast<uint32_t>(a.block_n) * BLOCK_K * 2;
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -158,7 +161,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         for (int kb = 0; kb < a.k_blocks; ++kb) {
           mbar_wait(&empty[stage], phase ^ 1);
           uint8_t* sa = ring + stage * Cfg::STAGE_BYTES;
-          uint8_t* sb = sa + A_BYTES;
+          uint8_t* sb = sa + MI * A_BYTES;
           mbar_expect_tx(&full[stage], tx_bytes);
           if (!kConv) {
             if (kb < a.kb_split) tma_load_2d(sa, &tmap_a, &full[stage], kb * BLOCK_K, tc.m0);
@@ -180,10 +183,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 
   // ===================== MMA warpgroups + epilogue =====================
   setmaxnreg_inc<232>();
-  const int wg = (warp >> 2) - 1;   // 0 / 1: rows [64 wg, 64 wg + 64) of the tile
-  const int wq = warp & 3;          // warp within the warpgroup: rows 16 wq .. 16 wq + 15 of the warpgroup's 64
+  const int wg = (warp >> 2) - 1;   // 0 / 1: rows [64 MI wg, 64 MI (wg + 1)) of the tile, as MI blocks of 64
+  const int wq = warp & 3;          // warp within the warpgroup: rows 16 wq .. 16 wq + 15 of each 64-row block
   const bool wg_leader = (threadIdx.x & 127) == 0;
-  const int r_base = wg * 64 + wq * 16 + (lane >> 2);  // tile rows r_base and r_base + 8 belong to this thread
+  const int r_base = wg * 64 * MI + wq * 16 + (lane >> 2);  // tile rows r_base + 64 mi and + 8 belong to this thread
   const int c_base = 2 * (lane & 3);                   // columns 8j + c_base, +1 of fragment j
   const uint32_t ring_u32 = smem_u32(ring);
   // staged epilogue: this warpgroup's slabs, and the offset of this thread's (row r_base, columns c_base, +1) in a slab; the
@@ -191,7 +194,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   // (lane >> 3) & 3: the 8 rows of a warp store land in 8 different chunks, 32 different banks
   const bool staged = kStaged && a.staged;
   uint8_t* stg = ring + STAGES * Cfg::STAGE_BYTES + wg * 64 * BN * 2;
-  const uint32_t stg_u32 = smem_u32(stg) + (r_base - wg * 64) * 64 + c_base * 2;
+  const uint32_t stg_u32 = smem_u32(stg) + (r_base - wg * 64 * MI) * 64 + c_base * 2;
   const int stg_xor = (lane >> 3) & 3;
   const bool has_res = (kEpi & E_RES) && !kGeglu && a.residual != nullptr;
   const int out_cols = kGeglu ? a.N / 2 : a.N;
@@ -199,7 +202,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 
   int stage = 0;
   uint32_t phase = 0;
-  float acc[BN / 2];
+  float acc[MI][BN / 2];
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
     const int m_tile = tile / a.n_tiles;
     const int n_tile = tile % a.n_tiles;
@@ -217,8 +220,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     int prev_stage = -1;
     for (int kb = 0; kb < a.k_blocks; ++kb) {
       mbar_wait(&full[stage], phase);
-      const uint32_t sa = ring_u32 + stage * Cfg::STAGE_BYTES + wg * 64 * 128;
-      const uint32_t sb = ring_u32 + stage * Cfg::STAGE_BYTES + A_BYTES;
+      const uint32_t sa = ring_u32 + stage * Cfg::STAGE_BYTES + wg * MI * 64 * 128;
+      const uint32_t sb = ring_u32 + stage * Cfg::STAGE_BYTES + MI * A_BYTES;
       const uint64_t adesc = make_wgmma_desc(sa, 16, 1024);
       const uint64_t bdesc = make_wgmma_desc(sb, 16, 1024);
       wgmma_fence();
@@ -226,11 +229,16 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       for (int k = 0; k < BLOCK_K / 16; ++k) {
         // advancing 16 bf16 along K inside the 128B swizzle atom = +32 bytes = +2 in the (addr >> 4) field
         const int scale_d = (kb | k) != 0 ? 1 : 0;
-        if constexpr (BN == 64) wgmma_ss_n64(acc, adesc + 2 * k, bdesc + 2 * k, scale_d);
-        else if constexpr (BN == 128) wgmma_ss_n128(acc, adesc + 2 * k, bdesc + 2 * k, scale_d);
-        else if constexpr (BN == 160) wgmma_ss_n160(acc, adesc + 2 * k, bdesc + 2 * k, scale_d);
-        else if constexpr (BN == 192) wgmma_ss_n192(acc, adesc + 2 * k, bdesc + 2 * k, scale_d);
-        else wgmma_ss_n256(acc, adesc + 2 * k, bdesc + 2 * k, scale_d);
+#pragma unroll
+        for (int mi = 0; mi < MI; ++mi) {
+          // the warpgroup's next 64 rows: + 64 * 128 bytes = + 512 in the (addr >> 4) field; same B descriptor
+          const uint64_t ad = adesc + 512 * mi + 2 * k, bd = bdesc + 2 * k;
+          if constexpr (BN == 64) wgmma_ss_n64(acc[mi], ad, bd, scale_d);
+          else if constexpr (BN == 128) wgmma_ss_n128(acc[mi], ad, bd, scale_d);
+          else if constexpr (BN == 160) wgmma_ss_n160(acc[mi], ad, bd, scale_d);
+          else if constexpr (BN == 192) wgmma_ss_n192(acc[mi], ad, bd, scale_d);
+          else wgmma_ss_n256(acc[mi], ad, bd, scale_d);
+        }
       }
       wgmma_commit();
       if (kb == 0 && staged && wg_leader) {
@@ -250,15 +258,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
     wgmma_wait<0>();
-    wgmma_fence_regs(acc);
+#pragma unroll
+    for (int mi = 0; mi < MI; ++mi) wgmma_fence_regs(acc[mi]);
     if (wg_leader) mbar_arrive(&empty[prev_stage]);
 
     // ---- epilogue: into the staging slabs, or straight from the accumulator registers to global memory
-    long long rows[2];
-    int imgs[2];
-    bool valid[2];
-    row_of<kConv>(a, tc, r_base, rows[0], imgs[0], valid[0]);
-    row_of<kConv>(a, tc, r_base + 8, rows[1], imgs[1], valid[1]);
     if (staged) {
       named_barrier_sync(1 + wg, 128);  // orders the slab writes below after the leader's bulk_wait_group_read
       if (has_res && stg_live) {
@@ -271,98 +275,108 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       return stg_u32 + h * 8 * 64 + (j >> 2) * SLAB_BYTES + (((j & 3) ^ stg_xor) << 4);
     };
 
-    if constexpr (kGeglu) {
-      // tile columns 16p .. 16p+7 are the a half, 16p+8 .. 16p+15 the g half of output columns n0/2 + 8p .. + 7
-      const bool has_bias = (kEpi & E_BIAS) && a.bias != nullptr;
+    // one pass per 64-row block of the warpgroup; a warp's 16 rows and their statistics are those of a 128-row tile
 #pragma unroll
-      for (int p = 0; p < BN / 16; ++p) {
-        if (16 * p >= a.block_n || n0 + 16 * p >= a.N) break;
-        float2 ba = make_float2(0.f, 0.f), bg = make_float2(0.f, 0.f);
-        if (has_bias) {
-          ba = __ldg(reinterpret_cast<const float2*>(a.bias + n0 + 16 * p + c_base));
-          bg = __ldg(reinterpret_cast<const float2*>(a.bias + n0 + 16 * p + 8 + c_base));
+    for (int mi = 0; mi < MI; ++mi) {
+      float (&accm)[BN / 2] = acc[mi];
+      long long rows[2];
+      int imgs[2];
+      bool valid[2];
+      row_of<kConv>(a, tc, r_base + 64 * mi, rows[0], imgs[0], valid[0]);
+      row_of<kConv>(a, tc, r_base + 64 * mi + 8, rows[1], imgs[1], valid[1]);
+      if constexpr (kGeglu) {
+        // tile columns 16p .. 16p+7 are the a half, 16p+8 .. 16p+15 the g half of output columns n0/2 + 8p .. + 7
+        const bool has_bias = (kEpi & E_BIAS) && a.bias != nullptr;
+#pragma unroll
+        for (int p = 0; p < BN / 16; ++p) {
+          if (16 * p >= a.block_n || n0 + 16 * p >= a.N) break;
+          float2 ba = make_float2(0.f, 0.f), bg = make_float2(0.f, 0.f);
+          if (has_bias) {
+            ba = __ldg(reinterpret_cast<const float2*>(a.bias + n0 + 16 * p + c_base));
+            bg = __ldg(reinterpret_cast<const float2*>(a.bias + n0 + 16 * p + 8 + c_base));
+          }
+          const int ocol = n0 / 2 + 8 * p + c_base;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            if (!valid[h]) continue;
+            const float a0 = accm[8 * p + 2 * h] + ba.x, a1 = accm[8 * p + 2 * h + 1] + ba.y;
+            const float g0 = accm[8 * p + 4 + 2 * h] + bg.x, g1 = accm[8 * p + 4 + 2 * h + 1] + bg.y;
+            const uint32_t o = pack_bf16x2(a0 * gelu_erf_f(g0), a1 * gelu_erf_f(g1));
+            if (staged) st_shared_u32(stg_addr(p, h), o);  // output column 8p + c_base of the tile: fragment p
+            else *reinterpret_cast<uint32_t*>(a.out + static_cast<size_t>(rows[h]) * a.ldo + ocol) = o;
+          }
         }
-        const int ocol = n0 / 2 + 8 * p + c_base;
+      } else {
+        const bool has_bias = (kEpi & E_BIAS) && a.bias != nullptr, has_rv = (kEpi & E_ROWVEC) && a.rowvec != nullptr;
+        const bool has_stats = (kEpi & E_STATS) && a.stats != nullptr;
+        const bool has_act = (kEpi & E_ACT) && a.act == 1, has_scale = (kEpi & E_ACT) && a.out_scale != 1.0f;
+        const bool has_kv = (kEpi & E_KV) && a.kv_world > 0;
+        // statistics: the 16 rows of a warp lie in ONE image (gemm_prepare checks it); the warp's first row has the
+        // smallest (x, y, image) / token index, so when it is outside the tensor the whole warp is
+        const long long row0 = __shfl_sync(0xffffffffu, rows[0], 0);
+        const bool stats_on = has_stats && __shfl_sync(0xffffffffu, valid[0] ? 1 : 0, 0);
+        const int stats_img = !kConv ? static_cast<int>(row0 / a.stats_rows) : __shfl_sync(0xffffffffu, imgs[0], 0);
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          if (!valid[h]) continue;
-          const float a0 = acc[8 * p + 2 * h] + ba.x, a1 = acc[8 * p + 2 * h + 1] + ba.y;
-          const float g0 = acc[8 * p + 4 + 2 * h] + bg.x, g1 = acc[8 * p + 4 + 2 * h + 1] + bg.y;
-          const uint32_t o = pack_bf16x2(a0 * gelu_erf_f(g0), a1 * gelu_erf_f(g1));
-          if (staged) st_shared_u32(stg_addr(p, h), o);  // output column 8p + c_base of the tile: fragment p
-          else *reinterpret_cast<uint32_t*>(a.out + static_cast<size_t>(rows[h]) * a.ldo + ocol) = o;
-        }
-      }
-    } else {
-      const bool has_bias = (kEpi & E_BIAS) && a.bias != nullptr, has_rv = (kEpi & E_ROWVEC) && a.rowvec != nullptr;
-      const bool has_stats = (kEpi & E_STATS) && a.stats != nullptr;
-      const bool has_act = (kEpi & E_ACT) && a.act == 1, has_scale = (kEpi & E_ACT) && a.out_scale != 1.0f;
-      const bool has_kv = (kEpi & E_KV) && a.kv_world > 0;
-      // statistics: the 16 rows of a warp lie in ONE image (gemm_prepare checks it); the warp's first row has the
-      // smallest (x, y, image) / token index, so when it is outside the tensor the whole warp is
-      const long long row0 = __shfl_sync(0xffffffffu, rows[0], 0);
-      const bool stats_on = has_stats && __shfl_sync(0xffffffffu, valid[0] ? 1 : 0, 0);
-      const int stats_img = !kConv ? static_cast<int>(row0 / a.stats_rows) : __shfl_sync(0xffffffffu, imgs[0], 0);
+        for (int j = 0; j < BN / 8; ++j) {
+          const int cl = 8 * j + c_base;
+          const int col = n0 + cl;
+          if (8 * j >= a.block_n || n0 + 8 * j >= a.N) break;  // (warp-uniform: N and block_n are multiples of 16)
+          float2 b2 = make_float2(0.f, 0.f);
+          if (has_bias) b2 = __ldg(reinterpret_cast<const float2*>(a.bias + col));
+          float sv[2][2];
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int cl = 8 * j + c_base;
-        const int col = n0 + cl;
-        if (8 * j >= a.block_n || n0 + 8 * j >= a.N) break;  // (warp-uniform: N and block_n are multiples of 16)
-        float2 b2 = make_float2(0.f, 0.f);
-        if (has_bias) b2 = __ldg(reinterpret_cast<const float2*>(a.bias + col));
-        float sv[2][2];
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          sv[h][0] = sv[h][1] = 0.f;
-          if (!valid[h]) continue;
-          float f0 = acc[4 * j + 2 * h] + b2.x, f1 = acc[4 * j + 2 * h + 1] + b2.y;
-          if (has_rv) {
-            const float2 v = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(a.rowvec + static_cast<size_t>(imgs[h]) * a.ld_rowvec + col));
-            f0 += v.x; f1 += v.y;
-          }
-          if (has_act) { f0 = silu_f(f0); f1 = silu_f(f1); }
-          if (has_scale) { f0 *= a.out_scale; f1 *= a.out_scale; }
-          if (has_res) {  // plain load: the residual may alias the output (in-place add)
-            const float2 v = unpack_bf16x2(staged ? ld_shared_u32(stg_addr(j, h))
-                                                  : *reinterpret_cast<const uint32_t*>(a.residual + static_cast<size_t>(rows[h]) * a.ld_res + col));
-            f0 += v.x; f1 += v.y;
-          }
-          const uint32_t o = pack_bf16x2(f0, f1);
-          if (has_stats) {  // statistics of what is stored: the rounded values
-            const float2 rv = unpack_bf16x2(o);
-            sv[h][0] = rv.x; sv[h][1] = rv.y;
-          }
-          if (has_kv && col >= a.kv_col0) {
-            // fused all-gather: the K|V columns of the QKV projection go straight into every rank's gathered K/V buffer
-            // (peer memory over NVLink; own rank included) at this rank's global token rows
-            const long long half = rows[h] / a.kv_rows_local;
-            const long long grow = half * a.kv_rows_global + a.kv_row_offset + (rows[h] - half * a.kv_rows_local);
-            const size_t off = static_cast<size_t>(grow) * a.kv_ld + (col - a.kv_col0);
+          for (int h = 0; h < 2; ++h) {
+            sv[h][0] = sv[h][1] = 0.f;
+            if (!valid[h]) continue;
+            float f0 = accm[4 * j + 2 * h] + b2.x, f1 = accm[4 * j + 2 * h + 1] + b2.y;
+            if (has_rv) {
+              const float2 v = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(a.rowvec + static_cast<size_t>(imgs[h]) * a.ld_rowvec + col));
+              f0 += v.x; f1 += v.y;
+            }
+            if (has_act) { f0 = silu_f(f0); f1 = silu_f(f1); }
+            if (has_scale) { f0 *= a.out_scale; f1 *= a.out_scale; }
+            if (has_res) {  // plain load: the residual may alias the output (in-place add)
+              const float2 v = unpack_bf16x2(staged ? ld_shared_u32(stg_addr(j, h))
+                                                    : *reinterpret_cast<const uint32_t*>(a.residual + static_cast<size_t>(rows[h]) * a.ld_res + col));
+              f0 += v.x; f1 += v.y;
+            }
+            const uint32_t o = pack_bf16x2(f0, f1);
+            if (has_stats) {  // statistics of what is stored: the rounded values
+              const float2 rv = unpack_bf16x2(o);
+              sv[h][0] = rv.x; sv[h][1] = rv.y;
+            }
+            if (has_kv && col >= a.kv_col0) {
+              // fused all-gather: the K|V columns of the QKV projection go straight into every rank's gathered K/V buffer
+              // (peer memory over NVLink; own rank included) at this rank's global token rows
+              const long long half = rows[h] / a.kv_rows_local;
+              const long long grow = half * a.kv_rows_global + a.kv_row_offset + (rows[h] - half * a.kv_rows_local);
+              const size_t off = static_cast<size_t>(grow) * a.kv_ld + (col - a.kv_col0);
 #pragma unroll 1
-            for (int rk = 0; rk < a.kv_world; ++rk) *reinterpret_cast<uint32_t*>(a.kv_dst[rk] + off) = o;
-          } else if (staged) {
-            st_shared_u32(stg_addr(j, h), o);
-          } else {
-            *reinterpret_cast<uint32_t*>(a.out + static_cast<size_t>(rows[h]) * a.ldo + col) = o;
+              for (int rk = 0; rk < a.kv_world; ++rk) *reinterpret_cast<uint32_t*>(a.kv_dst[rk] + off) = o;
+            } else if (staged) {
+              st_shared_u32(stg_addr(j, h), o);
+            } else {
+              *reinterpret_cast<uint32_t*>(a.out + static_cast<size_t>(rows[h]) * a.ldo + col) = o;
+            }
           }
-        }
-        if (has_stats) {
-          // column sums over the warp's 16 rows: lanes with equal lane % 4 hold the same two columns
-          float s0 = sv[0][0] + sv[1][0], s1 = sv[0][1] + sv[1][1];
-          float q0 = sv[0][0] * sv[0][0] + sv[1][0] * sv[1][0], q1 = sv[0][1] * sv[0][1] + sv[1][1] * sv[1][1];
+          if (has_stats) {
+            // column sums over the warp's 16 rows: lanes with equal lane % 4 hold the same two columns
+            float s0 = sv[0][0] + sv[1][0], s1 = sv[0][1] + sv[1][1];
+            float q0 = sv[0][0] * sv[0][0] + sv[1][0] * sv[1][0], q1 = sv[0][1] * sv[0][1] + sv[1][1] * sv[1][1];
 #pragma unroll
-          for (int m = 4; m < 32; m <<= 1) {
-            s0 += __shfl_xor_sync(0xffffffffu, s0, m);
-            s1 += __shfl_xor_sync(0xffffffffu, s1, m);
-            q0 += __shfl_xor_sync(0xffffffffu, q0, m);
-            q1 += __shfl_xor_sync(0xffffffffu, q1, m);
-          }
-          if (stats_on && lane < 4) {  // fixed point: integer adds commute, the result is independent of tile order
-            unsigned long long* st = reinterpret_cast<unsigned long long*>(a.stats) + (static_cast<size_t>(stats_img) * a.N + col) * 2;
-            atomicAdd(st + 0, static_cast<unsigned long long>(__float2ll_rn(s0 * kGnSumScale)));
-            atomicAdd(st + 1, static_cast<unsigned long long>(__float2ll_rn(q0 * kGnSqScale)));
-            atomicAdd(st + 2, static_cast<unsigned long long>(__float2ll_rn(s1 * kGnSumScale)));
-            atomicAdd(st + 3, static_cast<unsigned long long>(__float2ll_rn(q1 * kGnSqScale)));
+            for (int m = 4; m < 32; m <<= 1) {
+              s0 += __shfl_xor_sync(0xffffffffu, s0, m);
+              s1 += __shfl_xor_sync(0xffffffffu, s1, m);
+              q0 += __shfl_xor_sync(0xffffffffu, q0, m);
+              q1 += __shfl_xor_sync(0xffffffffu, q1, m);
+            }
+            if (stats_on && lane < 4) {  // fixed point: integer adds commute, the result is independent of tile order
+              unsigned long long* st = reinterpret_cast<unsigned long long*>(a.stats) + (static_cast<size_t>(stats_img) * a.N + col) * 2;
+              atomicAdd(st + 0, static_cast<unsigned long long>(__float2ll_rn(s0 * kGnSumScale)));
+              atomicAdd(st + 1, static_cast<unsigned long long>(__float2ll_rn(q0 * kGnSqScale)));
+              atomicAdd(st + 2, static_cast<unsigned long long>(__float2ll_rn(s1 * kGnSumScale)));
+              atomicAdd(st + 3, static_cast<unsigned long long>(__float2ll_rn(q1 * kGnSqScale)));
+            }
           }
         }
       }
@@ -383,6 +397,70 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 
 }  // namespace
 
+namespace {
+
+// conv: the grid of output positions per image and the sub-pixel phases of one launch
+void conv_out_grid(const GemmDesc& d, int* oh, int* ow, int* phases) {
+  *oh = d.conv_kind == 1 ? d.H / 2 : d.H;
+  *ow = d.conv_kind == 1 ? d.W / 2 : d.W;
+  *phases = d.conv_kind == 3 ? 4 : 1;
+}
+
+// conv: the spatial tile BW x BH x BN_img = `rows` output positions on an oh x ow grid, and the tiles per phase.  H, W need
+// not be powers of two: the tile may overhang, TMA zero-fills and the epilogue masks
+struct ConvTile { int bw, bh, bn_img; long long tiles; };
+ConvTile conv_tile(int rows, int n_img, int oh, int ow) {
+  ConvTile t;
+  t.bw = 16; while (t.bw > ow) t.bw >>= 1;
+  t.bh = rows / t.bw; while (t.bh > oh && t.bh > 1) t.bh >>= 1;
+  t.bn_img = rows / (t.bw * t.bh);
+  t.tiles = static_cast<long long>((ow + t.bw - 1) / t.bw) * ((oh + t.bh - 1) / t.bh) * ((n_img + t.bn_img - 1) / t.bn_img);
+  return t;
+}
+
+}  // namespace
+
+// A k-block of a rows x bn tile does rows * bn * 64 multiply-adds on (rows + bn) * 128 operand bytes from L2, so the time of
+// a tile goes as rows * bn + kOperandWeight * (rows + bn); at 128 rows that is 256 * (bn + 64).  The weight is fitted to
+// the per-tile times of tools/conv_tile_sweep.py (DESIGN section 5).
+constexpr int kOperandWeight = 128;
+constexpr int kMinKBlocks256 = 16;
+
+int gemm_choose_tile(const GemmDesc& d, int sms, int* block_m, int* block_n) {
+  D4D_REQUIRE(d.block_m == 0 || d.block_m == 128 || d.block_m == 256, "block_m must be 0 (automatic), 128 or 256");
+  D4D_REQUIRE(d.block_m != 256 || d.conv, "256-row tiles: convolutions only (a plain GEMM stages a 128-row tile for its TMA store)");
+  D4D_REQUIRE(d.block_m != 256 || d.block_n <= 0 || d.block_n == 128 || d.block_n == 160,
+              "256-row tiles run at block_n 128 or 160 (the accumulators of wider tiles do not fit the register file)");
+  int oh = 0, ow = 0, phases = 1;
+  if (d.conv) conv_out_grid(d, &oh, &ow, &phases);
+  D4D_REQUIRE(!d.conv || (d.n_img > 0 && oh > 0 && ow > 0), "empty conv");
+  // rows 128 or 256 (convs at widths 128 / 160 with at least one tile per SM and at least kMinKBlocks256 k-blocks per tile:
+  // a shorter tile is bound by its register epilogue, and 64 -> 128 channels at 64x64 ran 40% slower at 256 rows), width 64, 128, 160, 192 or 256 (the last N
+  // tile may overhang; its extra columns are not stored): the pair with the fewest SM-waves of the persistent grid, weighted
+  // by the tile's time, plus the work of the padded columns; ties to the larger tile.  GEGLU keeps to widths whose halves
+  // fill whole 32-column store slabs.
+  long long best_cost = -1;
+  for (int r : {128, 256}) {
+    if (d.block_m > 0 ? r != d.block_m : (r == 256 && !d.conv)) continue;
+    const int k_blocks = d.conv ? (d.conv_kind >= 2 ? 4 : 9) * ((d.Cin + BLOCK_K - 1) / BLOCK_K) : 0;
+    const long long m_tiles = d.conv ? conv_tile(r, d.n_img, oh, ow).tiles * phases : (static_cast<long long>(d.M) + r - 1) / r;
+    for (int c : {64, 128, 160, 192, 256}) {
+      if (d.block_n > 0) c = d.block_n;
+      else if (d.geglu && c % 64 != 0) continue;
+      const long long n_tiles = (d.N + c - 1) / c, tiles = m_tiles * n_tiles;
+      const bool fits = r == 128 || ((c == 128 || c == 160) && (d.block_m == 256 || (tiles >= sms && k_blocks >= kMinKBlocks256)));
+      if (fits) {
+        const long long waves = (tiles + sms - 1) / sms;
+        const long long cost = waves * (static_cast<long long>(r) * c + kOperandWeight * (r + c)) + (n_tiles * c - d.N) * (r / 2);
+        if (best_cost < 0 || cost <= best_cost) { best_cost = cost; *block_m = r; *block_n = c; }
+      }
+      if (d.block_n > 0) break;
+    }
+  }
+  D4D_REQUIRE(best_cost >= 0, "no tile for this block_m / block_n");
+  return 0;
+}
+
 int gemm_prepare(const GemmDesc& d, GemmLaunch* L) {
   D4D_REQUIRE(d.N % 16 == 0, "GEMM N must be a multiple of 16");
   D4D_REQUIRE(d.out != nullptr && d.A != nullptr && d.Wt != nullptr, "null operand");
@@ -402,23 +480,12 @@ int gemm_prepare(const GemmDesc& d, GemmLaunch* L) {
   int dev = 0, sms = 0;
   D4D_CUDA_OK(cudaGetDevice(&dev));
   D4D_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  int bn = d.block_n;
-  if (bn <= 0) {
-    // tile width 64, 128, 160, 192 or 256 (the last N tile may overhang; its extra columns are not stored): the one with
-    // the fewest SM-waves of the persistent grid, weighted by the tile's work (cost ~ waves * (block_n + fixed per-tile
-    // work)), ties to the wider.  GEGLU keeps to widths whose halves fill whole 32-column store slabs.
-    const long long rows = d.conv ? static_cast<long long>(d.n_img) * d.H * d.W : d.M;
-    const long long m_tiles_est = (rows + BLOCK_M - 1) / BLOCK_M;
-    long long best_cost = -1;
-    for (int c : {64, 128, 160, 192, 256}) {
-      if (d.geglu && c % 64 != 0) continue;
-      const long long tiles = m_tiles_est * ((d.N + c - 1) / c);
-      const long long waves = (tiles + sms - 1) / sms;
-      const long long cost = waves * (c + 64) + (static_cast<long long>((d.N + c - 1) / c) * c - d.N) / 4;
-      if (best_cost < 0 || cost <= best_cost) { best_cost = cost; bn = c; }
-    }
-  }
-  D4D_REQUIRE(bn >= 16 && bn <= 256 && bn % 16 == 0 && (d.block_n <= 0 || d.N % bn == 0), "no valid block_n");
+  D4D_REQUIRE(d.block_n <= 0 || (d.block_n >= 16 && d.block_n <= 256 && d.block_n % 16 == 0 && d.N % d.block_n == 0),
+              "no valid block_n");
+  D4D_REQUIRE(!d.conv || (d.conv_kind >= 0 && d.conv_kind <= 3), "conv_kind");
+  int bm = 0, bn = 0;
+  if (int rc = gemm_choose_tile(d, sms, &bm, &bn)) return rc;
+  a.block_m = bm;
   a.block_n = bn;
   a.n_tiles = (d.N + bn - 1) / bn;
   a.N = d.N;
@@ -479,7 +546,6 @@ int gemm_prepare(const GemmDesc& d, GemmLaunch* L) {
     }
   } else {
     D4D_REQUIRE(d.Cin % 8 == 0, "conv Cin must be a multiple of 8");
-    D4D_REQUIRE(d.conv_kind >= 0 && d.conv_kind <= 3, "conv_kind");
     D4D_REQUIRE(d.conv_kind != 1 || (d.H % 2 == 0 && d.W % 2 == 0), "stride-2 conv needs even H, W");
     a.mode = 1;
     a.n_img = d.n_img; a.Cin = d.Cin;
@@ -510,18 +576,15 @@ int gemm_prepare(const GemmDesc& d, GemmLaunch* L) {
     a.cin_blocks = (d.Cin + BLOCK_K - 1) / BLOCK_K;
     a.k_blocks = a.n_taps * a.cin_blocks;
     a.kb_split = a.k_blocks;
-    // spatial tile: BW x BH x BN = 128 output positions
-    int bw = 16; while (bw > a.W) bw >>= 1;
-    int bh = 128 / bw; while (bh > a.H && bh > 1) bh >>= 1;
-    // H, W need not be powers of two: the tile may overhang, TMA zero-fills and the epilogue masks
-    int bnimg = 128 / (bw * bh);
-    D4D_REQUIRE(bw * bh * bnimg == 128 && bnimg <= 256, "conv tile shape");
+    // spatial tile: BW x BH x BN = block_m output positions, one 4-D TMA box
+    const ConvTile ct = conv_tile(bm, d.n_img, a.H, a.W);
+    const int bw = ct.bw, bh = ct.bh, bnimg = ct.bn_img;
+    D4D_REQUIRE(bw * bh * bnimg == bm && bnimg <= 256, "conv tile shape");
     D4D_REQUIRE(d.stats == nullptr || (bw * bh) % 32 == 0, "statistics need 32-row warps inside one image");
     a.BW = bw; a.BH = bh; a.BN = bnimg;
     a.tiles_x = (a.W + bw - 1) / bw;
     a.tiles_y = (a.H + bh - 1) / bh;
-    const int tiles_n = (d.n_img + bnimg - 1) / bnimg;
-    a.tiles_per_phase = a.tiles_x * a.tiles_y * tiles_n;
+    a.tiles_per_phase = static_cast<int>(ct.tiles);
     a.m_tiles = a.tiles_per_phase * a.n_phases;
     a.M *= a.n_phases;  // output positions of the launch (FLOP count)
     if (int rc = make_tmap_nhwc(&L->tmap_a, d.A, d.n_img, d.H, d.W, d.Cin, BLOCK_K, bw, bh, bnimg, 128, a.in_stride)) return rc;
@@ -539,36 +602,40 @@ namespace {
 using GemmKernelFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
                               const CUtensorMap, const GemmKernelArgs);
 struct GemmVariant {
-  int bn;
+  int bn, bm;
   bool geglu, conv;
   int epi;
   GemmKernelFn fn;
   int smem;
 };
-#define D4D_GV(BN, G, C, E) {BN, G, C, E, gemm_wgmma_kernel<BN, G, C, E>, GemmCfg<BN, gemm_staged(C, E)>::SMEM}
+#define D4D_GV_M(BN, MI, G, C, E) \
+  {BN, 128 * MI, G, C, E, gemm_wgmma_kernel<BN, MI, G, C, E>, GemmCfg<BN, MI, gemm_staged(C, E)>::SMEM}
+#define D4D_GV(BN, G, C, E) D4D_GV_M(BN, 1, G, C, E)
 #define D4D_GV_PLAIN(BN)                                                                                              \
   /* plain GEMM: qkv | proj_in, shortcut | attn out, ff2 | proj_out, conv_in */                                       \
   D4D_GV(BN, false, false, 0), D4D_GV(BN, false, false, E_BIAS), D4D_GV(BN, false, false, E_BIAS | E_RES),           \
   D4D_GV(BN, false, false, E_BIAS | E_RES | E_STATS), D4D_GV(BN, false, false, E_ALL)
-#define D4D_GV_CONV(BN)                                                                                               \
+#define D4D_GV_CONV(BN, MI)                                                                                           \
   /* 3x3 convs: resnet conv1 | conv2 | down / up sampling */                                                          \
-  D4D_GV(BN, false, true, E_BIAS | E_ROWVEC | E_STATS), D4D_GV(BN, false, true, E_BIAS | E_RES | E_STATS),           \
-  D4D_GV(BN, false, true, E_BIAS | E_STATS), D4D_GV(BN, false, true, E_ALL)
+  D4D_GV_M(BN, MI, false, true, E_BIAS | E_ROWVEC | E_STATS), D4D_GV_M(BN, MI, false, true, E_BIAS | E_RES | E_STATS), \
+  D4D_GV_M(BN, MI, false, true, E_BIAS | E_STATS), D4D_GV_M(BN, MI, false, true, E_ALL)
 // the feature sets the UNet plan launches (csrc/unet.cu) at the tile widths it picks, plus E_ALL kernels for the rest.
 // GEGLU (only the bias bit matters) runs at widths whose output halves fill whole store slabs; no conv picks 192.
+// 256-row conv tiles (MI = 2) exist where 2 * BN / 2 accumulators per thread fit the 232 registers: widths 128 and 160.
 const GemmVariant kGemmVariants[] = {
-    D4D_GV_PLAIN(128), D4D_GV_CONV(128), D4D_GV(128, true, false, E_BIAS),
-    D4D_GV_PLAIN(160), D4D_GV_CONV(160),
+    D4D_GV_PLAIN(128), D4D_GV_CONV(128, 1), D4D_GV_CONV(128, 2), D4D_GV(128, true, false, E_BIAS),
+    D4D_GV_PLAIN(160), D4D_GV_CONV(160, 1), D4D_GV_CONV(160, 2),
     D4D_GV_PLAIN(192),
-    D4D_GV_PLAIN(256), D4D_GV_CONV(256), D4D_GV(256, true, false, E_BIAS),
+    D4D_GV_PLAIN(256), D4D_GV_CONV(256, 1), D4D_GV(256, true, false, E_BIAS),
     D4D_GV(64, false, false, E_ALL), D4D_GV(64, false, true, E_ALL), D4D_GV(64, true, false, E_BIAS),
 };
 #undef D4D_GV_CONV
 #undef D4D_GV_PLAIN
 #undef D4D_GV
+#undef D4D_GV_M
 constexpr int kNumGemmVariants = sizeof(kGemmVariants) / sizeof(kGemmVariants[0]);
 
-// the instantiation of kernel width bn whose feature bits equal the launch's, else the E_ALL one (-1: none)
+// the instantiation of kernel width bn (and the launch's tile rows) whose feature bits equal the launch's, else the E_ALL one (-1: none)
 int gemm_variant_at(const GemmKernelArgs& a, int bn) {
   const bool conv = a.mode != 0, geglu = a.geglu != 0;
   int need = 0;
@@ -583,7 +650,7 @@ int gemm_variant_at(const GemmKernelArgs& a, int bn) {
   int generic = -1;
   for (int i = 0; i < kNumGemmVariants; ++i) {
     const GemmVariant& v = kGemmVariants[i];
-    if (v.bn != bn || v.geglu != geglu || v.conv != conv) continue;
+    if (v.bn != bn || v.bm != a.block_m || v.geglu != geglu || v.conv != conv) continue;
     if (v.epi == need) return i;
     if ((v.epi & need) == need && (generic < 0 || v.epi == E_ALL)) generic = i;  // geglu: E_BIAS covers {} as well
   }

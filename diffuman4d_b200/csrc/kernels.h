@@ -20,6 +20,7 @@ constexpr float kGnSqScale = 16777216.f;    // 2^24
 
 struct GemmKernelArgs {
   int M, N, k_blocks, block_n, n_tiles, m_tiles;
+  int block_m;   // tile rows: 128, or 256 (conv; each MMA warpgroup owns two 64-row blocks)
   int mode;      // 0 plain, 1 implicit-GEMM convolution over NHWC (tap table below; TMA zero fill = padding)
   int kb_split;  // plain: k-blocks served by A (rest by A2)
   int H, W, n_img, Cin, cin_blocks, BW, BH, BN, tiles_x, tiles_y;  // H, W: the grid of output positions the tiles walk
@@ -75,6 +76,7 @@ struct GemmDesc {
   int act = 0;
   float out_scale = 1.0f;
   int block_n = 0;  // 0 = auto (64, 128, 160, 192 or 256; the last N tile may overhang)
+  int block_m = 0;  // 0 = auto, 128, or 256 (conv at block_n 128 / 160 only)
   // GroupNorm statistics of the output (see GemmKernelArgs::stats); plain GEMM: stats_rows = rows per image
   long long* stats = nullptr;
   int stats_rows = 0;
@@ -98,6 +100,8 @@ struct GemmLaunch {
   int grid;
 };
 
+// the tile rows and width gemm_prepare runs d at on a device of `sms` SMs (shape fields and block_m / block_n only)
+int gemm_choose_tile(const GemmDesc& d, int sms, int* block_m, int* block_n);
 int gemm_prepare(const GemmDesc& d, GemmLaunch* L);
 int gemm_run(const GemmLaunch& L, cudaStream_t stream);
 double gemm_flops(const GemmLaunch& L);

@@ -225,6 +225,16 @@ int d4d_op_gemm_kv_scatter(const void* A, int lda, int K, const void* W, int M, 
 int d4d_op_conv3x3(const void* x_nhwc, int n_img, int H, int W, int Cin, const void* Wt, int Cout, const float* bias,
                    const void* rowvec, int ld_rowvec, const void* residual, int act, void* out, int block_n,
                    int64_t* stats, void* stream);
+/* The three convolutions of the UNet at an explicit tile (d4d_version() 108 and later).  kind 0: d4d_op_conv3x3; kind 1 / 3:
+ * d4d_op_conv_resample's stride-2 conv / four-phase upsampling conv (residual then has the output's shape).
+ * block_m: 0 (automatic), 128 or 256 output positions per tile; 256 needs block_n 0, 128 or 160.  The output and the
+ * statistics do not depend on the tile: every sum runs in the same order.  Anything else returns 1, before any launch. */
+int d4d_op_conv_tiled(const void* x_nhwc, int n_img, int H, int W, int Cin, const void* Wt, int Cout, const float* bias,
+                      const void* rowvec, int ld_rowvec, const void* residual, int act, void* out, int kind, int block_m,
+                      int block_n, int64_t* stats, void* stream);
+/* The tile (rows, width) an automatic conv launch of this shape (kind as d4d_op_conv_tiled) takes on a device with `sms`
+ * SMs; needs no device. */
+int d4d_conv_tile_choice(int n_img, int H, int W, int Cin, int Cout, int kind, int sms, int* block_m, int* block_n);
 /* q: column slice of a row-major [batch*seq, ld_qkv] matrix; head hd = columns [hd*D, (hd+1)*D).  k, v: column slices of a
  * row-major [batch*seq_kv, ld_kv] matrix, the keys of batch entry b in rows [b*seq_kv, (b+1)*seq_kv).  seq_kv = 0 means
  * seq and ld_kv = 0 means ld_qkv (k and v in the QKV matrix). */

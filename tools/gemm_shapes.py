@@ -5,7 +5,7 @@
 Every distinct launch shape of the plan (csrc/unet.cu: PlanBuilder::resnet, transformer, self_attention, the down /
 up-sampling convs, conv_in, the pose encoder's GEMM-kernel layers and the time embedding) runs with the epilogue features
 the plan gives it, through the C ABI on pre-allocated buffers, captured `reps` times into a CUDA graph and timed with CUDA
-events after warm-up.  Per shape: launches per forward, the tile width gemm_prepare picks, µs per launch, TFLOP/s
+events after warm-up.  Per shape: launches per forward, the tile rows and width gemm_prepare picks, µs per launch, TFLOP/s
 (executed FLOPs: the upsampling convs run 4 taps per phase), compulsory HBM bytes and GB/s, and the least time the card
 could take: the larger of FLOPs / tensor peak and bytes / 3.35 TB/s, naming which bounds the shape.  The tensor peak is
 4096 dense BF16 FLOP/clk/SM at the card's maximum SM clock; a power-limited card runs below it under load.
@@ -104,18 +104,48 @@ def plan_shapes():
     return list(shapes.values())
 
 
-def auto_block_n(rows, N, geglu, sms):
-    """Mirror of gemm_prepare's automatic tile width (csrc/gemm_wgmma.cu)."""
+OPERAND_WEIGHT = 128  # kOperandWeight of csrc/gemm_wgmma.cu
+MIN_K_BLOCKS_256 = 16  # kMinKBlocks256
+
+
+def conv_tiles(rows, n, oh, ow):
+    """Tiles per phase of a conv on an oh x ow output grid at `rows` positions per tile (conv_tile of csrc/gemm_wgmma.cu)."""
+    bw = 16
+    while bw > ow:
+        bw >>= 1
+    bh = rows // bw
+    while bh > oh and bh > 1:
+        bh >>= 1
+    bn_img = rows // (bw * bh)
+    return -(-ow // bw) * -(-oh // bh) * -(-n // bn_img)
+
+
+def tile_cost(r, c, tiles, N, sms):
+    """Cost of running `tiles` r x c tiles on `sms` SMs (gemm_choose_tile): waves x tile time + the padded columns."""
+    n_tiles = -(-N // c)
+    return -(-tiles // sms) * (r * c + OPERAND_WEIGHT * (r + c)) + (n_tiles * c - N) * (r // 2)
+
+
+def auto_tile(N, sms, M=0, geglu=False, conv=None):
+    """Mirror of gemm_choose_tile (csrc/gemm_wgmma.cu): the (rows, width) of an automatic launch.  conv = (n, H, W, Cin, mode)
+    with mode "s1" / "s2" / "up" on the H x W input, else a plain GEMM of M rows."""
+    if conv:
+        n, H, W, Cin, mode = conv
+        oh, ow, phases = (H // 2, W // 2, 1) if mode == "s2" else (H, W, 4 if mode == "up" else 1)
+        k_blocks = (4 if mode == "up" else 9) * -(-Cin // 64)
     best = None
-    for c in (64, 128, 160, 192, 256):
-        if geglu and c % 64:
-            continue
-        n_tiles = -(-N // c)
-        waves = -(-(-(-rows // 128) * n_tiles) // sms)
-        cost = waves * (c + 64) + (n_tiles * c - N) // 4
-        if best is None or cost <= best[0]:
-            best = (cost, c)
-    return best[1]
+    for r in (128, 256) if conv else (128,):
+        m_tiles = conv_tiles(r, n, oh, ow) * phases if conv else -(-M // r)
+        for c in (64, 128, 160, 192, 256):
+            if geglu and c % 64:
+                continue
+            tiles = m_tiles * -(-N // c)
+            if r == 256 and not (c in (128, 160) and tiles >= sms and k_blocks >= MIN_K_BLOCKS_256):
+                continue
+            cost = tile_cost(r, c, tiles, N, sms)
+            if best is None or cost <= best[0]:
+                best = (cost, r, c)
+    return best[1], best[2]
 
 
 def card():
@@ -158,7 +188,7 @@ def make_launch(kind, spec, dev):
         K = K1 + K2
         flops = 2.0 * M * N * K
         byts = 2.0 * (M * K + N * K + M * nout + (M * N if res is not None else 0))
-        return run, flops, byts, auto_block_n(M, N, geglu, torch.cuda.get_device_properties(0).multi_processor_count)
+        return run, flops, byts, auto_tile(N, torch.cuda.get_device_properties(0).multi_processor_count, M=M, geglu=geglu)
     n, H, W, Cin, Cout, mode = spec["n"], spec["H"], spec["W"], spec["Cin"], spec["Cout"], spec["mode"]
     x = r(n, H, W, Cin)
     bias = torch.randn(Cout, generator=g).to(dev) if "bias" in f else None
@@ -173,7 +203,6 @@ def make_launch(kind, spec, dev):
         def run():
             check(lib().d4d_op_conv_resample(x.data_ptr(), n, H, W, Cin, wp.data_ptr(), Cout, p(bias), 3, 0, 0, out.data_ptr(),
                                              p(stats), stream()), "d4d_op_conv_resample")
-        rows = n * H * W
     elif mode == "s2":
         taps, Mo = 9, n * (H // 2) * (W // 2)
         wt = r(Cout, 9, Cin) * (9 * Cin) ** -0.5
@@ -182,7 +211,6 @@ def make_launch(kind, spec, dev):
         def run():
             check(lib().d4d_op_conv_resample(x.data_ptr(), n, H, W, Cin, wt.data_ptr(), Cout, p(bias), 1, 0, 0, out.data_ptr(),
                                              p(stats), stream()), "d4d_op_conv_resample")
-        rows = n * H * W  # gemm_prepare sizes the tile width on the input grid
     else:
         taps, Mo = 9, n * H * W
         wt = r(Cout, 9, Cin) * (9 * Cin) ** -0.5
@@ -195,10 +223,9 @@ def make_launch(kind, spec, dev):
             check(lib().d4d_op_conv3x3(x.data_ptr(), n, H, W, Cin, wt.data_ptr(), Cout, p(bias), p(rowvec), Cout, p(res), act,
                                        out.data_ptr(), 0, p(stats), stream()),
                   "d4d_op_conv3x3")
-        rows = Mo
     flops = 2.0 * Mo * Cout * taps * Cin
     byts = 2.0 * (x.numel() + taps * Cin * Cout + Mo * Cout * (2 if "residual" in f else 1))
-    return run, flops, byts, auto_block_n(rows, Cout, False, torch.cuda.get_device_properties(0).multi_processor_count)
+    return run, flops, byts, auto_tile(Cout, torch.cuda.get_device_properties(0).multi_processor_count, conv=(n, H, W, Cin, mode))
 
 
 def time_launch(run, reps):
@@ -232,11 +259,11 @@ def main():
     peak = 4096.0 * sms * max_mhz * 1e6
     print(f"# {name}, power limit {power_w:.0f} W, max SM clock {max_mhz:.0f} MHz, {sms} SMs; "
           f"tensor peak {peak / 1e12:.0f} TFLOP/s (4096 FLOP/clk/SM at max clock), HBM 3.35 TB/s")
-    hdr = f"{'kind':5} {'shape':58} {'cnt':>3} {'bn':>4} {'us':>9} {'TFLOP/s':>8} {'MB':>8} {'GB/s':>7} {'min us':>8} {'bound':>6} {'eff':>5}"
+    hdr = f"{'kind':5} {'shape':58} {'cnt':>3} {'rows':>4} {'bn':>4} {'us':>9} {'TFLOP/s':>8} {'MB':>8} {'GB/s':>7} {'min us':>8} {'bound':>6} {'eff':>5}"
     print(hdr)
     rows, tot = [], {"gemm": 0.0, "conv": 0.0}
     for kind, nm, cnt, spec in plan_shapes():
-        run, flops, byts, bn = make_launch(kind, spec, dev)
+        run, flops, byts, (bm, bn) = make_launch(kind, spec, dev)
         us = time_launch(run, args.reps)
         t_f, t_b = flops / peak * 1e6, byts / HBM_BPS * 1e6
         bound = "tensor" if t_f >= t_b else "HBM"
@@ -244,11 +271,11 @@ def main():
         dims = (f"M{spec['M']} N{spec['N']} K{spec['K1']}" + (f"+{spec['K2']}" if spec["K2"] else "")) if kind == "gemm" else \
             f"{spec['n']}x{spec['H']}x{spec['W']} {spec['Cin']}->{spec['Cout']} {spec['mode']}"
         label = f"{nm}: {dims} [{','.join(spec['feats']) or '-'}]"
-        print(f"{kind:5} {label:58} {cnt:3d} {bn:4d} {us:9.1f} {flops / us / 1e6:8.1f} {byts / 1e6:8.1f} "
+        print(f"{kind:5} {label:58} {cnt:3d} {bm:4d} {bn:4d} {us:9.1f} {flops / us / 1e6:8.1f} {byts / 1e6:8.1f} "
               f"{byts / us / 1e3:7.0f} {tmin:8.1f} {bound:>6} {tmin / us:5.2f}")
         tot[kind] += cnt * us
         rows.append({"kind": kind, "name": nm, "spec": {k: (list(v) if isinstance(v, tuple) else v) for k, v in spec.items()},
-                     "count": cnt, "block_n": bn, "us": us, "tflops": flops / us / 1e6, "bytes": byts,
+                     "count": cnt, "block_m": bm, "block_n": bn, "us": us, "tflops": flops / us / 1e6, "bytes": byts,
                      "gbps": byts / us / 1e3, "min_us": tmin, "bound": bound})
         del run
         torch.cuda.empty_cache()
