@@ -17,7 +17,7 @@ EXPORTS = [
     "d4d_op_attention", "d4d_op_groupnorm", "d4d_op_conv3x3_groupnorm", "d4d_op_conv_resample", "d4d_op_layernorm", "d4d_op_pose_conv0", "d4d_op_pose_conv", "d4d_debug_tap", "d4d_exchange_alloc",
     "d4d_exchange_open", "d4d_unet_forward_sharded", "d4d_denoise_window_sharded", "d4d_denoise_window_dpm_sharded",
     "d4d_window_exchange", "d4d_op_window_scatter", "d4d_denoise_window_unipc", "d4d_cfg_unipc_step",
-    "d4d_op_conv_tiled", "d4d_conv_tile_choice",
+    "d4d_op_conv_tiled", "d4d_conv_tile_choice", "d4d_op_gemm_tiled", "d4d_gemm_tile_choice",
 ]
 
 
@@ -103,6 +103,9 @@ def _load(path: str) -> C.CDLL:
                                      i32, vp, vp]
     l.d4d_op_gemm.argtypes = [vp, i32, i32, vp, i32, i32, vp, i32, i32, f32p, vp, i32, i32, vp, i32, vp, i32, i32,
                               i32, f32, i32, vp, i32, vp]
+    l.d4d_op_gemm_tiled.argtypes = [vp, i32, i32, vp, i32, i32, vp, i32, i32, f32p, vp, i32, i32, vp, i32, vp, i32, i32,
+                                    i32, f32, i32, i32, vp, i32, vp]
+    l.d4d_gemm_tile_choice.argtypes = [i32, i32, i32, i32, i32, i32, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     l.d4d_op_gemm_kv_scatter.argtypes = [vp, i32, i32, vp, i32, i32, vp, i32, i32, i32, C.c_int64, C.c_int64, C.c_int64,
                                          i32, vp, i32, vp]
     l.d4d_op_conv3x3.argtypes = [vp, i32, i32, i32, i32, vp, i32, f32p, vp, i32, vp, i32, vp, i32, vp, vp]
@@ -133,7 +136,7 @@ def _load(path: str) -> C.CDLL:
                 "d4d_create", "d4d_load_weight", "d4d_finalize_weights", "d4d_unet_forward", "d4d_denoise_window",
                 "d4d_denoise_window_dpm", "d4d_exchange_alloc", "d4d_exchange_open", "d4d_unet_forward_sharded",
                 "d4d_denoise_window_sharded", "d4d_denoise_window_dpm_sharded", "d4d_window_exchange", "d4d_debug_tap",
-                "d4d_denoise_window_unipc", "d4d_conv_tile_choice"):
+                "d4d_denoise_window_unipc", "d4d_conv_tile_choice", "d4d_gemm_tile_choice"):
             fn.restype = C.c_int
     return l
 

@@ -99,6 +99,14 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
   }
 }
+// The same bounded wait for kernels that issue wgmma: a call (printf) anywhere in such a kernel makes ptxas serialize
+// every wgmma of it (C7510), so a timeout traps without a message.
+__device__ __forceinline__ void mbar_wait_nocall(uint64_t* bar, uint32_t parity) {
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if (++spins > D4D_SPIN_LIMIT) __trap();
+  }
+}
 
 // ---- proxies / fences ----------------------------------------------------------------------
 __device__ __forceinline__ void fence_proxy_async_smem() {
@@ -107,6 +115,10 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
 // barrier over `threads` threads (a multiple of 32) on hardware barrier `id` (0 is __syncthreads)
 __device__ __forceinline__ void named_barrier_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+// arrive on hardware barrier `id` without waiting: the other threads of the `threads` count bar.sync on it
+__device__ __forceinline__ void named_barrier_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 __device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
   asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");

@@ -86,7 +86,7 @@ d4d::WindowStep dpm_step(const d4d_dpm_sched* sched, void* x0_prev, int32_t* low
 extern "C" {
 
 const char* d4d_last_error(void) { return d4d::g_last_error.c_str(); }
-int d4d_version(void) { return 108; }
+int d4d_version(void) { return 109; }
 
 int d4d_create(const d4d_config* cfg, int device, d4d_handle** out) {
   D4D_API_BEGIN
@@ -309,6 +309,14 @@ int d4d_op_gemm(const void* A, int lda, int K1, const void* A2, int lda2, int K2
                 const float* bias, const void* rowvec, int ld_rowvec, int rows_per_image, const void* residual,
                 int ld_res, void* out, int ldo, int geglu, int act, float out_scale, int block_n, int64_t* stats,
                 int stats_rows, void* stream) {
+  return d4d_op_gemm_tiled(A, lda, K1, A2, lda2, K2, W, M, N, bias, rowvec, ld_rowvec, rows_per_image, residual, ld_res, out,
+                           ldo, geglu, act, out_scale, block_n, 0, stats, stats_rows, stream);
+}
+
+int d4d_op_gemm_tiled(const void* A, int lda, int K1, const void* A2, int lda2, int K2, const void* W, int M, int N,
+                      const float* bias, const void* rowvec, int ld_rowvec, int rows_per_image, const void* residual,
+                      int ld_res, void* out, int ldo, int geglu, int act, float out_scale, int block_n, int schedule,
+                      int64_t* stats, int stats_rows, void* stream) {
   D4D_API_BEGIN
   d4d::GemmDesc d;
   d.A = static_cast<const bf16*>(A); d.lda = lda; d.K1 = K1;
@@ -317,11 +325,23 @@ int d4d_op_gemm(const void* A, int lda, int K1, const void* A2, int lda2, int K2
   d.rowvec = static_cast<const bf16*>(rowvec); d.ld_rowvec = ld_rowvec; d.rows_per_image = rows_per_image;
   d.residual = static_cast<const bf16*>(residual); d.ld_res = ld_res;
   d.out = static_cast<bf16*>(out); d.ldo = ldo; d.geglu = geglu; d.act = act; d.out_scale = out_scale; d.block_n = block_n;
+  d.schedule = schedule;
   d.stats = reinterpret_cast<long long*>(stats); d.stats_rows = stats_rows;
   D4D_REQUIRE(M > 0, "empty GEMM");
   d4d::GemmLaunch L;
   if (int rc = d4d::gemm_prepare(d, &L)) return rc;
   return d4d::gemm_run(L, static_cast<cudaStream_t>(stream));
+  D4D_API_END
+}
+
+int d4d_gemm_tile_choice(int M, int N, int K1, int K2, int geglu, int sms, int* block_n, int* schedule) {
+  D4D_API_BEGIN
+  D4D_REQUIRE(M > 0 && N > 0 && K1 > 0 && K2 >= 0 && sms > 0 && block_n && schedule, "gemm_tile_choice arguments");
+  d4d::GemmDesc d;
+  D4D_REQUIRE(K2 == 0 || K1 % 64 == 0, "two-source GEMM needs K1 % 64 == 0");
+  d.M = M; d.N = N; d.K1 = K1 + K2; d.geglu = geglu;  // K1 % 64 == 0: the k-blocks of A | A2 are those of one source
+  int block_m = 0;
+  return d4d::gemm_choose_tile(d, sms, &block_m, block_n, schedule);
   D4D_API_END
 }
 

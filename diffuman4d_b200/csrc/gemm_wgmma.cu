@@ -12,6 +12,11 @@
 // * plain GEMMs stage the epilogue in shared memory: each MMA warpgroup writes its finished 64 x BN bf16 rows into 32-column
 //   slabs (64B-swizzled, conflict-free), and one thread TMA-stores them and goes on into the next tile's MMAs while the
 //   stores drain.  The residual tile is TMA-loaded into the same slabs during the first k-block.
+// * ping-pong schedule (plain staged GEMMs, chosen per shape): each MMA warpgroup owns whole 128-row tiles, as two 64-row
+//   blocks (MI = 2, staging slabs for 128 rows each), and the two take turns: warpgroup i & 1 runs the i-th tile of the
+//   CTA's sequence.  Two named barriers order the main loops (tile i's MMAs are all issued before tile i + 1's start), so
+//   one warpgroup's epilogue runs while the other's MMAs keep the tensor cores busy.  The epilogue body is the same per
+//   64-row block, so outputs and statistics are bit-identical to the cooperative schedule.
 // * "conv" mode turns the A loader into an implicit-GEMM gather: the A tile for k-block (tap, c0) is a 4-D TMA box
 //   {64 ch, BW, BH, BN} of the NHWC activation at spatial offset (ky-1, kx-1); out-of-bounds rows/cols are zero-filled
 //   by TMA, which is exactly the conv's zero padding.  K = 9*Cin, weights are pre-laid-out as [Cout][tap][Cin].
@@ -42,12 +47,14 @@ constexpr int MAX_SMEM = 227 * 1024;
 constexpr int SLAB_COLS = 32;
 constexpr int SLAB_BYTES = 64 * SLAB_COLS * 2;
 
-// Tile width BN (the wgmma N) and the m64 blocks per warpgroup MI (tile rows = 128 MI) are template parameters; after the
-// staging slabs of both warpgroups (plain GEMM only), the ring takes as many stages as fit (at most 8).
-template <int BN, int MI, bool kStaged>
+// Tile width BN (the wgmma N) and the m64 blocks per warpgroup MI (tile rows = 128 MI, or 128 under ping-pong, where one
+// warpgroup owns the whole tile) are template parameters; after the staging slabs of both warpgroups (64 MI rows each;
+// plain GEMM only), the ring takes as many stages as fit (at most 8).
+template <int BN, int MI, bool kStaged, bool kPingPong>
 struct GemmCfg {
-  static constexpr int STAGE_BYTES = MI * A_BYTES + BN * BLOCK_K * 2;
-  static constexpr int STAGING_BYTES = kStaged ? 2 * 64 * BN * 2 : 0;
+  static constexpr int TILE_A_BYTES = kPingPong ? A_BYTES : MI * A_BYTES;
+  static constexpr int STAGE_BYTES = TILE_A_BYTES + BN * BLOCK_K * 2;
+  static constexpr int STAGING_BYTES = kStaged ? 2 * 64 * MI * BN * 2 : 0;
   static constexpr int STAGES_FIT = (MAX_SMEM - 1024 - BAR_BYTES - STAGING_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;
   static constexpr int SMEM = 1024 + BAR_BYTES + STAGES * STAGE_BYTES + STAGING_BYTES;
@@ -103,19 +110,23 @@ __device__ __forceinline__ void row_of(const GemmKernelArgs& a, const TileCoord&
 
 // Epilogue feature bits of the kernel template: a CLEAR bit compiles the feature out, a set bit is still checked at run
 // time.  gemm_run picks the instantiation whose bits equal the launch's features, or the E_ALL one.
-enum : int { E_BIAS = 1, E_ROWVEC = 2, E_ACT = 4, E_RES = 8, E_STATS = 16, E_KV = 32, E_ALL = 63 };
+enum : int { E_BIAS = 1, E_ROWVEC = 2, E_ACT = 4, E_RES = 8, E_STATS = 16, E_KV = 32, E_ALL = 63, E_STAGED_ALL = E_ALL & ~E_KV };
 // Instantiations with the staged epilogue: plain GEMMs.  Convs store from registers (their output pixels are not a row
 // range), and so do the E_KV kernels (they serve the K/V scatter and, as E_ALL, the rare feature sets no other kernel has).
 __host__ __device__ constexpr bool gemm_staged(bool conv, int epi) { return !conv && !(epi & E_KV); }
 
-template <int BN, int MI, bool kGeglu, bool kConv, int kEpi>
+// ping-pong: hardware barriers 3 and 4 hand the turn to issue MMAs to warpgroup 0 / 1 (1 and 2 are the epilogue barriers)
+constexpr int ORDER_BAR = 3;
+
+template <int BN, int MI, bool kGeglu, bool kConv, int kEpi, bool kPingPong>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_a2,
                   const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ CUtensorMap tmap_c,
                   const __grid_constant__ CUtensorMap tmap_r, const GemmKernelArgs a) {
   constexpr bool kStaged = gemm_staged(kConv, kEpi);
-  static_assert(MI == 1 || (kConv && MI == 2), "256-row tiles: conv mode only (a plain tile is 128 rows, as are its staging slabs)");
-  using Cfg = GemmCfg<BN, MI, kStaged>;
+  static_assert(MI == 1 || (kConv && MI == 2) || kPingPong, "256-row tiles: conv mode only (a plain tile is 128 rows)");
+  static_assert(!kPingPong || (kStaged && MI == 2), "ping-pong: staged plain GEMMs, one warpgroup per 128-row tile");
+  using Cfg = GemmCfg<BN, MI, kStaged, kPingPong>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment for the 128B swizzle atoms
@@ -135,7 +146,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     if (a.kb_split < a.k_blocks) tma_prefetch_desc(&tmap_a2);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 2);  // one arrival per MMA warpgroup
+      mbar_init(&empty[i], kPingPong ? 1 : 2);  // one arrival per MMA warpgroup that reads the stage
     }
     mbar_init(&res_full[0], 1);
     mbar_init(&res_full[1], 1);
@@ -149,7 +160,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     // ===================== TMA producer =====================
     setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
-      const uint32_t tx_bytes = MI * A_BYTES + static_cast<uint32_t>(a.block_n) * BLOCK_K * 2;
+      const uint32_t tx_bytes = Cfg::TILE_A_BYTES + static_cast<uint32_t>(a.block_n) * BLOCK_K * 2;
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -159,9 +170,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         tile_coords<kConv>(a, m_tile, tc);
         const int n0 = n_tile * a.block_n;
         for (int kb = 0; kb < a.k_blocks; ++kb) {
-          mbar_wait(&empty[stage], phase ^ 1);
+          mbar_wait_nocall(&empty[stage], phase ^ 1);
           uint8_t* sa = ring + stage * Cfg::STAGE_BYTES;
-          uint8_t* sb = sa + MI * A_BYTES;
+          uint8_t* sb = sa + Cfg::TILE_A_BYTES;
           mbar_expect_tx(&full[stage], tx_bytes);
           if (!kConv) {
             if (kb < a.kb_split) tma_load_2d(sa, &tmap_a, &full[stage], kb * BLOCK_K, tc.m0);
@@ -183,18 +194,21 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 
   // ===================== MMA warpgroups + epilogue =====================
   setmaxnreg_inc<232>();
-  const int wg = (warp >> 2) - 1;   // 0 / 1: rows [64 MI wg, 64 MI (wg + 1)) of the tile, as MI blocks of 64
+  const int wg = (warp >> 2) - 1;   // 0 / 1: rows [64 MI wg, 64 MI (wg + 1)) of the tile (ping-pong: all rows of every
+                                    // other tile), as MI blocks of 64
   const int wq = warp & 3;          // warp within the warpgroup: rows 16 wq .. 16 wq + 15 of each 64-row block
   const bool wg_leader = (threadIdx.x & 127) == 0;
-  const int r_base = wg * 64 * MI + wq * 16 + (lane >> 2);  // tile rows r_base + 64 mi and + 8 belong to this thread
+  const int wg_row0 = kPingPong ? 0 : wg * 64 * MI;          // the warpgroup's first tile row
+  const int r_base = wg_row0 + wq * 16 + (lane >> 2);       // tile rows r_base + 64 mi and + 8 belong to this thread
   const int c_base = 2 * (lane & 3);                   // columns 8j + c_base, +1 of fragment j
   const uint32_t ring_u32 = smem_u32(ring);
-  // staged epilogue: this warpgroup's slabs, and the offset of this thread's (row r_base, columns c_base, +1) in a slab; the
-  // 64-byte swizzle moves the 16-byte chunk c of row r to c ^ ((r >> 1) & 3), which for rows r_base, r_base + 8 is
-  // (lane >> 3) & 3: the 8 rows of a warp store land in 8 different chunks, 32 different banks
+  // staged epilogue: this warpgroup's slabs (64 rows x BN per 64-row block), and the offset of this thread's (row r_base,
+  // columns c_base, +1) in a slab; the 64-byte swizzle moves the 16-byte chunk c of row r to c ^ ((r >> 1) & 3), which for
+  // rows r_base, r_base + 8 is (lane >> 3) & 3: the 8 rows of a warp store land in 8 different chunks, 32 different banks
+  constexpr int STG_BLOCK = 64 * BN * 2;
   const bool staged = kStaged && a.staged;
-  uint8_t* stg = ring + STAGES * Cfg::STAGE_BYTES + wg * 64 * BN * 2;
-  const uint32_t stg_u32 = smem_u32(stg) + (r_base - wg * 64 * MI) * 64 + c_base * 2;
+  uint8_t* stg = ring + STAGES * Cfg::STAGE_BYTES + wg * MI * STG_BLOCK;
+  const uint32_t stg_u32 = smem_u32(stg) + (r_base - wg_row0) * 64 + c_base * 2;
   const int stg_xor = (lane >> 3) & 3;
   const bool has_res = (kEpi & E_RES) && !kGeglu && a.residual != nullptr;
   const int out_cols = kGeglu ? a.N / 2 : a.N;
@@ -202,8 +216,18 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 
   int stage = 0;
   uint32_t phase = 0;
+  // ping-pong: the k-blocks of the other warpgroup's tiles pass this warpgroup's ring counters by
+  const auto skip_stages = [&](int n) {
+    stage += n;
+    while (stage >= STAGES) { stage -= STAGES; phase ^= 1; }
+  };
+  if (kPingPong && wg == 1) {
+    skip_stages(a.k_blocks);
+    named_barrier_arrive(ORDER_BAR, 256);  // warpgroup 0 issues the MMAs of the first tile
+  }
+  const int tile_step = kPingPong ? 2 * gridDim.x : gridDim.x;
   float acc[MI][BN / 2];
-  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+  for (int tile = blockIdx.x + (kPingPong ? wg * gridDim.x : 0); tile < total_tiles; tile += tile_step) {
     const int m_tile = tile / a.n_tiles;
     const int n_tile = tile % a.n_tiles;
     TileCoord tc;
@@ -213,15 +237,17 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     const int ocol0 = kGeglu ? n0 / 2 : n0;
     const int ocols = min(kGeglu ? a.block_n / 2 : a.block_n, out_cols - ocol0);
     const int n_slabs = (ocols + SLAB_COLS - 1) / SLAB_COLS;
-    const int orow0 = tc.m0 + wg * 64;
-    const bool stg_live = staged && orow0 < a.M;
+    // staged: this warpgroup's 64-row blocks of the tile that lie inside the tensor, from output row orow0 on
+    const int orow0 = tc.m0 + wg_row0;
+    const int live_blocks = staged ? max(0, min(MI, (a.M - orow0 + 63) / 64)) : 0;
 
     // ---- main loop: one k-block in flight behind the one being issued; a stage is released once its MMAs retired
+    if (kPingPong) named_barrier_sync(ORDER_BAR + wg, 256);  // the previous tile's MMAs are all issued
     int prev_stage = -1;
     for (int kb = 0; kb < a.k_blocks; ++kb) {
-      mbar_wait(&full[stage], phase);
-      const uint32_t sa = ring_u32 + stage * Cfg::STAGE_BYTES + wg * MI * 64 * 128;
-      const uint32_t sb = ring_u32 + stage * Cfg::STAGE_BYTES + MI * A_BYTES;
+      mbar_wait_nocall(&full[stage], phase);
+      const uint32_t sa = ring_u32 + stage * Cfg::STAGE_BYTES + wg_row0 * 128;
+      const uint32_t sb = ring_u32 + stage * Cfg::STAGE_BYTES + Cfg::TILE_A_BYTES;
       const uint64_t adesc = make_wgmma_desc(sa, 16, 1024);
       const uint64_t bdesc = make_wgmma_desc(sb, 16, 1024);
       wgmma_fence();
@@ -246,16 +272,23 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         // after the barrier there); then the residual tile comes in under this tile's MMAs.  A tile reads only the
         // residual rows and columns it stores itself, so the residual may alias the output.
         bulk_wait_group_read<0>();
-        if (has_res && stg_live) {
-          mbar_expect_tx(&res_full[wg], n_slabs * SLAB_BYTES);
-          for (int s = 0; s < n_slabs; ++s)
-            tma_load_2d(stg + s * SLAB_BYTES, &tmap_r, &res_full[wg], ocol0 + s * SLAB_COLS, orow0);
+        if (has_res && live_blocks > 0) {
+          mbar_expect_tx(&res_full[wg], live_blocks * n_slabs * SLAB_BYTES);
+          for (int mi = 0; mi < live_blocks; ++mi)
+            for (int s = 0; s < n_slabs; ++s)
+              tma_load_2d(stg + mi * STG_BLOCK + s * SLAB_BYTES, &tmap_r, &res_full[wg], ocol0 + s * SLAB_COLS, orow0 + 64 * mi);
         }
       }
       wgmma_wait<1>();
       if (prev_stage >= 0 && wg_leader) mbar_arrive(&empty[prev_stage]);
       prev_stage = stage;
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    // ping-pong: hand the tensor cores to the other warpgroup (if the CTA has a next tile), run this tile's epilogue under
+    // its MMAs, and let the ring counters pass its k-blocks
+    if (kPingPong) {
+      if (tile + gridDim.x < total_tiles) named_barrier_arrive(ORDER_BAR + (wg ^ 1), 256);
+      skip_stages(a.k_blocks);
     }
     wgmma_wait<0>();
 #pragma unroll
@@ -265,19 +298,18 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     // ---- epilogue: into the staging slabs, or straight from the accumulator registers to global memory
     if (staged) {
       named_barrier_sync(1 + wg, 128);  // orders the slab writes below after the leader's bulk_wait_group_read
-      if (has_res && stg_live) {
-        mbar_wait(&res_full[wg], res_phase);
+      if (has_res && live_blocks > 0) {
+        mbar_wait_nocall(&res_full[wg], res_phase);
         res_phase ^= 1;
       }
     }
-    // shared address of this thread's pair (fragment j, row half h) in the slabs
-    auto stg_addr = [&](int j, int h) {
-      return stg_u32 + h * 8 * 64 + (j >> 2) * SLAB_BYTES + (((j & 3) ^ stg_xor) << 4);
-    };
-
     // one pass per 64-row block of the warpgroup; a warp's 16 rows and their statistics are those of a 128-row tile
 #pragma unroll
     for (int mi = 0; mi < MI; ++mi) {
+      // shared address of this thread's pair (fragment j, row half h) in the slabs of this block
+      auto stg_addr = [&](int j, int h) {
+        return stg_u32 + mi * STG_BLOCK + h * 8 * 64 + (j >> 2) * SLAB_BYTES + (((j & 3) ^ stg_xor) << 4);
+      };
       float (&accm)[BN / 2] = acc[mi];
       long long rows[2];
       int imgs[2];
@@ -385,8 +417,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       // the slab writes (generic proxy) become visible to the TMA store (async proxy); TMA clips rows >= M, columns >= N
       fence_proxy_async_smem();
       named_barrier_sync(1 + wg, 128);
-      if (wg_leader && stg_live) {
-        for (int s = 0; s < n_slabs; ++s) tma_store_2d(&tmap_c, stg + s * SLAB_BYTES, ocol0 + s * SLAB_COLS, orow0);
+      if (wg_leader && live_blocks > 0) {
+        for (int mi = 0; mi < live_blocks; ++mi)
+          for (int s = 0; s < n_slabs; ++s)
+            tma_store_2d(&tmap_c, stg + mi * STG_BLOCK + s * SLAB_BYTES, ocol0 + s * SLAB_COLS, orow0 + 64 * mi);
         bulk_commit_group();
       }
     }
@@ -425,12 +459,27 @@ ConvTile conv_tile(int rows, int n_img, int oh, int ow) {
 // the per-tile times of tools/conv_tile_sweep.py (DESIGN section 5).
 constexpr int kOperandWeight = 128;
 constexpr int kMinKBlocks256 = 16;
+// Schedule of a plain GEMM: a tile's main loop costs k_blocks * (128 bn + kOperandWeight (128 + bn)) and its epilogue
+// kEpilogueWeight * bn in the same units.  Cooperative CTAs run main loop and epilogue in turn; a ping-pong CTA overlaps
+// each epilogue with the next tile's main loop, so only the longer of the two counts, plus the last tile's epilogue.
+// The weight is fitted to the per-shape times of tools/gemm_schedule_sweep.py (DESIGN section 5).
+constexpr int kEpilogueWeight = 3072;
 
-int gemm_choose_tile(const GemmDesc& d, int sms, int* block_m, int* block_n) {
+namespace {
+bool pingpong_width(int bn, bool geglu) { return bn == 128 || (bn == 64 && !geglu); }
+}  // namespace
+
+int gemm_choose_tile(const GemmDesc& d, int sms, int* block_m, int* block_n, int* schedule) {
   D4D_REQUIRE(d.block_m == 0 || d.block_m == 128 || d.block_m == 256, "block_m must be 0 (automatic), 128 or 256");
   D4D_REQUIRE(d.block_m != 256 || d.conv, "256-row tiles: convolutions only (a plain GEMM stages a 128-row tile for its TMA store)");
   D4D_REQUIRE(d.block_m != 256 || d.block_n <= 0 || d.block_n == 128 || d.block_n == 160,
               "256-row tiles run at block_n 128 or 160 (the accumulators of wider tiles do not fit the register file)");
+  D4D_REQUIRE(d.schedule == 0 || d.schedule == kSchedCooperative || d.schedule == kSchedPingPong,
+              "schedule must be 0 (automatic), 1 (cooperative) or 2 (ping-pong)");
+  const bool pp_ok = !d.conv && d.kv_world == 0;
+  D4D_REQUIRE(d.schedule != kSchedPingPong || pp_ok, "ping-pong: plain GEMMs without the K/V scatter only");
+  D4D_REQUIRE(d.schedule != kSchedPingPong || d.block_n <= 0 || pingpong_width(d.block_n, d.geglu),
+              "ping-pong runs at block_n 64 or 128 (GEGLU: 128; wider accumulators do not fit the register file)");
   int oh = 0, ow = 0, phases = 1;
   if (d.conv) conv_out_grid(d, &oh, &ow, &phases);
   D4D_REQUIRE(!d.conv || (d.n_img > 0 && oh > 0 && ow > 0), "empty conv");
@@ -438,26 +487,49 @@ int gemm_choose_tile(const GemmDesc& d, int sms, int* block_m, int* block_n) {
   // a shorter tile is bound by its register epilogue, and 64 -> 128 channels at 64x64 ran 40% slower at 256 rows), width 64, 128, 160, 192 or 256 (the last N
   // tile may overhang; its extra columns are not stored): the pair with the fewest SM-waves of the persistent grid, weighted
   // by the tile's time, plus the work of the padded columns; ties to the larger tile.  GEGLU keeps to widths whose halves
-  // fill whole 32-column store slabs.
-  long long best_cost = -1;
-  for (int r : {128, 256}) {
-    if (d.block_m > 0 ? r != d.block_m : (r == 256 && !d.conv)) continue;
-    const int k_blocks = d.conv ? (d.conv_kind >= 2 ? 4 : 9) * ((d.Cin + BLOCK_K - 1) / BLOCK_K) : 0;
-    const long long m_tiles = d.conv ? conv_tile(r, d.n_img, oh, ow).tiles * phases : (static_cast<long long>(d.M) + r - 1) / r;
-    for (int c : {64, 128, 160, 192, 256}) {
-      if (d.block_n > 0) c = d.block_n;
-      else if (d.geglu && c % 64 != 0) continue;
-      const long long n_tiles = (d.N + c - 1) / c, tiles = m_tiles * n_tiles;
-      const bool fits = r == 128 || ((c == 128 || c == 160) && (d.block_m == 256 || (tiles >= sms && k_blocks >= kMinKBlocks256)));
-      if (fits) {
-        const long long waves = (tiles + sms - 1) / sms;
-        const long long cost = waves * (static_cast<long long>(r) * c + kOperandWeight * (r + c)) + (n_tiles * c - d.N) * (r / 2);
-        if (best_cost < 0 || cost <= best_cost) { best_cost = cost; *block_m = r; *block_n = c; }
+  // fill whole 32-column store slabs.  The same choice among the ping-pong widths gives that schedule's tile.
+  const auto best_tile = [&](bool pingpong, int* bm, int* bn) {
+    long long best_cost = -1;
+    for (int r : {128, 256}) {
+      if (d.block_m > 0 ? r != d.block_m : (r == 256 && !d.conv)) continue;
+      if (pingpong && r != 128) continue;
+      const int k_blocks = d.conv ? (d.conv_kind >= 2 ? 4 : 9) * ((d.Cin + BLOCK_K - 1) / BLOCK_K) : 0;
+      const long long m_tiles = d.conv ? conv_tile(r, d.n_img, oh, ow).tiles * phases : (static_cast<long long>(d.M) + r - 1) / r;
+      for (int c : {64, 128, 160, 192, 256}) {
+        if (d.block_n > 0) c = d.block_n;
+        else if ((d.geglu && c % 64 != 0) || (pingpong && !pingpong_width(c, d.geglu))) continue;
+        const long long n_tiles = (d.N + c - 1) / c, tiles = m_tiles * n_tiles;
+        const bool fits = r == 128 || ((c == 128 || c == 160) && (d.block_m == 256 || (tiles >= sms && k_blocks >= kMinKBlocks256)));
+        if (fits) {
+          const long long waves = (tiles + sms - 1) / sms;
+          const long long cost = waves * (static_cast<long long>(r) * c + kOperandWeight * (r + c)) + (n_tiles * c - d.N) * (r / 2);
+          if (best_cost < 0 || cost <= best_cost) { best_cost = cost; *bm = r; *bn = c; }
+        }
+        if (d.block_n > 0) break;
       }
-      if (d.block_n > 0) break;
     }
+    return best_cost >= 0;
+  };
+  // the time of the tiles an SM runs on either schedule (gemm_choose_tile's header comment), ping-pong strictly faster
+  const auto plain_time = [&](bool pingpong, int bn) {
+    const long long k_blocks = (d.K1 + BLOCK_K - 1) / BLOCK_K + (d.A2 ? (d.K2 + BLOCK_K - 1) / BLOCK_K : 0);
+    const long long tiles = ((static_cast<long long>(d.M) + BLOCK_M - 1) / BLOCK_M) * ((d.N + bn - 1) / bn);
+    const long long per_sm = (tiles + sms - 1) / sms;
+    const long long main = k_blocks * (static_cast<long long>(BLOCK_M) * bn + kOperandWeight * (BLOCK_M + bn));
+    const long long epi = static_cast<long long>(kEpilogueWeight) * bn;
+    return pingpong ? per_sm * std::max(main, epi) + std::min(main, epi) : per_sm * (main + epi);
+  };
+  int sched = d.schedule;
+  if (sched == 0) {
+    int pbm = 0, pbn = 0, cbm = 0, cbn = 0;
+    // an overhanging last N tile costs ping-pong more than the overlap saves (N = 320 at width 128, DESIGN section 5)
+    const bool pp_fits = pp_ok && (d.block_n <= 0 || pingpong_width(d.block_n, d.geglu)) && best_tile(true, &pbm, &pbn) &&
+                         d.N % pbn == 0;
+    D4D_REQUIRE(best_tile(false, &cbm, &cbn), "no tile for this block_m / block_n");
+    sched = pp_fits && plain_time(true, pbn) < plain_time(false, cbn) ? kSchedPingPong : kSchedCooperative;
   }
-  D4D_REQUIRE(best_cost >= 0, "no tile for this block_m / block_n");
+  D4D_REQUIRE(best_tile(sched == kSchedPingPong, block_m, block_n), "no tile for this block_m / block_n");
+  if (schedule) *schedule = sched;
   return 0;
 }
 
@@ -483,8 +555,8 @@ int gemm_prepare(const GemmDesc& d, GemmLaunch* L) {
   D4D_REQUIRE(d.block_n <= 0 || (d.block_n >= 16 && d.block_n <= 256 && d.block_n % 16 == 0 && d.N % d.block_n == 0),
               "no valid block_n");
   D4D_REQUIRE(!d.conv || (d.conv_kind >= 0 && d.conv_kind <= 3), "conv_kind");
-  int bm = 0, bn = 0;
-  if (int rc = gemm_choose_tile(d, sms, &bm, &bn)) return rc;
+  int bm = 0, bn = 0, sched = 0;
+  if (int rc = gemm_choose_tile(d, sms, &bm, &bn, &sched)) return rc;
   a.block_m = bm;
   a.block_n = bn;
   a.n_tiles = (d.N + bn - 1) / bn;
@@ -538,6 +610,9 @@ int gemm_prepare(const GemmDesc& d, GemmLaunch* L) {
     const auto aligned16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
     a.staged = d.kv_world == 0 && (d.geglu ? bn % (2 * SLAB_COLS) : bn % SLAB_COLS) == 0 && aligned16(d.out) &&
                (d.residual == nullptr || aligned16(d.residual));
+    // ping-pong stages its epilogue; an automatic launch that cannot runs cooperatively from registers
+    D4D_REQUIRE(d.schedule != kSchedPingPong || a.staged, "ping-pong needs the staged epilogue (16-byte aligned out / residual)");
+    a.pingpong = a.staged && sched == kSchedPingPong;
     L->tmap_c = L->tmap_r = L->tmap_a;
     if (a.staged) {
       if (int rc = make_tmap_2d(&L->tmap_c, d.out, d.M, d.geglu ? d.N / 2 : d.N, d.ldo, SLAB_COLS, 64, 64)) return rc;
@@ -605,16 +680,22 @@ struct GemmVariant {
   int bn, bm;
   bool geglu, conv;
   int epi;
+  bool pingpong;
   GemmKernelFn fn;
   int smem;
 };
 #define D4D_GV_M(BN, MI, G, C, E) \
-  {BN, 128 * MI, G, C, E, gemm_wgmma_kernel<BN, MI, G, C, E>, GemmCfg<BN, MI, gemm_staged(C, E)>::SMEM}
+  {BN, 128 * MI, G, C, E, false, gemm_wgmma_kernel<BN, MI, G, C, E, false>, GemmCfg<BN, MI, gemm_staged(C, E), false>::SMEM}
 #define D4D_GV(BN, G, C, E) D4D_GV_M(BN, 1, G, C, E)
-#define D4D_GV_PLAIN(BN)                                                                                              \
+#define D4D_GV_PP(BN, G, E) \
+  {BN, 128, G, false, E, true, gemm_wgmma_kernel<BN, 2, G, false, E, true>, GemmCfg<BN, 2, true, true>::SMEM}
+#define D4D_GV_PLAIN(BN, GV)                                                                                          \
   /* plain GEMM: qkv | proj_in, shortcut | attn out, ff2 | proj_out, conv_in */                                       \
-  D4D_GV(BN, false, false, 0), D4D_GV(BN, false, false, E_BIAS), D4D_GV(BN, false, false, E_BIAS | E_RES),           \
-  D4D_GV(BN, false, false, E_BIAS | E_RES | E_STATS), D4D_GV(BN, false, false, E_ALL)
+  GV(BN, false, 0), GV(BN, false, E_BIAS), GV(BN, false, E_BIAS | E_RES), GV(BN, false, E_BIAS | E_RES | E_STATS),     \
+  GV(BN, false, GV##_ALL)
+#define D4D_GV_COOP_ALL E_ALL
+#define D4D_GV_PP_ALL E_STAGED_ALL
+#define D4D_GV_COOP(BN, G, E) D4D_GV(BN, G, false, E)
 #define D4D_GV_CONV(BN, MI)                                                                                           \
   /* 3x3 convs: resnet conv1 | conv2 | down / up sampling */                                                          \
   D4D_GV_M(BN, MI, false, true, E_BIAS | E_ROWVEC | E_STATS), D4D_GV_M(BN, MI, false, true, E_BIAS | E_RES | E_STATS), \
@@ -622,15 +703,22 @@ struct GemmVariant {
 // the feature sets the UNet plan launches (csrc/unet.cu) at the tile widths it picks, plus E_ALL kernels for the rest.
 // GEGLU (only the bias bit matters) runs at widths whose output halves fill whole store slabs; no conv picks 192.
 // 256-row conv tiles (MI = 2) exist where 2 * BN / 2 accumulators per thread fit the 232 registers: widths 128 and 160.
+// Ping-pong kernels (MI = 2 as well) exist at width 128, plain and GEGLU, and at 64 for the all-features set (all but the
+// K/V scatter: ping-pong stages its epilogue).  At 160 the staged epilogue of two 64-row blocks spills.
 const GemmVariant kGemmVariants[] = {
-    D4D_GV_PLAIN(128), D4D_GV_CONV(128, 1), D4D_GV_CONV(128, 2), D4D_GV(128, true, false, E_BIAS),
-    D4D_GV_PLAIN(160), D4D_GV_CONV(160, 1), D4D_GV_CONV(160, 2),
-    D4D_GV_PLAIN(192),
-    D4D_GV_PLAIN(256), D4D_GV_CONV(256, 1), D4D_GV(256, true, false, E_BIAS),
+    D4D_GV_PLAIN(128, D4D_GV_COOP), D4D_GV_CONV(128, 1), D4D_GV_CONV(128, 2), D4D_GV(128, true, false, E_BIAS),
+    D4D_GV_PLAIN(160, D4D_GV_COOP), D4D_GV_CONV(160, 1), D4D_GV_CONV(160, 2),
+    D4D_GV_PLAIN(192, D4D_GV_COOP),
+    D4D_GV_PLAIN(256, D4D_GV_COOP), D4D_GV_CONV(256, 1), D4D_GV(256, true, false, E_BIAS),
     D4D_GV(64, false, false, E_ALL), D4D_GV(64, false, true, E_ALL), D4D_GV(64, true, false, E_BIAS),
+    D4D_GV_PLAIN(128, D4D_GV_PP), D4D_GV_PP(128, true, E_BIAS), D4D_GV_PP(64, false, E_STAGED_ALL),
 };
+#undef D4D_GV_COOP
+#undef D4D_GV_COOP_ALL
+#undef D4D_GV_PP_ALL
 #undef D4D_GV_CONV
 #undef D4D_GV_PLAIN
+#undef D4D_GV_PP
 #undef D4D_GV
 #undef D4D_GV_M
 constexpr int kNumGemmVariants = sizeof(kGemmVariants) / sizeof(kGemmVariants[0]);
@@ -650,7 +738,7 @@ int gemm_variant_at(const GemmKernelArgs& a, int bn) {
   int generic = -1;
   for (int i = 0; i < kNumGemmVariants; ++i) {
     const GemmVariant& v = kGemmVariants[i];
-    if (v.bn != bn || v.bm != a.block_m || v.geglu != geglu || v.conv != conv) continue;
+    if (v.bn != bn || v.bm != a.block_m || v.geglu != geglu || v.conv != conv || v.pingpong != (a.pingpong != 0)) continue;
     if (v.epi == need) return i;
     if ((v.epi & need) == need && (generic < 0 || v.epi == E_ALL)) generic = i;  // geglu: E_BIAS covers {} as well
   }

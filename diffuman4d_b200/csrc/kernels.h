@@ -42,6 +42,7 @@ struct GemmKernelArgs {
   // plain GEMM: the MMA warpgroups stage the output tile in shared memory and TMA stores it (tmap_c); the residual tile
   // arrives by TMA into the same buffer (tmap_r).  0: stores from registers (conv, K/V scatter, narrow block_n)
   int staged;
+  int pingpong;  // staged plain GEMM on the ping-pong schedule: each MMA warpgroup owns every other 128-row tile
   int geglu;
   int act;          // 0 none, 1 SiLU applied to (acc + bias + rowvec) before scale/residual
   float out_scale;  // multiplies (acc + bias + rowvec) after the activation
@@ -77,6 +78,8 @@ struct GemmDesc {
   float out_scale = 1.0f;
   int block_n = 0;  // 0 = auto (64, 128, 160, 192 or 256; the last N tile may overhang)
   int block_m = 0;  // 0 = auto, 128, or 256 (conv at block_n 128 / 160 only)
+  // plain GEMM: 0 = auto, kSchedCooperative, or kSchedPingPong (block_n 64 or 128; GEGLU 128; staged epilogue only)
+  int schedule = 0;
   // GroupNorm statistics of the output (see GemmKernelArgs::stats); plain GEMM: stats_rows = rows per image
   long long* stats = nullptr;
   int stats_rows = 0;
@@ -100,8 +103,11 @@ struct GemmLaunch {
   int grid;
 };
 
-// the tile rows and width gemm_prepare runs d at on a device of `sms` SMs (shape fields and block_m / block_n only)
-int gemm_choose_tile(const GemmDesc& d, int sms, int* block_m, int* block_n);
+constexpr int kSchedCooperative = 1, kSchedPingPong = 2;
+// the tile rows, width and schedule gemm_prepare runs d at on a device of `sms` SMs (shape fields and block_m / block_n /
+// schedule only; `schedule` may be null).  Ping-pong is chosen on shape alone: gemm_prepare runs a launch that cannot
+// stage its epilogue cooperatively.
+int gemm_choose_tile(const GemmDesc& d, int sms, int* block_m, int* block_n, int* schedule = nullptr);
 int gemm_prepare(const GemmDesc& d, GemmLaunch* L);
 int gemm_run(const GemmLaunch& L, cudaStream_t stream);
 double gemm_flops(const GemmLaunch& L);

@@ -235,6 +235,17 @@ int d4d_op_conv_tiled(const void* x_nhwc, int n_img, int H, int W, int Cin, cons
 /* The tile (rows, width) an automatic conv launch of this shape (kind as d4d_op_conv_tiled) takes on a device with `sms`
  * SMs; needs no device. */
 int d4d_conv_tile_choice(int n_img, int H, int W, int Cin, int Cout, int kind, int sms, int* block_m, int* block_n);
+/* d4d_op_gemm at an explicit schedule (d4d_version() 109 and later): 0 automatic, 1 cooperative (both MMA warpgroups
+ * share each 128-row tile), 2 ping-pong (each MMA warpgroup owns every other tile, so one tile's epilogue runs under the
+ * other's MMAs; block_n 0, 64 or 128, GEGLU 0 or 128, 16-byte aligned out and residual).  The output and the
+ * statistics do not depend on the schedule: every sum runs in the same order.  Anything else returns 1, before any launch. */
+int d4d_op_gemm_tiled(const void* A, int lda, int K1, const void* A2, int lda2, int K2, const void* W, int M, int N,
+                      const float* bias, const void* rowvec, int ld_rowvec, int rows_per_image, const void* residual,
+                      int ld_res, void* out, int ldo, int geglu, int act, float out_scale, int block_n, int schedule,
+                      int64_t* stats, int stats_rows, void* stream);
+/* The width and schedule (1 cooperative, 2 ping-pong) an automatic plain GEMM launch of this shape takes on a device with
+ * `sms` SMs (K2: columns of the second source, 0 for none); needs no device. */
+int d4d_gemm_tile_choice(int M, int N, int K1, int K2, int geglu, int sms, int* block_n, int* schedule);
 /* q: column slice of a row-major [batch*seq, ld_qkv] matrix; head hd = columns [hd*D, (hd+1)*D).  k, v: column slices of a
  * row-major [batch*seq_kv, ld_kv] matrix, the keys of batch entry b in rows [b*seq_kv, (b+1)*seq_kv).  seq_kv = 0 means
  * seq and ld_kv = 0 means ld_qkv (k and v in the QKV matrix). */

@@ -30,8 +30,10 @@ HW = (64, 32, 16, 8)
 B, F = 32, 16
 
 
-def plan_shapes():
-    """(kind, name, count, spec) for one forward.  spec: plain {M, N, K1, K2, feats} / conv {n, H, W, Cin, Cout, mode, feats}."""
+def plan_shapes(B=B, s0=HW[0]):
+    """(kind, name, count, spec) for one forward of B images of s0 x s0 latents (default: W16@64², 16 frames with CFG).
+    spec: plain {M, N, K1, K2, feats} / conv {n, H, W, Cin, Cout, mode, feats}."""
+    HW = tuple(s0 >> lvl for lvl in range(4))
     shapes = {}
 
     def add(kind, name, **spec):
@@ -66,7 +68,7 @@ def plan_shapes():
     add("gemm", "tem2", M=B, N=TE, K1=TE, K2=0, feats=("bias", "residual"))
     add("gemm", "temb_all", M=B, N=ldt, K1=TE, K2=0, feats=("bias",))
     # pose encoder (the 2F-image batch of bench.py's by_kind forward): layer 5 as a GEMM over im2col, 6 and 7 as convs
-    PB, s0 = 2 * F, HW[0]
+    PB = B
     add("gemm", "pose l5", M=PB * s0 * s0, N=64, K1=512, K2=0, feats=("bias", "act"))
     add("conv", "pose l6", n=PB, H=s0, W=s0, Cin=64, Cout=64, mode="s1", feats=("bias", "act"))
     add("conv", "pose l7", n=PB, H=s0, W=s0, Cin=64, Cout=128, mode="s1", feats=("bias", "act"))
@@ -106,6 +108,8 @@ def plan_shapes():
 
 OPERAND_WEIGHT = 128  # kOperandWeight of csrc/gemm_wgmma.cu
 MIN_K_BLOCKS_256 = 16  # kMinKBlocks256
+EPILOGUE_WEIGHT = 3072  # kEpilogueWeight
+COOPERATIVE, PINGPONG = 1, 2  # kSchedCooperative, kSchedPingPong
 
 
 def conv_tiles(rows, n, oh, ow):
@@ -126,9 +130,33 @@ def tile_cost(r, c, tiles, N, sms):
     return -(-tiles // sms) * (r * c + OPERAND_WEIGHT * (r + c)) + (n_tiles * c - N) * (r // 2)
 
 
-def auto_tile(N, sms, M=0, geglu=False, conv=None):
+def pingpong_width(c, geglu):
+    return c == 128 or (c == 64 and not geglu)
+
+
+def plain_time(pingpong, c, M, N, K, sms):
+    """gemm_choose_tile's time of the tiles an SM runs on either schedule: ping-pong overlaps each epilogue with the next
+    tile's main loop."""
+    per_sm = -(-(-(-M // 128) * -(-N // c)) // sms)
+    main = -(-K // 64) * (128 * c + OPERAND_WEIGHT * (128 + c))
+    epi = EPILOGUE_WEIGHT * c
+    return per_sm * max(main, epi) + min(main, epi) if pingpong else per_sm * (main + epi)
+
+
+def auto_tile(N, sms, M=0, geglu=False, conv=None, K=0):
     """Mirror of gemm_choose_tile (csrc/gemm_wgmma.cu): the (rows, width) of an automatic launch.  conv = (n, H, W, Cin, mode)
-    with mode "s1" / "s2" / "up" on the H x W input, else a plain GEMM of M rows."""
+    with mode "s1" / "s2" / "up" on the H x W input; else a plain GEMM of M rows and K = K1 + K2 columns, for which the
+    schedule (COOPERATIVE or PINGPONG) comes third."""
+    if not conv:
+        coop = _best_tile(N, sms, M=M, geglu=geglu)
+        pp = _best_tile(N, sms, M=M, geglu=geglu, pingpong=True)
+        if N % pp[1] == 0 and plain_time(True, pp[1], M, N, K, sms) < plain_time(False, coop[1], M, N, K, sms):
+            return pp + (PINGPONG,)
+        return coop + (COOPERATIVE,)
+    return _best_tile(N, sms, conv=conv)
+
+
+def _best_tile(N, sms, M=0, geglu=False, conv=None, pingpong=False):
     if conv:
         n, H, W, Cin, mode = conv
         oh, ow, phases = (H // 2, W // 2, 1) if mode == "s2" else (H, W, 4 if mode == "up" else 1)
@@ -137,7 +165,7 @@ def auto_tile(N, sms, M=0, geglu=False, conv=None):
     for r in (128, 256) if conv else (128,):
         m_tiles = conv_tiles(r, n, oh, ow) * phases if conv else -(-M // r)
         for c in (64, 128, 160, 192, 256):
-            if geglu and c % 64:
+            if (geglu and c % 64) or (pingpong and not pingpong_width(c, geglu)):
                 continue
             tiles = m_tiles * -(-N // c)
             if r == 256 and not (c in (128, 160) and tiles >= sms and k_blocks >= MIN_K_BLOCKS_256):
@@ -188,7 +216,7 @@ def make_launch(kind, spec, dev):
         K = K1 + K2
         flops = 2.0 * M * N * K
         byts = 2.0 * (M * K + N * K + M * nout + (M * N if res is not None else 0))
-        return run, flops, byts, auto_tile(N, torch.cuda.get_device_properties(0).multi_processor_count, M=M, geglu=geglu)
+        return run, flops, byts, auto_tile(N, torch.cuda.get_device_properties(0).multi_processor_count, M=M, geglu=geglu, K=K)
     n, H, W, Cin, Cout, mode = spec["n"], spec["H"], spec["W"], spec["Cin"], spec["Cout"], spec["mode"]
     x = r(n, H, W, Cin)
     bias = torch.randn(Cout, generator=g).to(dev) if "bias" in f else None
@@ -225,7 +253,7 @@ def make_launch(kind, spec, dev):
                   "d4d_op_conv3x3")
     flops = 2.0 * Mo * Cout * taps * Cin
     byts = 2.0 * (x.numel() + taps * Cin * Cout + Mo * Cout * (2 if "residual" in f else 1))
-    return run, flops, byts, auto_tile(Cout, torch.cuda.get_device_properties(0).multi_processor_count, conv=(n, H, W, Cin, mode))
+    return run, flops, byts, auto_tile(Cout, torch.cuda.get_device_properties(0).multi_processor_count, conv=(n, H, W, Cin, mode)) + (0,)
 
 
 def time_launch(run, reps):
@@ -259,11 +287,12 @@ def main():
     peak = 4096.0 * sms * max_mhz * 1e6
     print(f"# {name}, power limit {power_w:.0f} W, max SM clock {max_mhz:.0f} MHz, {sms} SMs; "
           f"tensor peak {peak / 1e12:.0f} TFLOP/s (4096 FLOP/clk/SM at max clock), HBM 3.35 TB/s")
-    hdr = f"{'kind':5} {'shape':58} {'cnt':>3} {'rows':>4} {'bn':>4} {'us':>9} {'TFLOP/s':>8} {'MB':>8} {'GB/s':>7} {'min us':>8} {'bound':>6} {'eff':>5}"
+    hdr = f"{'kind':5} {'shape':58} {'cnt':>3} {'rows':>4} {'bn':>4} {'sched':>5} {'us':>9} {'TFLOP/s':>8} {'MB':>8} {'GB/s':>7} {'min us':>8} {'bound':>6} {'eff':>5}"
     print(hdr)
     rows, tot = [], {"gemm": 0.0, "conv": 0.0}
     for kind, nm, cnt, spec in plan_shapes():
-        run, flops, byts, (bm, bn) = make_launch(kind, spec, dev)
+        run, flops, byts, (bm, bn, sched) = make_launch(kind, spec, dev)
+        sched_name = {0: "-", COOPERATIVE: "coop", PINGPONG: "pp"}[sched]
         us = time_launch(run, args.reps)
         t_f, t_b = flops / peak * 1e6, byts / HBM_BPS * 1e6
         bound = "tensor" if t_f >= t_b else "HBM"
@@ -271,11 +300,11 @@ def main():
         dims = (f"M{spec['M']} N{spec['N']} K{spec['K1']}" + (f"+{spec['K2']}" if spec["K2"] else "")) if kind == "gemm" else \
             f"{spec['n']}x{spec['H']}x{spec['W']} {spec['Cin']}->{spec['Cout']} {spec['mode']}"
         label = f"{nm}: {dims} [{','.join(spec['feats']) or '-'}]"
-        print(f"{kind:5} {label:58} {cnt:3d} {bm:4d} {bn:4d} {us:9.1f} {flops / us / 1e6:8.1f} {byts / 1e6:8.1f} "
+        print(f"{kind:5} {label:58} {cnt:3d} {bm:4d} {bn:4d} {sched_name:>5} {us:9.1f} {flops / us / 1e6:8.1f} {byts / 1e6:8.1f} "
               f"{byts / us / 1e3:7.0f} {tmin:8.1f} {bound:>6} {tmin / us:5.2f}")
         tot[kind] += cnt * us
         rows.append({"kind": kind, "name": nm, "spec": {k: (list(v) if isinstance(v, tuple) else v) for k, v in spec.items()},
-                     "count": cnt, "block_m": bm, "block_n": bn, "us": us, "tflops": flops / us / 1e6, "bytes": byts,
+                     "count": cnt, "block_m": bm, "block_n": bn, "schedule": sched_name, "us": us, "tflops": flops / us / 1e6, "bytes": byts,
                      "gbps": byts / us / 1e3, "min_us": tmin, "bound": bound})
         del run
         torch.cuda.empty_cache()
