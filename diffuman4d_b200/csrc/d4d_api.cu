@@ -78,8 +78,25 @@ d4d::WindowStep ddim_step(const d4d_sched* sched) {
 
 d4d::WindowStep dpm_step(const d4d_dpm_sched* sched, void* x0_prev, int32_t* lower_order_nums) {
   d4d::WindowStep s;
-  s.dpm = sched; s.x0_prev = static_cast<bf16*>(x0_prev); s.lower_order_nums = lower_order_nums;
+  s.dpm = sched;
+  s.state.x0_prev = static_cast<bf16*>(x0_prev);
+  s.state.lower_order_nums = s.state.lower_order_nums_out = lower_order_nums;
   return s;
+}
+
+// the step arguments of every d4d_cfg_*_step entry point
+d4d::StepArgs step_args(const void* noise, const void* latents, const void* cond_mask, const int64_t* timestep_indices,
+                        int64_t* timestep_indices_out, float guidance_scale, int cfg, int F, int height, int width,
+                        void* latents_out) {
+  d4d::StepArgs a;
+  const int hw = height * width;
+  a.noise = static_cast<const bf16*>(noise); a.latents = static_cast<const bf16*>(latents);
+  a.mask = static_cast<const bf16*>(cond_mask);
+  a.timestep_indices = reinterpret_cast<const long long*>(timestep_indices);
+  a.F = F; a.chw = 4 * hw; a.hw = hw; a.cfg = cfg; a.guidance = guidance_scale;
+  a.out = static_cast<bf16*>(latents_out);
+  a.ts_out = reinterpret_cast<long long*>(timestep_indices_out);
+  return a;
 }
 }  // namespace
 
@@ -209,8 +226,10 @@ int d4d_denoise_window_unipc(d4d_handle* h, void* latents, const void* pixel_lat
                              int num_steps, void* x0_prev, void* x0_prev2, void* last_sample, int32_t* lower_order_nums,
                              void* stream) {
   d4d::WindowStep s;
-  s.unipc = sched; s.x0_prev = static_cast<bf16*>(x0_prev); s.x0_prev2 = static_cast<bf16*>(x0_prev2);
-  s.last_sample = static_cast<bf16*>(last_sample); s.lower_order_nums = lower_order_nums;
+  s.unipc = sched;
+  s.state.x0_prev = static_cast<bf16*>(x0_prev); s.state.x0_prev2 = static_cast<bf16*>(x0_prev2);
+  s.state.last_sample = static_cast<bf16*>(last_sample);
+  s.state.lower_order_nums = s.state.lower_order_nums_out = lower_order_nums;
   return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, s, guidance_scale,
                         domain, F, 0, height, width, num_steps, stream);
 }
@@ -241,21 +260,10 @@ int d4d_cfg_ddim_step(const void* noise, const void* latents, const void* cond_m
                       int64_t* timestep_indices_out, const d4d_sched* sched, float guidance_scale, int cfg, int F,
                       int height, int width, void* latents_out, void* stream) {
   D4D_API_BEGIN
-  D4D_REQUIRE(noise && latents && cond_mask && timestep_indices && timestep_indices_out && sched && latents_out,
-              "null argument");
-  D4D_REQUIRE(timestep_indices != timestep_indices_out, "timestep_indices_out must not alias timestep_indices");
-  d4d::DdimArgs d;
-  const int hw = height * width;
-  d.noise = static_cast<const bf16*>(noise); d.latents = static_cast<const bf16*>(latents);
-  d.mask = static_cast<const bf16*>(cond_mask);
-  d.timestep_indices = reinterpret_cast<const long long*>(timestep_indices);
-  d.timesteps_table = reinterpret_cast<const long long*>(sched->timesteps_table);
-  d.alphas_cumprod = sched->alphas_cumprod;
-  d.n_steps = sched->n_steps; d.T = sched->num_train_timesteps; d.final_alpha_cumprod = sched->final_alpha_cumprod;
-  d.F = F; d.chw = 4 * hw; d.hw = hw; d.cfg = cfg; d.guidance = guidance_scale;
-  d.prediction_type = sched->prediction_type; d.clip_sample = sched->clip_sample; d.clip_range = sched->clip_sample_range;
-  d.emulate_bf16 = sched->emulate_bf16; d.out = static_cast<bf16*>(latents_out);
-  return d4d::cfg_ddim_step_run(d, reinterpret_cast<long long*>(timestep_indices_out), static_cast<cudaStream_t>(stream));
+  D4D_REQUIRE(sched != nullptr, "null argument");
+  return d4d::cfg_step_run(step_args(noise, latents, cond_mask, timestep_indices, timestep_indices_out, guidance_scale, cfg,
+                                     F, height, width, latents_out),
+                           *sched, d4d::SolverState(), static_cast<cudaStream_t>(stream));
   D4D_API_END
 }
 
@@ -264,21 +272,13 @@ int d4d_cfg_dpm_step(const void* noise, const void* latents, const void* cond_ma
                      int32_t* lower_order_nums_out, const d4d_dpm_sched* sched, float guidance_scale, int cfg, int F,
                      int height, int width, void* latents_out, void* stream) {
   D4D_API_BEGIN
-  D4D_REQUIRE(noise && latents && cond_mask && timestep_indices && timestep_indices_out && x0_prev && lower_order_nums &&
-                  lower_order_nums_out && sched && sched->timesteps_table && sched->coefs && latents_out,
-              "null argument");
-  d4d::DpmArgs d;
-  const int hw = height * width;
-  d.noise = static_cast<const bf16*>(noise); d.latents = static_cast<const bf16*>(latents);
-  d.mask = static_cast<const bf16*>(cond_mask);
-  d.timestep_indices = reinterpret_cast<const long long*>(timestep_indices);
-  d.coefs = sched->coefs; d.n_steps = sched->n_steps;
-  d.F = F; d.chw = 4 * hw; d.hw = hw; d.cfg = cfg; d.guidance = guidance_scale;
-  d.prediction_type = sched->prediction_type; d.solver_order = sched->solver_order;
-  d.final_first_order = sched->final_first_order; d.emulate_bf16 = sched->emulate_bf16;
-  d.x0_prev = static_cast<bf16*>(x0_prev); d.lower_order_nums = lower_order_nums;
-  d.lower_order_nums_out = lower_order_nums_out; d.out = static_cast<bf16*>(latents_out);
-  return d4d::cfg_dpm_step_run(d, reinterpret_cast<long long*>(timestep_indices_out), static_cast<cudaStream_t>(stream));
+  D4D_REQUIRE(sched != nullptr, "null argument");
+  d4d::SolverState st;
+  st.x0_prev = static_cast<bf16*>(x0_prev);
+  st.lower_order_nums = lower_order_nums; st.lower_order_nums_out = lower_order_nums_out;
+  return d4d::cfg_step_run(step_args(noise, latents, cond_mask, timestep_indices, timestep_indices_out, guidance_scale, cfg,
+                                     F, height, width, latents_out),
+                           *sched, st, static_cast<cudaStream_t>(stream));
   D4D_API_END
 }
 
@@ -287,21 +287,14 @@ int d4d_cfg_unipc_step(const void* noise, const void* latents, const void* cond_
                        const int32_t* lower_order_nums, int32_t* lower_order_nums_out, const d4d_unipc_sched* sched,
                        float guidance_scale, int cfg, int F, int height, int width, void* latents_out, void* stream) {
   D4D_API_BEGIN
-  D4D_REQUIRE(noise && latents && cond_mask && timestep_indices && timestep_indices_out && x0_prev && last_sample &&
-                  lower_order_nums && lower_order_nums_out && sched && sched->timesteps_table && sched->coefs && latents_out,
-              "null argument");
-  d4d::UniPCArgs d;
-  const int hw = height * width;
-  d.noise = static_cast<const bf16*>(noise); d.latents = static_cast<const bf16*>(latents);
-  d.mask = static_cast<const bf16*>(cond_mask);
-  d.timestep_indices = reinterpret_cast<const long long*>(timestep_indices);
-  d.coefs = sched->coefs; d.n_steps = sched->n_steps;
-  d.F = F; d.chw = 4 * hw; d.hw = hw; d.cfg = cfg; d.guidance = guidance_scale;
-  d.prediction_type = sched->prediction_type; d.solver_order = sched->solver_order; d.emulate_bf16 = sched->emulate_bf16;
-  d.x0_prev = static_cast<bf16*>(x0_prev); d.x0_prev2 = static_cast<bf16*>(x0_prev2);
-  d.last_sample = static_cast<bf16*>(last_sample); d.lower_order_nums = lower_order_nums;
-  d.lower_order_nums_out = lower_order_nums_out; d.out = static_cast<bf16*>(latents_out);
-  return d4d::cfg_unipc_step_run(d, reinterpret_cast<long long*>(timestep_indices_out), static_cast<cudaStream_t>(stream));
+  D4D_REQUIRE(sched != nullptr, "null argument");
+  d4d::SolverState st;
+  st.x0_prev = static_cast<bf16*>(x0_prev); st.x0_prev2 = static_cast<bf16*>(x0_prev2);
+  st.last_sample = static_cast<bf16*>(last_sample);
+  st.lower_order_nums = lower_order_nums; st.lower_order_nums_out = lower_order_nums_out;
+  return d4d::cfg_step_run(step_args(noise, latents, cond_mask, timestep_indices, timestep_indices_out, guidance_scale, cfg,
+                                     F, height, width, latents_out),
+                           *sched, st, static_cast<cudaStream_t>(stream));
   D4D_API_END
 }
 

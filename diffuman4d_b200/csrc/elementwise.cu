@@ -1,6 +1,6 @@
 // HBM-/latency-bound helper kernels of the denoise step: embeddings, layout changes feeding the
 // tensor-core kernels, the pose-encoder's small-channel convolutions, and the fused pipeline pieces
-// (input assembly, CFG combine + per-frame DDIM update).  All global traffic is 128-bit where the
+// (input assembly, CFG combine + per-frame scheduler step).  All global traffic is 128-bit where the
 // layout allows it.
 #include "kernels.h"
 
@@ -318,107 +318,103 @@ __global__ void fill_bf16_kernel(bf16* __restrict__ p, long long n, float v) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// a-13 + a-14: CFG combine + per-frame DDIM step (pipeline_diffuman4d.py:408-423, upstream DDIMScheduler.step)
+// a-13 + a-14: CFG combine + per-frame scheduler step (pipeline_diffuman4d.py:408-423).  One kernel per scheduler, one CTA
+// row per frame (blockIdx.y); a frame's step index is its timestep index.  The helpers below are the part all three share.
 // ---------------------------------------------------------------------------------------------
 template <bool EMU>
 __device__ __forceinline__ float rnd(float x) { return EMU ? bf16_round(x) : x; }
-
-template <bool EMU>
-__global__ void cfg_ddim_kernel(const DdimArgs a, long long* ts_out) {
-  const int f = blockIdx.y;
-  const bool is_cond = __bfloat162float(a.mask[static_cast<size_t>(f) * a.hw]) == 0.f;
-  long long idx = a.timestep_indices[f];
-  if (blockIdx.x == 0 && threadIdx.x == 0) ts_out[f] = is_cond ? 0 : idx + 1;
-  const size_t base = static_cast<size_t>(f) * a.chw;
-  if (is_cond) {
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.chw; i += gridDim.x * blockDim.x)
-      a.out[base + i] = a.latents[base + i];
-    return;
-  }
-  idx = idx < 0 ? 0 : (idx >= a.n_steps ? a.n_steps - 1 : idx);
-  const long long t = a.timesteps_table[idx];
-  const long long prev_t = t - a.T / a.n_steps;
-  const float a_t = a.alphas_cumprod[t];
-  const float a_prev = prev_t >= 0 ? a.alphas_cumprod[prev_t] : a.final_alpha_cumprod;
-  const float b_t = 1.0f - a_t;
-  const float sa = sqrtf(a_t), sb = sqrtf(b_t);
-  const float sa_prev = sqrtf(a_prev), sdir = sqrtf(1.0f - a_prev);
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.chw; i += gridDim.x * blockDim.x) {
-    float eps_in;
-    if (a.cfg) {
-      const float u = __bfloat162float(a.noise[base + i]);
-      const float c = __bfloat162float(a.noise[static_cast<size_t>(a.F) * a.chw + base + i]);
-      // u + g * (c - u)
-      eps_in = rnd<EMU>(u + rnd<EMU>(a.guidance * rnd<EMU>(c - u)));
-    } else {
-      eps_in = __bfloat162float(a.noise[base + i]);
-    }
-    const float x = __bfloat162float(a.latents[base + i]);
-    float x0, eps;
-    if (a.prediction_type == 0) {        // epsilon
-      x0 = rnd<EMU>(rnd<EMU>(x - rnd<EMU>(sb * eps_in)) / sa);
-      eps = eps_in;
-    } else if (a.prediction_type == 1) { // v_prediction
-      x0 = rnd<EMU>(rnd<EMU>(sa * x) - rnd<EMU>(sb * eps_in));
-      eps = rnd<EMU>(rnd<EMU>(sa * eps_in) + rnd<EMU>(sb * x));
-    } else {                             // sample
-      x0 = eps_in;
-      eps = rnd<EMU>(rnd<EMU>(x - rnd<EMU>(sa * x0)) / sb);
-    }
-    if (a.clip_sample) x0 = fminf(fmaxf(x0, -a.clip_range), a.clip_range);
-    const float dir = rnd<EMU>(sdir * eps);
-    const float prev = rnd<EMU>(rnd<EMU>(sa_prev * x0) + dir);
-    a.out[base + i] = __float2bfloat16_rn(prev);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// CFG combine + per-frame DPM-Solver++ step (upstream DPMSolverMultistepScheduler.step, dpmsolver++ / midpoint, order
-// <= 2).  Every frame carries its own history (x0_prev, lower_order_nums); its step index is its timestep index.
-// ---------------------------------------------------------------------------------------------
 // fp32 a - b without contraction into an FMA with a preceding product (the reference evaluates each op separately)
 template <bool EMU>
 __device__ __forceinline__ float sub_nc(float a, float b) { return EMU ? __fsub_rn(a, b) : a - b; }
 template <bool EMU>
 __device__ __forceinline__ float mul_nc(float a, float b) { return EMU ? __fmul_rn(a, b) : a * b; }
 
-template <bool EMU>
-__global__ void cfg_dpm_kernel(const DpmArgs a, long long* ts_out) {
+// The frame prologue: writes the frame's advanced timestep index and, for a multistep solver (lon_in != null), its
+// advanced order count.  A conditioning frame is never stepped: its latents pass through and its history stays untouched;
+// the function returns false for it.  Otherwise idx receives the step index clamped to the table, lon the order count.
+__device__ __forceinline__ bool step_frame(const StepArgs& a, int n_steps, const int* lon_in, int* lon_out,
+                                           int solver_order, long long& idx, int& lon) {
   const int f = blockIdx.y;
   const bool is_cond = __bfloat162float(a.mask[static_cast<size_t>(f) * a.hw]) == 0.f;
-  long long idx = a.timestep_indices[f];
-  const int lon = a.lower_order_nums[f];
+  idx = a.timestep_indices[f];
+  lon = lon_in ? lon_in[f] : 0;
   if (blockIdx.x == 0 && threadIdx.x == 0) {
-    ts_out[f] = is_cond ? 0 : idx + 1;
-    a.lower_order_nums_out[f] = is_cond ? lon : min(lon + 1, a.solver_order);
+    a.ts_out[f] = is_cond ? 0 : idx + 1;
+    if (lon_out) lon_out[f] = is_cond ? lon : min(lon + 1, solver_order);
   }
-  const size_t base = static_cast<size_t>(f) * a.chw;
-  if (is_cond) {  // never stepped: latents pass through, history untouched
+  if (is_cond) {
+    const size_t base = static_cast<size_t>(f) * a.chw;
     if (a.out != a.latents)
       for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.chw; i += gridDim.x * blockDim.x)
         a.out[base + i] = a.latents[base + i];
-    return;
+    return false;
   }
-  idx = idx < 0 ? 0 : (idx >= a.n_steps ? a.n_steps - 1 : idx);
-  const float* k = a.coefs + idx * kDpmCoefs;
-  const float alpha_s = k[0], sigma_s = k[1], ratio = k[2], c = k[3], half_c = k[4], inv_r0 = k[5];
-  const bool first = a.solver_order == 1 || lon < 1 || (a.final_first_order && idx == a.n_steps - 1);
+  idx = idx < 0 ? 0 : (idx >= n_steps ? n_steps - 1 : idx);
+  return true;
+}
+
+// The model output at element j of the frames: the CFG combine u + g * (c - u) of the two halves, or the one prediction.
+template <bool EMU>
+__device__ __forceinline__ float model_output(const StepArgs& a, size_t j) {
+  if (!a.cfg) return __bfloat162float(a.noise[j]);
+  const float u = __bfloat162float(a.noise[j]);
+  const float c = __bfloat162float(a.noise[static_cast<size_t>(a.F) * a.chw + j]);
+  return rnd<EMU>(u + rnd<EMU>(a.guidance * rnd<EMU>(c - u)));
+}
+
+// convert_model_output: the data prediction of model output m at sample x (alpha_t, sigma_t of the step), computed in
+// the model output's dtype.
+template <bool EMU>
+__device__ __forceinline__ float data_prediction(int prediction_type, float x, float m, float alpha, float sigma) {
+  if (prediction_type == 0) return rnd<EMU>(rnd<EMU>(x - rnd<EMU>(sigma * m)) / alpha);   // epsilon
+  if (prediction_type == 1) return rnd<EMU>(rnd<EMU>(alpha * x) - rnd<EMU>(sigma * m));   // v_prediction
+  return m;                                                                             // sample
+}
+
+// upstream DDIMScheduler.step
+template <bool EMU>
+__global__ void cfg_ddim_kernel(const StepArgs a, const d4d_sched s) {
+  long long idx;
+  int lon;
+  if (!step_frame(a, s.n_steps, nullptr, nullptr, 0, idx, lon)) return;
+  const size_t base = static_cast<size_t>(blockIdx.y) * a.chw;
+  const long long t = s.timesteps_table[idx];
+  const long long prev_t = t - s.num_train_timesteps / s.n_steps;
+  const float a_t = s.alphas_cumprod[t];
+  const float a_prev = prev_t >= 0 ? s.alphas_cumprod[prev_t] : s.final_alpha_cumprod;
+  const float b_t = 1.0f - a_t;
+  const float sa = sqrtf(a_t), sb = sqrtf(b_t);
+  const float sa_prev = sqrtf(a_prev), sdir = sqrtf(1.0f - a_prev);
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.chw; i += gridDim.x * blockDim.x) {
-    float m;
-    if (a.cfg) {
-      const float u = __bfloat162float(a.noise[base + i]);
-      const float cn = __bfloat162float(a.noise[static_cast<size_t>(a.F) * a.chw + base + i]);
-      m = rnd<EMU>(u + rnd<EMU>(a.guidance * rnd<EMU>(cn - u)));   // u + g * (c - u), as in cfg_ddim_kernel
-    } else {
-      m = __bfloat162float(a.noise[base + i]);
-    }
+    const float eps_in = model_output<EMU>(a, base + i);
     const float x = __bfloat162float(a.latents[base + i]);
-    float x0;  // convert_model_output: runs in the model output's dtype
-    if (a.prediction_type == 0) x0 = rnd<EMU>(rnd<EMU>(x - rnd<EMU>(sigma_s * m)) / alpha_s);
-    else if (a.prediction_type == 1) x0 = rnd<EMU>(rnd<EMU>(alpha_s * x) - rnd<EMU>(sigma_s * m));
-    else x0 = m;
-    const float m1 = __bfloat162float(a.x0_prev[base + i]);
-    a.x0_prev[base + i] = __float2bfloat16_rn(x0);
+    float x0 = data_prediction<EMU>(s.prediction_type, x, eps_in, sa, sb);
+    float eps = eps_in;
+    if (s.prediction_type == 1) eps = rnd<EMU>(rnd<EMU>(sa * eps_in) + rnd<EMU>(sb * x));
+    else if (s.prediction_type == 2) eps = rnd<EMU>(rnd<EMU>(x - rnd<EMU>(sa * x0)) / sb);
+    if (s.clip_sample) x0 = fminf(fmaxf(x0, -s.clip_sample_range), s.clip_sample_range);
+    const float dir = rnd<EMU>(sdir * eps);
+    const float prev = rnd<EMU>(rnd<EMU>(sa_prev * x0) + dir);
+    a.out[base + i] = __float2bfloat16_rn(prev);
+  }
+}
+
+// upstream DPMSolverMultistepScheduler.step (dpmsolver++ / midpoint, order <= 2); history x0_prev, lower_order_nums
+template <bool EMU>
+__global__ void cfg_dpm_kernel(const StepArgs a, const d4d_dpm_sched s, const SolverState st) {
+  long long idx;
+  int lon;
+  if (!step_frame(a, s.n_steps, st.lower_order_nums, st.lower_order_nums_out, s.solver_order, idx, lon)) return;
+  const size_t base = static_cast<size_t>(blockIdx.y) * a.chw;
+  const float* k = s.coefs + idx * kDpmCoefs;
+  const float alpha_s = k[0], sigma_s = k[1], ratio = k[2], c = k[3], half_c = k[4], inv_r0 = k[5];
+  const bool first = s.solver_order == 1 || lon < 1 || (s.final_first_order && idx == s.n_steps - 1);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.chw; i += gridDim.x * blockDim.x) {
+    const float m = model_output<EMU>(a, base + i);
+    const float x = __bfloat162float(a.latents[base + i]);
+    const float x0 = data_prediction<EMU>(s.prediction_type, x, m, alpha_s, sigma_s);
+    const float m1 = __bfloat162float(st.x0_prev[base + i]);
+    st.x0_prev[base + i] = __float2bfloat16_rn(x0);
     // sample is upcast to fp32: (sigma_t / sigma_s) * sample stays fp32, each coef * (bf16 tensor) rounds to bf16
     float prev = sub_nc<EMU>(mul_nc<EMU>(ratio, x), rnd<EMU>(c * x0));
     if (!first) {
@@ -429,56 +425,32 @@ __global__ void cfg_dpm_kernel(const DpmArgs a, long long* ts_out) {
   }
 }
 
-// ---------------------------------------------------------------------------------------------
-// CFG combine + per-frame UniPC step (upstream UniPCMultistepScheduler.step, predict_x0, bh1 / bh2, order <= 2).  Every
-// frame carries its own history (x0_prev, x0_prev2, last_sample, lower_order_nums); its step index is its timestep index.
-// Unlike DPM-Solver++, upstream does not upcast the sample: every product and difference rounds to bf16 in EMU mode.
-// ---------------------------------------------------------------------------------------------
+// upstream UniPCMultistepScheduler.step (predict_x0, bh1 / bh2, order <= 2); history x0_prev, x0_prev2, last_sample,
+// lower_order_nums.  Unlike DPM-Solver++, upstream does not upcast the sample: every product and difference rounds to
+// bf16 in EMU mode.
 template <bool EMU>
-__global__ void cfg_unipc_kernel(const UniPCArgs a, long long* ts_out) {
-  const int f = blockIdx.y;
-  const bool is_cond = __bfloat162float(a.mask[static_cast<size_t>(f) * a.hw]) == 0.f;
-  long long idx = a.timestep_indices[f];
-  const int lon = a.lower_order_nums[f];
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    ts_out[f] = is_cond ? 0 : idx + 1;
-    a.lower_order_nums_out[f] = is_cond ? lon : min(lon + 1, a.solver_order);
-  }
-  const size_t base = static_cast<size_t>(f) * a.chw;
-  if (is_cond) {  // never stepped: latents pass through, history untouched
-    if (a.out != a.latents)
-      for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.chw; i += gridDim.x * blockDim.x)
-        a.out[base + i] = a.latents[base + i];
-    return;
-  }
-  idx = idx < 0 ? 0 : (idx >= a.n_steps ? a.n_steps - 1 : idx);
-  const float* k = a.coefs + idx * kUniPCCoefs;
+__global__ void cfg_unipc_kernel(const StepArgs a, const d4d_unipc_sched s, const SolverState st) {
+  long long idx;
+  int lon;
+  if (!step_frame(a, s.n_steps, st.lower_order_nums, st.lower_order_nums_out, s.solver_order, idx, lon)) return;
+  const size_t base = static_cast<size_t>(blockIdx.y) * a.chw;
+  const float* k = s.coefs + idx * kUniPCCoefs;
   const float alpha_s = k[0], sigma_s = k[1];
   const float p_ratio = k[2], p_cphi = k[3], p_cB = k[4], p_rk = k[5];
   const float c_ratio = k[6], c_cphi = k[7], c_cB = k[8], c_rk = k[9];
   const float rho0 = rnd<EMU>(k[10]), rho1 = rnd<EMU>(k[11]);   // upstream casts the solved rhos to the sample dtype
   // the corrector runs at the previous step's order, which is lon; the predictor's order is capped by the row
   const bool correct = lon >= 1 && k[12] != 0.f;
-  const int c_order = min(lon, a.solver_order);
+  const int c_order = min(lon, s.solver_order);
   const int p_order = min(static_cast<int>(k[13]), lon + 1);
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.chw; i += gridDim.x * blockDim.x) {
-    float m;
-    if (a.cfg) {
-      const float u = __bfloat162float(a.noise[base + i]);
-      const float cn = __bfloat162float(a.noise[static_cast<size_t>(a.F) * a.chw + base + i]);
-      m = rnd<EMU>(u + rnd<EMU>(a.guidance * rnd<EMU>(cn - u)));   // u + g * (c - u), as in cfg_ddim_kernel
-    } else {
-      m = __bfloat162float(a.noise[base + i]);
-    }
+    const float m = model_output<EMU>(a, base + i);
     float x = __bfloat162float(a.latents[base + i]);
-    float x0;  // convert_model_output: runs in the model output's dtype
-    if (a.prediction_type == 0) x0 = rnd<EMU>(rnd<EMU>(x - rnd<EMU>(sigma_s * m)) / alpha_s);
-    else if (a.prediction_type == 1) x0 = rnd<EMU>(rnd<EMU>(alpha_s * x) - rnd<EMU>(sigma_s * m));
-    else x0 = m;
-    const float m0 = __bfloat162float(a.x0_prev[base + i]);
-    const float m1 = a.x0_prev2 ? __bfloat162float(a.x0_prev2[base + i]) : 0.f;
+    const float x0 = data_prediction<EMU>(s.prediction_type, x, m, alpha_s, sigma_s);
+    const float m0 = __bfloat162float(st.x0_prev[base + i]);
+    const float m1 = st.x0_prev2 ? __bfloat162float(st.x0_prev2[base + i]) : 0.f;
     if (correct) {  // UniC: recompute the sample from last_sample with this step's data prediction
-      const float last = __bfloat162float(a.last_sample[base + i]);
+      const float last = __bfloat162float(st.last_sample[base + i]);
       const float xt = rnd<EMU>(sub_nc<EMU>(rnd<EMU>(c_ratio * last), rnd<EMU>(c_cphi * m0)));
       const float d1t = rnd<EMU>(x0 - m0);
       float inner;
@@ -490,9 +462,9 @@ __global__ void cfg_unipc_kernel(const UniPCArgs a, long long* ts_out) {
       }
       x = rnd<EMU>(sub_nc<EMU>(xt, rnd<EMU>(c_cB * inner)));
     }
-    if (a.x0_prev2) a.x0_prev2[base + i] = __float2bfloat16_rn(m0);
-    a.x0_prev[base + i] = __float2bfloat16_rn(x0);
-    a.last_sample[base + i] = __float2bfloat16_rn(x);
+    if (st.x0_prev2) st.x0_prev2[base + i] = __float2bfloat16_rn(m0);
+    st.x0_prev[base + i] = __float2bfloat16_rn(x0);
+    st.last_sample[base + i] = __float2bfloat16_rn(x);
     // UniP from the (corrected) sample
     const float xt = rnd<EMU>(sub_nc<EMU>(rnd<EMU>(p_ratio * x), rnd<EMU>(p_cphi * x0)));
     float prev;
@@ -708,41 +680,55 @@ int fill_bf16_run(bf16* p, long long n, float v, cudaStream_t stream) {
   return 0;
 }
 
-int cfg_ddim_step_run(const DdimArgs& a, long long* ts_out, cudaStream_t stream) {
-  D4D_REQUIRE(a.n_steps > 0 && a.T > 0 && a.F > 0, "ddim args");
+// The checks every scheduler step shares.  coefs: the table the kernel reads besides the timesteps (alphas_cumprod for
+// DDIM); st: the solver state of a multistep solver, null for DDIM.  A block advancing a frame's counters must not change
+// what the frame's other blocks still read, hence no aliasing of the counter outputs.
+static int check_step(const StepArgs& a, const int64_t* timesteps_table, const float* coefs, int n_steps,
+                      int prediction_type, const SolverState* st) {
+  D4D_REQUIRE(a.noise && a.latents && a.mask && a.timestep_indices && a.out && a.ts_out && timesteps_table && coefs,
+              "null argument");
+  D4D_REQUIRE(a.F > 0 && n_steps > 0, "the frame and step counts must be positive");
+  D4D_REQUIRE(prediction_type >= 0 && prediction_type <= 2, "prediction_type");
+  D4D_REQUIRE(a.ts_out != a.timestep_indices, "timestep_indices_out must not alias timestep_indices");
+  if (st) {
+    D4D_REQUIRE(st->x0_prev && st->lower_order_nums && st->lower_order_nums_out, "null argument");
+    D4D_REQUIRE(st->lower_order_nums != st->lower_order_nums_out,
+                "the timestep index and order count outputs may not alias their inputs");
+  }
+  return 0;
+}
+
+// grid (blocks per frame, F) and the fp32 / bf16-emulating instantiation of a step kernel
+template <typename... Rest>
+static int launch_step(void (*emu)(StepArgs, Rest...), void (*fp32)(StepArgs, Rest...), bool emulate_bf16,
+                       cudaStream_t stream, const StepArgs& a, const Rest&... rest) {
   dim3 grid(min(64, blocks_for(a.chw, 256)), a.F);
-  if (a.emulate_bf16) cfg_ddim_kernel<true><<<grid, 256, 0, stream>>>(a, ts_out);
-  else cfg_ddim_kernel<false><<<grid, 256, 0, stream>>>(a, ts_out);
+  (emulate_bf16 ? emu : fp32)<<<grid, 256, 0, stream>>>(a, rest...);
   D4D_CUDA_OK(cudaGetLastError());
   return 0;
 }
 
-int cfg_dpm_step_run(const DpmArgs& a, long long* ts_out, cudaStream_t stream) {
-  D4D_REQUIRE(a.n_steps > 0 && a.F > 0 && a.coefs && a.x0_prev && a.lower_order_nums && a.lower_order_nums_out, "dpm args");
-  D4D_REQUIRE(a.solver_order == 1 || a.solver_order == 2, "solver_order must be 1 or 2");
-  D4D_REQUIRE(a.prediction_type >= 0 && a.prediction_type <= 2, "prediction_type");
-  D4D_REQUIRE(a.lower_order_nums != a.lower_order_nums_out && ts_out != a.timestep_indices,
-              "the timestep index and order count outputs may not alias their inputs");
-  dim3 grid(min(64, blocks_for(a.chw, 256)), a.F);
-  if (a.emulate_bf16) cfg_dpm_kernel<true><<<grid, 256, 0, stream>>>(a, ts_out);
-  else cfg_dpm_kernel<false><<<grid, 256, 0, stream>>>(a, ts_out);
-  D4D_CUDA_OK(cudaGetLastError());
-  return 0;
+int cfg_step_run(const StepArgs& a, const d4d_sched& s, const SolverState&, cudaStream_t stream, bool launch) {
+  if (int rc = check_step(a, s.timesteps_table, s.alphas_cumprod, s.n_steps, s.prediction_type, nullptr)) return rc;
+  D4D_REQUIRE(s.num_train_timesteps > 0, "ddim args");
+  if (!launch) return 0;
+  return launch_step(cfg_ddim_kernel<true>, cfg_ddim_kernel<false>, s.emulate_bf16, stream, a, s);
 }
 
-int cfg_unipc_step_run(const UniPCArgs& a, long long* ts_out, cudaStream_t stream) {
-  D4D_REQUIRE(a.n_steps > 0 && a.F > 0 && a.coefs && a.x0_prev && a.last_sample && a.lower_order_nums &&
-                  a.lower_order_nums_out, "unipc args");
-  D4D_REQUIRE(a.solver_order == 1 || a.solver_order == 2, "solver_order must be 1 or 2");
-  D4D_REQUIRE((a.x0_prev2 != nullptr) == (a.solver_order == 2), "x0_prev2 is given exactly when solver_order is 2");
-  D4D_REQUIRE(a.prediction_type >= 0 && a.prediction_type <= 2, "prediction_type");
-  D4D_REQUIRE(a.lower_order_nums != a.lower_order_nums_out && ts_out != a.timestep_indices,
-              "the timestep index and order count outputs may not alias their inputs");
-  dim3 grid(min(64, blocks_for(a.chw, 256)), a.F);
-  if (a.emulate_bf16) cfg_unipc_kernel<true><<<grid, 256, 0, stream>>>(a, ts_out);
-  else cfg_unipc_kernel<false><<<grid, 256, 0, stream>>>(a, ts_out);
-  D4D_CUDA_OK(cudaGetLastError());
-  return 0;
+int cfg_step_run(const StepArgs& a, const d4d_dpm_sched& s, const SolverState& st, cudaStream_t stream, bool launch) {
+  if (int rc = check_step(a, s.timesteps_table, s.coefs, s.n_steps, s.prediction_type, &st)) return rc;
+  D4D_REQUIRE(s.solver_order == 1 || s.solver_order == 2, "solver_order must be 1 or 2");
+  if (!launch) return 0;
+  return launch_step(cfg_dpm_kernel<true>, cfg_dpm_kernel<false>, s.emulate_bf16, stream, a, s, st);
+}
+
+int cfg_step_run(const StepArgs& a, const d4d_unipc_sched& s, const SolverState& st, cudaStream_t stream, bool launch) {
+  if (int rc = check_step(a, s.timesteps_table, s.coefs, s.n_steps, s.prediction_type, &st)) return rc;
+  D4D_REQUIRE(s.solver_order == 1 || s.solver_order == 2, "solver_order must be 1 or 2");
+  D4D_REQUIRE(st.last_sample != nullptr, "null argument");
+  D4D_REQUIRE((st.x0_prev2 != nullptr) == (s.solver_order == 2), "x0_prev2 is given exactly when solver_order is 2");
+  if (!launch) return 0;
+  return launch_step(cfg_unipc_kernel<true>, cfg_unipc_kernel<false>, s.emulate_bf16, stream, a, s, st);
 }
 
 }  // namespace d4d

@@ -6,6 +6,7 @@
 #include <utility>
 #include <string.h>
 
+#include "../../include/d4d.h"
 #include "common.cuh"
 
 namespace d4d {
@@ -189,78 +190,37 @@ struct AssembleArgs {
 };
 int assemble_input_run(const AssembleArgs& a, cudaStream_t stream);
 
-// a-13 + a-14: CFG combine + per-frame DDIM step (pipeline_diffuman4d.py:408-423)
-struct DdimArgs {
-  const bf16* noise;        // [(cfg?2:1)*F,4,h,w]
-  const bf16* latents;      // [F,4,h,w]
-  const bf16* mask;         // [F,1,h,w]  (cond frame <=> mask[f,0,0,0]==0)
-  const long long* timestep_indices;  // [F]
-  const long long* timesteps_table;   // [n_steps]
-  const float* alphas_cumprod;        // [T]
-  int n_steps, T;
-  float final_alpha_cumprod;
-  int F, chw, hw, cfg;
-  float guidance;
-  int prediction_type;      // 0 epsilon, 1 v_prediction, 2 sample
-  int clip_sample;
-  float clip_range;
-  int emulate_bf16;         // 1: round after every op like the reference's bf16 eager arithmetic
-  bf16* out;                // [F,4,h,w]
-};
-// ts_out[F]: updated timestep indices (targets +1, cond 0); may not alias a.timestep_indices
-int cfg_ddim_step_run(const DdimArgs& a, long long* ts_out, cudaStream_t stream);
-
-// CFG combine + per-frame DPM-Solver++ step (upstream DPMSolverMultistepScheduler, dpmsolver++ / midpoint, order <= 2).
-// Per-step coefficients row i of `coefs` (fp32, built on the host like the upstream scheduler builds them from its sigma
-// table): alpha_s, sigma_s (alpha_t / sigma_t of sigma_i), sigma_t(i+1) / sigma_t(i), c = alpha_t(i+1) * (exp(-h) - 1),
-// 0.5 * c, 1 / r0 (0 in row 0).
+// a-13 + a-14: CFG combine + per-frame scheduler step (pipeline_diffuman4d.py:408-423): DDIM, DPM-Solver++ (dpmsolver++ /
+// midpoint, order <= 2) or UniPC (predict_x0, bh1 / bh2, order <= 2; the UniC corrector of the frame's previous step,
+// then the UniP predictor).  The scheduler's constants, step count, prediction type and bf16 emulation come from its table
+// struct in include/d4d.h, passed as it is; the multistep solvers' coefficient rows are laid out there too.
 constexpr int kDpmCoefs = 6;
-struct DpmArgs {
-  const bf16* noise;        // [(cfg?2:1)*F,4,h,w]
-  const bf16* latents;      // [F,4,h,w]
-  const bf16* mask;         // [F,1,h,w]  (cond frame <=> mask[f,0,0,0]==0; never stepped, state untouched)
-  const long long* timestep_indices;  // [F] = the step index of each frame
-  const float* coefs;       // [n_steps][kDpmCoefs]
-  int n_steps;
-  int F, chw, hw, cfg;
-  float guidance;
-  int prediction_type;      // 0 epsilon, 1 v_prediction, 2 sample
-  int solver_order;         // 1 or 2
-  int final_first_order;    // 1: step n_steps-1 is first order
-  int emulate_bf16;
-  bf16* x0_prev;            // [F,4,h,w] in/out: each frame's previous data prediction
-  const int* lower_order_nums;        // [F]
-  int* lower_order_nums_out;          // [F] (may not alias lower_order_nums)
-  bf16* out;                // [F,4,h,w] (may alias latents)
-};
-// ts_out[F]: updated timestep indices (targets +1, cond 0); may not alias a.timestep_indices
-int cfg_dpm_step_run(const DpmArgs& a, long long* ts_out, cudaStream_t stream);
-
-// CFG combine + per-frame UniPC step (upstream UniPCMultistepScheduler, predict_x0, bh1 / bh2, order <= 2): the UniC
-// corrector of the frame's previous step, then the UniP predictor.  Coefficient row i of `coefs` (fp32, built on the host
-// in the upstream order of operations, layout in include/d4d.h d4d_unipc_sched).
 constexpr int kUniPCCoefs = 14;
-struct UniPCArgs {
+struct StepArgs {
   const bf16* noise;        // [(cfg?2:1)*F,4,h,w]
   const bf16* latents;      // [F,4,h,w]
-  const bf16* mask;         // [F,1,h,w]  (cond frame <=> mask[f,0,0,0]==0; never stepped, state untouched)
+  const bf16* mask;         // [F,1,h,w]  (cond frame <=> mask[f,0,0,0]==0; never stepped, solver state untouched)
   const long long* timestep_indices;  // [F] = the step index of each frame
-  const float* coefs;       // [n_steps][kUniPCCoefs]
-  int n_steps;
   int F, chw, hw, cfg;
   float guidance;
-  int prediction_type;      // 0 epsilon, 1 v_prediction, 2 sample
-  int solver_order;         // 1 or 2
-  int emulate_bf16;
-  bf16* x0_prev;            // [F,4,h,w] in/out: each frame's previous data prediction
-  bf16* x0_prev2;           // [F,4,h,w] in/out: the one before (solver_order 2; nullptr for order 1)
-  bf16* last_sample;        // [F,4,h,w] in/out: the sample each frame's last predictor started from
-  const int* lower_order_nums;        // [F]
-  int* lower_order_nums_out;          // [F] (may not alias lower_order_nums)
   bf16* out;                // [F,4,h,w] (may alias latents)
+  long long* ts_out;        // [F] updated timestep indices (targets +1, cond 0); may not alias timestep_indices
 };
-// ts_out[F]: updated timestep indices (targets +1, cond 0); may not alias a.timestep_indices
-int cfg_unipc_step_run(const UniPCArgs& a, long long* ts_out, cudaStream_t stream);
+// The multistep solvers' per-frame history, read and updated in place; members a scheduler does not keep are null (all
+// of them for DDIM).
+struct SolverState {
+  bf16* x0_prev = nullptr;      // [F,4,h,w]: each frame's previous data prediction
+  bf16* x0_prev2 = nullptr;     // [F,4,h,w]: the one before (UniPC at solver_order 2)
+  bf16* last_sample = nullptr;  // [F,4,h,w]: the sample each frame's last predictor started from (UniPC)
+  const int* lower_order_nums = nullptr;  // [F]: steps each frame has taken, capped at solver_order
+  int* lower_order_nums_out = nullptr;    // [F]: the advanced counts (may not alias lower_order_nums)
+};
+// Each checks its arguments, then launches one kernel (launch = false: only the checks, so that a caller can refuse bad
+// arguments before it enqueues the work that precedes the step).
+int cfg_step_run(const StepArgs& a, const d4d_sched& s, const SolverState& st, cudaStream_t stream, bool launch = true);
+int cfg_step_run(const StepArgs& a, const d4d_dpm_sched& s, const SolverState& st, cudaStream_t stream, bool launch = true);
+int cfg_step_run(const StepArgs& a, const d4d_unipc_sched& s, const SolverState& st, cudaStream_t stream,
+                 bool launch = true);
 
 // cross-rank K/V arrival flags (frame-sharded window): signal = system-scope release of `epoch` into slot `my_rank` of
 // every rank's flag array; wait = acquire-spin until all `world` slots of the local array reach `epoch`

@@ -79,7 +79,6 @@ WindowBufs::~WindowBufs() {
   cudaFree(timestep);
   cudaFree(skel);
   cudaFree(noise);
-  cudaFree(latents_tmp);
   cudaFree(ts_tmp);
   cudaFree(order_tmp);
 }
@@ -1195,71 +1194,13 @@ int Model::profile(const bf16* sample, const long long* timestep, const bf16* sk
   return 0;
 }
 
-// The scheduler step of one window step: writes the frames' new latents and solver state, and their advanced timestep
-// indices into ts_out (copied back by the caller).
-static int scheduler_step(const WindowStep& st, WindowBufs& wb, bf16* latents, const bf16* mask, const long long* ts_idx,
-                          int F, int hw, bool cfg_on, float guidance, cudaStream_t stream) {
-  if (const d4d_sched* ddim = st.ddim) {
-    DdimArgs d;
-    d.noise = wb.noise; d.latents = latents; d.mask = mask; d.timestep_indices = ts_idx;
-    d.timesteps_table = reinterpret_cast<const long long*>(ddim->timesteps_table); d.alphas_cumprod = ddim->alphas_cumprod;
-    d.n_steps = ddim->n_steps; d.T = ddim->num_train_timesteps; d.final_alpha_cumprod = ddim->final_alpha_cumprod;
-    d.F = F; d.chw = 4 * hw; d.hw = hw; d.cfg = cfg_on ? 1 : 0; d.guidance = guidance;
-    d.prediction_type = ddim->prediction_type; d.clip_sample = ddim->clip_sample; d.clip_range = ddim->clip_sample_range;
-    d.emulate_bf16 = ddim->emulate_bf16; d.out = wb.latents_tmp;
-    if (int rc = cfg_ddim_step_run(d, wb.ts_tmp, stream)) return rc;
-    D4D_CUDA_OK(cudaMemcpyAsync(latents, wb.latents_tmp, sizeof(bf16) * F * 4 * hw, cudaMemcpyDeviceToDevice, stream));
-    return 0;
-  }
-  if (const d4d_dpm_sched* dpm = st.dpm) {
-    DpmArgs d;
-    d.noise = wb.noise; d.latents = latents; d.mask = mask; d.timestep_indices = ts_idx; d.coefs = dpm->coefs;
-    d.n_steps = dpm->n_steps; d.F = F; d.chw = 4 * hw; d.hw = hw; d.cfg = cfg_on ? 1 : 0; d.guidance = guidance;
-    d.prediction_type = dpm->prediction_type; d.solver_order = dpm->solver_order;
-    d.final_first_order = dpm->final_first_order; d.emulate_bf16 = dpm->emulate_bf16;
-    d.x0_prev = st.x0_prev; d.lower_order_nums = st.lower_order_nums; d.lower_order_nums_out = wb.order_tmp;
-    d.out = latents;  // each element is read and written by the same thread
-    if (int rc = cfg_dpm_step_run(d, wb.ts_tmp, stream)) return rc;
-  } else {
-    const d4d_unipc_sched* u = st.unipc;
-    UniPCArgs d;
-    d.noise = wb.noise; d.latents = latents; d.mask = mask; d.timestep_indices = ts_idx; d.coefs = u->coefs;
-    d.n_steps = u->n_steps; d.F = F; d.chw = 4 * hw; d.hw = hw; d.cfg = cfg_on ? 1 : 0; d.guidance = guidance;
-    d.prediction_type = u->prediction_type; d.solver_order = u->solver_order; d.emulate_bf16 = u->emulate_bf16;
-    d.x0_prev = st.x0_prev; d.x0_prev2 = st.x0_prev2; d.last_sample = st.last_sample;
-    d.lower_order_nums = st.lower_order_nums; d.lower_order_nums_out = wb.order_tmp;
-    d.out = latents;  // each element is read and written by the same thread
-    if (int rc = cfg_unipc_step_run(d, wb.ts_tmp, stream)) return rc;
-  }
-  D4D_CUDA_OK(cudaMemcpyAsync(st.lower_order_nums, wb.order_tmp, sizeof(int) * F, cudaMemcpyDeviceToDevice, stream));
-  return 0;
-}
-
 int Model::denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
                           long long* ts_idx, const WindowStep& step, float guidance, int domain, int F, int h, int w,
                           int num_steps, cudaStream_t stream, int F_total) {
-  const bool multistep = step.dpm || step.unipc;
   D4D_REQUIRE(latents && pixel && plucker && mask && ts_idx &&
-                  (step.ddim != nullptr) + (step.dpm != nullptr) + (step.unipc != nullptr) == 1 &&
-                  (!multistep || (step.x0_prev && step.lower_order_nums)) && (!step.unipc || step.last_sample),
+                  (step.ddim != nullptr) + (step.dpm != nullptr) + (step.unipc != nullptr) == 1,
               "null argument");
-  const void* table = nullptr;
-  int n_steps = 0;
-  if (step.ddim) {
-    D4D_REQUIRE(step.ddim->timesteps_table && step.ddim->alphas_cumprod, "scheduler tables");
-    table = step.ddim->timesteps_table; n_steps = step.ddim->n_steps;
-  } else if (step.dpm) {
-    D4D_REQUIRE(step.dpm->timesteps_table && step.dpm->coefs, "scheduler tables");
-    table = step.dpm->timesteps_table; n_steps = step.dpm->n_steps;
-  } else {
-    D4D_REQUIRE(step.unipc->timesteps_table && step.unipc->coefs, "scheduler tables");
-    D4D_REQUIRE((step.x0_prev2 != nullptr) == (step.unipc->solver_order == 2),
-                "x0_prev2 is given exactly when solver_order is 2");
-    table = step.unipc->timesteps_table; n_steps = step.unipc->n_steps;
-  }
-  D4D_REQUIRE(n_steps > 0, "scheduler tables");
   D4D_REQUIRE(domain == 0 || domain == 1, "Invalid domain");
-  const long long* timesteps_table = static_cast<const long long*>(table);
   const bool cfg_on = guidance > 1.0f;
   const int B = cfg_on ? 2 * F : F;
   const bool pose = cfg_.enable_pose_encoder != 0;
@@ -1279,18 +1220,35 @@ int Model::denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker,
       if (int rc = fill_bf16_run(wb->skel, static_cast<long long>(3) * 64 * hw, -1.0f, stream)) return rc;  // constant negative image
     }
     D4D_CUDA_OK(cudaMalloc(&wb->noise, sizeof(bf16) * B * cfg_.out_channels * hw));
-    D4D_CUDA_OK(cudaMalloc(&wb->latents_tmp, sizeof(bf16) * F * 4 * hw));
     D4D_CUDA_OK(cudaMalloc(&wb->ts_tmp, sizeof(long long) * F));
     it = wbufs_.emplace(key, std::move(wb)).first;
   }
   WindowBufs& wb = *it->second;
+  const bool multistep = step.state.lower_order_nums != nullptr;
   if (multistep && !wb.order_tmp) D4D_CUDA_OK(cudaMalloc(&wb.order_tmp, sizeof(int) * F));
   const int doms[2] = {domain, domain};
   const int hw = h * w;
+  // The scheduler step runs in place (each element is read and written by the same thread); the counters go through
+  // ts_tmp / order_tmp, since a kernel may not overwrite the counters its other blocks still read.
+  StepArgs sa;
+  sa.noise = wb.noise; sa.latents = latents; sa.mask = mask; sa.timestep_indices = ts_idx;
+  sa.F = F; sa.chw = 4 * hw; sa.hw = hw; sa.cfg = cfg_on ? 1 : 0; sa.guidance = guidance;
+  sa.out = latents; sa.ts_out = wb.ts_tmp;
+  SolverState state = step.state;
+  state.lower_order_nums_out = wb.order_tmp;
+  // the scheduler's checks, before the window's work is enqueued; the input assembly reads its timestep table
+  const int64_t* timesteps_table = nullptr;
+  int n_steps = 0;
+  if (int rc = step.with_table([&](const auto& s) {
+        timesteps_table = s.timesteps_table;
+        n_steps = s.n_steps;
+        return cfg_step_run(sa, s, state, stream, false);
+      }))
+    return rc;
   for (int s = 0; s < num_steps; ++s) {
     AssembleArgs a;
     a.latents = latents; a.pixel = pixel; a.plucker = plucker; a.skel_latents = pose ? nullptr : skeletons; a.mask = mask;
-    a.timestep_indices = ts_idx; a.timesteps_table = timesteps_table;
+    a.timestep_indices = ts_idx; a.timesteps_table = reinterpret_cast<const long long*>(timesteps_table);
     a.n_steps = n_steps; a.F = F; a.h = h; a.w = w; a.cfg = cfg_on ? 1 : 0;
     a.sample = wb.sample; a.timestep_out = wb.timestep;
     if (int rc = assemble_input_run(a, stream)) return rc;
@@ -1305,8 +1263,11 @@ int Model::denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker,
       }
     }
     if (int rc = forward(wb.sample, wb.timestep, skel_in, doms, cfg_on ? 2 : 1, B, F, h, w, wb.noise, stream, F_total, pose && cfg_on)) return rc;
-    if (int rc = scheduler_step(step, wb, latents, mask, ts_idx, F, hw, cfg_on, guidance, stream)) return rc;
+    if (int rc = step.with_table([&](const auto& s) { return cfg_step_run(sa, s, state, stream); })) return rc;
     D4D_CUDA_OK(cudaMemcpyAsync(ts_idx, wb.ts_tmp, sizeof(long long) * F, cudaMemcpyDeviceToDevice, stream));
+    if (multistep)
+      D4D_CUDA_OK(cudaMemcpyAsync(step.state.lower_order_nums_out, wb.order_tmp, sizeof(int) * F, cudaMemcpyDeviceToDevice,
+                                  stream));
   }
   return 0;
 }

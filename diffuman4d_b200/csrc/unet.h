@@ -86,23 +86,22 @@ struct WindowBufs {  // scratch of d4d_denoise_window for one (F, h, w, cfg)
   long long* timestep = nullptr;
   bf16* skel = nullptr;
   bf16* noise = nullptr;
-  bf16* latents_tmp = nullptr;
   long long* ts_tmp = nullptr;
   int* order_tmp = nullptr;  // multistep schedulers only (allocated on first use)
   ~WindowBufs();
 };
 
 // The scheduler of a window step: exactly one of the tables is set.  The multistep schedulers (DPM-Solver++, UniPC) also
-// get the window frames' solver state, read and updated in place: x0_prev [F,4,h,w] and lower_order_nums [F] for both,
-// and for UniPC last_sample [F,4,h,w] and, at solver_order 2, x0_prev2 [F,4,h,w].  Unused members are null.
+// get the window frames' solver state, read and updated in place: the order counts are read from
+// state.lower_order_nums and the advanced ones end up in state.lower_order_nums_out, both the caller's array.
 struct WindowStep {
   const d4d_sched* ddim = nullptr;
   const d4d_dpm_sched* dpm = nullptr;
   const d4d_unipc_sched* unipc = nullptr;
-  bf16* x0_prev = nullptr;
-  bf16* x0_prev2 = nullptr;
-  bf16* last_sample = nullptr;
-  int* lower_order_nums = nullptr;
+  SolverState state;
+  // fn(table) with whichever table is set
+  template <typename Fn>
+  int with_table(Fn&& fn) const { return ddim ? fn(*ddim) : dpm ? fn(*dpm) : fn(*unipc); }
 };
 
 struct Exchange {  // K/V exchange buffers in peer memory (cudaIpc), two parities

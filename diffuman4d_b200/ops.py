@@ -290,37 +290,13 @@ def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: flo
     return out
 
 
-def cfg_dpm_step(noise: torch.Tensor, latents: torch.Tensor, cond_mask: torch.Tensor, timestep_indices: torch.Tensor,
-                 x0_prev: torch.Tensor, lower_order_nums: torch.Tensor, sched, guidance_scale: float, cfg: bool):
-    """One CFG + DPM-Solver++ step of F frames (``sched``: a ``d4d_dpm_sched`` from ``DPMSolverTables.c_struct``).
-    ``noise`` [(cfg?2:1)*F,4,h,w]; ``x0_prev`` [F,4,h,w] bf16 is updated in place.  Returns (new latents, advanced
-    timestep indices, advanced ``lower_order_nums``)."""
-    _bf16c(noise, "noise"), _bf16c(latents, "latents"), _bf16c(cond_mask, "cond_mask"), _bf16c(x0_prev, "x0_prev")
-    F, _, h, w = latents.shape
-    if x0_prev.shape != latents.shape:
-        raise ValueError("x0_prev must have the shape of latents")
-    if lower_order_nums.dtype != torch.int32 or not lower_order_nums.is_cuda or lower_order_nums.numel() != F:
-        raise ValueError("lower_order_nums must be a CUDA int32 [F] tensor")
-    if timestep_indices.dtype != torch.int64 or not timestep_indices.is_cuda or timestep_indices.numel() != F:
-        raise ValueError("timestep_indices must be a CUDA int64 [F] tensor")
-    out = torch.empty_like(latents)
-    ti_out = torch.empty_like(timestep_indices)
-    lon_out = torch.empty_like(lower_order_nums)
-    check(lib().d4d_cfg_dpm_step(_p(noise), _p(latents), _p(cond_mask), _p(timestep_indices), _p(ti_out), _p(x0_prev),
-                                 _p(lower_order_nums), _p(lon_out), C.byref(sched), float(guidance_scale), int(cfg), F, h, w,
-                                 _p(out), _stream()), "d4d_cfg_dpm_step")
-    return out, ti_out, lon_out
-
-
-def cfg_unipc_step(noise: torch.Tensor, latents: torch.Tensor, cond_mask: torch.Tensor, timestep_indices: torch.Tensor,
-                   x0_prev: torch.Tensor, x0_prev2: Optional[torch.Tensor], last_sample: torch.Tensor,
-                   lower_order_nums: torch.Tensor, sched, guidance_scale: float, cfg: bool):
-    """One CFG + UniPC step of F frames (``sched``: a ``d4d_unipc_sched`` from ``UniPCTables.c_struct``).  ``noise``
-    [(cfg?2:1)*F,4,h,w]; ``x0_prev``, ``x0_prev2`` (None at solver_order 1) and ``last_sample`` [F,4,h,w] bf16 are updated
-    in place.  Returns (new latents, advanced timestep indices, advanced ``lower_order_nums``)."""
+def _multistep_step(entry: str, noise, latents, cond_mask, timestep_indices, planes, lower_order_nums, sched,
+                    guidance_scale, cfg):
+    """``cfg_dpm_step`` / ``cfg_unipc_step``: ``planes`` are the (name, bf16 [F,4,h,w] tensor or None) state planes in the
+    order ``entry`` takes them."""
     _bf16c(noise, "noise"), _bf16c(latents, "latents"), _bf16c(cond_mask, "cond_mask")
     F, _, h, w = latents.shape
-    for name, t in (("x0_prev", x0_prev), ("x0_prev2", x0_prev2), ("last_sample", last_sample)):
+    for name, t in planes:
         if t is not None:
             _bf16c(t, name)
             if t.shape != latents.shape:
@@ -332,7 +308,27 @@ def cfg_unipc_step(noise: torch.Tensor, latents: torch.Tensor, cond_mask: torch.
     out = torch.empty_like(latents)
     ti_out = torch.empty_like(timestep_indices)
     lon_out = torch.empty_like(lower_order_nums)
-    check(lib().d4d_cfg_unipc_step(_p(noise), _p(latents), _p(cond_mask), _p(timestep_indices), _p(ti_out), _p(x0_prev),
-                                   _p(x0_prev2), _p(last_sample), _p(lower_order_nums), _p(lon_out), C.byref(sched),
-                                   float(guidance_scale), int(cfg), F, h, w, _p(out), _stream()), "d4d_cfg_unipc_step")
+    check(getattr(lib(), entry)(_p(noise), _p(latents), _p(cond_mask), _p(timestep_indices), _p(ti_out),
+                                *(_p(t) for _, t in planes), _p(lower_order_nums), _p(lon_out), C.byref(sched),
+                                float(guidance_scale), int(cfg), F, h, w, _p(out), _stream()), entry)
     return out, ti_out, lon_out
+
+
+def cfg_dpm_step(noise: torch.Tensor, latents: torch.Tensor, cond_mask: torch.Tensor, timestep_indices: torch.Tensor,
+                 x0_prev: torch.Tensor, lower_order_nums: torch.Tensor, sched, guidance_scale: float, cfg: bool):
+    """One CFG + DPM-Solver++ step of F frames (``sched``: a ``d4d_dpm_sched`` from ``DPMSolverTables.c_struct``).
+    ``noise`` [(cfg?2:1)*F,4,h,w]; ``x0_prev`` [F,4,h,w] bf16 is updated in place.  Returns (new latents, advanced
+    timestep indices, advanced ``lower_order_nums``)."""
+    return _multistep_step("d4d_cfg_dpm_step", noise, latents, cond_mask, timestep_indices, [("x0_prev", x0_prev)],
+                           lower_order_nums, sched, guidance_scale, cfg)
+
+
+def cfg_unipc_step(noise: torch.Tensor, latents: torch.Tensor, cond_mask: torch.Tensor, timestep_indices: torch.Tensor,
+                   x0_prev: torch.Tensor, x0_prev2: Optional[torch.Tensor], last_sample: torch.Tensor,
+                   lower_order_nums: torch.Tensor, sched, guidance_scale: float, cfg: bool):
+    """One CFG + UniPC step of F frames (``sched``: a ``d4d_unipc_sched`` from ``UniPCTables.c_struct``).  ``noise``
+    [(cfg?2:1)*F,4,h,w]; ``x0_prev``, ``x0_prev2`` (None at solver_order 1) and ``last_sample`` [F,4,h,w] bf16 are updated
+    in place.  Returns (new latents, advanced timestep indices, advanced ``lower_order_nums``)."""
+    return _multistep_step("d4d_cfg_unipc_step", noise, latents, cond_mask, timestep_indices,
+                           [("x0_prev", x0_prev), ("x0_prev2", x0_prev2), ("last_sample", last_sample)], lower_order_nums,
+                           sched, guidance_scale, cfg)

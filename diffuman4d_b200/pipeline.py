@@ -23,7 +23,7 @@ import torch
 
 from ._lib import check, lib
 from .config import DPMSolverConfig, SchedulerConfig, UniPCConfig
-from .scheduler import DDIMTables, DPMSolverFrame, DPMSolverState, DPMSolverTables, UniPCState, UniPCTables
+from .scheduler import DDIMTables, DPMSolverFrame, DPMSolverTables, SolverState, UniPCTables
 from .unet import _DOMAIN_IDS, B200MultiviewUNet
 
 
@@ -97,7 +97,7 @@ class B200Diffuman4DPipeline:
 
     @property
     def _multistep(self) -> bool:
-        return isinstance(self.scheduler, (DPMSolverTables, UniPCTables))
+        return self.scheduler.state_planes is not None
 
     def parepare_schedulers(self, num_inference_steps: int, num_frames: int):
         """PIPE:265-271.  The per-frame deep copies exist in the reference only because scheduler objects are
@@ -111,7 +111,7 @@ class B200Diffuman4DPipeline:
     # B-3 -----------------------------------------------------------------------------------------------
     def denoise_window(self, *, latents, pixel_values_latents, plucker_embeds_latents, skeletons_latents,
                        cond_masks_latents, timestep_indices, domain: str, guidance_scale: float,
-                       num_inference_steps: int = 1, solver_state: Optional[DPMSolverState] = None):
+                       num_inference_steps: int = 1, solver_state: Optional[SolverState] = None):
         """One window: ``num_inference_steps`` x (assemble -> UNet -> CFG -> per-frame scheduler step).  ``latents``
         [F,4,h,w] and ``timestep_indices`` [F] (int64, device) are updated IN PLACE and returned.  With DPM-Solver++ or
         UniPC, ``solver_state`` is the window frames' ``DPMSolverState`` / ``UniPCState`` (``take``), also updated in
@@ -124,13 +124,13 @@ class B200Diffuman4DPipeline:
 
     def _window_step(self, *, latents, pixel_values_latents, plucker_embeds_latents, skeletons_latents,
                      cond_masks_latents, timestep_indices, domain: str, guidance_scale: float,
-                     num_inference_steps: int = 1, solver_state: Optional[DPMSolverState] = None,
+                     num_inference_steps: int = 1, solver_state: Optional[SolverState] = None,
                      F_total: Optional[int] = None):
         """``denoise_window``'s checks and library call.  ``F_total`` given: the tensors hold this rank's frames of a
         frame-sharded window of ``F_total`` frames (``FrameShardedPipeline.denoise_window``)."""
-        unipc = isinstance(self.scheduler, UniPCTables)
-        if unipc and F_total is not None:
-            raise NotImplementedError("the frame-sharded window does not run the UniPC scheduler")
+        name = self.scheduler.window_entry_points[F_total is not None]
+        if name is None:
+            raise NotImplementedError(f"the frame-sharded window does not run the {self.scheduler.name} scheduler")
         if domain not in _DOMAIN_IDS:
             raise ValueError(f"Invalid domain for temporal embedding: {domain}")
         dev = self.device
@@ -155,32 +155,23 @@ class B200Diffuman4DPipeline:
         args = [self.unet._h, latents.data_ptr(), pix.data_ptr(), plk.data_ptr(), skl.data_ptr(), msk.data_ptr(),
                 timestep_indices.data_ptr(), C.byref(sched), float(g), _DOMAIN_IDS[domain], *frames, h, w,
                 int(num_inference_steps)]
-        if self._multistep:
+        if self._multistep:   # the state planes in ABI order (None: passed as NULL), then lower_order_nums
             st = solver_state
             if st is None:
-                raise ValueError(f"the {'UniPC' if unipc else 'DPM-Solver++'} scheduler needs the window frames' "
-                                 "solver_state")
+                raise ValueError(f"the {self.scheduler.name} scheduler needs the window frames' solver_state")
 
-            def state_tensor(name):
-                t = getattr(st, name, None)
+            def state_plane(plane):
+                t = getattr(st, plane, None)
                 if not (t is not None and t.is_cuda and t.dtype == torch.bfloat16 and t.is_contiguous()
                         and t.shape == latents.shape):
-                    raise ValueError(f"solver_state.{name} must be a contiguous CUDA bfloat16 tensor shaped like latents")
+                    raise ValueError(f"solver_state.{plane} must be a contiguous CUDA bfloat16 tensor shaped like latents")
                 return t.data_ptr()
 
-            x0_prev = state_tensor("x0_prev")
+            args += [None if plane is None else state_plane(plane) for plane in self.scheduler.state_planes]
             lon = st.lower_order_nums
             if not (lon.is_cuda and lon.dtype == torch.int32 and lon.is_contiguous() and lon.numel() == F_):
                 raise ValueError("solver_state.lower_order_nums must be a contiguous CUDA int32 [F] tensor")
-            if unipc:
-                x0_prev2 = state_tensor("x0_prev2") if self.scheduler.config.solver_order == 2 else None
-                args += [x0_prev, x0_prev2, state_tensor("last_sample"), lon.data_ptr()]
-                name = "d4d_denoise_window_unipc"
-            else:
-                args += [x0_prev, lon.data_ptr()]
-                name = "d4d_denoise_window_dpm" if F_total is None else "d4d_denoise_window_dpm_sharded"
-        else:
-            name = "d4d_denoise_window" if F_total is None else "d4d_denoise_window_sharded"
+            args.append(lon.data_ptr())
         with torch.cuda.device(dev):
             check(getattr(lib(), name)(*args, torch.cuda.current_stream().cuda_stream), name)
         return latents, timestep_indices

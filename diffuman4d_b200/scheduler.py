@@ -10,10 +10,13 @@ the sigma table and the per-step solver coefficients (``cfg_dpm_kernel``).  That
 reference deep-copies it per frame; here the state of every frame of a task is a ``DPMSolverState`` on the device.
 ``UniPCTables`` / ``UniPCState`` do the same for ``UniPCMultistepScheduler`` (``cfg_unipc_kernel``), whose corrector also
 needs each frame's previous sample and, at order 2, a second data prediction of history.
+
+Each tables class names the C entry points of its window step (``window_entry_points``: plain and frame-sharded, None
+where there is none) and the bf16 state planes they take, in ABI order (``state_planes``; None for the stateless DDIM).
 """
 from __future__ import annotations
 
-import ctypes as C
+import copy
 
 import numpy as np
 import torch
@@ -26,17 +29,13 @@ _PRED = {"epsilon": 0, "v_prediction": 1, "sample": 2}
 
 class DDIMTables:
     init_noise_sigma = 1.0  # DDIM: scale_model_input is the identity, init sigma 1 (reference PIPE:189,376)
+    window_entry_points = ("d4d_denoise_window", "d4d_denoise_window_sharded")
+    state_planes = None     # stateless: one table serves every frame
 
     def __init__(self, cfg: SchedulerConfig = None, device="cuda:0"):
         self.config = cfg or SchedulerConfig()
         c = self.config
-        T = c.num_train_timesteps
-        if c.beta_schedule == "scaled_linear":
-            betas = torch.linspace(c.beta_start ** 0.5, c.beta_end ** 0.5, T, dtype=torch.float32) ** 2
-        elif c.beta_schedule == "linear":
-            betas = torch.linspace(c.beta_start, c.beta_end, T, dtype=torch.float32)
-        else:
-            raise ValueError(f"{c.beta_schedule} is not implemented")
+        betas = _betas(c)
         if c.prediction_type not in _PRED:
             raise ValueError(f"prediction_type given as {c.prediction_type} must be one of {list(_PRED)}")
         self.alphas_cumprod = torch.cumprod(1.0 - betas, dim=0)
@@ -138,39 +137,71 @@ def dpm_step_coefficients(sigmas: torch.Tensor) -> torch.Tensor:
     return out
 
 
-class DPMSolverTables:
-    """Timesteps, sigmas and step coefficients of ``DPMSolverMultistepScheduler`` (diffusers 0.33.1) for
-    ``cfg_dpm_kernel``."""
+class _MultistepTables:
+    """What ``DPMSolverTables`` and ``UniPCTables`` share: the config checks common to both, the sigma table,
+    ``set_timesteps`` and the device copies behind ``c_struct``.  A subclass adds its own checks (``_check``), its
+    coefficient rows (``_coefficients``) and its C struct (``_struct``, plus the fields of ``_struct_fields``)."""
     init_noise_sigma = 1.0  # upstream: init_noise_sigma 1, scale_model_input is the identity
 
-    def __init__(self, cfg: DPMSolverConfig = None, device="cuda:0"):
-        self.config = cfg or DPMSolverConfig()
-        c = self.config
+    def __init__(self, cfg, device):
+        self.config = c = cfg
         if c.prediction_type not in _PRED:
             raise ValueError(f"prediction_type given as {c.prediction_type} must be one of {list(_PRED)}")
         if c.solver_order not in (1, 2):
             raise NotImplementedError(f"solver_order={c.solver_order}: the fused step implements orders 1 and 2")
         if c.final_sigmas_type not in ("zero", "sigma_min"):
             raise ValueError(f"final_sigmas_type {c.final_sigmas_type!r} must be 'zero' or 'sigma_min'")
+        self._check(c)
         self.alphas_cumprod = torch.cumprod(1.0 - _betas(c), dim=0)
         self.all_sigmas = ((1 - self.alphas_cumprod) / self.alphas_cumprod) ** 0.5   # fp32 [T]
         self.device = torch.device(device)
         self.num_inference_steps = None
         self.timesteps = None          # host int64 [n]
         self.sigmas = None             # host fp32 [n+1]
-        self.coefs = None              # host fp32 [n, 6]
+        self.coefs = None              # host fp32 [n, coefficients per step]
         self._dev = None
+
+    def _check(self, c):
+        pass
+
+    def _struct_fields(self) -> dict:
+        return {}
 
     def set_timesteps(self, n: int, device=None):
         c = self.config
-        ts = dpm_timesteps(c, n)
+        ts = dpm_timesteps(c, n)       # UniPC spaces its timesteps like DPM-Solver++
         last = 0.0 if c.final_sigmas_type == "zero" else float(self.all_sigmas[0])
         self.num_inference_steps = n
         self.timesteps = torch.from_numpy(ts)
         self.sigmas = torch.cat([self.all_sigmas[self.timesteps], torch.tensor([last], dtype=torch.float32)])
-        self.coefs = dpm_step_coefficients(self.sigmas)
+        self.coefs = self._coefficients(self.sigmas)
         self._dev = None
         return self.timesteps
+
+    def c_struct(self, emulate_bf16: bool = False):
+        if self.timesteps is None:
+            raise ValueError("call set_timesteps first")
+        if self._dev is None:
+            self._dev = (self.timesteps.to(self.device), self.coefs.to(self.device).contiguous())
+        c = self.config
+        return self._struct(timesteps_table=self._dev[0].data_ptr(), coefs=self._dev[1].data_ptr(),
+                            n_steps=int(self.num_inference_steps), prediction_type=_PRED[c.prediction_type],
+                            solver_order=int(c.solver_order), emulate_bf16=int(emulate_bf16), **self._struct_fields())
+
+
+class DPMSolverTables(_MultistepTables):
+    """Timesteps, sigmas and step coefficients of ``DPMSolverMultistepScheduler`` (diffusers 0.33.1) for
+    ``cfg_dpm_kernel``."""
+    name = "DPM-Solver++"
+    window_entry_points = ("d4d_denoise_window_dpm", "d4d_denoise_window_dpm_sharded")
+    state_planes = ("x0_prev",)
+    _struct = D4DDpmSched
+
+    def __init__(self, cfg: DPMSolverConfig = None, device="cuda:0"):
+        super().__init__(cfg or DPMSolverConfig(), device)
+
+    def _coefficients(self, sigmas: torch.Tensor) -> torch.Tensor:
+        return dpm_step_coefficients(sigmas)
 
     @property
     def final_first_order(self) -> bool:
@@ -179,35 +210,25 @@ class DPMSolverTables:
         return bool(c.euler_at_final or (c.lower_order_final and self.num_inference_steps < 15)
                     or c.final_sigmas_type == "zero")
 
+    def _struct_fields(self) -> dict:
+        return {"final_first_order": int(self.final_first_order)}
+
     def new_state(self, num_frames: int) -> "DPMSolverState":
         return DPMSolverState(num_frames, self.device)
 
-    def c_struct(self, emulate_bf16: bool = False) -> D4DDpmSched:
-        if self.timesteps is None:
-            raise ValueError("call set_timesteps first")
-        if self._dev is None:
-            self._dev = (self.timesteps.to(self.device), self.coefs.to(self.device).contiguous())
-        c = self.config
-        s = D4DDpmSched()
-        s.timesteps_table = self._dev[0].data_ptr()
-        s.coefs = self._dev[1].data_ptr()
-        s.n_steps = int(self.num_inference_steps)
-        s.prediction_type = _PRED[c.prediction_type]
-        s.solver_order = int(c.solver_order)
-        s.final_first_order = int(self.final_first_order)
-        s.emulate_bf16 = int(emulate_bf16)
-        return s
 
+class SolverState:
+    """The multistep solver history of every frame of one task, on the device: the bf16 planes named by ``planes``, each
+    [F,4,h,w] and allocated (zeroed) when the latent size is first known, and ``lower_order_nums`` [F] int32.  A new task
+    starts from zeros, which is the state of a freshly deep-copied upstream scheduler.  ``take`` / ``put`` gather and
+    scatter the frames of one window."""
 
-class DPMSolverState:
-    """The DPM-Solver++ history of every frame of one task, on the device: ``x0_prev`` [F,4,h,w] bf16 (each frame's
-    previous data prediction) and ``lower_order_nums`` [F] int32.  A new task starts from zeros, which is the state of a
-    freshly deep-copied upstream scheduler.  ``take`` / ``put`` gather and scatter the frames of one window."""
-
-    def __init__(self, num_frames: int, device, x0_prev: torch.Tensor = None, lower_order_nums: torch.Tensor = None):
+    def __init__(self, num_frames: int, device, planes: tuple, lower_order_nums: torch.Tensor = None, **tensors):
         self.num_frames = num_frames
         self.device = torch.device(device)
-        self.x0_prev = x0_prev         # allocated (zeroed) when the latent size is first known
+        self.planes = planes
+        for name, t in tensors.items():
+            setattr(self, name, t)
         self.lower_order_nums = (torch.zeros(num_frames, dtype=torch.int32, device=self.device)
                                  if lower_order_nums is None else lower_order_nums)
 
@@ -216,22 +237,34 @@ class DPMSolverState:
         return [DPMSolverFrame(self, i) for i in range(self.num_frames)]
 
     def _ensure(self, h: int, w: int):
-        if self.x0_prev is None:
-            self.x0_prev = torch.zeros(self.num_frames, 4, h, w, dtype=torch.bfloat16, device=self.device)
-        elif tuple(self.x0_prev.shape[2:]) != (h, w):
-            raise ValueError(f"solver state holds {tuple(self.x0_prev.shape[2:])} latents, got {(h, w)}")
+        for name in self.planes:
+            t = getattr(self, name)
+            if t is None:
+                setattr(self, name, torch.zeros(self.num_frames, 4, h, w, dtype=torch.bfloat16, device=self.device))
+            elif tuple(t.shape[2:]) != (h, w):
+                raise ValueError(f"solver state holds {tuple(t.shape[2:])} latents, got {(h, w)}")
 
-    def take(self, index: torch.Tensor, h: int, w: int) -> "DPMSolverState":
-        """The state of frames ``index`` as a new (contiguous) state, for one window."""
+    def take(self, index: torch.Tensor, h: int, w: int):
+        """The state of frames ``index`` as a new (contiguous) state of the same kind, for one window."""
         self._ensure(h, w)
         index = index.to(self.device)
-        return DPMSolverState(len(index), self.device, self.x0_prev[index].contiguous(),
-                              self.lower_order_nums[index].contiguous())
+        window = copy.copy(self)
+        window.num_frames = len(index)
+        for name in (*self.planes, "lower_order_nums"):
+            setattr(window, name, getattr(self, name)[index].contiguous())
+        return window
 
-    def put(self, index: torch.Tensor, window: "DPMSolverState"):
+    def put(self, index: torch.Tensor, window: "SolverState"):
         index = index.to(self.device)
-        self.x0_prev[index] = window.x0_prev
-        self.lower_order_nums[index] = window.lower_order_nums
+        for name in (*self.planes, "lower_order_nums"):
+            getattr(self, name)[index] = getattr(window, name)
+
+
+class DPMSolverState(SolverState):
+    """The DPM-Solver++ history: ``x0_prev`` (each frame's previous data prediction) and ``lower_order_nums``."""
+
+    def __init__(self, num_frames: int, device, x0_prev: torch.Tensor = None, lower_order_nums: torch.Tensor = None):
+        super().__init__(num_frames, device, DPMSolverTables.state_planes, lower_order_nums, x0_prev=x0_prev)
 
 
 class DPMSolverFrame:
@@ -239,7 +272,7 @@ class DPMSolverFrame:
     lists)."""
     __slots__ = ("state", "index")
 
-    def __init__(self, state: DPMSolverState, index: int):
+    def __init__(self, state: SolverState, index: int):
         self.state, self.index = state, index
 
 
@@ -295,97 +328,51 @@ def unipc_step_coefficients(c: UniPCConfig, sigmas: torch.Tensor) -> torch.Tenso
     return out
 
 
-class UniPCTables:
+def _unipc_planes(solver_order: int) -> tuple:
+    """UniPC's bf16 state planes in the order ``d4d_denoise_window_unipc`` takes them; ``x0_prev2`` exists at order 2
+    only (None: its argument is NULL)."""
+    return ("x0_prev", "x0_prev2" if solver_order == 2 else None, "last_sample")
+
+
+class UniPCTables(_MultistepTables):
     """Timesteps, sigmas and step coefficients of ``UniPCMultistepScheduler`` (diffusers 0.33.1) for
     ``cfg_unipc_kernel``."""
-    init_noise_sigma = 1.0  # upstream: init_noise_sigma 1, scale_model_input is the identity
+    name = "UniPC"
+    # no frame-sharded window: its window-result exchange carries DPM-Solver++'s state only
+    window_entry_points = ("d4d_denoise_window_unipc", None)
+    _struct = D4DUniPCSched
 
     def __init__(self, cfg: UniPCConfig = None, device="cuda:0"):
-        self.config = cfg or UniPCConfig()
-        c = self.config
-        if c.prediction_type not in _PRED:
-            raise ValueError(f"prediction_type given as {c.prediction_type} must be one of {list(_PRED)}")
-        if c.solver_order not in (1, 2):
-            raise NotImplementedError(f"solver_order={c.solver_order}: the fused step implements orders 1 and 2")
+        super().__init__(cfg or UniPCConfig(), device)
+
+    def _check(self, c):
         if c.solver_type not in ("bh1", "bh2"):
             raise ValueError(f"solver_type {c.solver_type!r} must be 'bh1' or 'bh2'")
-        if c.final_sigmas_type not in ("zero", "sigma_min"):
-            raise ValueError(f"final_sigmas_type {c.final_sigmas_type!r} must be 'zero' or 'sigma_min'")
         if c.final_sigmas_type == "zero" and c.solver_order == 2 and not c.lower_order_final:
             raise NotImplementedError("final_sigmas_type='zero' with lower_order_final=False at solver_order 2: the last "
                                       "step's second-order term divides by an infinite h")
         if c.final_sigmas_type == "zero" and c.solver_type == "bh1":
             raise NotImplementedError("final_sigmas_type='zero' with solver_type='bh1': the last step's B(h) = -h is "
                                       "infinite and upstream returns NaN")
-        self.alphas_cumprod = torch.cumprod(1.0 - _betas(c), dim=0)
-        self.all_sigmas = ((1 - self.alphas_cumprod) / self.alphas_cumprod) ** 0.5   # fp32 [T]
-        self.device = torch.device(device)
-        self.num_inference_steps = None
-        self.timesteps = None          # host int64 [n]
-        self.sigmas = None             # host fp32 [n+1]
-        self.coefs = None              # host fp32 [n, 14]
-        self._dev = None
 
-    def set_timesteps(self, n: int, device=None):
-        c = self.config
-        ts = dpm_timesteps(c, n)       # UniPC spaces its timesteps like DPM-Solver++
-        last = 0.0 if c.final_sigmas_type == "zero" else float(self.all_sigmas[0])
-        self.num_inference_steps = n
-        self.timesteps = torch.from_numpy(ts)
-        self.sigmas = torch.cat([self.all_sigmas[self.timesteps], torch.tensor([last], dtype=torch.float32)])
-        self.coefs = unipc_step_coefficients(c, self.sigmas)
-        self._dev = None
-        return self.timesteps
+    def _coefficients(self, sigmas: torch.Tensor) -> torch.Tensor:
+        return unipc_step_coefficients(self.config, sigmas)
+
+    @property
+    def state_planes(self) -> tuple:
+        return _unipc_planes(self.config.solver_order)
 
     def new_state(self, num_frames: int) -> "UniPCState":
         return UniPCState(num_frames, self.device, self.config.solver_order)
 
-    def c_struct(self, emulate_bf16: bool = False) -> D4DUniPCSched:
-        if self.timesteps is None:
-            raise ValueError("call set_timesteps first")
-        if self._dev is None:
-            self._dev = (self.timesteps.to(self.device), self.coefs.to(self.device).contiguous())
-        c = self.config
-        s = D4DUniPCSched()
-        s.timesteps_table = self._dev[0].data_ptr()
-        s.coefs = self._dev[1].data_ptr()
-        s.n_steps = int(self.num_inference_steps)
-        s.prediction_type = _PRED[c.prediction_type]
-        s.solver_order = int(c.solver_order)
-        s.emulate_bf16 = int(emulate_bf16)
-        return s
 
-
-class UniPCState(DPMSolverState):
-    """The UniPC history of every frame of one task, on the device: ``DPMSolverState``'s ``x0_prev`` and
-    ``lower_order_nums``, plus ``x0_prev2`` [F,4,h,w] bf16 (the data prediction before ``x0_prev``; order 2 only, else
-    None) and ``last_sample`` [F,4,h,w] bf16 (the sample each frame's last predictor started from, after correction).  A
-    new task starts from zeros, the state of a freshly deep-copied upstream scheduler."""
+class UniPCState(SolverState):
+    """The UniPC history: ``x0_prev`` and ``lower_order_nums`` as DPM-Solver++'s, plus ``x0_prev2`` (the data prediction
+    before ``x0_prev``; order 2 only, else None) and ``last_sample`` (the sample each frame's last predictor started from,
+    after correction)."""
 
     def __init__(self, num_frames: int, device, solver_order: int = 2, x0_prev: torch.Tensor = None,
                  lower_order_nums: torch.Tensor = None, x0_prev2: torch.Tensor = None, last_sample: torch.Tensor = None):
-        super().__init__(num_frames, device, x0_prev, lower_order_nums)
+        super().__init__(num_frames, device, tuple(p for p in _unipc_planes(solver_order) if p), lower_order_nums,
+                         x0_prev=x0_prev, x0_prev2=x0_prev2, last_sample=last_sample)
         self.solver_order = solver_order
-        self.x0_prev2 = x0_prev2
-        self.last_sample = last_sample
-
-    def _ensure(self, h: int, w: int):
-        super()._ensure(h, w)
-        if self.last_sample is None:
-            self.last_sample = torch.zeros_like(self.x0_prev)
-        if self.solver_order == 2 and self.x0_prev2 is None:
-            self.x0_prev2 = torch.zeros_like(self.x0_prev)
-
-    def take(self, index: torch.Tensor, h: int, w: int) -> "UniPCState":
-        self._ensure(h, w)
-        index = index.to(self.device)
-        g = lambda t: None if t is None else t[index].contiguous()
-        return UniPCState(len(index), self.device, self.solver_order, g(self.x0_prev), g(self.lower_order_nums),
-                          g(self.x0_prev2), g(self.last_sample))
-
-    def put(self, index: torch.Tensor, window: "UniPCState"):
-        super().put(index, window)
-        index = index.to(self.device)
-        self.last_sample[index] = window.last_sample
-        if self.x0_prev2 is not None:
-            self.x0_prev2[index] = window.x0_prev2

@@ -20,7 +20,7 @@ import torch.distributed as dist
 
 from ._lib import check, lib
 from .pipeline import B200Diffuman4DPipeline, _check_inplace, build_windows
-from .scheduler import DPMSolverState, UniPCTables
+from .scheduler import DPMSolverState
 from .sharding import frame_shard
 
 
@@ -47,8 +47,8 @@ def window_result_bytes(F_total: int, h: int, w: int, dpm: bool = True) -> int:
 
 class FrameShardedPipeline:
     def __init__(self, pipe: B200Diffuman4DPipeline, max_frames: int, h: int, w: int, group=None):
-        if isinstance(pipe.scheduler, UniPCTables):   # its window results would need two more per-frame tensors
-            raise NotImplementedError("the frame-sharded window does not run the UniPC scheduler; use "
+        if pipe.scheduler.window_entry_points[1] is None:
+            raise NotImplementedError(f"the frame-sharded window does not run the {pipe.scheduler.name} scheduler; use "
                                       "B200Diffuman4DPipeline on one GPU per task")
         if not dist.is_initialized():
             raise RuntimeError("torch.distributed must be initialised (one process per GPU)")
