@@ -7,7 +7,6 @@
 namespace d4d {
 static thread_local std::string g_last_error;
 void set_error(const std::string& msg) { g_last_error = msg; }
-int nhwc_to_nchw_run(const bf16* x, int ld, int n, int C, int hw, bf16* out, cudaStream_t stream);
 }  // namespace d4d
 
 struct d4d_handle {

@@ -533,6 +533,26 @@ int gemm_choose_tile(const GemmDesc& d, int sms, int* block_m, int* block_n, int
   return 0;
 }
 
+bool gemm_stats_fusable(const GemmDesc& d, int sms, const char** why) {
+  const auto refuse = [&](const char* msg) {
+    if (why) *why = msg;
+    return false;
+  };
+  if (d.geglu || d.kv_world != 0) return refuse("GroupNorm statistics: plain / conv epilogue only");
+  if (!d.conv) {
+    if (d.stats_rows <= 0 || d.stats_rows % 32 != 0) return refuse("statistics need rows-per-image % 32 == 0");
+    // rows past the last whole image would add into image M / stats_rows, past the [M / stats_rows][N][2] workspace
+    if (d.M % d.stats_rows != 0) return refuse("statistics need M % rows-per-image == 0");
+    return true;
+  }
+  int bm = 0, bn = 0, oh = 0, ow = 0, phases = 1;
+  if (gemm_choose_tile(d, sms, &bm, &bn)) return refuse("no tile for this block_m / block_n");
+  conv_out_grid(d, &oh, &ow, &phases);
+  const ConvTile t = conv_tile(bm, d.n_img, oh, ow);
+  if ((t.bw * t.bh) % 32 != 0) return refuse("statistics need 32-row warps inside one image");
+  return true;
+}
+
 int gemm_prepare(const GemmDesc& d, GemmLaunch* L) {
   D4D_REQUIRE(d.N % 16 == 0, "GEMM N must be a multiple of 16");
   D4D_REQUIRE(d.out != nullptr && d.A != nullptr && d.Wt != nullptr, "null operand");
@@ -574,10 +594,8 @@ int gemm_prepare(const GemmDesc& d, GemmLaunch* L) {
   a.out_scale = d.out_scale;
   a.stats = d.stats;
   a.stats_rows = d.stats_rows > 0 ? d.stats_rows : 1;
-  D4D_REQUIRE(d.stats == nullptr || (!d.geglu && d.kv_world == 0), "GroupNorm statistics: plain / conv epilogue only");
-  D4D_REQUIRE(d.stats == nullptr || d.conv || (d.stats_rows > 0 && d.stats_rows % 32 == 0), "statistics need rows-per-image % 32 == 0");
-  // rows past the last whole image would add into image M / stats_rows, past the [M / stats_rows][N][2] workspace
-  D4D_REQUIRE(d.stats == nullptr || d.conv || d.M % d.stats_rows == 0, "statistics need M % rows-per-image == 0");
+  const char* no_stats = nullptr;
+  D4D_REQUIRE(d.stats == nullptr || gemm_stats_fusable(d, sms, &no_stats), no_stats);
   a.kv_world = d.kv_world;
   a.kv_col0 = d.kv_col0;
   a.kv_ld = d.kv_ld;
@@ -655,7 +673,6 @@ int gemm_prepare(const GemmDesc& d, GemmLaunch* L) {
     const ConvTile ct = conv_tile(bm, d.n_img, a.H, a.W);
     const int bw = ct.bw, bh = ct.bh, bnimg = ct.bn_img;
     D4D_REQUIRE(bw * bh * bnimg == bm && bnimg <= 256, "conv tile shape");
-    D4D_REQUIRE(d.stats == nullptr || (bw * bh) % 32 == 0, "statistics need 32-row warps inside one image");
     a.BW = bw; a.BH = bh; a.BN = bnimg;
     a.tiles_x = (a.W + bw - 1) / bw;
     a.tiles_y = (a.H + bh - 1) / bh;

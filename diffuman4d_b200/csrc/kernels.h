@@ -109,6 +109,11 @@ constexpr int kSchedCooperative = 1, kSchedPingPong = 2;
 // schedule only; `schedule` may be null).  Ping-pong is chosen on shape alone: gemm_prepare runs a launch that cannot
 // stage its epilogue cooperatively.
 int gemm_choose_tile(const GemmDesc& d, int sms, int* block_m, int* block_n, int* schedule = nullptr);
+// whether the epilogue of d can accumulate the GroupNorm statistics of its output (GemmDesc::stats) on a device of `sms`
+// SMs: every 32-row warp of the tile gemm_choose_tile picks stays inside one image (plain GEMM: stats_rows % 32 == 0 and
+// M % stats_rows == 0).  Shape fields only; `why` (may be null) gets the reason when not.  gemm_prepare refuses stats
+// otherwise.
+bool gemm_stats_fusable(const GemmDesc& d, int sms, const char** why = nullptr);
 int gemm_prepare(const GemmDesc& d, GemmLaunch* L);
 int gemm_run(const GemmLaunch& L, cudaStream_t stream);
 double gemm_flops(const GemmLaunch& L);
@@ -173,6 +178,11 @@ int pose_conv_run(const bf16* x, int n, int Cin, int H, int W, const bf16* w, co
                   int stride, bf16* out_nhwc, cudaStream_t stream);
 // generic NHWC im2col, pad 1: [n,H,W,C] -> [n*Ho*Wo, k*k*C]
 int im2col_nhwc_run(const bf16* x, int n, int H, int W, int C, int ksize, int stride, bf16* out, cudaStream_t stream);
+// [1 + F images of per_img elements] -> [2F images]: images 0..F-1 <- small image 0, images F..2F-1 <- small images 1..F
+// (per_img % 8 == 0)
+int broadcast_neg_images_run(const bf16* small, long long per_img, int F, bf16* full, cudaStream_t stream);
+// p[0 .. n) = v
+int fill_bf16_run(bf16* p, long long n, float v, cudaStream_t stream);
 
 // a-1 input assembly (pipeline_diffuman4d.py:373-395), writes NCHW [2F or F, Cin, h, w] + timesteps
 struct AssembleArgs {

@@ -15,10 +15,6 @@
 
 namespace d4d {
 
-int silu_run(const bf16* x, long long n, bf16* out, cudaStream_t stream);
-int broadcast_neg_images_run(const bf16* small, long long per_img, int F, bf16* full, cudaStream_t stream);
-int fill_bf16_run(bf16* p, long long n, float v, cudaStream_t stream);
-
 namespace {
 
 inline uint16_t f2bf(float f) {
@@ -62,10 +58,11 @@ const struct { const char* path; int cin, cout, k; } kPoseLayers[8] = {
     {"pose_encoder.conv_layers.8", 32, 32, 3},  {"pose_encoder.conv_layers.10", 32, 64, 4},
     {"pose_encoder.conv_layers.12", 64, 64, 3}, {"pose_encoder.conv_layers.14", 64, 128, 3}};
 
-std::string plan_key(const int* dom, int nd, int B, int F, int h, int w) {
-  std::string k = std::to_string(B) + "_" + std::to_string(F) + "_" + std::to_string(h) + "_" + std::to_string(w) + "_";
-  for (int i = 0; i < nd; ++i) k += dom[i] ? 't' : 's';
-  return k;
+std::string plan_key(const PlanShape& s) {
+  std::string k = std::to_string(s.B) + "_" + std::to_string(s.F) + "_" + std::to_string(s.h) + "_" + std::to_string(s.w) + "_";
+  for (int d : s.domains) k += d ? 't' : 's';
+  if (s.F_total > 0) k += "_sh" + std::to_string(s.F_total);
+  return s.pose_shared_neg ? k + "_pn" : k;
 }
 
 }  // namespace
@@ -484,15 +481,11 @@ class PlanBuilder {
     return p;
   }
   // Runs the producer of `out` (d writes out.p) so that out.stats holds its statistics.  The epilogue accumulates them
-  // when every 32-row warp of the producer's tiles (grid H x W) stays inside one image: true at every level of the
-  // 64x64 and 128x128 latents.  Otherwise a statistics launch follows the producer.  Eager, not at the norm: a down-path
-  // output is read by two GroupNorms (the next block's and the up-path concat's) and must be summed once.
+  // where it can (gemm_stats_fusable) and the grid its tiles walk, H x W per image, has H > 1 and a multiple of 32
+  // positions: every level of the 64x64 and 128x128 latents.  Otherwise a statistics launch follows the producer.  Eager, not
+  // at the norm: a down-path output is read by two GroupNorms (the next block's and the up-path concat's), summed once.
   void gemm_stats(GemmDesc d, const Act& out, int n_img, int H, int W) {
-    int bw = 16;
-    while (bw > W) bw >>= 1;
-    int bh = 128 / bw;
-    while (bh > H && bh > 1) bh >>= 1;
-    if ((bw * bh) % 32 == 0 && (H * W) % 32 == 0) {
+    if (H > 1 && (H * W) % 32 == 0 && gemm_stats_fusable(d, sms_)) {
       d.stats = out.stats;
       gemm(d);
       return;
@@ -501,7 +494,7 @@ class PlanBuilder {
     const bf16* x = out.p;
     long long* st = out.stats;
     const int C = out.C, hw = out.H * out.W;
-    op([=](cudaStream_t s) { return groupnorm_stats_run(x, C, n_img, hw, st, s); }, 1, 3);
+    op([=](cudaStream_t s) { return groupnorm_stats_run(x, C, n_img, hw, st, s); }, kOpGroupNorm);
   }
   int rc() const { return rc_; }
 
@@ -544,13 +537,10 @@ class PlanBuilder {
     else free_.push_back({o, sz});
   }
 
-  void op(std::function<int(cudaStream_t)> f, int launches = 1, int kind = 5, double flops = 0.0) {
+  // the one place a plan's ops and launch count are recorded (the dry run counts launches only)
+  void op(std::function<int(cudaStream_t)> f, OpKind kind = kOpOther, int launches = 1, double flops = 0.0) {
     p_.launches += launches;
-    if (!dry_) {
-      p_.ops.push_back(std::move(f));
-      p_.op_kind.push_back(kind);
-      p_.op_flops.push_back(flops);
-    }
+    if (!dry_) p_.ops.push_back({std::move(f), kind, launches, flops});
   }
   void tap(const std::string& name, const Act& a) {
     if (!dry_) p_.taps.push_back({name, a.p, a.C, a.H, a.W, p_.ops.size()});
@@ -560,16 +550,17 @@ class PlanBuilder {
     if (!dry_) module_taps_.push_back({name, a.p, a.C, a.H, a.W, p_.ops.size()});
   }
   void gemm(const GemmDesc& d) {
-    if (dry_) { p_.launches += 1; return; }
+    const OpKind kind = d.conv ? kOpConv : kOpGemm;
+    if (dry_) { op(nullptr, kind); return; }
     GemmLaunch L;
     if (int rc = gemm_prepare(d, &L)) { if (!rc_) rc_ = rc; return; }
-    op([L](cudaStream_t s) { return gemm_run(L, s); }, 1, d.conv ? 1 : 0, gemm_flops(L));
+    op([L](cudaStream_t s) { return gemm_run(L, s); }, kind, 1, gemm_flops(L));
   }
   void attention(const AttnDesc& d) {
-    if (dry_) { p_.launches += 1; return; }
+    if (dry_) { op(nullptr, kOpAttention); return; }
     AttnLaunch L;
     if (int rc = attn_prepare(d, &L)) { if (!rc_) rc_ = rc; return; }
-    op([L](cudaStream_t s) { return attn_run(L, s); }, 1, 2, attn_flops(d));
+    op([L](cudaStream_t s) { return attn_run(L, s); }, kOpAttention, 1, attn_flops(d));
   }
   // GroupNorm(+SiLU) of (a | b) from their statistics (Act::stats, see gemm_stats): one apply launch
   void groupnorm(const Act& xa, const Act* xb, int n_img, float eps, const NormW& n, int silu, bf16* out) {
@@ -577,10 +568,11 @@ class PlanBuilder {
     const bf16 *x1 = xa.p, *x2 = xb ? xb->p : nullptr;
     const int C1 = xa.C, C2 = xb ? xb->C : 0;
     const long long *s1 = xa.stats, *s2 = xb ? xb->stats : nullptr;
-    op([=](cudaStream_t s) { return groupnorm_apply_run(x1, C1, s1, x2, C2, s2, n_img, hw, groups, eps, n.g, n.b, silu, out, s); }, 1, 3);
+    op([=](cudaStream_t s) { return groupnorm_apply_run(x1, C1, s1, x2, C2, s2, n_img, hw, groups, eps, n.g, n.b, silu, out, s); },
+       kOpGroupNorm);
   }
   void layernorm(const bf16* x, int rows, int C, const NormW& n, bf16* out) {
-    op([=](cudaStream_t s) { return layernorm_run(x, rows, C, 1e-5f, n.g, n.b, out, s); }, 1, 4);
+    op([=](cudaStream_t s) { return layernorm_run(x, rows, C, 1e-5f, n.g, n.b, out, s); }, kOpLayerNorm);
   }
   // GEMM descriptors of a weight: out[M, w.out] = A[M, w.in] * w^T + bias, and the conv (conv_kind `kind`) of n_img NHWC
   // images [H, W, w.in]; call sites set what differs
@@ -598,7 +590,7 @@ class PlanBuilder {
 
   // ResnetBlock2D on (xa | xb) -> new buffer   (reference semantics: SURVEY R-1)
   Act resnet(const ResnetW& r, Act xa, const Act* xb, const bf16* temb_all, int ld_temb) {
-    const int B = p_.B, hw = xa.H * xa.W, M = B * hw;
+    const int B = p_.shape.B, hw = xa.H * xa.W, M = B * hw;
     const int Cb = xb ? xb->C : 0;
     const int Cin = xa.C + Cb;
     bf16* h0 = alloc(static_cast<size_t>(M) * Cin);
@@ -640,15 +632,15 @@ class PlanBuilder {
     const int Cp = x.heads * x.dpad;
     const Exchange& X = m_.xch_;
     const int idx = p_.n3d++;
-    p_.launches += 4;
     const long long rows_local = seq;                                   // F_loc * hw tokens per CFG half
-    const long long rows_global = static_cast<long long>(seq) / p_.F * p_.F_total;
+    const long long rows_global = static_cast<long long>(seq) / p_.shape.F * p_.shape.F_total;
     if (static_cast<size_t>(batch) * rows_global * 2 * Cp * sizeof(bf16) > X.kv_bytes) {
       set_error("K/V exchange buffer too small for this window (d4d_exchange_alloc)");
       if (!rc_) rc_ = 1;
       return;
     }
-    if (dry_) return;
+    // two ops: QKV GEMM + flag signal + flag wait, then the attention
+    if (dry_) { op(nullptr, kOpGemm, 3); op(nullptr, kOpAttention); return; }
     GemmLaunch G[2];
     AttnLaunch A[2];
     for (int par = 0; par < 2; ++par) {
@@ -670,8 +662,7 @@ class PlanBuilder {
     Plan* pl = &p_;
     const GemmLaunch G0 = G[0], G1 = G[1];
     const AttnLaunch A0 = A[0], A1 = A[1];
-    const double fl_g = gemm_flops(G0), fl_a = attn_flops(A0.d);
-    p_.ops.push_back([=](cudaStream_t s) {
+    op([=](cudaStream_t s) {
       const unsigned int counter = pl->epoch0 + idx;
       const int par = counter & 1;
       if (int rc = gemm_run(par ? G1 : G0, s)) return rc;
@@ -680,15 +671,11 @@ class PlanBuilder {
       f.slot = par;
       if (int rc = kv_signal_run(f, s)) return rc;
       return kv_wait_run(f, s);
-    });
-    p_.op_kind.push_back(0);
-    p_.op_flops.push_back(fl_g);
-    p_.ops.push_back([=](cudaStream_t s) {
+    }, kOpGemm, 3, gemm_flops(G0));
+    op([=](cudaStream_t s) {
       const unsigned int counter = pl->epoch0 + idx;
       return attn_run((counter & 1) ? A1 : A0, s);
-    });
-    p_.op_kind.push_back(2);
-    p_.op_flops.push_back(fl_a);
+    }, kOpAttention, 1, attn_flops(A0.d));
   }
 
   void self_attention(const AttnW& a, const XfW& x, const bf16* normed, const bf16* resid, bf16* out, int M, int batch, int seq,
@@ -696,7 +683,7 @@ class PlanBuilder {
     const int Cp = x.heads * x.dpad;
     bf16* qkv = alloc(static_cast<size_t>(M) * 3 * Cp);
     bf16* o = nullptr;
-    if (is3d && p_.F_total > 0) {
+    if (is3d && p_.shape.F_total > 0) {
       o = alloc(static_cast<size_t>(M) * Cp);
       sharded_qkv_attention(a, x, normed, qkv, o, M, batch, seq);
     } else {
@@ -719,7 +706,7 @@ class PlanBuilder {
 
   // TransformerMultiviewModel (+ its single MultiviewTransformerBlock): x -> new buffer
   Act transformer(const XfW& x, Act in) {
-    const int B = p_.B, hw = in.H * in.W, M = B * hw, C = x.C, num_frames = x.is3d ? p_.F : 1;
+    const int B = p_.shape.B, hw = in.H * in.W, M = B * hw, C = x.C, num_frames = x.is3d ? p_.shape.F : 1;
     bf16* n = alloc(static_cast<size_t>(M) * C);
     groupnorm(in, nullptr, B, 1e-6f, x.gn, 0, n);
     bf16* t = alloc(static_cast<size_t>(M) * C);
@@ -763,7 +750,7 @@ class PlanBuilder {
   }
 
   Act conv3x3(const LinW& w, Act in, int act = 0, int n_img = 0) {
-    if (n_img <= 0) n_img = p_.B;
+    if (n_img <= 0) n_img = p_.shape.B;
     const int M = n_img * in.H * in.W;
     Act out{alloc(static_cast<size_t>(M) * w.out), w.out, in.H, in.W};
     GemmDesc d = conv(w, in.p, n_img, in.H, in.W, out.p);
@@ -776,10 +763,12 @@ class PlanBuilder {
     Model& m = m_;
     const d4d_config& cfg = m.cfg_;
     Plan* pl = &p_;
-    const int B = p_.B, F = p_.F, h = p_.h, w = p_.w;
+    const PlanShape& sh = p_.shape;
+    const int B = sh.B, F = sh.F, h = sh.h, w = sh.w;
     const int* ch = cfg.block_out_channels;
     const int C0 = ch[0], TE = 4 * C0, L = cfg.layers_per_block;
     const int M0 = B * h * w;
+    D4D_CUDA_OK(cudaDeviceGetAttribute(&sms_, cudaDevAttrMultiProcessorCount, m.device_));  // (gemm_stats)
 
     if (!dry_ && p_.stats_words > 0) {  // GroupNorm statistics pool (size from the dry run): zeroed once per forward
       stats_pool_ = reinterpret_cast<long long*>(alloc(p_.stats_words * 4));
@@ -806,8 +795,8 @@ class PlanBuilder {
       float* pos = reinterpret_cast<float*>(alloc(static_cast<size_t>(B) * 2));
       if (!dry_) {
         std::vector<float> hp(B);
-        for (int dmn = 0; dmn < p_.n_domains; ++dmn)
-          for (int f = 0; f < F; ++f) hp[dmn * F + f] = p_.domains[dmn] == 0 ? 0.f : static_cast<float>((p_.rank * F + f) % std::max(1, (p_.F_total > 0 ? p_.F_total : F) / 2));
+        for (int dmn = 0; dmn < sh.n_domains; ++dmn)
+          for (int f = 0; f < F; ++f) hp[dmn * F + f] = sh.domains[dmn] == 0 ? 0.f : static_cast<float>((sh.rank * F + f) % std::max(1, (sh.F_total > 0 ? sh.F_total : F) / 2));
         if (cudaMemcpy(pos, hp.data(), sizeof(float) * B, cudaMemcpyHostToDevice) != cudaSuccess) rc_ = 2;
       }
       op([=](cudaStream_t s) { return sinusoid_run(pos, B, C0, 1, 0.f, tsin, s); });
@@ -842,7 +831,7 @@ class PlanBuilder {
       // pose_shared_neg: the skeleton batch is [1 constant CFG-negative image | F positive images] instead of 2F images
       // (pipeline_diffuman4d.py:349-356 makes every negative skeleton the same all(-1) image); its embedding is computed
       // once per forward and broadcast to the F negative images below
-      const int PB = p_.pose_shared_neg ? F + 1 : B;
+      const int PB = sh.pose_shared_neg ? F + 1 : B;
       const int PM0 = PB * h * w;
       const PoseW& pw = m.pose_;
       bf16* a0 = alloc(static_cast<size_t>(PB) * Hs * Ws * 4);  // 3 channels padded to 4
@@ -881,7 +870,7 @@ class PlanBuilder {
         gemm(d);
       }
       release(x7.p);
-      if (p_.pose_shared_neg) {  // broadcast: images 0..F-1 <- embedding 0, images F..2F-1 <- embeddings 1..F
+      if (sh.pose_shared_neg) {  // broadcast: images 0..F-1 <- embedding 0, images F..2F-1 <- embeddings 1..F
         bf16* full = alloc(static_cast<size_t>(M0) * C0);
         bf16* small = pose_emb;
         const long long per_img = static_cast<long long>(h) * w * C0;
@@ -1001,14 +990,15 @@ class PlanBuilder {
   std::map<size_t, size_t> live_;
   long long* stats_pool_ = nullptr;
   size_t stats_used_ = 0;
+  int sms_ = 0;
   int rc_ = 0;
   std::vector<Plan::Tap> module_taps_;
 };
 
 Plan* Model::find_plan(int n_domains, int B, int F, int h, int w) {
   for (auto& kv : plans_) {
-    Plan* p = kv.second.get();
-    if (p->n_domains == n_domains && p->B == B && p->F == F && p->h == h && p->w == w) return p;
+    const PlanShape& s = kv.second->shape;
+    if (s.n_domains == n_domains && s.B == B && s.F == F && s.h == h && s.w == w) return kv.second.get();
   }
   return nullptr;
 }
@@ -1018,6 +1008,7 @@ int Model::get_plan(const int* domain_ids, int n_domains, int B, int F, int h, i
     set_error("weights not finalized (call d4d_finalize_weights)");
     return 3;
   }
+  D4D_REQUIRE(domain_ids != nullptr, "null argument");
   D4D_REQUIRE(B > 0 && F > 0 && n_domains > 0, "empty batch");
   if (n_domains * F != B) {
     // same message as the reference's ValueError (unet_multiview_condition.py:524-525)
@@ -1032,7 +1023,12 @@ int Model::get_plan(const int* domain_ids, int n_domains, int B, int F, int h, i
     D4D_REQUIRE(xch_.ready && xch_.world >= 1, "frame-sharded forward needs d4d_exchange_open first");
     D4D_REQUIRE(F * xch_.world == F_total, "F_total must equal world * local frames");
   }
-  const std::string key = plan_key(domain_ids, n_domains, B, F, h, w) + (sharded ? "_sh" + std::to_string(F_total) : std::string()) + (pose_shared_neg ? "_pn" : "");
+  PlanShape s;
+  s.n_domains = n_domains; s.B = B; s.F = F; s.h = h; s.w = w;
+  s.domains.assign(domain_ids, domain_ids + n_domains);
+  if (sharded) { s.F_total = F_total; s.rank = xch_.rank; s.world = xch_.world; }
+  s.pose_shared_neg = pose_shared_neg && cfg_.enable_pose_encoder && n_domains == 2;
+  const std::string key = plan_key(s);
   auto it = plans_.find(key);
   if (it != plans_.end()) {
     *out = it->second.get();
@@ -1040,17 +1036,11 @@ int Model::get_plan(const int* domain_ids, int n_domains, int B, int F, int h, i
   }
   D4D_CUDA_OK(cudaSetDevice(device_));
   std::unique_ptr<Plan> p(new Plan());
-  p->n_domains = n_domains; p->B = B; p->F = F; p->h = h; p->w = w;
-  p->domains.assign(domain_ids, domain_ids + n_domains);
-  if (sharded) { p->F_total = F_total; p->rank = xch_.rank; p->world = xch_.world; }
-  p->pose_shared_neg = pose_shared_neg && cfg_.enable_pose_encoder && n_domains == 2;
+  p->shape = s;
   size_t peak = 0;
   {
     Plan scratch;
-    scratch.n_domains = n_domains; scratch.B = B; scratch.F = F; scratch.h = h; scratch.w = w;
-    scratch.domains = p->domains;
-    scratch.F_total = p->F_total; scratch.rank = p->rank; scratch.world = p->world;
-    scratch.pose_shared_neg = p->pose_shared_neg;
+    scratch.shape = s;
     PlanBuilder dry(*this, scratch, true, nullptr);
     if (int rc = dry.build()) return rc;
     peak = dry.peak();
@@ -1066,28 +1056,38 @@ int Model::get_plan(const int* domain_ids, int n_domains, int B, int F, int h, i
   return 0;
 }
 
-int Model::forward(const bf16* sample, const long long* timestep, const bf16* skeletons, const int* domain_ids,
-                   int n_domains, int B, int F, int h, int w, bf16* out, cudaStream_t stream, int F_total, bool pose_shared_neg) {
-  D4D_REQUIRE(sample && timestep && out && domain_ids, "null argument");
+int Model::run_ops(Plan& p, const bf16* sample, const long long* timestep, const bf16* skeletons, bf16* out, size_t n,
+                   cudaStream_t stream, bool timed) {
+  D4D_REQUIRE(sample && timestep && (out || n < p.ops.size()), "null argument");
   D4D_REQUIRE(!cfg_.enable_pose_encoder || skeletons != nullptr, "skeletons are required when enable_pose_encoder");
   D4D_REQUIRE(!cfg_.center_input_sample, "center_input_sample is not supported");
+  D4D_CUDA_OK(cudaSetDevice(device_));
+  p.sample = sample; p.timestep = timestep; p.skeletons = skeletons; p.out = out;
+  p.epoch0 = xch_.epoch_base;  // global, monotonic exchange counter: every rank runs the same forwards in the same order
+  while (timed && p.events.size() < n + 1) {
+    cudaEvent_t e;
+    D4D_CUDA_OK(cudaEventCreate(&e));
+    p.events.push_back(e);
+  }
+  for (size_t i = 0; i < n; ++i) {
+    if (timed) D4D_CUDA_OK(cudaEventRecord(p.events[i], stream));
+    if (int rc = p.ops[i].run(stream)) return rc;
+  }
+  if (timed) D4D_CUDA_OK(cudaEventRecord(p.events[n], stream));
+  return 0;
+}
+
+int Model::forward(const bf16* sample, const long long* timestep, const bf16* skeletons, const int* domain_ids,
+                   int n_domains, int B, int F, int h, int w, bf16* out, cudaStream_t stream, int F_total, bool pose_shared_neg) {
   Plan* p = nullptr;
   if (int rc = get_plan(domain_ids, n_domains, B, F, h, w, &p, F_total, pose_shared_neg)) return rc;
-  D4D_CUDA_OK(cudaSetDevice(device_));
-  p->sample = sample;
-  p->timestep = timestep;
-  p->skeletons = skeletons;
-  p->out = out;
-  p->epoch0 = xch_.epoch_base;  // global, monotonic exchange counter: every rank runs the same forwards in the same order
-  for (auto& f : p->ops)
-    if (int rc = f(stream)) return rc;
+  if (int rc = run_ops(*p, sample, timestep, skeletons, out, p->ops.size(), stream)) return rc;
   xch_.epoch_base += static_cast<unsigned int>(p->n3d);
   return 0;
 }
 
 int Model::debug_tap(const bf16* sample, const long long* timestep, const bf16* skeletons, const int* domain_ids, int n_domains,
                      int B, int F, int h, int w, int tap, bf16* out, char* name64, int* dims3, cudaStream_t stream) {
-  D4D_REQUIRE(domain_ids != nullptr, "null argument");
   Plan* p = nullptr;
   if (int rc = get_plan(domain_ids, n_domains, B, F, h, w, &p)) return rc;
   if (tap < 0 || tap >= static_cast<int>(p->taps.size())) {
@@ -1101,12 +1101,7 @@ int Model::debug_tap(const bf16* sample, const long long* timestep, const bf16* 
   }
   if (dims3) { dims3[0] = t.C; dims3[1] = t.H; dims3[2] = t.W; }
   if (!out) return 0;
-  D4D_REQUIRE(sample && timestep, "null argument");
-  D4D_REQUIRE(!cfg_.enable_pose_encoder || skeletons != nullptr, "skeletons are required when enable_pose_encoder");
-  D4D_CUDA_OK(cudaSetDevice(device_));
-  p->sample = sample; p->timestep = timestep; p->skeletons = skeletons; p->out = nullptr;
-  for (size_t i = 0; i < t.n_ops; ++i)
-    if (int rc = p->ops[i](stream)) return rc;
+  if (int rc = run_ops(*p, sample, timestep, skeletons, nullptr, t.n_ops, stream)) return rc;
   return nhwc_to_nchw_run(t.p, t.C, B, t.C, t.H * t.W, out, stream);
 }
 
@@ -1165,31 +1160,20 @@ int Model::exchange_open(int rank, int world, const unsigned char* all_handles) 
 int Model::profile(const bf16* sample, const long long* timestep, const bf16* skeletons, const int* domain_ids, int n_domains,
                    int B, int F, int h, int w, bf16* out, cudaStream_t stream, float* ms_by_kind, int* launches_by_kind,
                    double* flops_by_kind) {
-  D4D_REQUIRE(sample && timestep && out && domain_ids && ms_by_kind && launches_by_kind && flops_by_kind, "null argument");
+  D4D_REQUIRE(ms_by_kind && launches_by_kind && flops_by_kind, "null argument");
   Plan* p = nullptr;
   if (int rc = get_plan(domain_ids, n_domains, B, F, h, w, &p)) return rc;
-  D4D_CUDA_OK(cudaSetDevice(device_));
-  p->sample = sample; p->timestep = timestep; p->skeletons = skeletons; p->out = out;
   const size_t n = p->ops.size();
-  while (p->events.size() < n + 1) {
-    cudaEvent_t e;
-    D4D_CUDA_OK(cudaEventCreate(&e));
-    p->events.push_back(e);
-  }
-  for (size_t i = 0; i < n; ++i) {
-    D4D_CUDA_OK(cudaEventRecord(p->events[i], stream));
-    if (int rc = p->ops[i](stream)) return rc;
-  }
-  D4D_CUDA_OK(cudaEventRecord(p->events[n], stream));
+  if (int rc = run_ops(*p, sample, timestep, skeletons, out, n, stream, true)) return rc;
   D4D_CUDA_OK(cudaEventSynchronize(p->events[n]));
-  for (int k = 0; k < 6; ++k) { ms_by_kind[k] = 0.f; launches_by_kind[k] = 0; flops_by_kind[k] = 0.0; }
+  for (int k = 0; k < kNumOpKinds; ++k) { ms_by_kind[k] = 0.f; launches_by_kind[k] = 0; flops_by_kind[k] = 0.0; }
   for (size_t i = 0; i < n; ++i) {
     float ms = 0.f;
     D4D_CUDA_OK(cudaEventElapsedTime(&ms, p->events[i], p->events[i + 1]));
-    const int k = p->op_kind[i];
-    ms_by_kind[k] += ms;
-    launches_by_kind[k] += 1;
-    flops_by_kind[k] += p->op_flops[i];
+    const PlanOp& op = p->ops[i];
+    ms_by_kind[op.kind] += ms;
+    launches_by_kind[op.kind] += op.launches;
+    flops_by_kind[op.kind] += op.flops;
   }
   return 0;
 }

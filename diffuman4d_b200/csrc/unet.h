@@ -52,28 +52,38 @@ struct PoseW {
   float scale = 1.f;
 };
 
-struct Plan {
+// Kernel kinds of d4d_profile_forward (include/d4d.h), in its order.
+enum OpKind { kOpGemm, kOpConv, kOpAttention, kOpGroupNorm, kOpLayerNorm, kOpOther, kNumOpKinds };
+static_assert(kNumOpKinds == 6, "d4d_profile_forward reports [6] arrays per kind");
+
+// one op of a plan: what it enqueues, its kernel launches and executed FLOPs (tensor-core ops, incl. tile / head padding)
+struct PlanOp { std::function<int(cudaStream_t)> run; OpKind kind; int launches; double flops; };
+
+// What a plan is built for, and so what it allocates.
+struct PlanShape {
   int n_domains = 0, B = 0, F = 0, h = 0, w = 0;
   std::vector<int> domains;
-  void* arena = nullptr;
-  size_t arena_bytes = 0;
-  int launches = 0;
   // frame-sharded window (DESIGN.md section 7): this rank owns F of F_total frames per CFG half
   int F_total = 0, rank = 0, world = 1;
   bool pose_shared_neg = false;  // skeleton batch = [1 CFG-negative image | F positive images] (window step)
+};
+
+struct Plan {
+  PlanShape shape;
+  void* arena = nullptr;
+  size_t arena_bytes = 0;
+  int launches = 0;            // sum of ops[i].launches
   size_t stats_words = 0;      // GroupNorm statistics pool: 64-bit fixed-point per-(image, channel) sums of every tensor a GroupNorm reads
   int n3d = 0;                 // number of 3-D attention layers (K/V exchanges) per forward
   unsigned int epoch0 = 0;     // exchange counter at the start of the current forward (epoch / buffer parity per layer)
-  std::vector<std::function<int(cudaStream_t)>> ops;
-  std::vector<int> op_kind;       // 0 gemm, 1 conv3x3, 2 attention, 3 groupnorm, 4 layernorm, 5 other
-  std::vector<double> op_flops;   // executed FLOPs (incl. tile/head padding) of tensor-core ops
-  std::vector<cudaEvent_t> events; // lazily created by profile()
+  std::vector<PlanOp> ops;
+  std::vector<cudaEvent_t> events; // lazily created by a timed Model::run_ops (profile)
   // debug taps (per-level drift report, tests/test_gpu_fullsize.py; per-module checks, tests/test_gpu_unet_modules.py): a
   // named intermediate activation [B*H*W, C] (NHWC) that is complete once ops[0 .. n_ops) have run; the arena may reuse its
   // storage afterwards.  The ten block taps come first, then the module taps in forward order (include/d4d.h).
   struct Tap { std::string name; const bf16* p; int C, H, W; size_t n_ops; };
   std::vector<Tap> taps;
-  // per-call externals, set by Model::forward before running the ops
+  // per-call externals, set by Model::run_ops before running the ops
   const bf16* sample = nullptr;
   const long long* timestep = nullptr;
   const bf16* skeletons = nullptr;
@@ -177,6 +187,10 @@ class Model {
   Exchange xch_;
 
   void need(const std::string& key, std::vector<int64_t> shape);
+  // checks and binds the per-call externals of p, then enqueues ops[0 .. n); timed: events[i] is recorded before op i and
+  // events[n] after the last
+  int run_ops(Plan& p, const bf16* sample, const long long* timestep, const bf16* skeletons, bf16* out, size_t n,
+              cudaStream_t stream, bool timed = false);
   int cin_pad() const { return 16; }
   int kp_in() const { return 192; }
 };
