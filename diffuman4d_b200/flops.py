@@ -5,75 +5,23 @@ n_l = (h / 2^l)(w / 2^l), F_l = F for 3-D blocks else 1:
     conv3(ci,co,n) = 18 ci co n        lin(ci,co,n) = 2 ci co n
     Resnet(ci,co,n) = conv3(ci,co,n) + conv3(co,co,n) + [ci != co] lin(ci,co,n) + 2*TE*co
     Transf(C,n,F_l) = 6 lin(C,C,n) + 4 n (F_l n) C + 24 C^2 n   [+ attn2: 4 lin(C,C,n) + 4 n^2 C]
-Embedding MLPs, the pose encoder and elementwise work are excluded (< 0.1 %).
+Embedding MLPs, the pose encoder and elementwise work are excluded (< 0.1 %).  Each launch of plan.launches carries its
+term of this sum.
 """
 from __future__ import annotations
 
 from typing import Dict
 
 from .config import UNetConfig
+from .plan import launches
 
 
 def unet_flops(cfg: UNetConfig, B: int, F: int, h: int, w: int) -> Dict[str, float]:
-    ch = cfg.block_out_channels
-    TE = cfg.time_embed_dim
-    L = cfg.layers_per_block
+    if B % F:
+        raise ValueError(f"B ({B}) must be a whole number of CFG halves of F ({F}) frames")
     out = {"conv3x3": 0.0, "linear": 0.0, "attn3d": 0.0, "attn2d": 0.0, "ff": 0.0}
-
-    def n(l):
-        return (h >> l) * (w >> l)
-
-    def conv3(ci, co, nn):
-        out["conv3x3"] += 18.0 * ci * co * nn * B
-
-    def lin(ci, co, nn, key="linear"):
-        out[key] += 2.0 * ci * co * nn * B
-
-    def resnet(ci, co, nn):
-        conv3(ci, co, nn)
-        conv3(co, co, nn)
-        if ci != co:
-            lin(ci, co, nn)
-        out["linear"] += 2.0 * TE * co * B
-
-    def transf(C, nn, Fl, attn2):
-        for _ in range(6):
-            lin(C, C, nn)
-        out["attn3d" if Fl > 1 else "attn2d"] += 4.0 * nn * (Fl * nn) * C * B
-        out["ff"] += 24.0 * C * C * nn * B
-        if attn2:
-            for _ in range(4):
-                lin(C, C, nn)
-            out["attn2d"] += 4.0 * nn * nn * C * B
-
-    conv3(cfg.in_channels, ch[0], n(0))
-    co = ch[0]
-    for i in range(4):
-        ci, co = co, ch[i]
-        Fl = F if (4 - i - 1) < cfg.num_3d_attn_blocks else 1
-        for j in range(L):
-            resnet(ci if j == 0 else co, co, n(i))
-            if i < 3:
-                transf(co, n(i), Fl, cfg.has_attn2(i))
-        if i < 3:
-            conv3(co, co, n(i + 1))
-    resnet(ch[3], ch[3], n(3))
-    transf(ch[3], n(3), F, cfg.has_attn2(3))
-    resnet(ch[3], ch[3], n(3))
-    co = ch[3]
-    for i in range(4):
-        cprev, co = co, ch[3 - i]
-        cin = ch[3 - min(i + 1, 3)]
-        lvl = 3 - i
-        Fl = F if i < cfg.num_3d_attn_blocks else 1
-        for j in range(L + 1):
-            skip = cin if j == L else co
-            rin = cprev if j == 0 else co
-            resnet(rin + skip, co, n(lvl))
-            if i > 0:
-                transf(co, n(lvl), Fl, cfg.has_attn2(lvl))
-        if i < 3:
-            conv3(co, co, n(lvl - 1))
-    conv3(ch[0], cfg.out_channels, n(0))
+    for launch in launches(cfg, F, h, w, halves=B // F):
+        if launch.algo:
+            out[launch.category] += launch.algo
     out["total"] = sum(out.values())
     return out

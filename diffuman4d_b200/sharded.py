@@ -20,23 +20,16 @@ import torch.distributed as dist
 
 from ._lib import check, lib
 from .pipeline import B200Diffuman4DPipeline, _check_inplace, build_windows
+from .plan import modules, pad_head_dim
 from .scheduler import DPMSolverState
 from .sharding import frame_shard
 
 
 def exchange_bytes(cfg, F_total: int, h: int, w: int, cfg_halves: int = 2) -> int:
-    """Size of one gathered K|V buffer: the largest 3-D attention layer.  The mid block (level 3) always runs one; level
-    L < 3 runs them (down_blocks.L, up_blocks.3-L) when 3 - L < num_3d_attn_blocks, so level 0 with 4."""
-    best = 0
-    for lvl in (0, 1, 2, 3):
-        if lvl < 3 and 3 - lvl >= cfg.num_3d_attn_blocks:
-            continue
-        d = cfg.head_dim(lvl)
-        dpad = 64 if d <= 64 else (128 if d <= 128 else 192)
-        cp = cfg.heads(lvl) * dpad
-        tokens = cfg_halves * F_total * (h >> lvl) * (w >> lvl)
-        best = max(best, tokens * 2 * cp * 2)
-    return best
+    """Size of one gathered K|V buffer: the largest 3-D attention layer, its K|V columns (heads x padded head dim each)
+    for every token of the window."""
+    return max((cfg_halves * F_total * (h >> m.level) * (w >> m.level) * 2 * cfg.heads(m.level)
+                * pad_head_dim(cfg.head_dim(m.level)) * 2 for m in modules(cfg) if m.is3d), default=0)
 
 
 def window_result_bytes(F_total: int, h: int, w: int, dpm: bool = True) -> int:

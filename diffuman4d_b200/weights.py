@@ -1,7 +1,8 @@
 """Weight-key contract of the UNet (diffusers layout, SURVEY.md section 8b) and seeded random weights.
 
 ``state_dict_spec`` lists every parameter of ``unet/diffusion_pytorch_model.safetensors`` for a given config with its
-diffusers shape; the C++ loader (the ``Model`` constructor in csrc/unet.cu) and the CPU oracle must agree with it (tested).
+diffusers shape, module by module of plan.modules; the C++ loader (the ``Model`` constructor in csrc/unet.cu) and the CPU
+oracle must agree with it (tested).
 """
 from __future__ import annotations
 
@@ -12,14 +13,14 @@ from typing import Dict, Tuple
 import torch
 
 from .config import UNetConfig
+from .plan import modules
 
 POSE_SPEC = [(3, 3, 3), (3, 16, 4), (16, 16, 3), (16, 32, 4), (32, 32, 3), (32, 64, 4), (64, 64, 3), (64, 128, 3)]
 
 
 def state_dict_spec(cfg: UNetConfig) -> "OrderedDict[str, Tuple[int, ...]]":
     spec: "OrderedDict[str, Tuple[int, ...]]" = OrderedDict()
-    ch = cfg.block_out_channels
-    C0, TE, L = ch[0], cfg.time_embed_dim, cfg.layers_per_block
+    C0, TE = cfg.block_out_channels[0], cfg.time_embed_dim
 
     def lin(p, out, inp, bias=True):
         spec[p + ".weight"] = (out, inp)
@@ -78,30 +79,13 @@ def state_dict_spec(cfg: UNetConfig) -> "OrderedDict[str, Tuple[int, ...]]":
             conv(f"pose_encoder.conv_layers.{2 * i}", co, ci, k)
         conv("pose_encoder.final_proj", C0, 128, 1)
         spec["pose_encoder.scale"] = (1,)
-    cout = C0
-    for i in range(4):
-        cin, cout = cout, ch[i]
-        for j in range(L):
-            resnet(f"down_blocks.{i}.resnets.{j}", cin if j == 0 else cout, cout)
-            if i < 3:
-                xf(f"down_blocks.{i}.attentions.{j}", cout, cfg.has_attn2(i))
-        if i < 3:
-            conv(f"down_blocks.{i}.downsamplers.0.conv", cout, cout, 3)
-    resnet("mid_block.resnets.0", ch[3], ch[3])
-    xf("mid_block.attentions.0", ch[3], cfg.has_attn2(3))
-    resnet("mid_block.resnets.1", ch[3], ch[3])
-    cout = ch[3]
-    for i in range(4):
-        cprev, cout = cout, ch[3 - i]
-        cin = ch[3 - min(i + 1, 3)]
-        for j in range(L + 1):
-            skip = cin if j == L else cout
-            rin = cprev if j == 0 else cout
-            resnet(f"up_blocks.{i}.resnets.{j}", rin + skip, cout)
-            if i > 0:
-                xf(f"up_blocks.{i}.attentions.{j}", cout, cfg.has_attn2(3 - i))
-        if i < 3:
-            conv(f"up_blocks.{i}.upsamplers.0.conv", cout, cout, 3)
+    for m in modules(cfg):
+        if m.type == "resnet":
+            resnet(m.path, m.cin + m.skip, m.cout)
+        elif m.type == "transformer":
+            xf(m.path, m.cout, m.attn2)
+        else:
+            conv(m.path + ".conv", m.cout, m.cin, 3)
     norm("conv_norm_out", C0)
     conv("conv_out", cfg.out_channels, C0, 3)
     return spec

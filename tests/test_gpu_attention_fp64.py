@@ -4,8 +4,8 @@ test_gpu_ops.py::test_attention accepts |out - ref| <= 1e-2 |ref| + 5e-3 max|ref
 about four times the kernel's rounding, so a kernel that truncates P to bf16 (a -2e-3 bias in every output) or whose
 exp2 is 5e-3 off on every other key passes it.  And the plan's own attention shapes (16384 to 65536 keys) are reached
 only by the whole-network tests, after sixty layers of drift.  Here every distinct d4d_op_attention call of one forward
-(attention_launches, restated from PlanBuilder::transformer and checked against d4d_profile_forward's attention count
-and FLOPs) runs on seeded bf16 inputs in the plan's memory layout, and is compared with
+(attention_launches, from plan.launches, which test_plan.py checks against d4d_profile_forward's launch counts and
+FLOPs) runs on seeded bf16 inputs in the plan's memory layout, and is compared with
 
   R64  softmax(scale q k^T) v in float64 on the same bf16 inputs, and A = softmax(scale q k^T) |v|;
   E    the rounding model of DESIGN section 2 in float64: P = bf16(p) with p = exp(s - max s), O = sum P v / sum p,
@@ -31,8 +31,6 @@ emulation passes with margin, and each of five plausible kernel defects fails a 
 test_gpu_kernel_edges.py::test_attention_key_census.  At 16384 keys one dropped key moves an output by ~1e-4, below
 what (a)-(c) see; the census, extended to the plan's key counts, covers that.
 """
-import ctypes as C
-import gc
 import math
 import time
 from collections import Counter
@@ -43,6 +41,7 @@ import torch
 import torch.nn.functional as F
 
 from diffuman4d_b200.config import UNetConfig
+from diffuman4d_b200.plan import launches
 from test_gpu_kernel_edges import census_misses, census_v  # noqa: E402
 
 BOUND_ULP = 2.0 ** -8      # (a): |K - R64| <= BOUND_ULP (|R64| + A)
@@ -54,42 +53,15 @@ DISTRIBUTIONS = ("flat", "sharp", "rising", "dominant", "offset_v")
 
 
 # ------------------------------------------------------------------------------------------------ the plan's launches
-def _dpad(d):
-    return 64 if d <= 64 else (128 if d <= 128 else 192)
-
-
 def _scale(d):
     """The softmax scale the plan passes: 1.0f / sqrtf(head_dim), from the real head_dim."""
     return float(np.float32(1.0) / np.sqrt(np.float32(d)))
 
 
 def attention_launches(cfg, F, h, w, halves=2, ranks=1):
-    """Every distinct d4d_op_attention call of one forward of `halves` CFG halves of F frames at an h x w latent, as
-    {(batch, seq, seq_kv, heads, head_dim padded, head_dim, scale): count}, restated from PlanBuilder::transformer and
-    self_attention (csrc/unet.cu).  Level L (channel level; the mid block is level 3) has 2 * layers_per_block + 1
-    transformers (down_blocks.L and up_blocks.3-L), the mid block one.  attn1 is 3-D (one sequence of F * hw tokens per
-    CFG half) at the mid block and where 3 - L < num_3d_attn_blocks, per image elsewhere; attn2 is per image.
-    ranks > 1: one rank's launches of the frame-sharded window, F / ranks frames local: a 3-D attention has
-    seq = F / ranks * hw local queries and seq_kv = F * hw gathered keys."""
-    calls = Counter()
-    B = halves * F // ranks
-    for lvl in range(4):
-        n_xf = 1 if lvl == 3 else 2 * cfg.layers_per_block + 1
-        hw = (h >> lvl) * (w >> lvl)
-        heads, d = cfg.heads(lvl), cfg.head_dim(lvl)
-        shape = (heads, _dpad(d), d, _scale(d))
-        if (lvl == 3 or 3 - lvl < cfg.num_3d_attn_blocks) and F // ranks > 1:
-            calls[(halves, F // ranks * hw, F * hw, *shape)] += n_xf
-        else:
-            calls[(B, hw, hw, *shape)] += n_xf
-        if cfg.has_attn2(lvl):
-            calls[(B, hw, hw, *shape)] += n_xf
-    return dict(calls)
-
-
-def attention_flops(launches):
-    """4 batch heads seq seq_kv dpad over every call: attn_flops (csrc/attention_wgmma.cu) summed over the plan."""
-    return sum(4.0 * b * hd * s * skv * dp * n for (b, s, skv, hd, dp, d, sc), n in launches.items())
+    """Every distinct d4d_op_attention call of plan.launches(cfg, F, h, w, halves, ranks), as
+    {(batch, seq, seq_kv, heads, head_dim padded, head_dim, scale): count}."""
+    return dict(Counter(tuple(a.spec.values()) for a in launches(cfg, F, h, w, halves, ranks) if a.kind == "attention"))
 
 
 SD21, CTOR = UNetConfig.sd21(), UNetConfig.ctor_default()
@@ -448,36 +420,3 @@ def test_attention_launch_vs_fp64(cuda, case):
     torch.cuda.synchronize()
     print("\n".join(lines) + f"\n  [{_case_id(case)}] {time.perf_counter() - t0:.1f} s")
     assert not fails, fails
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("plan", list(PLANS))
-def test_attention_launches_match_profile(cuda, plan):
-    """attention_launches is the plan's list: one profiled forward (d4d_profile_forward, the call bench.py makes)
-    reports the same number of attention launches and the same attention FLOPs."""
-    from diffuman4d_b200._lib import check, lib
-    from diffuman4d_b200.unet import B200MultiviewUNet
-    from diffuman4d_b200.weights import random_state_dict
-    cfg, F, h, w = PLANS[plan]
-    B = 2 * F
-    unet = B200MultiviewUNet(cfg, device=0).load_state_dict(random_state_dict(cfg, seed=1, device="cuda"))
-    try:
-        g = torch.Generator(device="cuda").manual_seed(0)
-        x = torch.randn(B, cfg.in_channels, h, w, generator=g, device="cuda").to(torch.bfloat16)
-        t = torch.randint(0, 1000, (B,), generator=g, device="cuda")
-        sk = (torch.rand(B, 3, 8 * h, 8 * w, generator=g, device="cuda") * 2 - 1).to(torch.bfloat16) \
-            if cfg.enable_pose_encoder else None
-        y = torch.empty(B, cfg.out_channels, h, w, device="cuda", dtype=torch.bfloat16)
-        ms, n, fl = (C.c_float * 6)(), (C.c_int32 * 6)(), (C.c_double * 6)()
-        check(lib().d4d_profile_forward(unet._h, x.data_ptr(), t.data_ptr(), None if sk is None else sk.data_ptr(),
-                                        (C.c_int32 * 2)(0, 1), 2, B, F, h, w, y.data_ptr(),
-                                        torch.cuda.current_stream().cuda_stream, ms, n, fl), "d4d_profile_forward")
-        launches = attention_launches(cfg, F, h, w)
-        print(f"\n  [{plan}] attention: {n[2]} launches, {fl[2] / 1e12:.3f} TFLOP, {ms[2]:.2f} ms; "
-              f"{len(launches)} distinct shapes")
-        assert n[2] == sum(launches.values())
-        assert fl[2] == attention_flops(launches)
-    finally:
-        del unet
-        gc.collect()
-        torch.cuda.empty_cache()

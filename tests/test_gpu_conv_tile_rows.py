@@ -20,6 +20,8 @@ import torch
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tools"))
 
+from diffuman4d_b200.config import UNetConfig  # noqa: E402
+from diffuman4d_b200.plan import launches  # noqa: E402
 from test_gpu_kernel_edges import _check_ws, _close, _conv_ref, _rand, _stats_ws, _stream  # noqa: E402
 
 KIND = {"s1": 0, "s2": 1, "up": 3}
@@ -122,19 +124,9 @@ def test_rows_256_refused_where_no_kernel_exists(cuda):
 
 
 def _plan_convs(n, s):
-    """(n, H, W, Cin, Cout, mode) of every conv of the SD-2.1 plan on n images of s x s latents (channels 320 / 640 / 1280 / 1280)."""
-    C = (320, 640, 1280, 1280)
-    out = [(n, s, s, 64, 64, "s1"), (n, s, s, 64, 128, "s1"), (n, s, s, 320, 16, "s1")]   # pose encoder, conv_out
-    for lvl in range(4):
-        hw = s >> lvl
-        out.append((n, hw, hw, C[lvl], C[lvl], "s1"))
-        if lvl < 3:
-            out.append((n, hw, hw, C[lvl], C[lvl], "s2"))
-            out.append((n, hw >> 1, hw >> 1, C[lvl], C[lvl + 1], "s1"))   # first resnet of the next level: the wider Cout
-        if lvl > 0:
-            out.append((n, hw, hw, C[lvl], C[lvl], "up"))
-            out.append((n, hw, hw, 2 * C[lvl], C[lvl], "s1"))            # up path: conv1 over the concat
-    return out
+    """(n, H, W, Cin, Cout, mode) of every distinct conv of the SD-2.1 plan (plan.launches) on n images of s x s latents."""
+    convs = (c for c in launches(UNetConfig.sd21(), n // 2, s, s) if c.kind == "conv")
+    return list(dict.fromkeys(tuple(c.spec.values()) for c in convs))
 
 
 @pytest.mark.parametrize("n,s", [(32, 64), (48, 64), (32, 128)], ids=["W16@64", "W24@64", "W16@128"])

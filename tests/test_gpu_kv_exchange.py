@@ -23,46 +23,26 @@ import pytest
 import torch
 
 from diffuman4d_b200.config import SchedulerConfig, UNetConfig
+from diffuman4d_b200.plan import launches, pad_head_dim
 from diffuman4d_b200.sharded import exchange_bytes
 
 SENT16 = 0x7FA5       # bf16 NaN bit pattern that no kernel produces
 WIDTHS = (64, 128, 160, 192, 256)
 
 
-def _pad(d):
-    return 64 if d <= 64 else (128 if d <= 128 else 192)
-
-
 # ------------------------------------------------------------------------------------------------ exchange buffer size (CPU)
-def _layers_3d(cfg):
-    """Level of every 3-D attention layer of the plan, in PlanBuilder::build's order: down_blocks.i (i < 3) when
-    4 - i - 1 < num_3d_attn_blocks, the mid block always, up_blocks.i (i > 0) when i < num_3d_attn_blocks (level 3 - i)."""
-    n3d, L = cfg.num_3d_attn_blocks, cfg.layers_per_block
-    levels = []
-    for i in range(3):
-        if 4 - i - 1 < n3d:
-            levels += [i] * L
-    levels.append(3)
-    for i in range(1, 4):
-        if i < n3d:
-            levels += [3 - i] * (L + 1)
-    return levels
-
-
 @pytest.mark.parametrize("n3d", [0, 1, 2, 3, 4])
 @pytest.mark.parametrize("name", ["tiny", "sd21", "ctor_default"])
 def test_exchange_bytes_is_the_largest_3d_layer(name, n3d):
     """exchange_bytes equals the largest batch * rows_global * 2 C' * 2 bytes that sharded_qkv_attention (csrc/unet.cu)
-    requires of the buffer, over the layers the plan builds: too small fails every sharded forward, and num_3d_attn_blocks
-    = 4 puts a 3-D layer on level 0 (full-resolution tokens)."""
+    requires of the buffer, over the 3-D attention launches of the plan: too small fails every sharded forward, and
+    num_3d_attn_blocks = 4 puts a 3-D layer on level 0 (full-resolution tokens)."""
     cfg = dataclasses.replace(getattr(UNetConfig, name)(), num_3d_attn_blocks=n3d)
     for F_total in (2, 4, 16, 24):
         for lat in (16, 24, 64, 128):
-            need = 0
-            for lvl in _layers_3d(cfg):
-                cp = cfg.heads(lvl) * _pad(cfg.head_dim(lvl))
-                rows_global = F_total * (lat >> lvl) ** 2     # seq / F * F_total: every frame's tokens of one CFG half
-                need = max(need, 2 * rows_global * 2 * cp * 2)  # batch (CFG halves) * rows * K|V columns * bf16
+            # batch (CFG halves) * rows_global (every frame's tokens of one half) * K|V columns * bf16
+            need = max(a.spec["batch"] * a.spec["seq_kv"] * 2 * a.spec["heads"] * a.spec["dpad"] * 2
+                       for a in launches(cfg, F_total, lat, lat) if a.category == "attn3d")
             assert exchange_bytes(cfg, F_total, lat, lat) == need, (F_total, lat)
 
 
@@ -147,7 +127,7 @@ SHAPES = [
 def _scatter_params():
     out = []
     for s in SHAPES:
-        N = 3 * s[2] * _pad(s[3])
+        N = 3 * s[2] * pad_head_dim(s[3])
         for bn in (0,) + tuple(b for b in WIDTHS if N % b == 0):
             out.append(pytest.param(s, bn, id=f"{s[0]}-bn{bn}"))
     return out
@@ -162,7 +142,7 @@ def _layer(shape):
         _CACHE.clear()
         from diffuman4d_b200 import ops
         _, K, heads, d, hw, F_total, _ = shape
-        dp = _pad(d)
+        dp = pad_head_dim(d)
         Cp = heads * dp
         g = torch.Generator().manual_seed(7)
         a = torch.randn(2 * F_total * hw, K, generator=g).to(torch.bfloat16).cuda()
@@ -202,7 +182,7 @@ def test_kv_scatter(cuda, shape, bn):
     GEMM at every width equal at the automatic one."""
     from diffuman4d_b200 import ops
     _, K, heads, d, hw, F_total, Rs = shape
-    Cp = heads * _pad(d)
+    Cp = heads * pad_head_dim(d)
     N = 3 * Cp
     L = _layer(shape)
     a, w, full, ref64 = L["a"], L["w"], L["full"], L["ref64"]
@@ -246,7 +226,7 @@ def test_attention_over_gathered_kv(cuda, shape):
     attention tolerance."""
     from diffuman4d_b200 import ops
     _, K, heads, d, hw, F_total, Rs = shape
-    dp = _pad(d)
+    dp = pad_head_dim(d)
     Cp = heads * dp
     L = _layer(shape)
     a, w, qkv_full = L["a"], L["w"], L["full"][0]

@@ -35,6 +35,7 @@ import torch
 import torch.nn.functional as F
 
 from diffuman4d_b200.config import UNetConfig
+from diffuman4d_b200.plan import modules
 from diffuman4d_b200.weights import random_state_dict
 from oracle.unet_oracle import (Downsample2D, OracleUNet, ResnetBlock2D, TransformerMultiviewModel, Upsample2D,
                                 timestep_embedding)
@@ -66,39 +67,12 @@ CASES = {
 
 # ------------------------------------------------------------------------------------------------ harness
 def module_plan(cfg, F):
-    """The modules in forward order as (name, input tap names, num_frames), restated from OracleUNet.forward and its
-    blocks.  A ResNet also reads time_embedding; an up-path ResNet reads cat(previous, skip), the skip popped from the
-    down path's outputs (conv_in, then every ResNet/transformer output and every downsampler)."""
-    L, plan, skips = cfg.layers_per_block, [], ["conv_in"]
-    prev = "conv_in"
-
-    def add(name, *inputs, nf=1):
-        nonlocal prev
-        plan.append((name, list(inputs), nf))
-        prev = name
-
-    for i in range(4):
-        nf = F if 3 - i < cfg.num_3d_attn_blocks else 1
-        for j in range(L):
-            add(f"down_blocks.{i}.resnets.{j}", prev)
-            if i < 3:
-                add(f"down_blocks.{i}.attentions.{j}", prev, nf=nf)
-            skips.append(prev)
-        if i < 3:
-            add(f"down_blocks.{i}.downsamplers.0", prev)
-            skips.append(prev)
-    add("mid_block.resnets.0", prev)
-    add("mid_block.attentions.0", prev, nf=F)
-    add("mid_block.resnets.1", prev)
-    for i in range(4):
-        nf = F if i < cfg.num_3d_attn_blocks else 1
-        for j in range(L + 1):
-            add(f"up_blocks.{i}.resnets.{j}", prev, skips.pop())
-            if i > 0:
-                add(f"up_blocks.{i}.attentions.{j}", prev, nf=nf)
-        if i < 3:
-            add(f"up_blocks.{i}.upsamplers.0", prev)
-    assert not skips
+    """The modules of plan.modules in forward order as (name, input tap names, num_frames).  A ResNet also reads
+    time_embedding; an up-path ResNet reads cat(previous, skip)."""
+    plan, prev = [], "conv_in"
+    for m in modules(cfg):
+        plan.append((m.path, [prev] + ([m.skip_from] if m.skip_from else []), F if m.is3d else 1))
+        prev = m.path
     return plan
 
 

@@ -2,10 +2,9 @@
 
     python tools/gemm_shapes.py [--reps 20] [--json OUT]
 
-Every distinct launch shape of the plan (csrc/unet.cu: PlanBuilder::resnet, transformer, self_attention, the down /
-up-sampling convs, conv_in, the pose encoder's GEMM-kernel layers and the time embedding) runs with the epilogue features
-the plan gives it, through the C ABI on pre-allocated buffers, captured `reps` times into a CUDA graph and timed with CUDA
-events after warm-up.  Per shape: launches per forward, the tile rows and width gemm_prepare picks, µs per launch, TFLOP/s
+Every distinct GEMM / conv launch shape of the plan (diffuman4d_b200/plan.py, which mirrors PlanBuilder in csrc/unet.cu)
+runs with the epilogue features the plan gives it, through the C ABI on pre-allocated buffers, captured `reps` times
+into a CUDA graph and timed with CUDA events after warm-up.  Per shape: launches per forward, the tile rows and width gemm_prepare picks, µs per launch, TFLOP/s
 (executed FLOPs: the upsampling convs run 4 taps per phase), compulsory HBM bytes and GB/s, and the least time the card
 could take: the larger of FLOPs / tensor peak and bytes / 3.35 TB/s, naming which bounds the shape.  The tensor peak is
 4096 dense BF16 FLOP/clk/SM at the card's maximum SM clock; a power-limited card runs below it under load.
@@ -24,85 +23,36 @@ sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
 
+from diffuman4d_b200.config import UNetConfig  # noqa: E402
+from diffuman4d_b200.plan import launches  # noqa: E402
+
 HBM_BPS = 3.35e12
-C = (320, 640, 1280, 1280)
-HW = (64, 32, 16, 8)
-B, F = 32, 16
+B = 32
 
 
-def plan_shapes(B=B, s0=HW[0]):
-    """(kind, name, count, spec) for one forward of B images of s0 x s0 latents (default: W16@64², 16 frames with CFG).
+def label(launch):
+    """The short name of a launch: its op, after its level (L1..L4; the mid block's transformer: mid)."""
+    if launch.op in ("time1", "tem1"):
+        return "time1 / tem1"
+    if "_blocks." not in launch.module and not launch.module.startswith("mid_block."):
+        return launch.op
+    tag = "mid" if launch.module.startswith("mid_block.attentions") else f"L{launch.level + 1}"
+    return f"{tag} {launch.op}"
+
+
+def plan_shapes(B=B, s0=64):
+    """(kind, name, count, spec) of every distinct GEMM / conv launch of one forward of B images (B / 2 frames with CFG)
+    of s0 x s0 latents, SD-2.1 layout (default: W16@64²), from plan.launches.
     spec: plain {M, N, K1, K2, feats} / conv {n, H, W, Cin, Cout, mode, feats}."""
-    HW = tuple(s0 >> lvl for lvl in range(4))
     shapes = {}
-
-    def add(kind, name, **spec):
-        key = (kind, tuple(sorted(spec.items())))
-        if key in shapes:
-            shapes[key][2] += 1
-        else:
-            shapes[key] = [kind, name, 1, spec]
-
-    def resnet(lvl, cin, cout, cskip=0):
-        n, s = B, HW[lvl]
-        add("conv", f"L{lvl + 1} conv1", n=n, H=s, W=s, Cin=cin + cskip, Cout=cout, mode="s1", feats=("bias", "rowvec", "stats"))
-        if cin + cskip != cout:
-            add("gemm", f"L{lvl + 1} shortcut", M=n * s * s, N=cout, K1=cin, K2=cskip, feats=("bias", "two_source") if cskip else ("bias",))
-        add("conv", f"L{lvl + 1} conv2", n=n, H=s, W=s, Cin=cout, Cout=cout, mode="s1", feats=("bias", "residual", "stats"))
-
-    def transformer(lvl, name="L"):
-        c, M = C[lvl], B * HW[lvl] ** 2
-        tag = f"{name}{lvl + 1}" if name == "L" else name
-        add("gemm", f"{tag} proj_in", M=M, N=c, K1=c, K2=0, feats=("bias",))
-        add("gemm", f"{tag} qkv", M=M, N=3 * c, K1=c, K2=0, feats=())
-        add("gemm", f"{tag} out-proj", M=M, N=c, K1=c, K2=0, feats=("bias", "residual"))
-        add("gemm", f"{tag} ff1 geglu", M=M, N=8 * c, K1=c, K2=0, feats=("bias", "geglu"))
-        add("gemm", f"{tag} ff2", M=M, N=c, K1=4 * c, K2=0, feats=("bias", "residual"))
-        add("gemm", f"{tag} proj_out", M=M, N=c, K1=c, K2=0, feats=("bias", "residual", "stats"))
-
-    TE = 4 * C[0]
-    ldt = sum([320, 320, 640, 640, 1280, 1280, 1280, 1280] + [1280, 1280] + [1280] * 6 + [640] * 3 + [320] * 3)
-    add("gemm", "time1 / tem1", M=B, N=TE, K1=C[0], K2=0, feats=("bias", "act"))
-    add("gemm", "time1 / tem1", M=B, N=TE, K1=C[0], K2=0, feats=("bias", "act"))
-    add("gemm", "time2", M=B, N=TE, K1=TE, K2=0, feats=("bias",))
-    add("gemm", "tem2", M=B, N=TE, K1=TE, K2=0, feats=("bias", "residual"))
-    add("gemm", "temb_all", M=B, N=ldt, K1=TE, K2=0, feats=("bias",))
-    # pose encoder (the 2F-image batch of bench.py's by_kind forward): layer 5 as a GEMM over im2col, 6 and 7 as convs
-    PB = B
-    add("gemm", "pose l5", M=PB * s0 * s0, N=64, K1=512, K2=0, feats=("bias", "act"))
-    add("conv", "pose l6", n=PB, H=s0, W=s0, Cin=64, Cout=64, mode="s1", feats=("bias", "act"))
-    add("conv", "pose l7", n=PB, H=s0, W=s0, Cin=64, Cout=128, mode="s1", feats=("bias", "act"))
-    add("gemm", "pose proj", M=PB * s0 * s0, N=C[0], K1=128, K2=0, feats=("bias", "scale"))
-    add("gemm", "conv_in", M=B * s0 * s0, N=C[0], K1=192, K2=0, feats=("bias", "residual", "stats"))
-    # down
-    x = C[0]
-    skips = [C[0]]
-    for i in range(4):
-        for _ in range(2):
-            resnet(i, x, C[i])
-            x = C[i]
-            if i < 3:
-                transformer(i)
-            skips.append(x)
-        if i < 3:
-            add("conv", f"L{i + 1} downsample", n=B, H=HW[i], W=HW[i], Cin=x, Cout=x, mode="s2", feats=("bias", "stats"))
-            skips.append(x)
-    # mid
-    resnet(3, x, x)
-    transformer(3, "mid")
-    resnet(3, x, x)
-    # up
-    for i in range(4):
-        lvl = 3 - i
-        for _ in range(3):
-            sk = skips.pop()
-            resnet(lvl, x, C[lvl], sk)
-            x = C[lvl]
-            if i > 0:
-                transformer(lvl)
-        if i < 3:
-            add("conv", f"L{lvl + 1} upsample", n=B, H=HW[lvl], W=HW[lvl], Cin=x, Cout=x, mode="up", feats=("bias", "stats"))
-    add("conv", "conv_out", n=B, H=s0, W=s0, Cin=C[0], Cout=16, mode="s1", feats=("bias",))
+    for launch in launches(UNetConfig.sd21(), B // 2, s0, s0):
+        if launch.kind != "attention":
+            spec = dict(launch.spec, feats=launch.feats)
+            key = (launch.kind, tuple(sorted(spec.items())))
+            if key in shapes:
+                shapes[key][2] += 1
+            else:
+                shapes[key] = [launch.kind, label(launch), 1, spec]
     return list(shapes.values())
 
 
