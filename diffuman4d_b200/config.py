@@ -161,3 +161,18 @@ class UniPCConfig:
 
     def __post_init__(self):
         self.disable_corrector = tuple(int(i) for i in self.disable_corrector)
+
+
+@dataclass
+class PNDMConfig:
+    """PNDM scheduler knobs (upstream diffusers==0.33.1 ``PNDMScheduler`` defaults, except ``skip_prk_steps``) that the
+    fused step implements: skip_prk_steps (the PLMS steps only, as Stable Diffusion ships it), epsilon or v prediction,
+    betas from a linear or scaled-linear schedule."""
+    num_train_timesteps: int = 1000
+    beta_start: float = 0.0001
+    beta_end: float = 0.02
+    beta_schedule: str = "linear"         # or "scaled_linear"
+    prediction_type: str = "epsilon"      # or "v_prediction"
+    set_alpha_to_one: bool = False
+    timestep_spacing: str = "leading"     # or "linspace", "trailing"
+    steps_offset: int = 0

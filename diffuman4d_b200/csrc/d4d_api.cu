@@ -59,7 +59,7 @@ int denoise_window(d4d_handle* h, void* latents, const void* pixel_latents, cons
                    const void* cond_mask, int64_t* timestep_indices, const d4d::WindowStep& step, float guidance_scale,
                    int domain, int F, int F_total, int height, int width, int num_steps, void* stream) {
   D4D_API_BEGIN
-  D4D_REQUIRE(h != nullptr && (step.ddim != nullptr || step.dpm != nullptr || step.unipc != nullptr), "null argument");
+  D4D_REQUIRE(h != nullptr && step.tables() > 0, "null argument");
   DeviceGuard g(h->model->device());
   return h->model->denoise_window(static_cast<bf16*>(latents), static_cast<const bf16*>(pixel_latents),
                                   static_cast<const bf16*>(plucker), static_cast<const bf16*>(skeletons),
@@ -83,6 +83,15 @@ d4d::WindowStep dpm_step(const d4d_dpm_sched* sched, void* x0_prev, int32_t* low
   return s;
 }
 
+// the PNDM state of d4d_denoise_window_pndm / d4d_cfg_pndm_step (the counter arrays are set by the caller)
+d4d::SolverState pndm_state(void* ets0, void* ets1, void* ets2, void* ets3, void* cur_sample) {
+  d4d::SolverState st;
+  void* const ets[4] = {ets0, ets1, ets2, ets3};
+  for (int i = 0; i < 4; ++i) st.ets[i] = static_cast<bf16*>(ets[i]);
+  st.cur_sample = static_cast<bf16*>(cur_sample);
+  return st;
+}
+
 // the step arguments of every d4d_cfg_*_step entry point
 d4d::StepArgs step_args(const void* noise, const void* latents, const void* cond_mask, const int64_t* timestep_indices,
                         int64_t* timestep_indices_out, float guidance_scale, int cfg, int F, int height, int width,
@@ -102,7 +111,7 @@ d4d::StepArgs step_args(const void* noise, const void* latents, const void* cond
 extern "C" {
 
 const char* d4d_last_error(void) { return d4d::g_last_error.c_str(); }
-int d4d_version(void) { return 109; }
+int d4d_version(void) { return 110; }
 
 int d4d_create(const d4d_config* cfg, int device, d4d_handle** out) {
   D4D_API_BEGIN
@@ -233,6 +242,19 @@ int d4d_denoise_window_unipc(d4d_handle* h, void* latents, const void* pixel_lat
                         domain, F, 0, height, width, num_steps, stream);
 }
 
+int d4d_denoise_window_pndm(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                            const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                            const d4d_pndm_sched* sched, float guidance_scale, int domain, int F, int height, int width,
+                            int num_steps, void* ets0, void* ets1, void* ets2, void* ets3, void* cur_sample,
+                            int32_t* counter, void* stream) {
+  d4d::WindowStep s;
+  s.pndm = sched;
+  s.state = pndm_state(ets0, ets1, ets2, ets3, cur_sample);
+  s.state.lower_order_nums = s.state.lower_order_nums_out = counter;
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, s, guidance_scale,
+                        domain, F, 0, height, width, num_steps, stream);
+}
+
 int d4d_assemble_input(void* latents, const void* pixel_latents, const void* plucker, const void* skel_latents,
                        const void* cond_mask, const int64_t* timestep_indices, const int64_t* timesteps_table,
                        int n_steps, int F, int height, int width, int cfg, void* sample_out, int64_t* timestep_out,
@@ -291,6 +313,20 @@ int d4d_cfg_unipc_step(const void* noise, const void* latents, const void* cond_
   st.x0_prev = static_cast<bf16*>(x0_prev); st.x0_prev2 = static_cast<bf16*>(x0_prev2);
   st.last_sample = static_cast<bf16*>(last_sample);
   st.lower_order_nums = lower_order_nums; st.lower_order_nums_out = lower_order_nums_out;
+  return d4d::cfg_step_run(step_args(noise, latents, cond_mask, timestep_indices, timestep_indices_out, guidance_scale, cfg,
+                                     F, height, width, latents_out),
+                           *sched, st, static_cast<cudaStream_t>(stream));
+  D4D_API_END
+}
+
+int d4d_cfg_pndm_step(const void* noise, const void* latents, const void* cond_mask, const int64_t* timestep_indices,
+                      int64_t* timestep_indices_out, void* ets0, void* ets1, void* ets2, void* ets3, void* cur_sample,
+                      const int32_t* counter, int32_t* counter_out, const d4d_pndm_sched* sched, float guidance_scale,
+                      int cfg, int F, int height, int width, void* latents_out, void* stream) {
+  D4D_API_BEGIN
+  D4D_REQUIRE(sched != nullptr, "null argument");
+  d4d::SolverState st = pndm_state(ets0, ets1, ets2, ets3, cur_sample);
+  st.lower_order_nums = counter; st.lower_order_nums_out = counter_out;
   return d4d::cfg_step_run(step_args(noise, latents, cond_mask, timestep_indices, timestep_indices_out, guidance_scale, cfg,
                                      F, height, width, latents_out),
                            *sched, st, static_cast<cudaStream_t>(stream));

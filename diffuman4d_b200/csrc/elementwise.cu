@@ -478,6 +478,61 @@ __global__ void cfg_unipc_kernel(const StepArgs a, const d4d_unipc_sched s, cons
   }
 }
 
+// upstream PNDMScheduler.step_plms (skip_prk_steps) and _get_prev_sample; history ets[4] (a ring of the last model
+// outputs), cur_sample and the frame's counter (lower_order_nums, uncapped).  Upstream does not upcast: in EMU mode every
+// product, sum and quotient rounds to bf16, the Adams-Bashforth sums one operation at a time as upstream writes them.
+constexpr int kPndmNoCap = 0x7fffffff;
+template <bool EMU>
+__global__ void cfg_pndm_kernel(const StepArgs a, const d4d_pndm_sched s, const SolverState st) {
+  long long idx;
+  int counter;
+  if (!step_frame(a, s.n_steps, st.lower_order_nums, st.lower_order_nums_out, kPndmNoCap, idx, counter)) return;
+  const size_t base = static_cast<size_t>(blockIdx.y) * a.chw;
+  const float* k = s.coefs + idx * kPndmCoefs + (counter == 1 ? 5 : 0);   // counter 1 steps from t + T/n to t
+  const float sqrt_a = k[0], sqrt_b = k[1], sample_coef = k[2], alpha_diff = k[3], denom = k[4];
+  // the output of counter c (c != 1) goes to ring slot (c == 0 ? 0 : c - 1) % 4; after it, the last min(c, 4) outputs
+  // are kept (1 at counters 0 and 1: counter 1's output is not kept)
+  const int slot = counter == 0 ? 0 : counter - 1;
+  const int kept = counter < 2 ? 1 : min(counter, 4);
+  bf16* const e1p = st.ets[slot & 3];
+  const bf16* const e2p = st.ets[(slot + 3) & 3];
+  const bf16* const e3p = st.ets[(slot + 2) & 3];
+  const bf16* const e4p = st.ets[(slot + 1) & 3];
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.chw; i += gridDim.x * blockDim.x) {
+    const float m = model_output<EMU>(a, base + i);
+    float x = __bfloat162float(a.latents[base + i]);
+    float eps;
+    if (counter == 0) {
+      eps = m;
+      e1p[base + i] = __float2bfloat16_rn(m);
+      st.cur_sample[base + i] = a.latents[base + i];
+    } else if (counter == 1) {  // (model_output + ets[-1]) / 2, from the sample counter 0 started from
+      eps = rnd<EMU>(rnd<EMU>(m + __bfloat162float(st.ets[0][base + i])) / 2.f);
+      x = __bfloat162float(st.cur_sample[base + i]);
+    } else {
+      e1p[base + i] = __float2bfloat16_rn(m);
+      const float e2 = __bfloat162float(e2p[base + i]);
+      if (kept == 2) {
+        eps = rnd<EMU>(rnd<EMU>(rnd<EMU>(3.f * m) - e2) / 2.f);
+      } else {
+        const float e3 = __bfloat162float(e3p[base + i]);
+        const float s3 = rnd<EMU>(rnd<EMU>(rnd<EMU>(kept == 3 ? 23.f * m : 55.f * m) -
+                                           rnd<EMU>(kept == 3 ? 16.f * e2 : 59.f * e2)) +
+                                  rnd<EMU>(kept == 3 ? 5.f * e3 : 37.f * e3));
+        if (kept == 3) {
+          eps = rnd<EMU>(s3 / 12.f);
+        } else {
+          const float e4 = __bfloat162float(e4p[base + i]);
+          eps = rnd<EMU>(static_cast<float>(1.0 / 24.0) * rnd<EMU>(s3 - rnd<EMU>(9.f * e4)));
+        }
+      }
+    }
+    if (s.prediction_type == 1) eps = rnd<EMU>(rnd<EMU>(sqrt_a * eps) + rnd<EMU>(sqrt_b * x));   // v -> epsilon
+    const float prev = rnd<EMU>(rnd<EMU>(sample_coef * x) - rnd<EMU>(rnd<EMU>(alpha_diff * eps) / denom));
+    a.out[base + i] = __float2bfloat16_rn(prev);
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 // frame-sharded window: K/V arrival flags in peer memory
 // ---------------------------------------------------------------------------------------------
@@ -691,7 +746,7 @@ static int check_step(const StepArgs& a, const int64_t* timesteps_table, const f
   D4D_REQUIRE(prediction_type >= 0 && prediction_type <= 2, "prediction_type");
   D4D_REQUIRE(a.ts_out != a.timestep_indices, "timestep_indices_out must not alias timestep_indices");
   if (st) {
-    D4D_REQUIRE(st->x0_prev && st->lower_order_nums && st->lower_order_nums_out, "null argument");
+    D4D_REQUIRE(st->lower_order_nums && st->lower_order_nums_out, "null argument");
     D4D_REQUIRE(st->lower_order_nums != st->lower_order_nums_out,
                 "the timestep index and order count outputs may not alias their inputs");
   }
@@ -717,6 +772,7 @@ int cfg_step_run(const StepArgs& a, const d4d_sched& s, const SolverState&, cuda
 
 int cfg_step_run(const StepArgs& a, const d4d_dpm_sched& s, const SolverState& st, cudaStream_t stream, bool launch) {
   if (int rc = check_step(a, s.timesteps_table, s.coefs, s.n_steps, s.prediction_type, &st)) return rc;
+  D4D_REQUIRE(st.x0_prev != nullptr, "null argument");
   D4D_REQUIRE(s.solver_order == 1 || s.solver_order == 2, "solver_order must be 1 or 2");
   if (!launch) return 0;
   return launch_step(cfg_dpm_kernel<true>, cfg_dpm_kernel<false>, s.emulate_bf16, stream, a, s, st);
@@ -725,10 +781,18 @@ int cfg_step_run(const StepArgs& a, const d4d_dpm_sched& s, const SolverState& s
 int cfg_step_run(const StepArgs& a, const d4d_unipc_sched& s, const SolverState& st, cudaStream_t stream, bool launch) {
   if (int rc = check_step(a, s.timesteps_table, s.coefs, s.n_steps, s.prediction_type, &st)) return rc;
   D4D_REQUIRE(s.solver_order == 1 || s.solver_order == 2, "solver_order must be 1 or 2");
-  D4D_REQUIRE(st.last_sample != nullptr, "null argument");
+  D4D_REQUIRE(st.x0_prev != nullptr && st.last_sample != nullptr, "null argument");
   D4D_REQUIRE((st.x0_prev2 != nullptr) == (s.solver_order == 2), "x0_prev2 is given exactly when solver_order is 2");
   if (!launch) return 0;
   return launch_step(cfg_unipc_kernel<true>, cfg_unipc_kernel<false>, s.emulate_bf16, stream, a, s, st);
+}
+
+int cfg_step_run(const StepArgs& a, const d4d_pndm_sched& s, const SolverState& st, cudaStream_t stream, bool launch) {
+  if (int rc = check_step(a, s.timesteps_table, s.coefs, s.n_steps, s.prediction_type, &st)) return rc;
+  D4D_REQUIRE(st.ets[0] && st.ets[1] && st.ets[2] && st.ets[3] && st.cur_sample, "null argument");
+  D4D_REQUIRE(s.prediction_type <= 1, "PNDM's prediction_type must be 0 (epsilon) or 1 (v_prediction)");
+  if (!launch) return 0;
+  return launch_step(cfg_pndm_kernel<true>, cfg_pndm_kernel<false>, s.emulate_bf16, stream, a, s, st);
 }
 
 }  // namespace d4d

@@ -1181,9 +1181,7 @@ int Model::profile(const bf16* sample, const long long* timestep, const bf16* sk
 int Model::denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
                           long long* ts_idx, const WindowStep& step, float guidance, int domain, int F, int h, int w,
                           int num_steps, cudaStream_t stream, int F_total) {
-  D4D_REQUIRE(latents && pixel && plucker && mask && ts_idx &&
-                  (step.ddim != nullptr) + (step.dpm != nullptr) + (step.unipc != nullptr) == 1,
-              "null argument");
+  D4D_REQUIRE(latents && pixel && plucker && mask && ts_idx && step.tables() == 1, "null argument");
   D4D_REQUIRE(domain == 0 || domain == 1, "Invalid domain");
   const bool cfg_on = guidance > 1.0f;
   const int B = cfg_on ? 2 * F : F;

@@ -19,7 +19,7 @@ from typing import Callable, List, Optional, Union
 
 import torch
 
-from .config import DPMSolverConfig, SchedulerConfig, UNetConfig, UniPCConfig
+from .config import DPMSolverConfig, PNDMConfig, SchedulerConfig, UNetConfig, UniPCConfig
 from .pipeline import B200Diffuman4DPipeline
 from .unet import B200MultiviewUNet
 
@@ -150,16 +150,45 @@ def unipc_config_from_json(d: dict) -> UniPCConfig:
         steps_offset=d.get("steps_offset", 0))
 
 
-def scheduler_config_from_json(d: dict) -> Union[SchedulerConfig, DPMSolverConfig, UniPCConfig]:
+def pndm_config_from_json(d: dict) -> PNDMConfig:
+    """Map a diffusers ``PNDMScheduler`` config; every knob the fused step does not implement raises
+    ``NotImplementedError`` naming the key."""
+    def refuse(key, why):
+        raise NotImplementedError(f"PNDMScheduler {key}={d.get(key)!r} is not supported by the CUDA path ({why})")
+
+    def want(key, allowed, default):
+        v = d.get(key, default)
+        if v not in allowed:
+            refuse(key, f"supported: {allowed}")
+        return v
+
+    if not d.get("skip_prk_steps", False):
+        refuse("skip_prk_steps", "only the PLMS steps (skip_prk_steps=True) are implemented, not the Runge-Kutta warm-up")
+    if d.get("trained_betas") is not None:
+        refuse("trained_betas", "betas come from beta_schedule")
+    want("beta_schedule", ("linear", "scaled_linear"), "linear")
+    want("prediction_type", ("epsilon", "v_prediction"), "epsilon")
+    want("timestep_spacing", ("linspace", "leading", "trailing"), "leading")
+    return PNDMConfig(
+        num_train_timesteps=d.get("num_train_timesteps", 1000), beta_start=d.get("beta_start", 0.0001),
+        beta_end=d.get("beta_end", 0.02), beta_schedule=d.get("beta_schedule", "linear"),
+        prediction_type=d.get("prediction_type", "epsilon"), set_alpha_to_one=d.get("set_alpha_to_one", False),
+        timestep_spacing=d.get("timestep_spacing", "leading"), steps_offset=d.get("steps_offset", 0))
+
+
+def scheduler_config_from_json(d: dict) -> Union[SchedulerConfig, DPMSolverConfig, UniPCConfig, PNDMConfig]:
     cls = d.get("_class_name", "DDIMScheduler")
     if cls == "DPMSolverMultistepScheduler":
         return dpm_solver_config_from_json(d)
     if cls == "UniPCMultistepScheduler":
         return unipc_config_from_json(d)
+    if cls == "PNDMScheduler":
+        return pndm_config_from_json(d)
     if cls != "DDIMScheduler":
         raise NotImplementedError(
-            f"scheduler {cls} is not fused on the CUDA path (DDIMScheduler, DPMSolverMultistepScheduler and "
-            "UniPCMultistepScheduler only); run the reference's Python scheduler loop for other classes")
+            f"scheduler {cls} is not fused on the CUDA path (DDIMScheduler, DPMSolverMultistepScheduler, "
+            "UniPCMultistepScheduler and PNDMScheduler only); run the reference's Python scheduler loop for other "
+            "classes")
     if d.get("thresholding", False):
         raise NotImplementedError("dynamic thresholding is not supported")
     return SchedulerConfig(

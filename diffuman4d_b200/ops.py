@@ -3,7 +3,7 @@ and the current stream; all arithmetic happens in libd4d.so."""
 from __future__ import annotations
 
 import ctypes as C
-from typing import List, Optional
+from typing import List, Optional, Sequence
 
 import torch
 
@@ -292,7 +292,7 @@ def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: flo
 
 def _multistep_step(entry: str, noise, latents, cond_mask, timestep_indices, planes, lower_order_nums, sched,
                     guidance_scale, cfg):
-    """``cfg_dpm_step`` / ``cfg_unipc_step``: ``planes`` are the (name, bf16 [F,4,h,w] tensor or None) state planes in the
+    """``cfg_dpm_step`` / ``cfg_unipc_step`` / ``cfg_pndm_step``: ``planes`` are the (name, bf16 [F,4,h,w] tensor or None) state planes in the
     order ``entry`` takes them."""
     _bf16c(noise, "noise"), _bf16c(latents, "latents"), _bf16c(cond_mask, "cond_mask")
     F, _, h, w = latents.shape
@@ -332,3 +332,16 @@ def cfg_unipc_step(noise: torch.Tensor, latents: torch.Tensor, cond_mask: torch.
     return _multistep_step("d4d_cfg_unipc_step", noise, latents, cond_mask, timestep_indices,
                            [("x0_prev", x0_prev), ("x0_prev2", x0_prev2), ("last_sample", last_sample)], lower_order_nums,
                            sched, guidance_scale, cfg)
+
+
+def cfg_pndm_step(noise: torch.Tensor, latents: torch.Tensor, cond_mask: torch.Tensor, timestep_indices: torch.Tensor,
+                  ets: Sequence[torch.Tensor], cur_sample: torch.Tensor, counter: torch.Tensor, sched,
+                  guidance_scale: float, cfg: bool):
+    """One CFG + PNDM step of F frames (``sched``: a ``d4d_pndm_sched`` from ``PNDMTables.c_struct``).  ``noise``
+    [(cfg?2:1)*F,4,h,w]; the four ``ets`` planes and ``cur_sample`` [F,4,h,w] bf16 are updated in place.  Returns (new
+    latents, advanced timestep indices, advanced ``counter``)."""
+    if len(ets) != 4:
+        raise ValueError("ets must be the four planes ets0 .. ets3")
+    return _multistep_step("d4d_cfg_pndm_step", noise, latents, cond_mask, timestep_indices,
+                           [*((f"ets{i}", t) for i, t in enumerate(ets)), ("cur_sample", cur_sample)], counter, sched,
+                           guidance_scale, cfg)

@@ -9,7 +9,9 @@ runs on the GPU (csrc/elementwise.cu ``cfg_ddim_kernel``).
 the sigma table and the per-step solver coefficients (``cfg_dpm_kernel``).  That scheduler is stateful, which is why the
 reference deep-copies it per frame; here the state of every frame of a task is a ``DPMSolverState`` on the device.
 ``UniPCTables`` / ``UniPCState`` do the same for ``UniPCMultistepScheduler`` (``cfg_unipc_kernel``), whose corrector also
-needs each frame's previous sample and, at order 2, a second data prediction of history.
+needs each frame's previous sample and, at order 2, a second data prediction of history.  ``PNDMTables`` / ``PNDMState``
+do the same for ``PNDMScheduler`` with ``skip_prk_steps`` (``cfg_pndm_kernel``), whose history is the last four model
+outputs, the sample of the frame's first step and its step counter.
 
 Each tables class names the C entry points of its window step (``window_entry_points``: plain and frame-sharded, None
 where there is none) and the bf16 state planes they take, in ABI order (``state_planes``; None for the stateless DDIM).
@@ -21,8 +23,8 @@ import copy
 import numpy as np
 import torch
 
-from ._lib import D4DDpmSched, D4DSched, D4DUniPCSched
-from .config import DPMSolverConfig, SchedulerConfig, UniPCConfig
+from ._lib import D4DDpmSched, D4DPndmSched, D4DSched, D4DUniPCSched
+from .config import DPMSolverConfig, PNDMConfig, SchedulerConfig, UniPCConfig
 
 _PRED = {"epsilon": 0, "v_prediction": 1, "sample": 2}
 
@@ -376,3 +378,114 @@ class UniPCState(SolverState):
         super().__init__(num_frames, device, tuple(p for p in _unipc_planes(solver_order) if p), lower_order_nums,
                          x0_prev=x0_prev, x0_prev2=x0_prev2, last_sample=last_sample)
         self.solver_order = solver_order
+
+
+# ---- PNDM -------------------------------------------------------------------------------------------------------------
+PNDM_COEFS = 10   # row layout in include/d4d.h ``d4d_pndm_sched``
+
+
+def pndm_timesteps(c: PNDMConfig, n: int) -> np.ndarray:
+    """``PNDMScheduler.set_timesteps(n)`` timesteps with ``skip_prk_steps``: the n spaced timesteps, the second-largest
+    repeated, in descending order (n + 1 entries from n = 2 on; the counter-1 step re-steps to the repeated one)."""
+    T = c.num_train_timesteps
+    if n < 1:
+        raise ValueError(f"num_inference_steps must be positive, got {n}")
+    if c.timestep_spacing == "linspace":
+        ts = np.linspace(0, T - 1, n).round().astype(np.int64)
+    elif c.timestep_spacing == "leading":
+        ts = (np.arange(0, n) * (T // n)).round() + c.steps_offset
+    elif c.timestep_spacing == "trailing":
+        ts = np.round(np.arange(T, 0, -T / n))[::-1].astype(np.int64) - 1
+    else:
+        raise ValueError(f"{c.timestep_spacing} is not supported")
+    return np.concatenate([ts[:-1], ts[-2:-1], ts[-1:]])[::-1].copy().astype(np.int64)
+
+
+def pndm_prev_sample_coefficients(alphas_cumprod: torch.Tensor, final_alpha_cumprod: torch.Tensor, t: int,
+                                  prev: int) -> list:
+    """The five scalars of ``PNDMScheduler._get_prev_sample`` from timestep ``t`` to ``prev``, evaluated on 0-dim tensors
+    in upstream's order: a_t^0.5, (1 - a_t)^0.5, (a_prev / a_t)^0.5, a_prev - a_t and the denominator
+    a_t (1 - a_prev)^0.5 + (a_t (1 - a_t) a_prev)^0.5."""
+    a_t = alphas_cumprod[t]
+    a_prev = alphas_cumprod[prev] if prev >= 0 else final_alpha_cumprod
+    b_t = 1 - a_t
+    b_prev = 1 - a_prev
+    return [a_t ** 0.5, b_t ** 0.5, (a_prev / a_t) ** 0.5, a_prev - a_t,
+            a_t * b_prev ** 0.5 + (a_t * b_t * a_prev) ** 0.5]
+
+
+def pndm_step_coefficients(alphas_cumprod: torch.Tensor, final_alpha_cumprod: torch.Tensor, timesteps, n: int
+                           ) -> torch.Tensor:
+    """[len(timesteps), 10] coefficients of ``cfg_pndm_kernel`` (layout in include/d4d.h ``d4d_pndm_sched``) for
+    ``n`` inference steps: each row's step from t to t - T // n, then the counter-1 step from t + T // n to t (NaN where
+    t + T // n is past the table, where upstream's lookup fails)."""
+    T = alphas_cumprod.numel()
+    ratio = T // n
+    out = torch.full((len(timesteps), PNDM_COEFS), float("nan"), dtype=alphas_cumprod.dtype)
+    for i, t in enumerate(int(v) for v in timesteps):
+        out[i, :5] = torch.stack(pndm_prev_sample_coefficients(alphas_cumprod, final_alpha_cumprod, t, t - ratio))
+        if t + ratio < T:
+            out[i, 5:] = torch.stack(pndm_prev_sample_coefficients(alphas_cumprod, final_alpha_cumprod, t + ratio, t))
+    return out
+
+
+class PNDMTables:
+    """Timesteps and step coefficients of ``PNDMScheduler`` with ``skip_prk_steps`` (diffusers 0.33.1) for
+    ``cfg_pndm_kernel``."""
+    name = "PNDM"
+    init_noise_sigma = 1.0  # upstream: init_noise_sigma 1, scale_model_input is the identity
+    # no frame-sharded window: its window-result exchange carries DPM-Solver++'s state only
+    window_entry_points = ("d4d_denoise_window_pndm", None)
+    state_planes = ("ets0", "ets1", "ets2", "ets3", "cur_sample")
+
+    def __init__(self, cfg: PNDMConfig = None, device="cuda:0"):
+        self.config = c = cfg or PNDMConfig()
+        if c.prediction_type not in ("epsilon", "v_prediction"):
+            raise NotImplementedError(f"prediction_type {c.prediction_type!r}: PNDM steps 'epsilon' or 'v_prediction'")
+        if c.timestep_spacing not in ("linspace", "leading", "trailing"):
+            raise ValueError(f"{c.timestep_spacing} is not supported")
+        self.alphas_cumprod = torch.cumprod(1.0 - _betas(c), dim=0)
+        self.final_alpha_cumprod = torch.tensor(1.0) if c.set_alpha_to_one else self.alphas_cumprod[0]
+        self.device = torch.device(device)
+        self.num_inference_steps = None
+        self.timesteps = None          # host int64 [n + 1] (n = 1: [1])
+        self.coefs = None              # host fp32 [len(timesteps), 10]
+        self._dev = None
+
+    def set_timesteps(self, n: int, device=None):
+        ts = pndm_timesteps(self.config, n)
+        self.num_inference_steps = n
+        self.timesteps = torch.from_numpy(ts)
+        self.coefs = pndm_step_coefficients(self.alphas_cumprod, self.final_alpha_cumprod, ts, n)
+        self._dev = None
+        return self.timesteps
+
+    def c_struct(self, emulate_bf16: bool = False) -> D4DPndmSched:
+        if self.timesteps is None:
+            raise ValueError("call set_timesteps first")
+        if self._dev is None:
+            self._dev = (self.timesteps.to(self.device), self.coefs.to(self.device).contiguous())
+        s = D4DPndmSched()
+        s.timesteps_table = self._dev[0].data_ptr()
+        s.coefs = self._dev[1].data_ptr()
+        s.n_steps = len(self.timesteps)
+        s.prediction_type = _PRED[self.config.prediction_type]
+        s.emulate_bf16 = int(emulate_bf16)
+        return s
+
+    def new_state(self, num_frames: int) -> "PNDMState":
+        return PNDMState(num_frames, self.device)
+
+
+class PNDMState(SolverState):
+    """The PNDM history: ``ets0`` .. ``ets3`` (a ring of each frame's last model outputs: the output of counter c, c != 1,
+    is in ``ets{(0 if c == 0 else c - 1) % 4}``), ``cur_sample`` (the sample each frame's first step started from) and,
+    in ``lower_order_nums``, each frame's step counter (upstream ``counter``, not capped)."""
+
+    def __init__(self, num_frames: int, device, counter: torch.Tensor = None, **planes):
+        super().__init__(num_frames, device, PNDMTables.state_planes, counter,
+                         **{name: planes.get(name) for name in PNDMTables.state_planes})
+
+    @property
+    def counter(self) -> torch.Tensor:
+        return self.lower_order_nums

@@ -109,6 +109,28 @@ typedef struct d4d_unipc_sched {
   int32_t emulate_bf16;             /* 1: round like the reference's bf16 eager maths (history, x0 and every op in bf16) */
 } d4d_unipc_sched;
 
+/* PNDM constants for the fused step (upstream diffusers PNDMScheduler with skip_prk_steps, i.e. the PLMS linear
+ * multistep steps only; d4d_version() 110 and later).  The solver's history is per frame and lives on the device (ets0..3 /
+ * cur_sample / counter of d4d_denoise_window_pndm); a frame's counter is the number of steps it has taken (upstream's
+ * `counter`), and its row of the table is its timestep index.  Counter 0 steps with the model output as it is and saves
+ * the sample; counter 1 re-steps from that saved sample with the mean of the two outputs, from t + T/n to t; counters
+ * 2, 3 and >= 4 use the Adams-Bashforth combinations of the last 2, 3 and 4 outputs (counter 1's output is not kept).
+ * The table has one row per entry of upstream's timesteps (num_inference_steps + 1 of them from 2 steps on).
+ * coefs row i (fp32), computed on the host in the upstream scheduler's fp32 order of operations (the device evaluates no
+ * pow), for t = timesteps[i], prev = t - T/n (T/n = num_train_timesteps // num_inference_steps), a_j = alphas_cumprod[j]
+ * (final_alpha_cumprod for j < 0):
+ *   [0] a_t^0.5  [1] (1 - a_t)^0.5                                          (v_prediction -> epsilon)
+ *   [2] (a_prev / a_t)^0.5  [3] a_prev - a_t  [4] a_t * (1 - a_prev)^0.5 + (a_t * (1 - a_t) * a_prev)^0.5
+ *   [5..9] the same for the counter-1 step, with (prev, t) = (t, t + T/n); NaN where t + T/n >= T, where upstream's
+ *          lookup fails */
+typedef struct d4d_pndm_sched {
+  const int64_t* timesteps_table;   /* device, [n_steps]  (scheduler.timesteps after set_timesteps) */
+  const float* coefs;               /* device, [n_steps][10], see above */
+  int32_t n_steps;                  /* rows of the table */
+  int32_t prediction_type;          /* 0 epsilon, 1 v_prediction */
+  int32_t emulate_bf16;             /* 1: round like the reference's bf16 eager maths (history and every op in bf16) */
+} d4d_pndm_sched;
+
 const char* d4d_last_error(void);
 int d4d_version(void);
 
@@ -179,6 +201,19 @@ int d4d_denoise_window_unipc(d4d_handle* h, void* latents, const void* pixel_lat
                              int num_steps, void* x0_prev, void* x0_prev2, void* last_sample, int32_t* lower_order_nums,
                              void* stream);
 
+/* The same window step with a PNDM scheduler (d4d_version() 110 and later).  Arguments as d4d_denoise_window, plus the
+ * window frames' solver state, read and updated in place (conditioning frames keep theirs; zeros for a new task):
+ *   ets0, ets1, ets2, ets3  device bf16 [F,4,h,w]: each frame's last model outputs, in a ring: the output of counter c
+ *                           (c != 1) is stored in ets((c == 0 ? 0 : c - 1) % 4)
+ *   cur_sample              device bf16 [F,4,h,w]: the sample each frame's counter-0 step started from
+ *   counter                 device int32 [F]: steps each frame has taken
+ * A caller carries them across the windows of one task, gathered and scattered with the frames like the latents. */
+int d4d_denoise_window_pndm(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                            const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                            const d4d_pndm_sched* sched, float guidance_scale, int domain, int F, int height, int width,
+                            int num_steps, void* ets0, void* ets1, void* ets2, void* ets3, void* cur_sample,
+                            int32_t* counter, void* stream);
+
 /* ---- building blocks of B-3, exported for parity tests ------------------------------------------------ */
 int d4d_assemble_input(void* latents, const void* pixel_latents, const void* plucker, const void* skel_latents,
                        const void* cond_mask, const int64_t* timestep_indices, const int64_t* timesteps_table,
@@ -201,6 +236,13 @@ int d4d_cfg_unipc_step(const void* noise, const void* latents, const void* cond_
                        int64_t* timestep_indices_out, void* x0_prev, void* x0_prev2, void* last_sample,
                        const int32_t* lower_order_nums, int32_t* lower_order_nums_out, const d4d_unipc_sched* sched,
                        float guidance_scale, int cfg, int F, int height, int width, void* latents_out, void* stream);
+/* One CFG + PNDM step of the frames (d4d_version() 110 and later; state as d4d_denoise_window_pndm).  ets0..3 and
+ * cur_sample are updated in place; counter_out and timestep_indices_out receive the advanced counters (they may not alias
+ * the inputs); latents_out may alias latents. */
+int d4d_cfg_pndm_step(const void* noise, const void* latents, const void* cond_mask, const int64_t* timestep_indices,
+                      int64_t* timestep_indices_out, void* ets0, void* ets1, void* ets2, void* ets3, void* cur_sample,
+                      const int32_t* counter, int32_t* counter_out, const d4d_pndm_sched* sched, float guidance_scale,
+                      int cfg, int F, int height, int width, void* latents_out, void* stream);
 
 /* ---- op-level entry points (each is one hot-path kernel; used by tests/ and bench.py) ------------------
  * d4d_op_gemm:   out[M,N] = act((A|A2)[M,K1+K2] . W[N,K]^T + bias + rowvec[row/rows_per_image]) * scale + residual

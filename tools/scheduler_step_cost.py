@@ -1,11 +1,12 @@
-"""What the DPM-Solver++ and UniPC steps cost against DDIM in the window step of bench.py's workload (W16 @ 64x64 latents,
-CFG 2.0, SD-2.1 channel layout, random weights), on one GPU in one process.
+"""What the DPM-Solver++, UniPC and PNDM steps cost against DDIM in the window step of bench.py's workload (W16 @ 64x64
+latents, CFG 2.0, SD-2.1 channel layout, random weights), on one GPU in one process.
 
-The three pipelines share one UNet; rounds alternate DDIM, DPM-Solver++ and UniPC so that clock drift hits all alike.  Each
-step restores its inputs (latents, timestep indices and, for the multistep schedulers, the frames' solver state) from
+The four pipelines share one UNet; rounds alternate DDIM, DPM-Solver++, UniPC and PNDM so that clock drift hits all alike.
+Each step restores its inputs (latents, timestep indices and, for the multistep schedulers, the frames' solver state) from
 device copies and then makes ONE public ``denoise_window`` call.  The multistep frames start with a full history, so the
 timed step is the second-order one; the UniPC target frames also sit two steps further into the schedule, so that both
-its corrector and its predictor run at order 2.  Also times the three fused step kernels alone.  Prints one JSON line (and writes it to --out) with the
+its corrector and its predictor run at order 2, and the PNDM frames have taken five steps, so that they combine four
+model outputs.  Also times the four fused step kernels alone.  Prints one JSON line (and writes it to --out) with the
 card's name, power limit and max SM clock beside the numbers.
 
     python tools/scheduler_step_cost.py --rounds 8 --steps 10 --out /tmp/scheduler_step_cost.json
@@ -38,9 +39,9 @@ def main():
     from bench import WORKLOAD, gpu_identity, synth_inputs
     from diffuman4d_b200 import ops
     from diffuman4d_b200._lib import check, lib
-    from diffuman4d_b200.config import DPMSolverConfig, SchedulerConfig, UNetConfig, UniPCConfig
+    from diffuman4d_b200.config import DPMSolverConfig, PNDMConfig, SchedulerConfig, UNetConfig, UniPCConfig
     from diffuman4d_b200.pipeline import B200Diffuman4DPipeline
-    from diffuman4d_b200.scheduler import DPMSolverState, UniPCState
+    from diffuman4d_b200.scheduler import DPMSolverState, PNDMState, UniPCState
     from diffuman4d_b200.unet import B200MultiviewUNet
     from diffuman4d_b200.weights import random_state_dict
 
@@ -53,7 +54,8 @@ def main():
     ddim = B200Diffuman4DPipeline(unet, SchedulerConfig())
     dpm = B200Diffuman4DPipeline(unet, DPMSolverConfig())
     unipc = B200Diffuman4DPipeline(unet, UniPCConfig())
-    for p in (ddim, dpm, unipc):
+    pndm = B200Diffuman4DPipeline(unet, PNDMConfig())
+    for p in (ddim, dpm, unipc, pndm):
         p.parepare_schedulers(wl["n_steps"], F)
 
     inp = {k: (v.to(torch.bfloat16) if v.dtype.is_floating_point else v).to(dev)
@@ -69,12 +71,19 @@ def main():
     x0_init2 = torch.randn(F, 4, h, w, device=dev, generator=g).to(torch.bfloat16)
     last_init = torch.randn(F, 4, h, w, device=dev, generator=g).to(torch.bfloat16)
     state_u = UniPCState(F, dev).take(torch.arange(F), h, w)
+    ets_init = [torch.randn(F, 4, h, w, device=dev, generator=g).to(torch.bfloat16) for _ in range(4)]
+    cnt_init = torch.full((F,), 5, dtype=torch.int32, device=dev)           # four kept outputs: the 4-term sum
+    state_p = PNDMState(F, dev).take(torch.arange(F), h, w)
 
     def window(p, solver_state=None, ts_init=inp["ts"]):
         def step():
             lat.copy_(inp["latents"])
             ts.copy_(ts_init)
-            if isinstance(solver_state, UniPCState):
+            if isinstance(solver_state, PNDMState):
+                for k in range(4):
+                    getattr(solver_state, f"ets{k}").copy_(ets_init[k])
+                solver_state.lower_order_nums.copy_(cnt_init)
+            elif isinstance(solver_state, UniPCState):
                 solver_state.x0_prev2.copy_(x0_init2)
                 solver_state.last_sample.copy_(last_init)
                 solver_state.x0_prev.copy_(x0_init)
@@ -87,14 +96,16 @@ def main():
                              domain=wl["domain"], guidance_scale=wl["guidance"], solver_state=solver_state)
         return step
 
-    # the two fused step kernels alone, on the window's shapes (CFG noise [2F,4,h,w])
+    # the fused step kernels alone, on the window's shapes (CFG noise [2F,4,h,w])
     noise = torch.randn(2 * F, 4, h, w, device=dev, generator=g).to(torch.bfloat16)
     ddim_s, dpm_s, unipc_s = ddim.scheduler.c_struct(), dpm.scheduler.c_struct(), unipc.scheduler.c_struct()
+    pndm_s = pndm.scheduler.c_struct()
     out = torch.empty_like(lat)
     ts_out = torch.empty_like(ts)
     x0_k, lon_k = x0_init.clone(), lon_init.clone()
     x0_u, x02_u, last_u, lon_u = x0_init.clone(), x0_init2.clone(), last_init.clone(), lon2_init.clone()
     ts_u = ts_unipc.clone()
+    ets_p, cur_p, cnt_p = [e.clone() for e in ets_init], x0_init.clone(), cnt_init.clone()
     stream = lambda: torch.cuda.current_stream().cuda_stream
 
     def ddim_kernel():
@@ -108,6 +119,9 @@ def main():
     def unipc_kernel():
         ops.cfg_unipc_step(noise, lat, inp["mask"], ts_u, x0_u, x02_u, last_u, lon_u, unipc_s, wl["guidance"], True)
 
+    def pndm_kernel():
+        ops.cfg_pndm_step(noise, lat, inp["mask"], ts, ets_p, cur_p, cnt_p, pndm_s, wl["guidance"], True)
+
     def timed(fn, n):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
@@ -117,19 +131,21 @@ def main():
         torch.cuda.synchronize()
         return e0.elapsed_time(e1) / n
 
-    arms = {"ddim": window(ddim), "dpm_solver++": window(dpm, state), "unipc": window(unipc, state_u, ts_unipc)}
+    arms = {"ddim": window(ddim), "dpm_solver++": window(dpm, state), "unipc": window(unipc, state_u, ts_unipc),
+            "pndm": window(pndm, state_p)}
     for fn in arms.values():                                             # warm-up: plans, buffers, clocks
         for _ in range(3):
             fn()
     torch.cuda.synchronize()
     per_round = {k: [] for k in arms}
-    kernel = {"ddim": [], "dpm_solver++": [], "unipc": []}
+    kernel = {"ddim": [], "dpm_solver++": [], "unipc": [], "pndm": []}
     for _ in range(args.rounds):
         for k, fn in arms.items():
             per_round[k].append(timed(fn, args.steps))
         kernel["ddim"].append(timed(ddim_kernel, args.kernel_iters))
         kernel["dpm_solver++"].append(timed(dpm_kernel, args.kernel_iters))
         kernel["unipc"].append(timed(unipc_kernel, args.kernel_iters))
+        kernel["pndm"].append(timed(pndm_kernel, args.kernel_iters))
     med = {k: statistics.median(v) for k, v in per_round.items()}
     kmed = {k: statistics.median(v) for k, v in kernel.items()}
     res = {"workload": wl["name"], "gpu": gpu_identity(0), "rounds": args.rounds, "steps_per_round": args.steps,
@@ -138,10 +154,11 @@ def main():
            "dpm_over_ddim": med["dpm_solver++"] / med["ddim"],
            "unipc_minus_ddim_ms": med["unipc"] - med["ddim"],
            "unipc_minus_dpm_ms": med["unipc"] - med["dpm_solver++"],
+           "pndm_minus_ddim_ms": med["pndm"] - med["ddim"],
            "step_kernel_us_median": {k: 1e3 * v for k, v in kmed.items()},
            "note": "DPM-Solver++ and UniPC steps timed in their second-order branches (every frame has a full history, "
-                   "UniPC corrects at order 2); the kernel-only DPM and UniPC times include the op wrappers' output "
-                   "allocations"}
+                   "UniPC corrects at order 2), PNDM in its four-output branch; the kernel-only multistep times include "
+                   "the op wrappers' output allocations"}
     line = json.dumps(res)
     print(line)
     if args.out:
