@@ -176,3 +176,19 @@ class PNDMConfig:
     set_alpha_to_one: bool = False
     timestep_spacing: str = "leading"     # or "linspace", "trailing"
     steps_offset: int = 0
+
+
+@dataclass
+class DEISConfig:
+    """DEIS scheduler knobs (upstream diffusers==0.33.1 ``DEISMultistepScheduler`` defaults) that the fused step
+    implements: algorithm_type "deis", solver_type "logrho", solver_order 1, 2 or 3, no thresholding, sigmas straight from
+    the beta schedule (the last one is sigma_min: upstream has no final_sigmas_type knob for DEIS)."""
+    num_train_timesteps: int = 1000
+    beta_start: float = 0.0001
+    beta_end: float = 0.02
+    beta_schedule: str = "linear"         # or "scaled_linear"
+    solver_order: int = 2                 # 1, 2 or 3
+    prediction_type: str = "epsilon"      # or "v_prediction", "sample"
+    lower_order_final: bool = True
+    timestep_spacing: str = "linspace"    # or "leading", "trailing"
+    steps_offset: int = 0

@@ -111,7 +111,7 @@ d4d::StepArgs step_args(const void* noise, const void* latents, const void* cond
 extern "C" {
 
 const char* d4d_last_error(void) { return d4d::g_last_error.c_str(); }
-int d4d_version(void) { return 110; }
+int d4d_version(void) { return 111; }
 
 int d4d_create(const d4d_config* cfg, int device, d4d_handle** out) {
   D4D_API_BEGIN
@@ -255,6 +255,18 @@ int d4d_denoise_window_pndm(d4d_handle* h, void* latents, const void* pixel_late
                         domain, F, 0, height, width, num_steps, stream);
 }
 
+int d4d_denoise_window_deis(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                            const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                            const d4d_deis_sched* sched, float guidance_scale, int domain, int F, int height, int width,
+                            int num_steps, void* m_prev, void* m_prev2, int32_t* lower_order_nums, void* stream) {
+  d4d::WindowStep s;
+  s.deis = sched;
+  s.state.m_prev = static_cast<bf16*>(m_prev); s.state.m_prev2 = static_cast<bf16*>(m_prev2);
+  s.state.lower_order_nums = s.state.lower_order_nums_out = lower_order_nums;
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, s, guidance_scale,
+                        domain, F, 0, height, width, num_steps, stream);
+}
+
 int d4d_assemble_input(void* latents, const void* pixel_latents, const void* plucker, const void* skel_latents,
                        const void* cond_mask, const int64_t* timestep_indices, const int64_t* timesteps_table,
                        int n_steps, int F, int height, int width, int cfg, void* sample_out, int64_t* timestep_out,
@@ -327,6 +339,21 @@ int d4d_cfg_pndm_step(const void* noise, const void* latents, const void* cond_m
   D4D_REQUIRE(sched != nullptr, "null argument");
   d4d::SolverState st = pndm_state(ets0, ets1, ets2, ets3, cur_sample);
   st.lower_order_nums = counter; st.lower_order_nums_out = counter_out;
+  return d4d::cfg_step_run(step_args(noise, latents, cond_mask, timestep_indices, timestep_indices_out, guidance_scale, cfg,
+                                     F, height, width, latents_out),
+                           *sched, st, static_cast<cudaStream_t>(stream));
+  D4D_API_END
+}
+
+int d4d_cfg_deis_step(const void* noise, const void* latents, const void* cond_mask, const int64_t* timestep_indices,
+                      int64_t* timestep_indices_out, void* m_prev, void* m_prev2, const int32_t* lower_order_nums,
+                      int32_t* lower_order_nums_out, const d4d_deis_sched* sched, float guidance_scale, int cfg, int F,
+                      int height, int width, void* latents_out, void* stream) {
+  D4D_API_BEGIN
+  D4D_REQUIRE(sched != nullptr, "null argument");
+  d4d::SolverState st;
+  st.m_prev = static_cast<bf16*>(m_prev); st.m_prev2 = static_cast<bf16*>(m_prev2);
+  st.lower_order_nums = lower_order_nums; st.lower_order_nums_out = lower_order_nums_out;
   return d4d::cfg_step_run(step_args(noise, latents, cond_mask, timestep_indices, timestep_indices_out, guidance_scale, cfg,
                                      F, height, width, latents_out),
                            *sched, st, static_cast<cudaStream_t>(stream));

@@ -319,7 +319,7 @@ __global__ void fill_bf16_kernel(bf16* __restrict__ p, long long n, float v) {
 
 // ---------------------------------------------------------------------------------------------
 // a-13 + a-14: CFG combine + per-frame scheduler step (pipeline_diffuman4d.py:408-423).  One kernel per scheduler, one CTA
-// row per frame (blockIdx.y); a frame's step index is its timestep index.  The helpers below are the part all three share.
+// row per frame (blockIdx.y); a frame's step index is its timestep index.  The helpers below are the part they all share.
 // ---------------------------------------------------------------------------------------------
 template <bool EMU>
 __device__ __forceinline__ float rnd(float x) { return EMU ? bf16_round(x) : x; }
@@ -529,6 +529,43 @@ __global__ void cfg_pndm_kernel(const StepArgs a, const d4d_pndm_sched s, const 
     }
     if (s.prediction_type == 1) eps = rnd<EMU>(rnd<EMU>(sqrt_a * eps) + rnd<EMU>(sqrt_b * x));   // v -> epsilon
     const float prev = rnd<EMU>(rnd<EMU>(sample_coef * x) - rnd<EMU>(rnd<EMU>(alpha_diff * eps) / denom));
+    a.out[base + i] = __float2bfloat16_rn(prev);
+  }
+}
+
+// upstream DEISMultistepScheduler.step (deis / logrho, order <= 3); history m_prev, m_prev2 (the last model outputs in
+// their epsilon form), lower_order_nums.  Upstream does not upcast the sample: in EMU mode every product, sum and
+// quotient rounds to bf16, the higher-order sums one term at a time as upstream writes them.
+template <bool EMU>
+__global__ void cfg_deis_kernel(const StepArgs a, const d4d_deis_sched s, const SolverState st) {
+  long long idx;
+  int lon;
+  if (!step_frame(a, s.n_steps, st.lower_order_nums, st.lower_order_nums_out, s.solver_order, idx, lon)) return;
+  const size_t base = static_cast<size_t>(blockIdx.y) * a.chw;
+  const float* k = s.coefs + idx * kDeisCoefs;
+  const float alpha_s = k[0], sigma_s = k[1], ratio = k[2], c_first = k[3], alpha_t = k[4];
+  const int order = min(min(s.solver_order, lon + 1), static_cast<int>(k[10]));
+  const float c0 = order == 3 ? k[7] : k[5], c1 = order == 3 ? k[8] : k[6], c2 = k[9];
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.chw; i += gridDim.x * blockDim.x) {
+    const float m = model_output<EMU>(a, base + i);
+    const float x = __bfloat162float(a.latents[base + i]);
+    // convert_model_output: the data prediction, then back to its epsilon form (in the model output's dtype)
+    const float x0 = data_prediction<EMU>(s.prediction_type, x, m, alpha_s, sigma_s);
+    const float m0 = rnd<EMU>(rnd<EMU>(x - rnd<EMU>(alpha_s * x0)) / sigma_s);
+    const bf16 m1b = st.m_prev[base + i];
+    const float m1 = __bfloat162float(m1b);
+    const float m2 = st.m_prev2 ? __bfloat162float(st.m_prev2[base + i]) : 0.f;
+    if (st.m_prev2) st.m_prev2[base + i] = m1b;
+    st.m_prev[base + i] = __float2bfloat16_rn(m0);
+    float prev;
+    if (order == 1) {
+      prev = rnd<EMU>(rnd<EMU>(ratio * x) - rnd<EMU>(c_first * m0));
+    } else {
+      float acc = rnd<EMU>(rnd<EMU>(x / alpha_s) + rnd<EMU>(c0 * m0));
+      acc = rnd<EMU>(acc + rnd<EMU>(c1 * m1));
+      if (order == 3) acc = rnd<EMU>(acc + rnd<EMU>(c2 * m2));
+      prev = rnd<EMU>(alpha_t * acc);
+    }
     a.out[base + i] = __float2bfloat16_rn(prev);
   }
 }
@@ -793,6 +830,15 @@ int cfg_step_run(const StepArgs& a, const d4d_pndm_sched& s, const SolverState& 
   D4D_REQUIRE(s.prediction_type <= 1, "PNDM's prediction_type must be 0 (epsilon) or 1 (v_prediction)");
   if (!launch) return 0;
   return launch_step(cfg_pndm_kernel<true>, cfg_pndm_kernel<false>, s.emulate_bf16, stream, a, s, st);
+}
+
+int cfg_step_run(const StepArgs& a, const d4d_deis_sched& s, const SolverState& st, cudaStream_t stream, bool launch) {
+  if (int rc = check_step(a, s.timesteps_table, s.coefs, s.n_steps, s.prediction_type, &st)) return rc;
+  D4D_REQUIRE(s.solver_order >= 1 && s.solver_order <= 3, "solver_order must be 1, 2 or 3");
+  D4D_REQUIRE(st.m_prev != nullptr, "null argument");
+  D4D_REQUIRE((st.m_prev2 != nullptr) == (s.solver_order == 3), "m_prev2 is given exactly when solver_order is 3");
+  if (!launch) return 0;
+  return launch_step(cfg_deis_kernel<true>, cfg_deis_kernel<false>, s.emulate_bf16, stream, a, s, st);
 }
 
 }  // namespace d4d

@@ -102,19 +102,24 @@ struct WindowBufs {  // scratch of d4d_denoise_window for one (F, h, w, cfg)
 };
 
 // The scheduler of a window step: exactly one of the tables is set.  The multistep schedulers (DPM-Solver++, UniPC,
-// PNDM) also get the window frames' solver state, read and updated in place: the order counts are read from
+// PNDM, DEIS) also get the window frames' solver state, read and updated in place: the order counts are read from
 // state.lower_order_nums and the advanced ones end up in state.lower_order_nums_out, both the caller's array.
 struct WindowStep {
   const d4d_sched* ddim = nullptr;
   const d4d_dpm_sched* dpm = nullptr;
   const d4d_unipc_sched* unipc = nullptr;
   const d4d_pndm_sched* pndm = nullptr;
+  const d4d_deis_sched* deis = nullptr;
   SolverState state;
   // the number of tables set (a valid step has one)
-  int tables() const { return (ddim != nullptr) + (dpm != nullptr) + (unipc != nullptr) + (pndm != nullptr); }
+  int tables() const {
+    return (ddim != nullptr) + (dpm != nullptr) + (unipc != nullptr) + (pndm != nullptr) + (deis != nullptr);
+  }
   // fn(table) with whichever table is set
   template <typename Fn>
-  int with_table(Fn&& fn) const { return ddim ? fn(*ddim) : dpm ? fn(*dpm) : unipc ? fn(*unipc) : fn(*pndm); }
+  int with_table(Fn&& fn) const {
+    return ddim ? fn(*ddim) : dpm ? fn(*dpm) : unipc ? fn(*unipc) : pndm ? fn(*pndm) : fn(*deis);
+  }
 };
 
 struct Exchange {  // K/V exchange buffers in peer memory (cudaIpc), two parities

@@ -19,7 +19,7 @@ from typing import Callable, List, Optional, Union
 
 import torch
 
-from .config import DPMSolverConfig, PNDMConfig, SchedulerConfig, UNetConfig, UniPCConfig
+from .config import DEISConfig, DPMSolverConfig, PNDMConfig, SchedulerConfig, UNetConfig, UniPCConfig
 from .pipeline import B200Diffuman4DPipeline
 from .unet import B200MultiviewUNet
 
@@ -176,7 +176,42 @@ def pndm_config_from_json(d: dict) -> PNDMConfig:
         timestep_spacing=d.get("timestep_spacing", "leading"), steps_offset=d.get("steps_offset", 0))
 
 
-def scheduler_config_from_json(d: dict) -> Union[SchedulerConfig, DPMSolverConfig, UniPCConfig, PNDMConfig]:
+def deis_config_from_json(d: dict) -> DEISConfig:
+    """Map a diffusers ``DEISMultistepScheduler`` config; every knob the fused step does not implement raises
+    ``NotImplementedError`` naming the key."""
+    def refuse(key, why):
+        raise NotImplementedError(f"DEISMultistepScheduler {key}={d.get(key)!r} is not supported by the CUDA path ({why})")
+
+    def want(key, allowed, default):
+        v = d.get(key, default)
+        if v not in allowed:
+            refuse(key, f"supported: {allowed}")
+        return v
+
+    if d.get("thresholding", False):
+        refuse("thresholding", "dynamic thresholding is not implemented")
+    for key in ("use_karras_sigmas", "use_exponential_sigmas", "use_beta_sigmas", "use_flow_sigmas",
+                "use_dynamic_shifting"):
+        if d.get(key, False):
+            refuse(key, "sigmas come straight from the beta schedule")
+    if d.get("rescale_betas_zero_snr", False):
+        refuse("rescale_betas_zero_snr", "zero-SNR rescaling is not implemented")
+    if d.get("trained_betas") is not None:
+        refuse("trained_betas", "betas come from beta_schedule")
+    want("algorithm_type", ("deis",), "deis")
+    want("solver_type", ("logrho",), "logrho")
+    order = want("solver_order", (1, 2, 3), 2)
+    want("beta_schedule", ("linear", "scaled_linear"), "linear")
+    want("prediction_type", ("epsilon", "v_prediction", "sample"), "epsilon")
+    want("timestep_spacing", ("linspace", "leading", "trailing"), "linspace")
+    return DEISConfig(
+        num_train_timesteps=d.get("num_train_timesteps", 1000), beta_start=d.get("beta_start", 0.0001),
+        beta_end=d.get("beta_end", 0.02), beta_schedule=d.get("beta_schedule", "linear"), solver_order=order,
+        prediction_type=d.get("prediction_type", "epsilon"), lower_order_final=d.get("lower_order_final", True),
+        timestep_spacing=d.get("timestep_spacing", "linspace"), steps_offset=d.get("steps_offset", 0))
+
+
+def scheduler_config_from_json(d: dict) -> Union[SchedulerConfig, DPMSolverConfig, UniPCConfig, PNDMConfig, DEISConfig]:
     cls = d.get("_class_name", "DDIMScheduler")
     if cls == "DPMSolverMultistepScheduler":
         return dpm_solver_config_from_json(d)
@@ -184,11 +219,13 @@ def scheduler_config_from_json(d: dict) -> Union[SchedulerConfig, DPMSolverConfi
         return unipc_config_from_json(d)
     if cls == "PNDMScheduler":
         return pndm_config_from_json(d)
+    if cls == "DEISMultistepScheduler":
+        return deis_config_from_json(d)
     if cls != "DDIMScheduler":
         raise NotImplementedError(
             f"scheduler {cls} is not fused on the CUDA path (DDIMScheduler, DPMSolverMultistepScheduler, "
-            "UniPCMultistepScheduler and PNDMScheduler only); run the reference's Python scheduler loop for other "
-            "classes")
+            "UniPCMultistepScheduler, PNDMScheduler and DEISMultistepScheduler only); run the reference's Python "
+            "scheduler loop for other classes")
     if d.get("thresholding", False):
         raise NotImplementedError("dynamic thresholding is not supported")
     return SchedulerConfig(

@@ -1,4 +1,4 @@
-"""Host-side scheduler tables for the fused CFG + scheduler-step kernels: DDIM, DPM-Solver++ and UniPC.
+"""Host-side scheduler tables for the fused CFG + scheduler-step kernels: DDIM, DPM-Solver++, UniPC, PNDM and DEIS.
 
 Mirrors what the reference obtains from ``self.scheduler.set_timesteps(n)`` + per-frame deep copies
 (pipeline_diffuman4d.py:265-271) for upstream diffusers==0.33.1 ``DDIMScheduler``: the ``timesteps`` vector and
@@ -11,7 +11,9 @@ reference deep-copies it per frame; here the state of every frame of a task is a
 ``UniPCTables`` / ``UniPCState`` do the same for ``UniPCMultistepScheduler`` (``cfg_unipc_kernel``), whose corrector also
 needs each frame's previous sample and, at order 2, a second data prediction of history.  ``PNDMTables`` / ``PNDMState``
 do the same for ``PNDMScheduler`` with ``skip_prk_steps`` (``cfg_pndm_kernel``), whose history is the last four model
-outputs, the sample of the frame's first step and its step counter.
+outputs, the sample of the frame's first step and its step counter.  ``DEISTables`` / ``DEISState`` do the same for
+``DEISMultistepScheduler`` (``cfg_deis_kernel``, up to third order), whose history is the last two model outputs in their
+epsilon form.
 
 Each tables class names the C entry points of its window step (``window_entry_points``: plain and frame-sharded, None
 where there is none) and the bf16 state planes they take, in ABI order (``state_planes``; None for the stateless DDIM).
@@ -23,8 +25,8 @@ import copy
 import numpy as np
 import torch
 
-from ._lib import D4DDpmSched, D4DPndmSched, D4DSched, D4DUniPCSched
-from .config import DPMSolverConfig, PNDMConfig, SchedulerConfig, UniPCConfig
+from ._lib import D4DDeisSched, D4DDpmSched, D4DPndmSched, D4DSched, D4DUniPCSched
+from .config import DEISConfig, DPMSolverConfig, PNDMConfig, SchedulerConfig, UniPCConfig
 
 _PRED = {"epsilon": 0, "v_prediction": 1, "sample": 2}
 
@@ -140,19 +142,22 @@ def dpm_step_coefficients(sigmas: torch.Tensor) -> torch.Tensor:
 
 
 class _MultistepTables:
-    """What ``DPMSolverTables`` and ``UniPCTables`` share: the config checks common to both, the sigma table,
-    ``set_timesteps`` and the device copies behind ``c_struct``.  A subclass adds its own checks (``_check``), its
+    """What ``DPMSolverTables``, ``UniPCTables`` and ``DEISTables`` share: the config checks common to all, the sigma
+    table, ``set_timesteps`` and the device copies behind ``c_struct``.  A subclass adds its own checks (``_check``), its
     coefficient rows (``_coefficients``) and its C struct (``_struct``, plus the fields of ``_struct_fields``)."""
     init_noise_sigma = 1.0  # upstream: init_noise_sigma 1, scale_model_input is the identity
+    solver_orders = (1, 2)  # the orders the fused step implements
 
     def __init__(self, cfg, device):
         self.config = c = cfg
         if c.prediction_type not in _PRED:
             raise ValueError(f"prediction_type given as {c.prediction_type} must be one of {list(_PRED)}")
-        if c.solver_order not in (1, 2):
-            raise NotImplementedError(f"solver_order={c.solver_order}: the fused step implements orders 1 and 2")
-        if c.final_sigmas_type not in ("zero", "sigma_min"):
-            raise ValueError(f"final_sigmas_type {c.final_sigmas_type!r} must be 'zero' or 'sigma_min'")
+        if c.solver_order not in self.solver_orders:
+            orders = ", ".join(str(o) for o in self.solver_orders[:-1])
+            raise NotImplementedError(f"solver_order={c.solver_order}: the fused step implements orders {orders} and "
+                                      f"{self.solver_orders[-1]}")
+        if self.final_sigmas_type not in ("zero", "sigma_min"):
+            raise ValueError(f"final_sigmas_type {self.final_sigmas_type!r} must be 'zero' or 'sigma_min'")
         self._check(c)
         self.alphas_cumprod = torch.cumprod(1.0 - _betas(c), dim=0)
         self.all_sigmas = ((1 - self.alphas_cumprod) / self.alphas_cumprod) ** 0.5   # fp32 [T]
@@ -166,13 +171,18 @@ class _MultistepTables:
     def _check(self, c):
         pass
 
+    @property
+    def final_sigmas_type(self) -> str:
+        """The last sigma of the table: 0 ("zero") or that of the first training timestep ("sigma_min")."""
+        return self.config.final_sigmas_type
+
     def _struct_fields(self) -> dict:
         return {}
 
     def set_timesteps(self, n: int, device=None):
         c = self.config
-        ts = dpm_timesteps(c, n)       # UniPC spaces its timesteps like DPM-Solver++
-        last = 0.0 if c.final_sigmas_type == "zero" else float(self.all_sigmas[0])
+        ts = dpm_timesteps(c, n)       # UniPC and DEIS space their timesteps like DPM-Solver++
+        last = 0.0 if self.final_sigmas_type == "zero" else float(self.all_sigmas[0])
         self.num_inference_steps = n
         self.timesteps = torch.from_numpy(ts)
         self.sigmas = torch.cat([self.all_sigmas[self.timesteps], torch.tensor([last], dtype=torch.float32)])
@@ -489,3 +499,117 @@ class PNDMState(SolverState):
     @property
     def counter(self) -> torch.Tensor:
         return self.lower_order_nums
+
+
+# ---- DEIS -------------------------------------------------------------------------------------------------------------
+DEIS_COEFS = 11   # row layout in include/d4d.h ``d4d_deis_sched``
+
+
+def _np_log(v: torch.Tensor) -> torch.Tensor:
+    """``np.log`` of a 0-dim tensor, as upstream's ``ind_fn`` takes it: numpy's log in the tensor's dtype."""
+    return torch.from_numpy(np.asarray(np.log(v.numpy())))
+
+
+def deis_ind_coefficients(rho_t: torch.Tensor, rho_s: list) -> list:
+    """The ``ind_fn`` coefficients of ``multistep_deis_second_order_update`` (``rho_s`` = [rho_s0, rho_s1]) or
+    ``multistep_deis_third_order_update`` (``rho_s`` = [rho_s0, rho_s1, rho_s2]), evaluated like upstream: np.log of
+    each 0-dim rho, every other operation on 0-dim tensors, in upstream's order."""
+    def ind2(t, b, c):
+        lt, lb, lc = _np_log(t), _np_log(b), _np_log(c)
+        return t * (-lc + lt - 1) / (lb - lc)
+
+    def ind3(t, b, c, d):
+        lt, lb, lc, ld = _np_log(t), _np_log(b), _np_log(c), _np_log(d)
+        numerator = t * (lc * (ld - lt + 1) - ld * lt + ld + lt ** 2 - 2 * lt + 2)
+        denominator = (lb - lc) * (lb - ld)
+        return numerator / denominator
+
+    s0 = rho_s[0]
+    if len(rho_s) == 2:
+        s1 = rho_s[1]
+        return [ind2(rho_t, s0, s1) - ind2(s0, s0, s1), ind2(rho_t, s1, s0) - ind2(s0, s1, s0)]
+    s1, s2 = rho_s[1], rho_s[2]
+    return [ind3(rho_t, s0, s1, s2) - ind3(s0, s0, s1, s2), ind3(rho_t, s1, s2, s0) - ind3(s0, s1, s2, s0),
+            ind3(rho_t, s2, s0, s1) - ind3(s0, s2, s0, s1)]
+
+
+def deis_order_cap(c: DEISConfig, i: int, n: int) -> int:
+    """The highest order step i of n may take: ``solver_order``; 1 at the last step and 2 at the one before with
+    ``lower_order_final`` below 15 steps (upstream ``lower_order_final`` / ``lower_order_second``); at most i + 1, as a
+    frame has never taken more steps than its step index."""
+    cap = min(c.solver_order, i + 1)
+    if c.lower_order_final and n < 15:
+        cap = min(cap, 1 if i == n - 1 else 2 if i == n - 2 else cap)
+    return cap
+
+
+def deis_step_coefficients(c: DEISConfig, sigmas: torch.Tensor) -> torch.Tensor:
+    """[n, 11] fp32 coefficients of the n steps over ``sigmas`` [n+1] (layout in include/d4d.h ``d4d_deis_sched``), each
+    evaluated on 0-dim fp32 tensors in the order ``DEISMultistepScheduler``'s ``convert_model_output`` /
+    ``deis_first_order_update`` / ``multistep_deis_second_order_update`` / ``multistep_deis_third_order_update``
+    evaluate them."""
+    def alpha_sigma(j):
+        alpha_t = 1 / ((sigmas[j] ** 2 + 1) ** 0.5)
+        return alpha_t, sigmas[j] * alpha_t
+
+    def lam(j):
+        a, s = alpha_sigma(j)
+        return torch.log(a) - torch.log(s)
+
+    def rho(j):
+        a, s = alpha_sigma(j)
+        return s / a
+
+    n = sigmas.numel() - 1
+    zero = torch.tensor(0.0)
+    out = torch.zeros(n, DEIS_COEFS, dtype=torch.float32)
+    for i in range(n):
+        alpha_s, sigma_s = alpha_sigma(i)
+        alpha_t, sigma_t = alpha_sigma(i + 1)
+        h = lam(i + 1) - lam(i)
+        second = deis_ind_coefficients(rho(i + 1), [rho(i), rho(i - 1)]) if i >= 1 else [zero] * 2
+        third = deis_ind_coefficients(rho(i + 1), [rho(i), rho(i - 1), rho(i - 2)]) if i >= 2 else [zero] * 3
+        out[i] = torch.stack([alpha_s, sigma_s, alpha_t / alpha_s, sigma_t * (torch.exp(h) - 1.0), alpha_t, *second,
+                              *third, torch.tensor(float(deis_order_cap(c, i, n)))])
+    return out
+
+
+def _deis_planes(solver_order: int) -> tuple:
+    """DEIS's bf16 state planes in the order ``d4d_denoise_window_deis`` takes them; ``m_prev2`` exists at order 3 only
+    (None: its argument is NULL)."""
+    return ("m_prev", "m_prev2" if solver_order == 3 else None)
+
+
+class DEISTables(_MultistepTables):
+    """Timesteps, sigmas and step coefficients of ``DEISMultistepScheduler`` (algorithm_type "deis", solver_type
+    "logrho"; diffusers 0.33.1) for ``cfg_deis_kernel``."""
+    name = "DEIS"
+    solver_orders = (1, 2, 3)
+    # no frame-sharded window: its window-result exchange carries DPM-Solver++'s state only
+    window_entry_points = ("d4d_denoise_window_deis", None)
+    final_sigmas_type = "sigma_min"   # upstream's table always ends on the sigma of the first training timestep
+    _struct = D4DDeisSched
+
+    def __init__(self, cfg: DEISConfig = None, device="cuda:0"):
+        super().__init__(cfg or DEISConfig(), device)
+
+    def _coefficients(self, sigmas: torch.Tensor) -> torch.Tensor:
+        return deis_step_coefficients(self.config, sigmas)
+
+    @property
+    def state_planes(self) -> tuple:
+        return _deis_planes(self.config.solver_order)
+
+    def new_state(self, num_frames: int) -> "DEISState":
+        return DEISState(num_frames, self.device, self.config.solver_order)
+
+
+class DEISState(SolverState):
+    """The DEIS history: ``m_prev`` (each frame's previous model output, converted to its epsilon form), ``m_prev2`` (the
+    one before; order 3 only, else None) and ``lower_order_nums``."""
+
+    def __init__(self, num_frames: int, device, solver_order: int = 2, m_prev: torch.Tensor = None,
+                 m_prev2: torch.Tensor = None, lower_order_nums: torch.Tensor = None):
+        super().__init__(num_frames, device, tuple(p for p in _deis_planes(solver_order) if p), lower_order_nums,
+                         m_prev=m_prev, m_prev2=m_prev2)
+        self.solver_order = solver_order

@@ -131,6 +131,32 @@ typedef struct d4d_pndm_sched {
   int32_t emulate_bf16;             /* 1: round like the reference's bf16 eager maths (history and every op in bf16) */
 } d4d_pndm_sched;
 
+/* DEIS constants for the fused step (upstream diffusers DEISMultistepScheduler with algorithm_type "deis", solver_type
+ * "logrho", solver_order 1, 2 or 3; d4d_version() 111 and later).  The solver's history is per frame and lives on the
+ * device (m_prev / m_prev2 / lower_order_nums of d4d_denoise_window_deis); a frame's step index is its timestep index.
+ * The history holds model outputs converted to their epsilon form, m = (x - alpha_i * x0) / sigma'_i with x0 the data
+ * prediction.  Step i runs at order min(solver_order, lower_order_nums + 1, row i's cap).  Every sigma is nonzero: the
+ * table ends on the sigma of the first training timestep.
+ * coefs row i (fp32), computed on the host in the upstream scheduler's fp32 order of operations (the device evaluates no
+ * log / exp), with alpha_j = 1 / sqrt(sigma_j^2 + 1), sigma'_j = sigma_j * alpha_j, lambda_j = log alpha_j - log sigma'_j,
+ * rho_j = sigma'_j / alpha_j, and upstream's ind_fn integrals of the Lagrange basis in log rho (np.log in fp32):
+ *   [0] alpha_i   [1] sigma'_i                                               (convert_model_output)
+ *   [2] alpha_(i+1) / alpha_i   [3] sigma'_(i+1) * (exp(lambda_(i+1) - lambda_i) - 1)
+ *                                                     (first order: x' = [2] * x - [3] * m0)
+ *   [4] alpha_(i+1)                                   (higher orders: x' = [4] * (x / alpha_i + sum_k c_k * m_k))
+ *   [5] c_0  [6] c_1 of the second-order update from rho_i, rho_(i-1) to rho_(i+1)         (0 in row 0)
+ *   [7] c_0  [8] c_1  [9] c_2 of the third-order update from rho_i, rho_(i-1), rho_(i-2)    (0 in rows 0, 1)
+ *   [10] the order cap: min(solver_order, i + 1), and with lower_order_final below 15 steps 1 in the last row and 2 in
+ *        the row before it */
+typedef struct d4d_deis_sched {
+  const int64_t* timesteps_table;   /* device, [n_steps]  (scheduler.timesteps after set_timesteps) */
+  const float* coefs;               /* device, [n_steps][11], see above */
+  int32_t n_steps;
+  int32_t prediction_type;          /* 0 epsilon, 1 v_prediction, 2 sample */
+  int32_t solver_order;             /* 1, 2 or 3 */
+  int32_t emulate_bf16;             /* 1: round like the reference's bf16 eager maths (history and every op in bf16) */
+} d4d_deis_sched;
+
 const char* d4d_last_error(void);
 int d4d_version(void);
 
@@ -214,6 +240,17 @@ int d4d_denoise_window_pndm(d4d_handle* h, void* latents, const void* pixel_late
                             int num_steps, void* ets0, void* ets1, void* ets2, void* ets3, void* cur_sample,
                             int32_t* counter, void* stream);
 
+/* The same window step with a DEIS scheduler (d4d_version() 111 and later).  Arguments as d4d_denoise_window, plus the
+ * window frames' solver state, read and updated in place (conditioning frames keep theirs; zeros for a new task):
+ *   m_prev            device bf16 [F,4,h,w]: each frame's previous model output in its epsilon form
+ *   m_prev2           device bf16 [F,4,h,w]: the one before (solver_order 3; NULL exactly when solver_order is 1 or 2)
+ *   lower_order_nums  device int32 [F]: steps each frame has taken, capped at solver_order
+ * A caller carries them across the windows of one task, gathered and scattered with the frames like the latents. */
+int d4d_denoise_window_deis(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                            const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                            const d4d_deis_sched* sched, float guidance_scale, int domain, int F, int height, int width,
+                            int num_steps, void* m_prev, void* m_prev2, int32_t* lower_order_nums, void* stream);
+
 /* ---- building blocks of B-3, exported for parity tests ------------------------------------------------ */
 int d4d_assemble_input(void* latents, const void* pixel_latents, const void* plucker, const void* skel_latents,
                        const void* cond_mask, const int64_t* timestep_indices, const int64_t* timesteps_table,
@@ -243,6 +280,13 @@ int d4d_cfg_pndm_step(const void* noise, const void* latents, const void* cond_m
                       int64_t* timestep_indices_out, void* ets0, void* ets1, void* ets2, void* ets3, void* cur_sample,
                       const int32_t* counter, int32_t* counter_out, const d4d_pndm_sched* sched, float guidance_scale,
                       int cfg, int F, int height, int width, void* latents_out, void* stream);
+/* One CFG + DEIS step of the frames (d4d_version() 111 and later; state as d4d_denoise_window_deis).  m_prev and m_prev2
+ * are updated in place; lower_order_nums_out and timestep_indices_out receive the advanced counters (they may not alias
+ * the inputs); latents_out may alias latents. */
+int d4d_cfg_deis_step(const void* noise, const void* latents, const void* cond_mask, const int64_t* timestep_indices,
+                      int64_t* timestep_indices_out, void* m_prev, void* m_prev2, const int32_t* lower_order_nums,
+                      int32_t* lower_order_nums_out, const d4d_deis_sched* sched, float guidance_scale, int cfg, int F,
+                      int height, int width, void* latents_out, void* stream);
 
 /* ---- op-level entry points (each is one hot-path kernel; used by tests/ and bench.py) ------------------
  * d4d_op_gemm:   out[M,N] = act((A|A2)[M,K1+K2] . W[N,K]^T + bias + rowvec[row/rows_per_image]) * scale + residual

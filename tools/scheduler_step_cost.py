@@ -1,12 +1,14 @@
-"""What the DPM-Solver++, UniPC and PNDM steps cost against DDIM in the window step of bench.py's workload (W16 @ 64x64
-latents, CFG 2.0, SD-2.1 channel layout, random weights), on one GPU in one process.
+"""What the DPM-Solver++, UniPC, PNDM and DEIS steps cost against DDIM in the window step of bench.py's workload (W16 @
+64x64 latents, CFG 2.0, SD-2.1 channel layout, random weights), on one GPU in one process.
 
-The four pipelines share one UNet; rounds alternate DDIM, DPM-Solver++, UniPC and PNDM so that clock drift hits all alike.
+The five pipelines share one UNet; rounds alternate DDIM, DPM-Solver++, UniPC, PNDM and DEIS so that clock drift hits all
+alike.
 Each step restores its inputs (latents, timestep indices and, for the multistep schedulers, the frames' solver state) from
 device copies and then makes ONE public ``denoise_window`` call.  The multistep frames start with a full history, so the
 timed step is the second-order one; the UniPC target frames also sit two steps further into the schedule, so that both
-its corrector and its predictor run at order 2, and the PNDM frames have taken five steps, so that they combine four
-model outputs.  Also times the four fused step kernels alone.  Prints one JSON line (and writes it to --out) with the
+its corrector and its predictor run at order 2, the PNDM frames have taken five steps, so that they combine four
+model outputs, and the DEIS (solver_order 3) frames sit at the UniPC rows with a full history, so that every one takes
+the third-order step.  Also times the five fused step kernels alone.  Prints one JSON line (and writes it to --out) with the
 card's name, power limit and max SM clock beside the numbers.
 
     python tools/scheduler_step_cost.py --rounds 8 --steps 10 --out /tmp/scheduler_step_cost.json
@@ -39,9 +41,9 @@ def main():
     from bench import WORKLOAD, gpu_identity, synth_inputs
     from diffuman4d_b200 import ops
     from diffuman4d_b200._lib import check, lib
-    from diffuman4d_b200.config import DPMSolverConfig, PNDMConfig, SchedulerConfig, UNetConfig, UniPCConfig
+    from diffuman4d_b200.config import DEISConfig, DPMSolverConfig, PNDMConfig, SchedulerConfig, UNetConfig, UniPCConfig
     from diffuman4d_b200.pipeline import B200Diffuman4DPipeline
-    from diffuman4d_b200.scheduler import DPMSolverState, PNDMState, UniPCState
+    from diffuman4d_b200.scheduler import DEISState, DPMSolverState, PNDMState, UniPCState
     from diffuman4d_b200.unet import B200MultiviewUNet
     from diffuman4d_b200.weights import random_state_dict
 
@@ -55,7 +57,8 @@ def main():
     dpm = B200Diffuman4DPipeline(unet, DPMSolverConfig())
     unipc = B200Diffuman4DPipeline(unet, UniPCConfig())
     pndm = B200Diffuman4DPipeline(unet, PNDMConfig())
-    for p in (ddim, dpm, unipc, pndm):
+    deis = B200Diffuman4DPipeline(unet, DEISConfig(solver_order=3))
+    for p in (ddim, dpm, unipc, pndm, deis):
         p.parepare_schedulers(wl["n_steps"], F)
 
     inp = {k: (v.to(torch.bfloat16) if v.dtype.is_floating_point else v).to(dev)
@@ -74,12 +77,18 @@ def main():
     ets_init = [torch.randn(F, 4, h, w, device=dev, generator=g).to(torch.bfloat16) for _ in range(4)]
     cnt_init = torch.full((F,), 5, dtype=torch.int32, device=dev)           # four kept outputs: the 4-term sum
     state_p = PNDMState(F, dev).take(torch.arange(F), h, w)
+    lon3_init = torch.full((F,), 3, dtype=torch.int32, device=dev)         # two outputs of history: third order
+    state_d = DEISState(F, dev, solver_order=3).take(torch.arange(F), h, w)
 
     def window(p, solver_state=None, ts_init=inp["ts"]):
         def step():
             lat.copy_(inp["latents"])
             ts.copy_(ts_init)
-            if isinstance(solver_state, PNDMState):
+            if isinstance(solver_state, DEISState):
+                solver_state.m_prev.copy_(x0_init)
+                solver_state.m_prev2.copy_(x0_init2)
+                solver_state.lower_order_nums.copy_(lon3_init)
+            elif isinstance(solver_state, PNDMState):
                 for k in range(4):
                     getattr(solver_state, f"ets{k}").copy_(ets_init[k])
                 solver_state.lower_order_nums.copy_(cnt_init)
@@ -99,13 +108,14 @@ def main():
     # the fused step kernels alone, on the window's shapes (CFG noise [2F,4,h,w])
     noise = torch.randn(2 * F, 4, h, w, device=dev, generator=g).to(torch.bfloat16)
     ddim_s, dpm_s, unipc_s = ddim.scheduler.c_struct(), dpm.scheduler.c_struct(), unipc.scheduler.c_struct()
-    pndm_s = pndm.scheduler.c_struct()
+    pndm_s, deis_s = pndm.scheduler.c_struct(), deis.scheduler.c_struct()
     out = torch.empty_like(lat)
     ts_out = torch.empty_like(ts)
     x0_k, lon_k = x0_init.clone(), lon_init.clone()
     x0_u, x02_u, last_u, lon_u = x0_init.clone(), x0_init2.clone(), last_init.clone(), lon2_init.clone()
     ts_u = ts_unipc.clone()
     ets_p, cur_p, cnt_p = [e.clone() for e in ets_init], x0_init.clone(), cnt_init.clone()
+    m_d, m2_d, lon_d = x0_init.clone(), x0_init2.clone(), lon3_init.clone()
     stream = lambda: torch.cuda.current_stream().cuda_stream
 
     def ddim_kernel():
@@ -122,6 +132,9 @@ def main():
     def pndm_kernel():
         ops.cfg_pndm_step(noise, lat, inp["mask"], ts, ets_p, cur_p, cnt_p, pndm_s, wl["guidance"], True)
 
+    def deis_kernel():
+        ops.cfg_deis_step(noise, lat, inp["mask"], ts_u, m_d, m2_d, lon_d, deis_s, wl["guidance"], True)
+
     def timed(fn, n):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
@@ -132,13 +145,13 @@ def main():
         return e0.elapsed_time(e1) / n
 
     arms = {"ddim": window(ddim), "dpm_solver++": window(dpm, state), "unipc": window(unipc, state_u, ts_unipc),
-            "pndm": window(pndm, state_p)}
+            "pndm": window(pndm, state_p), "deis": window(deis, state_d, ts_unipc)}
     for fn in arms.values():                                             # warm-up: plans, buffers, clocks
         for _ in range(3):
             fn()
     torch.cuda.synchronize()
     per_round = {k: [] for k in arms}
-    kernel = {"ddim": [], "dpm_solver++": [], "unipc": [], "pndm": []}
+    kernel = {"ddim": [], "dpm_solver++": [], "unipc": [], "pndm": [], "deis": []}
     for _ in range(args.rounds):
         for k, fn in arms.items():
             per_round[k].append(timed(fn, args.steps))
@@ -146,6 +159,7 @@ def main():
         kernel["dpm_solver++"].append(timed(dpm_kernel, args.kernel_iters))
         kernel["unipc"].append(timed(unipc_kernel, args.kernel_iters))
         kernel["pndm"].append(timed(pndm_kernel, args.kernel_iters))
+        kernel["deis"].append(timed(deis_kernel, args.kernel_iters))
     med = {k: statistics.median(v) for k, v in per_round.items()}
     kmed = {k: statistics.median(v) for k, v in kernel.items()}
     res = {"workload": wl["name"], "gpu": gpu_identity(0), "rounds": args.rounds, "steps_per_round": args.steps,
@@ -155,10 +169,11 @@ def main():
            "unipc_minus_ddim_ms": med["unipc"] - med["ddim"],
            "unipc_minus_dpm_ms": med["unipc"] - med["dpm_solver++"],
            "pndm_minus_ddim_ms": med["pndm"] - med["ddim"],
+           "deis_minus_ddim_ms": med["deis"] - med["ddim"],
            "step_kernel_us_median": {k: 1e3 * v for k, v in kmed.items()},
            "note": "DPM-Solver++ and UniPC steps timed in their second-order branches (every frame has a full history, "
-                   "UniPC corrects at order 2), PNDM in its four-output branch; the kernel-only multistep times include "
-                   "the op wrappers' output allocations"}
+                   "UniPC corrects at order 2), PNDM in its four-output branch, DEIS in its third-order branch; the "
+                   "kernel-only multistep times include the op wrappers' output allocations"}
     line = json.dumps(res)
     print(line)
     if args.out:
