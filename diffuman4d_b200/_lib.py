@@ -19,6 +19,7 @@ EXPORTS = [
     "d4d_window_exchange", "d4d_op_window_scatter", "d4d_denoise_window_unipc", "d4d_cfg_unipc_step",
     "d4d_op_conv_tiled", "d4d_conv_tile_choice", "d4d_op_gemm_tiled", "d4d_gemm_tile_choice",
     "d4d_denoise_window_pndm", "d4d_cfg_pndm_step", "d4d_denoise_window_deis", "d4d_cfg_deis_step",
+    "d4d_denoise_window_dpm_single", "d4d_cfg_dpm_single_step",
 ]
 
 
@@ -62,6 +63,13 @@ class D4DPndmSched(C.Structure):
 
 
 class D4DDeisSched(C.Structure):
+    _fields_ = [
+        ("timesteps_table", C.c_void_p), ("coefs", C.c_void_p), ("n_steps", C.c_int32), ("prediction_type", C.c_int32),
+        ("solver_order", C.c_int32), ("emulate_bf16", C.c_int32),
+    ]
+
+
+class D4DDpmSingleSched(C.Structure):
     _fields_ = [
         ("timesteps_table", C.c_void_p), ("coefs", C.c_void_p), ("n_steps", C.c_int32), ("prediction_type", C.c_int32),
         ("solver_order", C.c_int32), ("emulate_bf16", C.c_int32),
@@ -115,6 +123,8 @@ def _load(path: str) -> C.CDLL:
                                           i32, vp, vp, vp, vp, vp, vp, vp]
     l.d4d_denoise_window_deis.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.POINTER(D4DDeisSched), f32, i32, i32, i32, i32,
                                           i32, vp, vp, vp, vp]
+    l.d4d_denoise_window_dpm_single.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.POINTER(D4DDpmSingleSched), f32, i32, i32,
+                                                i32, i32, i32, vp, vp, vp, vp, vp]
     l.d4d_assemble_input.argtypes = [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]
     l.d4d_cfg_ddim_step.argtypes = [vp, vp, vp, vp, vp, C.POINTER(D4DSched), f32, i32, i32, i32, i32, vp, vp]
     l.d4d_cfg_dpm_step.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, C.POINTER(D4DDpmSched), f32, i32, i32, i32, i32, vp, vp]
@@ -124,6 +134,8 @@ def _load(path: str) -> C.CDLL:
                                     i32, i32, i32, vp, vp]
     l.d4d_cfg_deis_step.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, C.POINTER(D4DDeisSched), f32, i32, i32, i32, i32,
                                     vp, vp]
+    l.d4d_cfg_dpm_single_step.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.POINTER(D4DDpmSingleSched), f32, i32,
+                                          i32, i32, i32, vp, vp]
     l.d4d_op_gemm.argtypes = [vp, i32, i32, vp, i32, i32, vp, i32, i32, f32p, vp, i32, i32, vp, i32, vp, i32, i32,
                               i32, f32, i32, vp, i32, vp]
     l.d4d_op_gemm_tiled.argtypes = [vp, i32, i32, vp, i32, i32, vp, i32, i32, f32p, vp, i32, i32, vp, i32, vp, i32, i32,
@@ -160,7 +172,8 @@ def _load(path: str) -> C.CDLL:
                 "d4d_denoise_window_dpm", "d4d_exchange_alloc", "d4d_exchange_open", "d4d_unet_forward_sharded",
                 "d4d_denoise_window_sharded", "d4d_denoise_window_dpm_sharded", "d4d_window_exchange", "d4d_debug_tap",
                 "d4d_denoise_window_unipc", "d4d_conv_tile_choice", "d4d_gemm_tile_choice", "d4d_denoise_window_pndm",
-                "d4d_cfg_pndm_step", "d4d_denoise_window_deis", "d4d_cfg_deis_step"):
+                "d4d_cfg_pndm_step", "d4d_denoise_window_deis", "d4d_cfg_deis_step", "d4d_denoise_window_dpm_single",
+                "d4d_cfg_dpm_single_step"):
             fn.restype = C.c_int
     return l
 

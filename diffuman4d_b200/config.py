@@ -192,3 +192,21 @@ class DEISConfig:
     lower_order_final: bool = True
     timestep_spacing: str = "linspace"    # or "leading", "trailing"
     steps_offset: int = 0
+
+
+@dataclass
+class DPMSingleConfig:
+    """DPM-Solver++ singlestep scheduler knobs (upstream diffusers==0.33.1 ``DPMSolverSinglestepScheduler`` defaults) that
+    the fused step implements: algorithm_type "dpmsolver++", solver_type "midpoint", solver_order 1, 2 or 3, no
+    thresholding, sigmas straight from the beta schedule.  Upstream spaces the timesteps one way only (linspace over n + 1
+    points, without the last), and its ``set_timesteps`` switches ``lower_order_final`` on when n is not a multiple of
+    ``solver_order`` or the final sigma is zero."""
+    num_train_timesteps: int = 1000
+    beta_start: float = 0.0001
+    beta_end: float = 0.02
+    beta_schedule: str = "linear"         # or "scaled_linear"
+    solver_order: int = 2                 # 1, 2 or 3
+    prediction_type: str = "epsilon"      # or "v_prediction", "sample"
+    lower_order_final: bool = False
+    final_sigmas_type: str = "zero"       # or "sigma_min"
+    timestep_spacing: str = "linspace"    # the only spacing upstream has

@@ -111,7 +111,7 @@ d4d::StepArgs step_args(const void* noise, const void* latents, const void* cond
 extern "C" {
 
 const char* d4d_last_error(void) { return d4d::g_last_error.c_str(); }
-int d4d_version(void) { return 111; }
+int d4d_version(void) { return 112; }
 
 int d4d_create(const d4d_config* cfg, int device, d4d_handle** out) {
   D4D_API_BEGIN
@@ -267,6 +267,20 @@ int d4d_denoise_window_deis(d4d_handle* h, void* latents, const void* pixel_late
                         domain, F, 0, height, width, num_steps, stream);
 }
 
+int d4d_denoise_window_dpm_single(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                  const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                  const d4d_dpm_single_sched* sched, float guidance_scale, int domain, int F, int height,
+                                  int width, int num_steps, void* x0_prev, void* x0_prev2, void* cur_sample,
+                                  int32_t* lower_order_nums, void* stream) {
+  d4d::WindowStep s;
+  s.dpm_single = sched;
+  s.state.x0_prev = static_cast<bf16*>(x0_prev); s.state.x0_prev2 = static_cast<bf16*>(x0_prev2);
+  s.state.cur_sample = static_cast<bf16*>(cur_sample);
+  s.state.lower_order_nums = s.state.lower_order_nums_out = lower_order_nums;
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, s, guidance_scale,
+                        domain, F, 0, height, width, num_steps, stream);
+}
+
 int d4d_assemble_input(void* latents, const void* pixel_latents, const void* plucker, const void* skel_latents,
                        const void* cond_mask, const int64_t* timestep_indices, const int64_t* timesteps_table,
                        int n_steps, int F, int height, int width, int cfg, void* sample_out, int64_t* timestep_out,
@@ -353,6 +367,23 @@ int d4d_cfg_deis_step(const void* noise, const void* latents, const void* cond_m
   D4D_REQUIRE(sched != nullptr, "null argument");
   d4d::SolverState st;
   st.m_prev = static_cast<bf16*>(m_prev); st.m_prev2 = static_cast<bf16*>(m_prev2);
+  st.lower_order_nums = lower_order_nums; st.lower_order_nums_out = lower_order_nums_out;
+  return d4d::cfg_step_run(step_args(noise, latents, cond_mask, timestep_indices, timestep_indices_out, guidance_scale, cfg,
+                                     F, height, width, latents_out),
+                           *sched, st, static_cast<cudaStream_t>(stream));
+  D4D_API_END
+}
+
+int d4d_cfg_dpm_single_step(const void* noise, const void* latents, const void* cond_mask,
+                            const int64_t* timestep_indices, int64_t* timestep_indices_out, void* x0_prev,
+                            void* x0_prev2, void* cur_sample, const int32_t* lower_order_nums,
+                            int32_t* lower_order_nums_out, const d4d_dpm_single_sched* sched, float guidance_scale,
+                            int cfg, int F, int height, int width, void* latents_out, void* stream) {
+  D4D_API_BEGIN
+  D4D_REQUIRE(sched != nullptr, "null argument");
+  d4d::SolverState st;
+  st.x0_prev = static_cast<bf16*>(x0_prev); st.x0_prev2 = static_cast<bf16*>(x0_prev2);
+  st.cur_sample = static_cast<bf16*>(cur_sample);
   st.lower_order_nums = lower_order_nums; st.lower_order_nums_out = lower_order_nums_out;
   return d4d::cfg_step_run(step_args(noise, latents, cond_mask, timestep_indices, timestep_indices_out, guidance_scale, cfg,
                                      F, height, width, latents_out),

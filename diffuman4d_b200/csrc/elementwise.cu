@@ -570,6 +570,48 @@ __global__ void cfg_deis_kernel(const StepArgs a, const d4d_deis_sched s, const 
   }
 }
 
+// upstream DPMSolverSinglestepScheduler.step (dpmsolver++ / midpoint, order <= 3); history x0_prev, x0_prev2 (the last
+// data predictions), cur_sample (the sample the frame's current block started from), lower_order_nums.  A step at order
+// 1 starts a block and saves its sample; a step at order 2 or 3 updates from that sample with the block start's data
+// prediction (x0_prev at order 2, x0_prev2 at order 3).  Upstream does not upcast the sample: in EMU mode every product
+// and difference rounds to bf16, the sums one term at a time as upstream writes them.
+template <bool EMU>
+__global__ void cfg_dpm_single_kernel(const StepArgs a, const d4d_dpm_single_sched s, const SolverState st) {
+  long long idx;
+  int lon;
+  if (!step_frame(a, s.n_steps, st.lower_order_nums, st.lower_order_nums_out, s.solver_order, idx, lon)) return;
+  const size_t base = static_cast<size_t>(blockIdx.y) * a.chw;
+  const float* k = s.coefs + idx * kDpmSingleCoefs;
+  const float alpha_s = k[0], sigma_s = k[1];
+  // upstream lowers the row's order while the history it needs is missing
+  const int order = min(static_cast<int>(k[12]), lon + 1);
+  const float* u = k + (order == 1 ? 2 : order == 2 ? 4 : 8);
+  const float ratio = u[0], c = u[1], c_d1 = u[2], inv_r0 = u[3];
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.chw; i += gridDim.x * blockDim.x) {
+    const float m = model_output<EMU>(a, base + i);
+    const bf16 xb = a.latents[base + i];
+    const float x = __bfloat162float(xb);
+    const float x0 = data_prediction<EMU>(s.prediction_type, x, m, alpha_s, sigma_s);
+    const bf16 m1b = st.x0_prev[base + i];
+    const float m1 = __bfloat162float(m1b);
+    const float m2 = st.x0_prev2 ? __bfloat162float(st.x0_prev2[base + i]) : 0.f;
+    if (st.x0_prev2) st.x0_prev2[base + i] = m1b;
+    st.x0_prev[base + i] = __float2bfloat16_rn(x0);
+    float prev;
+    if (order == 1) {
+      st.cur_sample[base + i] = xb;
+      prev = rnd<EMU>(rnd<EMU>(ratio * x) - rnd<EMU>(c * x0));
+    } else {
+      const float xs = __bfloat162float(st.cur_sample[base + i]);
+      const float d0 = order == 2 ? m1 : m2;     // the block start's data prediction
+      const float d1 = rnd<EMU>(inv_r0 * rnd<EMU>(x0 - d0));
+      prev = rnd<EMU>(rnd<EMU>(ratio * xs) - rnd<EMU>(c * d0));
+      prev = order == 2 ? rnd<EMU>(prev - rnd<EMU>(c_d1 * d1)) : rnd<EMU>(prev + rnd<EMU>(c_d1 * d1));
+    }
+    a.out[base + i] = __float2bfloat16_rn(prev);
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 // frame-sharded window: K/V arrival flags in peer memory
 // ---------------------------------------------------------------------------------------------
@@ -839,6 +881,16 @@ int cfg_step_run(const StepArgs& a, const d4d_deis_sched& s, const SolverState& 
   D4D_REQUIRE((st.m_prev2 != nullptr) == (s.solver_order == 3), "m_prev2 is given exactly when solver_order is 3");
   if (!launch) return 0;
   return launch_step(cfg_deis_kernel<true>, cfg_deis_kernel<false>, s.emulate_bf16, stream, a, s, st);
+}
+
+int cfg_step_run(const StepArgs& a, const d4d_dpm_single_sched& s, const SolverState& st, cudaStream_t stream,
+                 bool launch) {
+  if (int rc = check_step(a, s.timesteps_table, s.coefs, s.n_steps, s.prediction_type, &st)) return rc;
+  D4D_REQUIRE(s.solver_order >= 1 && s.solver_order <= 3, "solver_order must be 1, 2 or 3");
+  D4D_REQUIRE(st.x0_prev != nullptr && st.cur_sample != nullptr, "null argument");
+  D4D_REQUIRE((st.x0_prev2 != nullptr) == (s.solver_order == 3), "x0_prev2 is given exactly when solver_order is 3");
+  if (!launch) return 0;
+  return launch_step(cfg_dpm_single_kernel<true>, cfg_dpm_single_kernel<false>, s.emulate_bf16, stream, a, s, st);
 }
 
 }  // namespace d4d

@@ -202,13 +202,15 @@ int assemble_input_run(const AssembleArgs& a, cudaStream_t stream);
 
 // a-13 + a-14: CFG combine + per-frame scheduler step (pipeline_diffuman4d.py:408-423): DDIM, DPM-Solver++ (dpmsolver++ /
 // midpoint, order <= 2), UniPC (predict_x0, bh1 / bh2, order <= 2; the UniC corrector of the frame's previous step,
-// then the UniP predictor), PNDM (skip_prk_steps: the PLMS steps) or DEIS (deis / logrho, order <= 3).  The scheduler's
-// constants, step count, prediction type and bf16 emulation come from its table struct in include/d4d.h, passed as it
-// is; the multistep solvers' coefficient rows are laid out there too.
+// then the UniP predictor), PNDM (skip_prk_steps: the PLMS steps), DEIS (deis / logrho, order <= 3) or DPM-Solver++
+// singlestep (dpmsolver++ / midpoint, order <= 3).  The scheduler's constants, step count, prediction type and bf16
+// emulation come from its table struct in include/d4d.h, passed as it is; the multistep solvers' coefficient rows are
+// laid out there too.
 constexpr int kDpmCoefs = 6;
 constexpr int kUniPCCoefs = 14;
 constexpr int kPndmCoefs = 10;
 constexpr int kDeisCoefs = 11;
+constexpr int kDpmSingleCoefs = 13;
 struct StepArgs {
   const bf16* noise;        // [(cfg?2:1)*F,4,h,w]
   const bf16* latents;      // [F,4,h,w]
@@ -223,10 +225,13 @@ struct StepArgs {
 // of them for DDIM).
 struct SolverState {
   bf16* x0_prev = nullptr;      // [F,4,h,w]: each frame's previous data prediction
-  bf16* x0_prev2 = nullptr;     // [F,4,h,w]: the one before (UniPC at solver_order 2)
+  // [F,4,h,w]: the one before (UniPC at solver_order 2, DPM-Solver++ singlestep at solver_order 3)
+  bf16* x0_prev2 = nullptr;
   bf16* last_sample = nullptr;  // [F,4,h,w]: the sample each frame's last predictor started from (UniPC)
   bf16* ets[4] = {};            // [F,4,h,w] each: the ring of PNDM's last model outputs (d4d_denoise_window_pndm)
-  bf16* cur_sample = nullptr;   // [F,4,h,w]: the sample each frame's PNDM counter-0 step started from
+  // [F,4,h,w]: the sample the frame's first step started from: PNDM's counter-0 step, or the order-1 step that started
+  // the frame's current DPM-Solver++ singlestep block
+  bf16* cur_sample = nullptr;
   bf16* m_prev = nullptr;       // [F,4,h,w]: each frame's previous DEIS model output, in its epsilon form
   bf16* m_prev2 = nullptr;      // [F,4,h,w]: the one before (DEIS at solver_order 3)
   // [F]: steps each frame has taken, capped at solver_order (PNDM: uncapped, its `counter`)
@@ -242,6 +247,8 @@ int cfg_step_run(const StepArgs& a, const d4d_unipc_sched& s, const SolverState&
 int cfg_step_run(const StepArgs& a, const d4d_pndm_sched& s, const SolverState& st, cudaStream_t stream,
                  bool launch = true);
 int cfg_step_run(const StepArgs& a, const d4d_deis_sched& s, const SolverState& st, cudaStream_t stream,
+                 bool launch = true);
+int cfg_step_run(const StepArgs& a, const d4d_dpm_single_sched& s, const SolverState& st, cudaStream_t stream,
                  bool launch = true);
 
 // cross-rank K/V arrival flags (frame-sharded window): signal = system-scope release of `epoch` into slot `my_rank` of

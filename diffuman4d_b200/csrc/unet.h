@@ -101,24 +101,27 @@ struct WindowBufs {  // scratch of d4d_denoise_window for one (F, h, w, cfg)
   ~WindowBufs();
 };
 
-// The scheduler of a window step: exactly one of the tables is set.  The multistep schedulers (DPM-Solver++, UniPC,
-// PNDM, DEIS) also get the window frames' solver state, read and updated in place: the order counts are read from
-// state.lower_order_nums and the advanced ones end up in state.lower_order_nums_out, both the caller's array.
+// The scheduler of a window step: exactly one of the tables is set.  The stateful schedulers (DPM-Solver++, UniPC,
+// PNDM, DEIS, DPM-Solver++ singlestep) also get the window frames' solver state, read and updated in place: the order
+// counts are read from state.lower_order_nums and the advanced ones end up in state.lower_order_nums_out, both the
+// caller's array.
 struct WindowStep {
   const d4d_sched* ddim = nullptr;
   const d4d_dpm_sched* dpm = nullptr;
   const d4d_unipc_sched* unipc = nullptr;
   const d4d_pndm_sched* pndm = nullptr;
   const d4d_deis_sched* deis = nullptr;
+  const d4d_dpm_single_sched* dpm_single = nullptr;
   SolverState state;
   // the number of tables set (a valid step has one)
   int tables() const {
-    return (ddim != nullptr) + (dpm != nullptr) + (unipc != nullptr) + (pndm != nullptr) + (deis != nullptr);
+    return (ddim != nullptr) + (dpm != nullptr) + (unipc != nullptr) + (pndm != nullptr) + (deis != nullptr) +
+           (dpm_single != nullptr);
   }
   // fn(table) with whichever table is set
   template <typename Fn>
   int with_table(Fn&& fn) const {
-    return ddim ? fn(*ddim) : dpm ? fn(*dpm) : unipc ? fn(*unipc) : pndm ? fn(*pndm) : fn(*deis);
+    return ddim ? fn(*ddim) : dpm ? fn(*dpm) : unipc ? fn(*unipc) : pndm ? fn(*pndm) : deis ? fn(*deis) : fn(*dpm_single);
   }
 };
 

@@ -19,7 +19,8 @@ from typing import Callable, List, Optional, Union
 
 import torch
 
-from .config import DEISConfig, DPMSolverConfig, PNDMConfig, SchedulerConfig, UNetConfig, UniPCConfig
+from .config import (DEISConfig, DPMSingleConfig, DPMSolverConfig, PNDMConfig, SchedulerConfig, UNetConfig,
+                     UniPCConfig)
 from .pipeline import B200Diffuman4DPipeline
 from .unet import B200MultiviewUNet
 
@@ -211,7 +212,48 @@ def deis_config_from_json(d: dict) -> DEISConfig:
         timestep_spacing=d.get("timestep_spacing", "linspace"), steps_offset=d.get("steps_offset", 0))
 
 
-def scheduler_config_from_json(d: dict) -> Union[SchedulerConfig, DPMSolverConfig, UniPCConfig, PNDMConfig, DEISConfig]:
+def dpm_single_config_from_json(d: dict) -> DPMSingleConfig:
+    """Map a diffusers ``DPMSolverSinglestepScheduler`` config; every knob the fused step does not implement raises
+    ``NotImplementedError`` naming the key."""
+    def refuse(key, why):
+        raise NotImplementedError(f"DPMSolverSinglestepScheduler {key}={d.get(key)!r} is not supported by the CUDA path "
+                                  f"({why})")
+
+    def want(key, allowed, default):
+        v = d.get(key, default)
+        if v not in allowed:
+            refuse(key, f"supported: {allowed}")
+        return v
+
+    if d.get("thresholding", False):
+        refuse("thresholding", "dynamic thresholding is not implemented")
+    for key in ("use_karras_sigmas", "use_exponential_sigmas", "use_beta_sigmas", "use_flow_sigmas",
+                "use_dynamic_shifting"):
+        if d.get(key, False):
+            refuse(key, "sigmas come straight from the beta schedule")
+    lmc = d.get("lambda_min_clipped", -math.inf)
+    if lmc is not None and math.isfinite(float(lmc)):
+        refuse("lambda_min_clipped", "only -inf (no clipping)")
+    if d.get("variance_type") is not None:
+        refuse("variance_type", "only None")
+    if d.get("trained_betas") is not None:
+        refuse("trained_betas", "betas come from beta_schedule")
+    want("algorithm_type", ("dpmsolver++",), "dpmsolver++")
+    want("solver_type", ("midpoint",), "midpoint")
+    order = want("solver_order", (1, 2, 3), 2)
+    want("beta_schedule", ("linear", "scaled_linear"), "linear")
+    want("prediction_type", ("epsilon", "v_prediction", "sample"), "epsilon")
+    want("final_sigmas_type", ("zero", "sigma_min"), "zero")
+    want("timestep_spacing", ("linspace",), "linspace")    # upstream has no other spacing for this class
+    return DPMSingleConfig(
+        num_train_timesteps=d.get("num_train_timesteps", 1000), beta_start=d.get("beta_start", 0.0001),
+        beta_end=d.get("beta_end", 0.02), beta_schedule=d.get("beta_schedule", "linear"), solver_order=order,
+        prediction_type=d.get("prediction_type", "epsilon"), lower_order_final=d.get("lower_order_final", False),
+        final_sigmas_type=d.get("final_sigmas_type", "zero"))
+
+
+def scheduler_config_from_json(d: dict) -> Union[SchedulerConfig, DPMSolverConfig, UniPCConfig, PNDMConfig, DEISConfig,
+                                                 DPMSingleConfig]:
     cls = d.get("_class_name", "DDIMScheduler")
     if cls == "DPMSolverMultistepScheduler":
         return dpm_solver_config_from_json(d)
@@ -221,11 +263,13 @@ def scheduler_config_from_json(d: dict) -> Union[SchedulerConfig, DPMSolverConfi
         return pndm_config_from_json(d)
     if cls == "DEISMultistepScheduler":
         return deis_config_from_json(d)
+    if cls == "DPMSolverSinglestepScheduler":
+        return dpm_single_config_from_json(d)
     if cls != "DDIMScheduler":
         raise NotImplementedError(
             f"scheduler {cls} is not fused on the CUDA path (DDIMScheduler, DPMSolverMultistepScheduler, "
-            "UniPCMultistepScheduler, PNDMScheduler and DEISMultistepScheduler only); run the reference's Python "
-            "scheduler loop for other classes")
+            "UniPCMultistepScheduler, PNDMScheduler, DEISMultistepScheduler and DPMSolverSinglestepScheduler only); run "
+            "the reference's Python scheduler loop for other classes")
     if d.get("thresholding", False):
         raise NotImplementedError("dynamic thresholding is not supported")
     return SchedulerConfig(

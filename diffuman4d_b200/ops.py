@@ -292,8 +292,8 @@ def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: flo
 
 def _multistep_step(entry: str, noise, latents, cond_mask, timestep_indices, planes, lower_order_nums, sched,
                     guidance_scale, cfg):
-    """``cfg_dpm_step`` / ``cfg_unipc_step`` / ``cfg_pndm_step`` / ``cfg_deis_step``: ``planes`` are the (name, bf16
-    [F,4,h,w] tensor or None) state planes in the order ``entry`` takes them."""
+    """``cfg_dpm_step`` / ``cfg_unipc_step`` / ``cfg_pndm_step`` / ``cfg_deis_step`` / ``cfg_dpm_single_step``:
+    ``planes`` are the (name, bf16 [F,4,h,w] tensor or None) state planes in the order ``entry`` takes them."""
     _bf16c(noise, "noise"), _bf16c(latents, "latents"), _bf16c(cond_mask, "cond_mask")
     F, _, h, w = latents.shape
     for name, t in planes:
@@ -355,3 +355,15 @@ def cfg_deis_step(noise: torch.Tensor, latents: torch.Tensor, cond_mask: torch.T
     Returns (new latents, advanced timestep indices, advanced ``lower_order_nums``)."""
     return _multistep_step("d4d_cfg_deis_step", noise, latents, cond_mask, timestep_indices,
                            [("m_prev", m_prev), ("m_prev2", m_prev2)], lower_order_nums, sched, guidance_scale, cfg)
+
+
+def cfg_dpm_single_step(noise: torch.Tensor, latents: torch.Tensor, cond_mask: torch.Tensor,
+                        timestep_indices: torch.Tensor, x0_prev: torch.Tensor, x0_prev2: Optional[torch.Tensor],
+                        cur_sample: torch.Tensor, lower_order_nums: torch.Tensor, sched, guidance_scale: float, cfg: bool):
+    """One CFG + DPM-Solver++ singlestep step of F frames (``sched``: a ``d4d_dpm_single_sched`` from
+    ``DPMSingleTables.c_struct``).  ``noise`` [(cfg?2:1)*F,4,h,w]; ``x0_prev``, ``x0_prev2`` (None below solver_order 3)
+    and ``cur_sample`` [F,4,h,w] bf16 are updated in place.  Returns (new latents, advanced timestep indices, advanced
+    ``lower_order_nums``)."""
+    return _multistep_step("d4d_cfg_dpm_single_step", noise, latents, cond_mask, timestep_indices,
+                           [("x0_prev", x0_prev), ("x0_prev2", x0_prev2), ("cur_sample", cur_sample)], lower_order_nums,
+                           sched, guidance_scale, cfg)

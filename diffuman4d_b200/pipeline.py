@@ -4,9 +4,10 @@ Seams (SURVEY.md section 8b):
   B-3  ``denoise_window``  == ``Diffuman4DPipeline.__call__`` with latents given
        (reference src/diffusers/pipelines/diffuman4d/pipeline_diffuman4d.py:345-425): input assembly, UNet, CFG
        combine and the F per-frame scheduler steps run as ONE C-ABI call (no per-frame host sync).  The scheduler is DDIM
-       (``SchedulerConfig``), DPM-Solver++ (``DPMSolverConfig``), UniPC (``UniPCConfig``), PNDM (``PNDMConfig``) or DEIS
-       (``DEISConfig``); the multistep ones keep a per-frame history on the device (``DPMSolverState`` / ``UniPCState`` /
-       ``PNDMState`` / ``DEISState``) in place of the reference's per-frame scheduler copies.
+       (``SchedulerConfig``), DPM-Solver++ (``DPMSolverConfig``), UniPC (``UniPCConfig``), PNDM (``PNDMConfig``), DEIS
+       (``DEISConfig``) or DPM-Solver++ singlestep (``DPMSingleConfig``); the stateful ones keep a per-frame history on
+       the device (``DPMSolverState`` / ``UniPCState`` / ``PNDMState`` / ``DEISState`` / ``DPMSingleState``) in place of
+       the reference's per-frame scheduler copies.
   B-4  ``sliding_iterative_denoise`` == PIPE:439-559: same arguments, same ValueErrors, same returned dict.  The VAE
        (stock AutoencoderKL, out of scope per SURVEY section 8f) is pluggable: pass ``vae`` with ``encode_latents(x)`` /
        ``decode_latents(z)`` callables, or feed latents directly (``pixel_values_latents=...``).
@@ -22,9 +23,9 @@ from typing import Callable, List, Optional, Union
 import torch
 
 from ._lib import check, lib
-from .config import DEISConfig, DPMSolverConfig, PNDMConfig, SchedulerConfig, UniPCConfig
-from .scheduler import (DDIMTables, DEISTables, DPMSolverFrame, DPMSolverTables, PNDMTables, SolverState,
-                        UniPCTables)
+from .config import DEISConfig, DPMSingleConfig, DPMSolverConfig, PNDMConfig, SchedulerConfig, UniPCConfig
+from .scheduler import (DDIMTables, DEISTables, DPMSingleTables, DPMSolverFrame, DPMSolverTables, PNDMTables,
+                        SolverState, UniPCTables)
 from .unet import _DOMAIN_IDS, B200MultiviewUNet
 
 
@@ -67,7 +68,7 @@ def resize_conditions(plucker_embeds: torch.Tensor, cond_masks: torch.Tensor, h:
 class B200Diffuman4DPipeline:
     def __init__(self, unet: B200MultiviewUNet,
                  scheduler_config: Union[SchedulerConfig, DPMSolverConfig, UniPCConfig, PNDMConfig, DEISConfig,
-                                         None] = None,
+                                         DPMSingleConfig, None] = None,
                  vae=None, emulate_bf16_scheduler: bool = False):
         self.unet = unet
         self.vae = vae
@@ -81,6 +82,8 @@ class B200Diffuman4DPipeline:
             self.scheduler = PNDMTables(scheduler_config, device=self.device)
         elif isinstance(scheduler_config, DEISConfig):
             self.scheduler = DEISTables(scheduler_config, device=self.device)
+        elif isinstance(scheduler_config, DPMSingleConfig):
+            self.scheduler = DPMSingleTables(scheduler_config, device=self.device)
         else:
             self.scheduler = DDIMTables(scheduler_config, device=self.device)
         self.emulate_bf16_scheduler = emulate_bf16_scheduler
@@ -107,8 +110,9 @@ class B200Diffuman4DPipeline:
 
     def parepare_schedulers(self, num_inference_steps: int, num_frames: int):
         """PIPE:265-271.  The per-frame deep copies exist in the reference only because scheduler objects are
-        stateful; DDIM is stateless, so one table serves all frames.  DPM-Solver++, UniPC, PNDM and DEIS get a fresh
-        (zeroed) device state for the frames, and one ``DPMSolverFrame`` handle per frame in place of each copy."""
+        stateful; DDIM is stateless, so one table serves all frames.  DPM-Solver++ (multistep and singlestep), UniPC,
+        PNDM and DEIS get a fresh (zeroed) device state for the frames, and one ``DPMSolverFrame`` handle per frame in
+        place of each copy."""
         ts = self.scheduler.set_timesteps(num_inference_steps)
         if self._multistep:
             return self.scheduler.new_state(num_frames).frames(), ts
@@ -120,8 +124,8 @@ class B200Diffuman4DPipeline:
                        num_inference_steps: int = 1, solver_state: Optional[SolverState] = None):
         """One window: ``num_inference_steps`` x (assemble -> UNet -> CFG -> per-frame scheduler step).  ``latents``
         [F,4,h,w] and ``timestep_indices`` [F] (int64, device) are updated IN PLACE and returned.  With DPM-Solver++,
-        UniPC, PNDM or DEIS, ``solver_state`` is the window frames' ``DPMSolverState`` / ``UniPCState`` / ``PNDMState``
-        / ``DEISState`` (``take``), also updated in place."""
+        UniPC, PNDM, DEIS or DPM-Solver++ singlestep, ``solver_state`` is the window frames' ``DPMSolverState`` /
+        ``UniPCState`` / ``PNDMState`` / ``DEISState`` / ``DPMSingleState`` (``take``), also updated in place."""
         return self._window_step(latents=latents, pixel_values_latents=pixel_values_latents,
                                  plucker_embeds_latents=plucker_embeds_latents, skeletons_latents=skeletons_latents,
                                  cond_masks_latents=cond_masks_latents, timestep_indices=timestep_indices, domain=domain,

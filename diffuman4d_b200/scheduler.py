@@ -1,4 +1,5 @@
-"""Host-side scheduler tables for the fused CFG + scheduler-step kernels: DDIM, DPM-Solver++, UniPC, PNDM and DEIS.
+"""Host-side scheduler tables for the fused CFG + scheduler-step kernels: DDIM, DPM-Solver++ (multistep and singlestep),
+UniPC, PNDM and DEIS.
 
 Mirrors what the reference obtains from ``self.scheduler.set_timesteps(n)`` + per-frame deep copies
 (pipeline_diffuman4d.py:265-271) for upstream diffusers==0.33.1 ``DDIMScheduler``: the ``timesteps`` vector and
@@ -13,7 +14,9 @@ needs each frame's previous sample and, at order 2, a second data prediction of 
 do the same for ``PNDMScheduler`` with ``skip_prk_steps`` (``cfg_pndm_kernel``), whose history is the last four model
 outputs, the sample of the frame's first step and its step counter.  ``DEISTables`` / ``DEISState`` do the same for
 ``DEISMultistepScheduler`` (``cfg_deis_kernel``, up to third order), whose history is the last two model outputs in their
-epsilon form.
+epsilon form.  ``DPMSingleTables`` / ``DPMSingleState`` do the same for ``DPMSolverSinglestepScheduler``
+(``cfg_dpm_single_kernel``, up to third order), whose history is the last two data predictions and the sample the frame's
+current block started from.
 
 Each tables class names the C entry points of its window step (``window_entry_points``: plain and frame-sharded, None
 where there is none) and the bf16 state planes they take, in ABI order (``state_planes``; None for the stateless DDIM).
@@ -21,12 +24,13 @@ where there is none) and the bf16 state planes they take, in ABI order (``state_
 from __future__ import annotations
 
 import copy
+import dataclasses
 
 import numpy as np
 import torch
 
-from ._lib import D4DDeisSched, D4DDpmSched, D4DPndmSched, D4DSched, D4DUniPCSched
-from .config import DEISConfig, DPMSolverConfig, PNDMConfig, SchedulerConfig, UniPCConfig
+from ._lib import D4DDeisSched, D4DDpmSched, D4DDpmSingleSched, D4DPndmSched, D4DSched, D4DUniPCSched
+from .config import DEISConfig, DPMSingleConfig, DPMSolverConfig, PNDMConfig, SchedulerConfig, UniPCConfig
 
 _PRED = {"epsilon": 0, "v_prediction": 1, "sample": 2}
 
@@ -142,7 +146,8 @@ def dpm_step_coefficients(sigmas: torch.Tensor) -> torch.Tensor:
 
 
 class _MultistepTables:
-    """What ``DPMSolverTables``, ``UniPCTables`` and ``DEISTables`` share: the config checks common to all, the sigma
+    """What ``DPMSolverTables``, ``UniPCTables``, ``DEISTables`` and ``DPMSingleTables`` share: the config checks common to
+    all, the sigma
     table, ``set_timesteps`` and the device copies behind ``c_struct``.  A subclass adds its own checks (``_check``), its
     coefficient rows (``_coefficients``) and its C struct (``_struct``, plus the fields of ``_struct_fields``)."""
     init_noise_sigma = 1.0  # upstream: init_noise_sigma 1, scale_model_input is the identity
@@ -181,7 +186,7 @@ class _MultistepTables:
 
     def set_timesteps(self, n: int, device=None):
         c = self.config
-        ts = dpm_timesteps(c, n)       # UniPC and DEIS space their timesteps like DPM-Solver++
+        ts = dpm_timesteps(c, n)       # UniPC, DEIS and singlestep space their timesteps like DPM-Solver++
         last = 0.0 if self.final_sigmas_type == "zero" else float(self.all_sigmas[0])
         self.num_inference_steps = n
         self.timesteps = torch.from_numpy(ts)
@@ -612,4 +617,125 @@ class DEISState(SolverState):
                  m_prev2: torch.Tensor = None, lower_order_nums: torch.Tensor = None):
         super().__init__(num_frames, device, tuple(p for p in _deis_planes(solver_order) if p), lower_order_nums,
                          m_prev=m_prev, m_prev2=m_prev2)
+        self.solver_order = solver_order
+
+
+# ---- DPM-Solver++ singlestep ------------------------------------------------------------------------------------------
+DPM_SINGLE_COEFS = 13   # row layout in include/d4d.h ``d4d_dpm_single_sched``
+
+
+def dpm_single_order_list(solver_order: int, lower_order_final: bool, final_sigmas_type: str, n: int) -> list:
+    """The order of each of the n steps (upstream ``DPMSolverSinglestepScheduler.get_order_list``): blocks 1, 2, ..,
+    solver_order.  With ``lower_order_final`` the list ends on a shorter block: the last n % solver_order steps form one,
+    and when that is none, the last full block is split into 1, .., solver_order - 1 and 1.  Without it n must be a
+    multiple of solver_order (``set_timesteps`` switches it on otherwise).  A zero final sigma makes the last step first
+    order."""
+    block = list(range(1, solver_order + 1))
+    full, rest = divmod(n, solver_order)
+    if not lower_order_final:
+        if rest:
+            raise ValueError(f"{n} steps are not whole blocks of {solver_order} without lower_order_final")
+        orders = block * full
+    elif rest:
+        orders = block * full + block[:rest]
+    else:
+        orders = block * (full - 1) + block[:-1] + [1]
+    if final_sigmas_type == "zero":
+        orders[-1] = 1
+    return orders
+
+
+def dpm_single_step_coefficients(orders: list, sigmas: torch.Tensor) -> torch.Tensor:
+    """[n, 13] fp32 coefficients of the n steps over ``sigmas`` [n+1] with the rows' ``orders`` (layout in include/d4d.h
+    ``d4d_dpm_single_sched``), each evaluated on 0-dim fp32 tensors in the order ``DPMSolverSinglestepScheduler``'s
+    ``convert_model_output`` / ``dpm_solver_first_order_update`` / ``singlestep_dpm_solver_second_order_update`` /
+    ``singlestep_dpm_solver_third_order_update`` evaluate them.  The first-order scalars are DPM-Solver++ multistep's.
+    The update of order k at row i spans the block from row i - k + 1; entries of orders above the row's are 0."""
+    def alpha_sigma(sigma):
+        alpha_t = 1 / ((sigma ** 2 + 1) ** 0.5)
+        return alpha_t, sigma * alpha_t
+
+    def lam(j):
+        a, s = alpha_sigma(sigmas[j])
+        return torch.log(a) - torch.log(s)
+
+    first = dpm_step_coefficients(sigmas)
+    n = sigmas.numel() - 1
+    out = torch.zeros(n, DPM_SINGLE_COEFS, dtype=torch.float32)
+    out[:, :4] = first[:, :4]
+    for i, order in enumerate(orders):
+        alpha_t, sigma_t = alpha_sigma(sigmas[i + 1])
+        lambda_t, lambda_s0 = lam(i + 1), lam(i)
+        if order >= 2:
+            lambda_s1 = lam(i - 1)
+            h = lambda_t - lambda_s1
+            r0 = (lambda_s0 - lambda_s1) / h
+            c = alpha_t * (torch.exp(-h) - 1.0)
+            out[i, 4:8] = torch.stack([sigma_t / alpha_sigma(sigmas[i - 1])[1], c, 0.5 * c, 1.0 / r0])
+        if order == 3:
+            lambda_s2 = lam(i - 2)
+            h = lambda_t - lambda_s2
+            r0 = (lambda_s0 - lambda_s2) / h
+            c = alpha_t * (torch.exp(-h) - 1.0)
+            out[i, 8:12] = torch.stack([sigma_t / alpha_sigma(sigmas[i - 2])[1], c,
+                                        alpha_t * ((torch.exp(-h) - 1.0) / h + 1.0), 1.0 / r0])
+        out[i, 12] = float(order)
+    return out
+
+
+def _dpm_single_planes(solver_order: int) -> tuple:
+    """The singlestep solver's bf16 state planes in the order ``d4d_denoise_window_dpm_single`` takes them; ``x0_prev2``
+    exists at order 3 only (None: its argument is NULL)."""
+    return ("x0_prev", "x0_prev2" if solver_order == 3 else None, "cur_sample")
+
+
+class DPMSingleTables(_MultistepTables):
+    """Timesteps, sigmas, order list and step coefficients of ``DPMSolverSinglestepScheduler`` (algorithm_type
+    "dpmsolver++", solver_type "midpoint"; diffusers 0.33.1) for ``cfg_dpm_single_kernel``.
+
+    ``config`` is this object's own copy: like upstream's ``register_to_config``, ``set_timesteps`` switches its
+    ``lower_order_final`` on when the step count is not a multiple of ``solver_order`` or the final sigma is zero, and
+    the switch stays for later ``set_timesteps`` calls."""
+    name = "DPM-Solver++ singlestep"
+    solver_orders = (1, 2, 3)
+    # no frame-sharded window: its window-result exchange carries DPM-Solver++ multistep's state only
+    window_entry_points = ("d4d_denoise_window_dpm_single", None)
+    _struct = D4DDpmSingleSched
+
+    def __init__(self, cfg: DPMSingleConfig = None, device="cuda:0"):
+        super().__init__(dataclasses.replace(cfg or DPMSingleConfig()), device)
+        self.order_list = None          # the order of each step, after set_timesteps
+
+    def _check(self, c):
+        if c.timestep_spacing != "linspace":
+            raise ValueError(f"timestep_spacing {c.timestep_spacing!r}: DPMSolverSinglestepScheduler spaces its timesteps "
+                             "by 'linspace' only")
+
+    def set_timesteps(self, n: int, device=None):
+        c = self.config
+        if not c.lower_order_final and (n % c.solver_order != 0 or c.final_sigmas_type == "zero"):
+            c.lower_order_final = True
+        self.order_list = dpm_single_order_list(c.solver_order, c.lower_order_final, c.final_sigmas_type, n)
+        return super().set_timesteps(n, device)
+
+    def _coefficients(self, sigmas: torch.Tensor) -> torch.Tensor:
+        return dpm_single_step_coefficients(self.order_list, sigmas)
+
+    @property
+    def state_planes(self) -> tuple:
+        return _dpm_single_planes(self.config.solver_order)
+
+    def new_state(self, num_frames: int) -> "DPMSingleState":
+        return DPMSingleState(num_frames, self.device, self.config.solver_order)
+
+
+class DPMSingleState(SolverState):
+    """The DPM-Solver++ singlestep history: ``x0_prev`` (each frame's previous data prediction), ``x0_prev2`` (the one
+    before; order 3 only, else None), ``cur_sample`` (the sample the frame's current block started from) and
+    ``lower_order_nums``."""
+
+    def __init__(self, num_frames: int, device, solver_order: int = 2, x0_prev: torch.Tensor = None,
+                 x0_prev2: torch.Tensor = None, cur_sample: torch.Tensor = None, lower_order_nums: torch.Tensor = None):
+        super().__init__(num_frames, device, tuple(p for p in _dpm_single_planes(solver_order) if p), lower_order_nums,
+                         x0_prev=x0_prev, x0_prev2=x0_prev2, cur_sample=cur_sample)
         self.solver_order = solver_order

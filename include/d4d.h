@@ -157,6 +157,35 @@ typedef struct d4d_deis_sched {
   int32_t emulate_bf16;             /* 1: round like the reference's bf16 eager maths (history and every op in bf16) */
 } d4d_deis_sched;
 
+/* DPM-Solver++ singlestep constants for the fused step (upstream diffusers DPMSolverSinglestepScheduler with
+ * algorithm_type "dpmsolver++", solver_type "midpoint", solver_order 1, 2 or 3; d4d_version() 112 and later).  The
+ * solver's history is per frame and lives on the device (x0_prev / x0_prev2 / cur_sample / lower_order_nums of
+ * d4d_denoise_window_dpm_single); a frame's step index is its timestep index.  Upstream's order list splits the steps
+ * into blocks 1, 2, .., k; step i runs at order min(row i's order, lower_order_nums + 1).  A step at order 1 starts a
+ * block and saves its sample in cur_sample; a step at order k > 1 updates from that sample, k - 1 rows back, with the
+ * data predictions x0 (this step), x0_prev and, at order 3, x0_prev2 (the block start's).
+ * coefs row i (fp32), computed on the host in the upstream scheduler's fp32 order of operations (the device evaluates no
+ * log / exp), with alpha_j = 1 / sqrt(sigma_j^2 + 1), sigma'_j = sigma_j * alpha_j, lambda_j = log alpha_j - log sigma'_j
+ * and, for the update of order k, b = i - k + 1 (the block start), h = lambda_(i+1) - lambda_b,
+ * r0 = (lambda_i - lambda_b) / h, c = alpha_(i+1) * (exp(-h) - 1):
+ *   [0] alpha_i   [1] sigma'_i                                               (convert_model_output)
+ *   [2] sigma'_(i+1) / sigma'_i   [3] c                 (order 1: x' = [2] * x - [3] * x0; [2], [3] as d4d_dpm_sched's)
+ *   [4] sigma'_(i+1) / sigma'_(i-1)   [5] c   [6] 0.5 * c   [7] 1 / r0
+ *        (order 2: x' = [4] * s - [5] * x0_prev - [6] * ([7] * (x0 - x0_prev)), s = cur_sample)
+ *   [8] sigma'_(i+1) / sigma'_(i-2)   [9] c   [10] alpha_(i+1) * ((exp(-h) - 1) / h + 1)   [11] 1 / r0
+ *        (order 3: x' = [8] * s - [9] * x0_prev2 + [10] * ([11] * (x0 - x0_prev2)))
+ *   [12] the row's order from upstream's order list
+ * [4..7] are 0 in rows of order 1 and [8..11] in rows of order 1 or 2 (those rows never run the update; with
+ * final_sigmas_type "zero" the last row has order 1 and an infinite h). */
+typedef struct d4d_dpm_single_sched {
+  const int64_t* timesteps_table;   /* device, [n_steps]  (scheduler.timesteps after set_timesteps) */
+  const float* coefs;               /* device, [n_steps][13], see above */
+  int32_t n_steps;
+  int32_t prediction_type;          /* 0 epsilon, 1 v_prediction, 2 sample */
+  int32_t solver_order;             /* 1, 2 or 3 */
+  int32_t emulate_bf16;             /* 1: round like the reference's bf16 eager maths (history and every op in bf16) */
+} d4d_dpm_single_sched;
+
 const char* d4d_last_error(void);
 int d4d_version(void);
 
@@ -251,6 +280,20 @@ int d4d_denoise_window_deis(d4d_handle* h, void* latents, const void* pixel_late
                             const d4d_deis_sched* sched, float guidance_scale, int domain, int F, int height, int width,
                             int num_steps, void* m_prev, void* m_prev2, int32_t* lower_order_nums, void* stream);
 
+/* The same window step with a DPM-Solver++ singlestep scheduler (d4d_version() 112 and later).  Arguments as
+ * d4d_denoise_window, plus the window frames' solver state, read and updated in place (conditioning frames keep theirs;
+ * zeros for a new task):
+ *   x0_prev           device bf16 [F,4,h,w]: each frame's data prediction of its previous step
+ *   x0_prev2          device bf16 [F,4,h,w]: the one before (solver_order 3; NULL exactly when solver_order is 1 or 2)
+ *   cur_sample        device bf16 [F,4,h,w]: the sample each frame's current block started from
+ *   lower_order_nums  device int32 [F]: steps each frame has taken, capped at solver_order
+ * A caller carries them across the windows of one task, gathered and scattered with the frames like the latents. */
+int d4d_denoise_window_dpm_single(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                  const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                  const d4d_dpm_single_sched* sched, float guidance_scale, int domain, int F, int height,
+                                  int width, int num_steps, void* x0_prev, void* x0_prev2, void* cur_sample,
+                                  int32_t* lower_order_nums, void* stream);
+
 /* ---- building blocks of B-3, exported for parity tests ------------------------------------------------ */
 int d4d_assemble_input(void* latents, const void* pixel_latents, const void* plucker, const void* skel_latents,
                        const void* cond_mask, const int64_t* timestep_indices, const int64_t* timesteps_table,
@@ -287,6 +330,14 @@ int d4d_cfg_deis_step(const void* noise, const void* latents, const void* cond_m
                       int64_t* timestep_indices_out, void* m_prev, void* m_prev2, const int32_t* lower_order_nums,
                       int32_t* lower_order_nums_out, const d4d_deis_sched* sched, float guidance_scale, int cfg, int F,
                       int height, int width, void* latents_out, void* stream);
+/* One CFG + DPM-Solver++ singlestep step of the frames (d4d_version() 112 and later; state as
+ * d4d_denoise_window_dpm_single).  x0_prev, x0_prev2 and cur_sample are updated in place; lower_order_nums_out and
+ * timestep_indices_out receive the advanced counters (they may not alias the inputs); latents_out may alias latents. */
+int d4d_cfg_dpm_single_step(const void* noise, const void* latents, const void* cond_mask,
+                            const int64_t* timestep_indices, int64_t* timestep_indices_out, void* x0_prev,
+                            void* x0_prev2, void* cur_sample, const int32_t* lower_order_nums,
+                            int32_t* lower_order_nums_out, const d4d_dpm_single_sched* sched, float guidance_scale,
+                            int cfg, int F, int height, int width, void* latents_out, void* stream);
 
 /* ---- op-level entry points (each is one hot-path kernel; used by tests/ and bench.py) ------------------
  * d4d_op_gemm:   out[M,N] = act((A|A2)[M,K1+K2] . W[N,K]^T + bias + rowvec[row/rows_per_image]) * scale + residual
