@@ -5,8 +5,8 @@ same k-blocks in the same order, and the GroupNorm statistics are the same fixed
 the stored output and the statistics words must not depend on the tile rows: they are compared byte for byte, for the three
 conv kinds (stride 1, stride 2 through the strided tensor map, four-phase upsampling), the four epilogue instantiations of
 the conv kernels, both widths that have 256-row kernels, the level shapes of the UNet at a reduced image count, and grids
-that overhang the tile.  Each case is also held against the fp64 reference at the tolerance of test_gpu_kernel_edges.py, which
-guards the case of both tiles being wrong together.
+that overhang the tile.  Each case is also held to criterion (a) of test_gpu_gemm_conv_fp64.py (a correct rounding of a value
+within the accumulation allowance of the fp64 result), which guards the case of both tiles being wrong together.
 
 The tile chooser (gemm_choose_tile) is checked against its cost table (tools/gemm_shapes.py::auto_tile) for every conv of the
 W16@64², W24@64² and W16@128² plans; that test needs no device.
@@ -22,7 +22,8 @@ sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(
 
 from diffuman4d_b200.config import UNetConfig  # noqa: E402
 from diffuman4d_b200.plan import launches  # noqa: E402
-from test_gpu_kernel_edges import _check_ws, _close, _conv_ref, _rand, _stats_ws, _stream  # noqa: E402
+from test_gpu_gemm_conv_fp64 import Case, check_a  # noqa: E402
+from test_gpu_kernel_edges import _check_ws, _rand, _stats_ws, _stream  # noqa: E402
 
 KIND = {"s1": 0, "s2": 1, "up": 3}
 FEATS = {"bias+rowvec+stats": ("bias", "rowvec", "stats"),       # resnet conv1
@@ -43,7 +44,7 @@ def _conv_tiled(x, wt, Cout, kind, block_m, block_n, bias=None, rowvec=None, res
 
 
 def _run_both(n, H, W, Cin, Cout, kind, feats, bn, seed=300):
-    """The conv at 128 and at 256 rows: outputs, statistics workspaces, and the fp64-grade reference."""
+    """The conv at 128 and at 256 rows: outputs and statistics workspaces, and the launch and operands for check_a."""
     from diffuman4d_b200 import ops
     x = _rand((n, H, W, Cin), seed)
     w = _rand((Cout, Cin, 3, 3), seed + 1, std=(9 * Cin) ** -0.5)
@@ -53,28 +54,25 @@ def _run_both(n, H, W, Cin, Cout, kind, feats, bn, seed=300):
     rowvec = _rand((n, Cout), seed + 3) if "rowvec" in feats else None
     res = _rand((n, oh, ow, Cout), seed + 4) if "residual" in feats else None
     act = int("act" in feats)
-    ref = _conv_ref(x, w, bias, stride=2 if kind == "s2" else 1, up=kind == "up")
-    if rowvec is not None:
-        ref = ref + rowvec.float()[:, None, None, :]
-    if act:
-        ref = torch.nn.functional.silu(ref)
-    if res is not None:
-        ref = ref + res.float()
+    case = Case("tile-rows", "conv", dict(n=n, H=H, W=W, Cin=Cin, Cout=Cout, mode=kind), feats, {"rows": oh * ow})
+    inp = {"a": x, "a2": None, "w": w, "bias": bias, "rowvec": rowvec, "scale": 1.0,
+           "res": None if res is None else res.view(-1, Cout)}
     got = {}
     for bm in (128, 256):
         ws = _stats_ws(n * Cout * 2) if "stats" in feats else None
         got[bm] = (_conv_tiled(x, wt, Cout, kind, bm, bn, bias, rowvec, res, act, ws), ws)
-    return got, ref
+    return got, (case, inp)
 
 
 def _check_pair(got, ref, n, what):
+    """ref: (case, operands) of the launch, for criterion (a)."""
     (o128, s128), (o256, s256) = got[128], got[256]
     assert torch.equal(o128.view(torch.int16), o256.view(torch.int16)), \
         f"{what}: {int((o128.view(torch.int16) != o256.view(torch.int16)).sum())} output words differ between 128 and 256 rows"
     if s128 is not None:
         assert torch.equal(s128, s256), f"{what}: {int((s128 != s256).sum())} statistics words differ between 128 and 256 rows"
         _check_ws(s256, o256, n, what)
-    _close(o256, ref)
+    check_a(o256.view(-1, o256.shape[-1]), *ref, what)
 
 
 @pytest.mark.gpu
