@@ -54,10 +54,11 @@ int unet_forward(d4d_handle* h, const void* sample, const int64_t* timestep, con
 }
 
 // every d4d_denoise_window* entry point: `step` names the scheduler table and the frames' solver state; F_total = 0 runs
-// the single-GPU plan
+// the single-GPU plan; cfg_split runs this rank's CFG half (the *_cfg_split entry points)
 int denoise_window(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker, const void* skeletons,
                    const void* cond_mask, int64_t* timestep_indices, const d4d::WindowStep& step, float guidance_scale,
-                   int domain, int F, int F_total, int height, int width, int num_steps, void* stream) {
+                   int domain, int F, int F_total, int height, int width, int num_steps, void* stream,
+                   bool cfg_split = false) {
   D4D_API_BEGIN
   D4D_REQUIRE(h != nullptr && step.tables() > 0, "null argument");
   DeviceGuard g(h->model->device());
@@ -65,7 +66,7 @@ int denoise_window(d4d_handle* h, void* latents, const void* pixel_latents, cons
                                   static_cast<const bf16*>(plucker), static_cast<const bf16*>(skeletons),
                                   static_cast<const bf16*>(cond_mask), reinterpret_cast<long long*>(timestep_indices),
                                   step, guidance_scale, domain, F, height, width, num_steps,
-                                  static_cast<cudaStream_t>(stream), F_total);
+                                  static_cast<cudaStream_t>(stream), F_total, cfg_split);
   D4D_API_END
 }
 
@@ -83,6 +84,16 @@ d4d::WindowStep dpm_step(const d4d_dpm_sched* sched, void* x0_prev, int32_t* low
   return s;
 }
 
+d4d::WindowStep unipc_step(const d4d_unipc_sched* sched, void* x0_prev, void* x0_prev2, void* last_sample,
+                           int32_t* lower_order_nums) {
+  d4d::WindowStep s;
+  s.unipc = sched;
+  s.state.x0_prev = static_cast<bf16*>(x0_prev); s.state.x0_prev2 = static_cast<bf16*>(x0_prev2);
+  s.state.last_sample = static_cast<bf16*>(last_sample);
+  s.state.lower_order_nums = s.state.lower_order_nums_out = lower_order_nums;
+  return s;
+}
+
 // the PNDM state of d4d_denoise_window_pndm / d4d_cfg_pndm_step (the counter arrays are set by the caller)
 d4d::SolverState pndm_state(void* ets0, void* ets1, void* ets2, void* ets3, void* cur_sample) {
   d4d::SolverState st;
@@ -90,6 +101,33 @@ d4d::SolverState pndm_state(void* ets0, void* ets1, void* ets2, void* ets3, void
   for (int i = 0; i < 4; ++i) st.ets[i] = static_cast<bf16*>(ets[i]);
   st.cur_sample = static_cast<bf16*>(cur_sample);
   return st;
+}
+
+d4d::WindowStep pndm_step(const d4d_pndm_sched* sched, void* ets0, void* ets1, void* ets2, void* ets3, void* cur_sample,
+                          int32_t* counter) {
+  d4d::WindowStep s;
+  s.pndm = sched;
+  s.state = pndm_state(ets0, ets1, ets2, ets3, cur_sample);
+  s.state.lower_order_nums = s.state.lower_order_nums_out = counter;
+  return s;
+}
+
+d4d::WindowStep deis_step(const d4d_deis_sched* sched, void* m_prev, void* m_prev2, int32_t* lower_order_nums) {
+  d4d::WindowStep s;
+  s.deis = sched;
+  s.state.m_prev = static_cast<bf16*>(m_prev); s.state.m_prev2 = static_cast<bf16*>(m_prev2);
+  s.state.lower_order_nums = s.state.lower_order_nums_out = lower_order_nums;
+  return s;
+}
+
+d4d::WindowStep dpm_single_step(const d4d_dpm_single_sched* sched, void* x0_prev, void* x0_prev2, void* cur_sample,
+                                int32_t* lower_order_nums) {
+  d4d::WindowStep s;
+  s.dpm_single = sched;
+  s.state.x0_prev = static_cast<bf16*>(x0_prev); s.state.x0_prev2 = static_cast<bf16*>(x0_prev2);
+  s.state.cur_sample = static_cast<bf16*>(cur_sample);
+  s.state.lower_order_nums = s.state.lower_order_nums_out = lower_order_nums;
+  return s;
 }
 
 // the step arguments of every d4d_cfg_*_step entry point
@@ -111,7 +149,7 @@ d4d::StepArgs step_args(const void* noise, const void* latents, const void* cond
 extern "C" {
 
 const char* d4d_last_error(void) { return d4d::g_last_error.c_str(); }
-int d4d_version(void) { return 112; }
+int d4d_version(void) { return 113; }
 
 int d4d_create(const d4d_config* cfg, int device, d4d_handle** out) {
   D4D_API_BEGIN
@@ -233,13 +271,9 @@ int d4d_denoise_window_unipc(d4d_handle* h, void* latents, const void* pixel_lat
                              const d4d_unipc_sched* sched, float guidance_scale, int domain, int F, int height, int width,
                              int num_steps, void* x0_prev, void* x0_prev2, void* last_sample, int32_t* lower_order_nums,
                              void* stream) {
-  d4d::WindowStep s;
-  s.unipc = sched;
-  s.state.x0_prev = static_cast<bf16*>(x0_prev); s.state.x0_prev2 = static_cast<bf16*>(x0_prev2);
-  s.state.last_sample = static_cast<bf16*>(last_sample);
-  s.state.lower_order_nums = s.state.lower_order_nums_out = lower_order_nums;
-  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, s, guidance_scale,
-                        domain, F, 0, height, width, num_steps, stream);
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
+                        unipc_step(sched, x0_prev, x0_prev2, last_sample, lower_order_nums), guidance_scale, domain, F, 0,
+                        height, width, num_steps, stream);
 }
 
 int d4d_denoise_window_pndm(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
@@ -247,24 +281,18 @@ int d4d_denoise_window_pndm(d4d_handle* h, void* latents, const void* pixel_late
                             const d4d_pndm_sched* sched, float guidance_scale, int domain, int F, int height, int width,
                             int num_steps, void* ets0, void* ets1, void* ets2, void* ets3, void* cur_sample,
                             int32_t* counter, void* stream) {
-  d4d::WindowStep s;
-  s.pndm = sched;
-  s.state = pndm_state(ets0, ets1, ets2, ets3, cur_sample);
-  s.state.lower_order_nums = s.state.lower_order_nums_out = counter;
-  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, s, guidance_scale,
-                        domain, F, 0, height, width, num_steps, stream);
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
+                        pndm_step(sched, ets0, ets1, ets2, ets3, cur_sample, counter), guidance_scale, domain, F, 0, height,
+                        width, num_steps, stream);
 }
 
 int d4d_denoise_window_deis(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
                             const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
                             const d4d_deis_sched* sched, float guidance_scale, int domain, int F, int height, int width,
                             int num_steps, void* m_prev, void* m_prev2, int32_t* lower_order_nums, void* stream) {
-  d4d::WindowStep s;
-  s.deis = sched;
-  s.state.m_prev = static_cast<bf16*>(m_prev); s.state.m_prev2 = static_cast<bf16*>(m_prev2);
-  s.state.lower_order_nums = s.state.lower_order_nums_out = lower_order_nums;
-  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, s, guidance_scale,
-                        domain, F, 0, height, width, num_steps, stream);
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
+                        deis_step(sched, m_prev, m_prev2, lower_order_nums), guidance_scale, domain, F, 0, height, width,
+                        num_steps, stream);
 }
 
 int d4d_denoise_window_dpm_single(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
@@ -272,13 +300,9 @@ int d4d_denoise_window_dpm_single(d4d_handle* h, void* latents, const void* pixe
                                   const d4d_dpm_single_sched* sched, float guidance_scale, int domain, int F, int height,
                                   int width, int num_steps, void* x0_prev, void* x0_prev2, void* cur_sample,
                                   int32_t* lower_order_nums, void* stream) {
-  d4d::WindowStep s;
-  s.dpm_single = sched;
-  s.state.x0_prev = static_cast<bf16*>(x0_prev); s.state.x0_prev2 = static_cast<bf16*>(x0_prev2);
-  s.state.cur_sample = static_cast<bf16*>(cur_sample);
-  s.state.lower_order_nums = s.state.lower_order_nums_out = lower_order_nums;
-  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, s, guidance_scale,
-                        domain, F, 0, height, width, num_steps, stream);
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
+                        dpm_single_step(sched, x0_prev, x0_prev2, cur_sample, lower_order_nums), guidance_scale, domain, F,
+                        0, height, width, num_steps, stream);
 }
 
 int d4d_assemble_input(void* latents, const void* pixel_latents, const void* plucker, const void* skel_latents,
@@ -658,6 +682,63 @@ int d4d_op_window_scatter(const void* latents, const int64_t* timestep_indices, 
   a.x0_prev = static_cast<const bf16*>(x0_prev); a.lower_order_nums = lower_order_nums;
   return d4d::window_scatter_run(a, dst_bytes, static_cast<cudaStream_t>(stream));
   D4D_API_END
+}
+
+int d4d_denoise_window_cfg_split(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                 const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                 const d4d_sched* sched, float guidance_scale, int domain, int F, int height, int width,
+                                 int num_steps, void* stream) {
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, ddim_step(sched),
+                        guidance_scale, domain, F, 0, height, width, num_steps, stream, true);
+}
+
+int d4d_denoise_window_dpm_cfg_split(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                     const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                     const d4d_dpm_sched* sched, float guidance_scale, int domain, int F, int height,
+                                     int width, int num_steps, void* x0_prev, int32_t* lower_order_nums, void* stream) {
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
+                        dpm_step(sched, x0_prev, lower_order_nums), guidance_scale, domain, F, 0, height, width, num_steps,
+                        stream, true);
+}
+
+int d4d_denoise_window_unipc_cfg_split(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                       const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                       const d4d_unipc_sched* sched, float guidance_scale, int domain, int F, int height,
+                                       int width, int num_steps, void* x0_prev, void* x0_prev2, void* last_sample,
+                                       int32_t* lower_order_nums, void* stream) {
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
+                        unipc_step(sched, x0_prev, x0_prev2, last_sample, lower_order_nums), guidance_scale, domain, F, 0,
+                        height, width, num_steps, stream, true);
+}
+
+int d4d_denoise_window_pndm_cfg_split(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                      const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                      const d4d_pndm_sched* sched, float guidance_scale, int domain, int F, int height,
+                                      int width, int num_steps, void* ets0, void* ets1, void* ets2, void* ets3,
+                                      void* cur_sample, int32_t* counter, void* stream) {
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
+                        pndm_step(sched, ets0, ets1, ets2, ets3, cur_sample, counter), guidance_scale, domain, F, 0, height,
+                        width, num_steps, stream, true);
+}
+
+int d4d_denoise_window_deis_cfg_split(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                      const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                      const d4d_deis_sched* sched, float guidance_scale, int domain, int F, int height,
+                                      int width, int num_steps, void* m_prev, void* m_prev2, int32_t* lower_order_nums,
+                                      void* stream) {
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
+                        deis_step(sched, m_prev, m_prev2, lower_order_nums), guidance_scale, domain, F, 0, height, width,
+                        num_steps, stream, true);
+}
+
+int d4d_denoise_window_dpm_single_cfg_split(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                            const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                            const d4d_dpm_single_sched* sched, float guidance_scale, int domain, int F,
+                                            int height, int width, int num_steps, void* x0_prev, void* x0_prev2,
+                                            void* cur_sample, int32_t* lower_order_nums, void* stream) {
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
+                        dpm_single_step(sched, x0_prev, x0_prev2, cur_sample, lower_order_nums), guidance_scale, domain, F,
+                        0, height, width, num_steps, stream, true);
 }
 
 int d4d_exchange_alloc(d4d_handle* h, size_t kv_bytes, unsigned char* handles_out) {

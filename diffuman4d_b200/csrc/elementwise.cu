@@ -83,15 +83,16 @@ __global__ void im2col_nhwc_kernel(const bf16* __restrict__ x, int n, int H, int
   *reinterpret_cast<uint4*>(out + (r * kk + tap) * C + o8 * 8) = v;
 }
 
-// [n*H*W, ld] (first C columns) -> NCHW [n, C, H, W]
-__global__ void nhwc_to_nchw_kernel(const bf16* __restrict__ x, int ld, int n, int C, int hw, bf16* __restrict__ out) {
+// [n*H*W, ld] (first C columns) -> NCHW [n, C, H, W] in destination out.p[blockIdx.y]
+// (__grid_constant__: the destination is indexed in parameter space, not from a local copy of the array)
+__global__ void nhwc_to_nchw_kernel(const bf16* __restrict__ x, int ld, int n, int C, int hw, const __grid_constant__ NchwDst out) {
   const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   const long long total = static_cast<long long>(n) * C * hw;
   if (idx >= total) return;
   const int p = static_cast<int>(idx % hw);
   const int c = static_cast<int>((idx / hw) % C);
   const int img = static_cast<int>(idx / (static_cast<long long>(hw) * C));
-  out[idx] = x[(static_cast<size_t>(img) * hw + p) * ld + c];
+  out.p[blockIdx.y][idx] = x[(static_cast<size_t>(img) * hw + p) * ld + c];
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -254,6 +255,11 @@ __global__ void assemble_kernel(const AssembleArgs a, int Cin) {
   const int f = blockIdx.y;
   const int hw = a.h * a.w;
   const bool is_cond = __bfloat162float(a.mask[static_cast<size_t>(f) * hw]) == 0.f;
+  // the rows of frame f's positive and negative images (-1: not written); the positive half is the LAST half when cfg
+  // (torch.cat([negative, positive]))
+  const bool whole = a.half < 0;
+  const int pos_img = whole ? (a.cfg ? a.F + f : f) : (a.half == 1 ? f : -1);
+  const int neg_img = whole ? (a.cfg ? f : -1) : (a.half == 0 ? f : -1);
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     long long t = 0;
     if (!is_cond) {
@@ -261,11 +267,12 @@ __global__ void assemble_kernel(const AssembleArgs a, int Cin) {
       idx = idx < 0 ? 0 : (idx >= a.n_steps ? a.n_steps - 1 : idx);
       t = a.timesteps_table[idx];
     }
-    a.timestep_out[f] = t;
-    if (a.cfg) a.timestep_out[a.F + f] = t;
+    if (pos_img >= 0) a.timestep_out[pos_img] = t;
+    if (neg_img >= 0) a.timestep_out[neg_img] = t;
   }
   const bf16 one = __float2bfloat16_rn(1.f), zero = __float2bfloat16_rn(0.f), mone = __float2bfloat16_rn(-1.f);
-  const int halves = a.cfg ? 2 : 1;
+  bf16* const pos = pos_img >= 0 ? a.sample + static_cast<size_t>(pos_img) * Cin * hw : nullptr;
+  bf16* const neg = neg_img >= 0 ? a.sample + static_cast<size_t>(neg_img) * Cin * hw : nullptr;
   for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < hw; p += gridDim.x * blockDim.x) {
     const bf16 m = a.mask[static_cast<size_t>(f) * hw + p];
     for (int c = 0; c < 4; ++c) {
@@ -275,38 +282,34 @@ __global__ void assemble_kernel(const AssembleArgs a, int Cin) {
         lat = a.pixel[li];
         a.latents[li] = lat;  // reference aliasing quirk: latents <- image latents at cond frames (PIPE:375-379)
       }
-      // positive half is the LAST half when cfg (torch.cat([negative, positive]))
-      const int pos_img = a.cfg ? a.F + f : f;
-      a.sample[(static_cast<size_t>(pos_img) * Cin + c) * hw + p] = lat;
-      if (a.cfg) a.sample[(static_cast<size_t>(f) * Cin + c) * hw + p] = is_cond ? one : lat;
+      if (pos) pos[static_cast<size_t>(c) * hw + p] = lat;
+      if (neg) neg[static_cast<size_t>(c) * hw + p] = is_cond ? one : lat;
     }
     int ch = 4;
     for (int c = 0; c < 6; ++c, ++ch) {
-      const bf16 v = a.plucker[(static_cast<size_t>(f) * 6 + c) * hw + p];
-      const int pos_img = a.cfg ? a.F + f : f;
-      a.sample[(static_cast<size_t>(pos_img) * Cin + ch) * hw + p] = v;
-      if (a.cfg) a.sample[(static_cast<size_t>(f) * Cin + ch) * hw + p] = zero;
+      if (pos) pos[static_cast<size_t>(ch) * hw + p] = a.plucker[(static_cast<size_t>(f) * 6 + c) * hw + p];
+      if (neg) neg[static_cast<size_t>(ch) * hw + p] = zero;
     }
     if (a.skel_latents) {
       for (int c = 0; c < 4; ++c, ++ch) {
-        const bf16 v = a.skel_latents[(static_cast<size_t>(f) * 4 + c) * hw + p];
-        const int pos_img = a.cfg ? a.F + f : f;
-        a.sample[(static_cast<size_t>(pos_img) * Cin + ch) * hw + p] = v;
-        if (a.cfg) a.sample[(static_cast<size_t>(f) * Cin + ch) * hw + p] = mone;
+        if (pos) pos[static_cast<size_t>(ch) * hw + p] = a.skel_latents[(static_cast<size_t>(f) * 4 + c) * hw + p];
+        if (neg) neg[static_cast<size_t>(ch) * hw + p] = mone;
       }
     }
-    for (int hf = 0; hf < halves; ++hf)
-      a.sample[(static_cast<size_t>(hf * a.F + f) * Cin + ch) * hw + p] = m;
+    if (pos) pos[static_cast<size_t>(ch) * hw + p] = m;
+    if (neg) neg[static_cast<size_t>(ch) * hw + p] = m;
   }
 }
 
-// images 0..F-1 <- small image 0 ; images F..2F-1 <- small images 1..F   (per_img elements each, multiple of 8)
-__global__ void broadcast_neg_images_kernel(const bf16* __restrict__ small, long long per_img8, int F, bf16* __restrict__ full) {
-  const long long total = per_img8 * 2 * F;
+// images 0..n_neg-1 <- small image 0 ; images n_neg..n_neg+n_pos-1 <- small images 1..n_pos   (per_img elements each,
+// multiple of 8)
+__global__ void broadcast_neg_images_kernel(const bf16* __restrict__ small, long long per_img8, int n_neg, int n_pos,
+                                            bf16* __restrict__ full) {
+  const long long total = per_img8 * (n_neg + n_pos);
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const long long img = i / per_img8, off = i - img * per_img8;
-    const long long src = img < F ? 0 : img - F + 1;
+    const long long src = img < n_neg ? 0 : img - n_neg + 1;
     reinterpret_cast<uint4*>(full)[i] = __ldg(reinterpret_cast<const uint4*>(small) + src * per_img8 + off);
   }
 }
@@ -708,8 +711,16 @@ int im2col_nhwc_run(const bf16* x, int n, int H, int W, int C, int ksize, int st
 }
 
 int nhwc_to_nchw_run(const bf16* x, int ld, int n, int C, int hw, bf16* out, cudaStream_t stream) {
+  NchwDst d = {};
+  d.p[0] = out;
+  d.n = 1;
+  return nhwc_to_nchw_run(x, ld, n, C, hw, d, stream);
+}
+int nhwc_to_nchw_run(const bf16* x, int ld, int n, int C, int hw, const NchwDst& out, cudaStream_t stream) {
+  D4D_REQUIRE(out.n >= 1 && out.n <= 8, "nhwc_to_nchw: 1 to 8 destinations");
+  for (int i = 0; i < out.n; ++i) D4D_REQUIRE(out.p[i] != nullptr, "nhwc_to_nchw: null destination");
   const long long total = static_cast<long long>(n) * C * hw;
-  nhwc_to_nchw_kernel<<<blocks_for(total, 256), 256, 0, stream>>>(x, ld, n, C, hw, out);
+  nhwc_to_nchw_kernel<<<dim3(blocks_for(total, 256), out.n), 256, 0, stream>>>(x, ld, n, C, hw, out);
   D4D_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -802,9 +813,9 @@ int assemble_input_run(const AssembleArgs& a, cudaStream_t stream) {
   return 0;
 }
 
-int broadcast_neg_images_run(const bf16* small, long long per_img, int F, bf16* full, cudaStream_t stream) {
-  D4D_REQUIRE(per_img % 8 == 0 && F > 0, "broadcast_neg_images arguments");
-  broadcast_neg_images_kernel<<<132 * 8, 256, 0, stream>>>(small, per_img / 8, F, full);
+int broadcast_neg_images_run(const bf16* small, long long per_img, int n_neg, int n_pos, bf16* full, cudaStream_t stream) {
+  D4D_REQUIRE(per_img % 8 == 0 && n_neg > 0 && n_pos >= 0, "broadcast_neg_images arguments");
+  broadcast_neg_images_kernel<<<132 * 8, 256, 0, stream>>>(small, per_img / 8, n_neg, n_pos, full);
   D4D_CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -170,6 +170,13 @@ int silu_run(const bf16* x, long long n, bf16* out, cudaStream_t stream);
 int im2col_nchw_run(const bf16* x, int n, int Cin, int H, int W, int cin_pad, int KP, bf16* out, cudaStream_t stream);
 // [n*hw, ld] (first C columns) -> NCHW [n, C, hw]
 int nhwc_to_nchw_run(const bf16* x, int ld, int n, int C, int hw, bf16* out, cudaStream_t stream);
+// the same permute storing the same NCHW tensor into every p[i], i < n (the CFG-split window stores its half of the noise
+// into every rank's exchange buffer, peer memory mapped with cudaIpc, like the K/V scatter epilogue)
+struct NchwDst {
+  bf16* p[8];
+  int n;
+};
+int nhwc_to_nchw_run(const bf16* x, int ld, int n, int C, int hw, const NchwDst& out, cudaStream_t stream);
 // pose encoder layer 0: NCHW [n,3,H,W] -> NHWC [n,H,W,4] (channel 3 = 0), 3x3 pad 1 + SiLU; w [9][3][3] (tap, cin, cout)
 int pose_conv0_run(const bf16* x_nchw, int n, int H, int W, const bf16* w, const float* bias, bf16* out_nhwc4,
                    cudaStream_t stream);
@@ -178,14 +185,18 @@ int pose_conv_run(const bf16* x, int n, int Cin, int H, int W, const bf16* w, co
                   int stride, bf16* out_nhwc, cudaStream_t stream);
 // generic NHWC im2col, pad 1: [n,H,W,C] -> [n*Ho*Wo, k*k*C]
 int im2col_nhwc_run(const bf16* x, int n, int H, int W, int C, int ksize, int stride, bf16* out, cudaStream_t stream);
-// [1 + F images of per_img elements] -> [2F images]: images 0..F-1 <- small image 0, images F..2F-1 <- small images 1..F
-// (per_img % 8 == 0)
-int broadcast_neg_images_run(const bf16* small, long long per_img, int F, bf16* full, cudaStream_t stream);
+// [1 + n_pos images of per_img elements] -> [n_neg + n_pos images]: images 0..n_neg-1 <- small image 0, images
+// n_neg..n_neg+n_pos-1 <- small images 1..n_pos (per_img % 8 == 0)
+int broadcast_neg_images_run(const bf16* small, long long per_img, int n_neg, int n_pos, bf16* full, cudaStream_t stream);
 // p[0 .. n) = v
 int fill_bf16_run(bf16* p, long long n, float v, cudaStream_t stream);
 
 // a-1 input assembly (pipeline_diffuman4d.py:373-395), writes NCHW [2F or F, Cin, h, w] + timesteps
 struct AssembleArgs {
+  // -1: the whole batch, (cfg ? 2 : 1) * F images; 0 / 1: only CFG half k's F images (0 negative, 1 positive) at rows
+  // [0, F), the rows the whole batch has at [k*F, (k+1)*F) (cfg is then not read).  Every mode overwrites the cond frames'
+  // latents in place alike.
+  int half = -1;
   bf16* latents;            // [F,4,h,w]  (cond frames are overwritten in place like the reference)
   const bf16* pixel;        // [F,4,h,w]
   const bf16* plucker;      // [F,6,h,w]
@@ -195,8 +206,8 @@ struct AssembleArgs {
   const long long* timesteps_table;   // [n_steps] (device)
   int n_steps;
   int F, h, w, cfg;
-  bf16* sample;             // out [(cfg?2:1)*F, Cin, h, w]
-  long long* timestep_out;  // out [(cfg?2:1)*F]
+  bf16* sample;             // out [(cfg?2:1)*F, Cin, h, w]; [F, Cin, h, w] for one half
+  long long* timestep_out;  // out [(cfg?2:1)*F]; [F] for one half
 };
 int assemble_input_run(const AssembleArgs& a, cudaStream_t stream);
 

@@ -62,7 +62,14 @@ std::string plan_key(const PlanShape& s) {
   std::string k = std::to_string(s.B) + "_" + std::to_string(s.F) + "_" + std::to_string(s.h) + "_" + std::to_string(s.w) + "_";
   for (int d : s.domains) k += d ? 't' : 's';
   if (s.F_total > 0) k += "_sh" + std::to_string(s.F_total);
-  return s.pose_shared_neg ? k + "_pn" : k;
+  return s.pose_neg > 0 ? k + "_pn" + std::to_string(s.pose_neg) : k;
+}
+
+NchwDst one_dst(bf16* out) {
+  NchwDst d = {};
+  d.p[0] = out;
+  d.n = out ? 1 : 0;
+  return d;
 }
 
 }  // namespace
@@ -828,10 +835,10 @@ class PlanBuilder {
     bf16* pose_emb = nullptr;
     if (cfg.enable_pose_encoder) {
       const int Hs = 8 * h, Ws = 8 * w;
-      // pose_shared_neg: the skeleton batch is [1 constant CFG-negative image | F positive images] instead of 2F images
+      // pose_neg: the skeleton batch is [1 constant CFG-negative image | B - pose_neg positive images] instead of B images
       // (pipeline_diffuman4d.py:349-356 makes every negative skeleton the same all(-1) image); its embedding is computed
-      // once per forward and broadcast to the F negative images below
-      const int PB = sh.pose_shared_neg ? F + 1 : B;
+      // once per forward and broadcast to the pose_neg negative images below
+      const int PB = sh.pose_neg > 0 ? B - sh.pose_neg + 1 : B;
       const int PM0 = PB * h * w;
       const PoseW& pw = m.pose_;
       bf16* a0 = alloc(static_cast<size_t>(PB) * Hs * Ws * 4);  // 3 channels padded to 4
@@ -870,11 +877,12 @@ class PlanBuilder {
         gemm(d);
       }
       release(x7.p);
-      if (sh.pose_shared_neg) {  // broadcast: images 0..F-1 <- embedding 0, images F..2F-1 <- embeddings 1..F
+      if (sh.pose_neg > 0) {  // broadcast: images 0..pose_neg-1 <- embedding 0, the rest <- embeddings 1..B-pose_neg
         bf16* full = alloc(static_cast<size_t>(M0) * C0);
         bf16* small = pose_emb;
         const long long per_img = static_cast<long long>(h) * w * C0;
-        op([=](cudaStream_t s) { return broadcast_neg_images_run(small, per_img, F, full, s); });
+        const int n_neg = sh.pose_neg, n_pos = B - sh.pose_neg;
+        op([=](cudaStream_t s) { return broadcast_neg_images_run(small, per_img, n_neg, n_pos, full, s); });
         release(small);
         pose_emb = full;
       }
@@ -1003,7 +1011,7 @@ Plan* Model::find_plan(int n_domains, int B, int F, int h, int w) {
   return nullptr;
 }
 
-int Model::get_plan(const int* domain_ids, int n_domains, int B, int F, int h, int w, Plan** out, int F_total, bool pose_shared_neg) {
+int Model::get_plan(const int* domain_ids, int n_domains, int B, int F, int h, int w, Plan** out, int F_total, int pose_neg) {
   if (!finalized_) {
     set_error("weights not finalized (call d4d_finalize_weights)");
     return 3;
@@ -1027,7 +1035,8 @@ int Model::get_plan(const int* domain_ids, int n_domains, int B, int F, int h, i
   s.n_domains = n_domains; s.B = B; s.F = F; s.h = h; s.w = w;
   s.domains.assign(domain_ids, domain_ids + n_domains);
   if (sharded) { s.F_total = F_total; s.rank = xch_.rank; s.world = xch_.world; }
-  s.pose_shared_neg = pose_shared_neg && cfg_.enable_pose_encoder && n_domains == 2;
+  D4D_REQUIRE(pose_neg >= 0 && pose_neg <= B, "pose_neg must be in [0, B]");
+  s.pose_neg = cfg_.enable_pose_encoder ? pose_neg : 0;
   const std::string key = plan_key(s);
   auto it = plans_.find(key);
   if (it != plans_.end()) {
@@ -1056,9 +1065,9 @@ int Model::get_plan(const int* domain_ids, int n_domains, int B, int F, int h, i
   return 0;
 }
 
-int Model::run_ops(Plan& p, const bf16* sample, const long long* timestep, const bf16* skeletons, bf16* out, size_t n,
+int Model::run_ops(Plan& p, const bf16* sample, const long long* timestep, const bf16* skeletons, const NchwDst& out, size_t n,
                    cudaStream_t stream, bool timed) {
-  D4D_REQUIRE(sample && timestep && (out || n < p.ops.size()), "null argument");
+  D4D_REQUIRE(sample && timestep && (out.n > 0 || n < p.ops.size()), "null argument");
   D4D_REQUIRE(!cfg_.enable_pose_encoder || skeletons != nullptr, "skeletons are required when enable_pose_encoder");
   D4D_REQUIRE(!cfg_.center_input_sample, "center_input_sample is not supported");
   D4D_CUDA_OK(cudaSetDevice(device_));
@@ -1078,9 +1087,15 @@ int Model::run_ops(Plan& p, const bf16* sample, const long long* timestep, const
 }
 
 int Model::forward(const bf16* sample, const long long* timestep, const bf16* skeletons, const int* domain_ids,
-                   int n_domains, int B, int F, int h, int w, bf16* out, cudaStream_t stream, int F_total, bool pose_shared_neg) {
+                   int n_domains, int B, int F, int h, int w, bf16* out, cudaStream_t stream, int F_total, int pose_neg) {
+  return forward(sample, timestep, skeletons, domain_ids, n_domains, B, F, h, w, one_dst(out), stream, F_total, pose_neg);
+}
+
+int Model::forward(const bf16* sample, const long long* timestep, const bf16* skeletons, const int* domain_ids,
+                   int n_domains, int B, int F, int h, int w, const NchwDst& out, cudaStream_t stream, int F_total,
+                   int pose_neg) {
   Plan* p = nullptr;
-  if (int rc = get_plan(domain_ids, n_domains, B, F, h, w, &p, F_total, pose_shared_neg)) return rc;
+  if (int rc = get_plan(domain_ids, n_domains, B, F, h, w, &p, F_total, pose_neg)) return rc;
   if (int rc = run_ops(*p, sample, timestep, skeletons, out, p->ops.size(), stream)) return rc;
   xch_.epoch_base += static_cast<unsigned int>(p->n3d);
   return 0;
@@ -1101,7 +1116,7 @@ int Model::debug_tap(const bf16* sample, const long long* timestep, const bf16* 
   }
   if (dims3) { dims3[0] = t.C; dims3[1] = t.H; dims3[2] = t.W; }
   if (!out) return 0;
-  if (int rc = run_ops(*p, sample, timestep, skeletons, nullptr, t.n_ops, stream)) return rc;
+  if (int rc = run_ops(*p, sample, timestep, skeletons, one_dst(nullptr), t.n_ops, stream)) return rc;
   return nhwc_to_nchw_run(t.p, t.C, B, t.C, t.H * t.W, out, stream);
 }
 
@@ -1164,7 +1179,7 @@ int Model::profile(const bf16* sample, const long long* timestep, const bf16* sk
   Plan* p = nullptr;
   if (int rc = get_plan(domain_ids, n_domains, B, F, h, w, &p)) return rc;
   const size_t n = p->ops.size();
-  if (int rc = run_ops(*p, sample, timestep, skeletons, out, n, stream, true)) return rc;
+  if (int rc = run_ops(*p, sample, timestep, skeletons, one_dst(out), n, stream, true)) return rc;
   D4D_CUDA_OK(cudaEventSynchronize(p->events[n]));
   for (int k = 0; k < kNumOpKinds; ++k) { ms_by_kind[k] = 0.f; launches_by_kind[k] = 0; flops_by_kind[k] = 0.0; }
   for (size_t i = 0; i < n; ++i) {
@@ -1180,15 +1195,24 @@ int Model::profile(const bf16* sample, const long long* timestep, const bf16* sk
 
 int Model::denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
                           long long* ts_idx, const WindowStep& step, float guidance, int domain, int F, int h, int w,
-                          int num_steps, cudaStream_t stream, int F_total) {
+                          int num_steps, cudaStream_t stream, int F_total, bool cfg_split) {
   D4D_REQUIRE(latents && pixel && plucker && mask && ts_idx && step.tables() == 1, "null argument");
   D4D_REQUIRE(domain == 0 || domain == 1, "Invalid domain");
   const bool cfg_on = guidance > 1.0f;
+  const bool split = cfg_split && cfg_on;  // guidance <= 1 has no halves: the plain step runs and nothing is exchanged
   const int B = cfg_on ? 2 * F : F;
   const bool pose = cfg_.enable_pose_encoder != 0;
   const int Cin = 4 + 6 + (pose ? 0 : 4) + 1;
+  const int Co = cfg_.out_channels;
   D4D_REQUIRE(Cin == cfg_.in_channels, "in_channels does not match the latent/plucker/skeleton/mask channel layout");
   D4D_REQUIRE(skeletons != nullptr, "skeletons required");
+  if (split) {
+    D4D_REQUIRE(xch_.ready, "the CFG-split window needs d4d_exchange_open first");
+    D4D_REQUIRE(xch_.world <= 2, "the CFG-split window runs on 1 (loopback) or 2 ranks");
+    D4D_REQUIRE(F > 0 && h > 0 && w > 0, "empty window");
+    D4D_REQUIRE(2ull * F * Co * h * w * sizeof(bf16) <= xch_.kv_bytes,
+                "the window's noise (2 * F * out_channels * h * w bf16) does not fit the exchange buffer (d4d_exchange_alloc)");
+  }
   D4D_CUDA_OK(cudaSetDevice(device_));
   const std::string key = std::to_string(B) + "_" + std::to_string(F) + "_" + std::to_string(h) + "_" + std::to_string(w);
   auto it = wbufs_.find(key);
@@ -1201,7 +1225,7 @@ int Model::denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker,
       D4D_CUDA_OK(cudaMalloc(&wb->skel, sizeof(bf16) * (F + 1) * 3 * 64 * hw));
       if (int rc = fill_bf16_run(wb->skel, static_cast<long long>(3) * 64 * hw, -1.0f, stream)) return rc;  // constant negative image
     }
-    D4D_CUDA_OK(cudaMalloc(&wb->noise, sizeof(bf16) * B * cfg_.out_channels * hw));
+    D4D_CUDA_OK(cudaMalloc(&wb->noise, sizeof(bf16) * B * Co * hw));
     D4D_CUDA_OK(cudaMalloc(&wb->ts_tmp, sizeof(long long) * F));
     it = wbufs_.emplace(key, std::move(wb)).first;
   }
@@ -1233,18 +1257,42 @@ int Model::denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker,
     a.timestep_indices = ts_idx; a.timesteps_table = reinterpret_cast<const long long*>(timesteps_table);
     a.n_steps = n_steps; a.F = F; a.h = h; a.w = w; a.cfg = cfg_on ? 1 : 0;
     a.sample = wb.sample; a.timestep_out = wb.timestep;
-    if (int rc = assemble_input_run(a, stream)) return rc;
-    const bf16* skel_in = nullptr;
-    if (pose) {
-      if (cfg_on) {  // [negative (filled once) | F positive images]
-        D4D_CUDA_OK(cudaMemcpyAsync(wb.skel + static_cast<size_t>(3) * 64 * hw, skeletons, sizeof(bf16) * F * 3 * 64 * hw,
-                                    cudaMemcpyDeviceToDevice, stream));
-        skel_in = wb.skel;
-      } else {
-        skel_in = skeletons;
+    if (split) {
+      // CFG split (DESIGN.md section 7): the UNet on this rank's half k (a loopback runs both), its noise stored at rows
+      // [k*F, (k+1)*F) of exchange e's buffer parity on every rank; one flag round; the step reads the gathered [2F] noise
+      // in place.  Every rank then computes the step from the same bits.
+      const unsigned int e = xch_.epoch_base;
+      const int k0 = xch_.world == 1 ? 0 : xch_.rank, k1 = xch_.world == 1 ? 2 : xch_.rank + 1;
+      for (int k = k0; k < k1; ++k) {
+        a.half = k;
+        if (int rc = assemble_input_run(a, stream)) return rc;
+        NchwDst dst = {};
+        dst.n = xch_.world;
+        for (int r = 0; r < xch_.world; ++r)
+          dst.p[r] = static_cast<bf16*>(xch_.peer_kv[e & 1][r]) + static_cast<size_t>(k) * F * Co * hw;
+        // every negative skeleton is the constant image wb.skel[0]: the negative half encodes it once (pose_neg = F)
+        const bf16* skel_in = pose ? (k == 0 ? wb.skel : skeletons) : nullptr;
+        if (int rc = forward(wb.sample, wb.timestep, skel_in, doms, 1, F, F, h, w, dst, stream, 0, pose && k == 0 ? F : 0))
+          return rc;
       }
+      if (int rc = flag_round(stream)) return rc;
+      sa.noise = static_cast<const bf16*>(xch_.kv[e & 1]);
+    } else {
+      if (int rc = assemble_input_run(a, stream)) return rc;
+      const bf16* skel_in = nullptr;
+      if (pose) {
+        if (cfg_on) {  // [negative (filled once) | F positive images]
+          D4D_CUDA_OK(cudaMemcpyAsync(wb.skel + static_cast<size_t>(3) * 64 * hw, skeletons, sizeof(bf16) * F * 3 * 64 * hw,
+                                      cudaMemcpyDeviceToDevice, stream));
+          skel_in = wb.skel;
+        } else {
+          skel_in = skeletons;
+        }
+      }
+      if (int rc = forward(wb.sample, wb.timestep, skel_in, doms, cfg_on ? 2 : 1, B, F, h, w, wb.noise, stream, F_total,
+                           pose && cfg_on ? F : 0))
+        return rc;
     }
-    if (int rc = forward(wb.sample, wb.timestep, skel_in, doms, cfg_on ? 2 : 1, B, F, h, w, wb.noise, stream, F_total, pose && cfg_on)) return rc;
     if (int rc = step.with_table([&](const auto& s) { return cfg_step_run(sa, s, state, stream); })) return rc;
     D4D_CUDA_OK(cudaMemcpyAsync(ts_idx, wb.ts_tmp, sizeof(long long) * F, cudaMemcpyDeviceToDevice, stream));
     if (multistep)
@@ -1252,6 +1300,18 @@ int Model::denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker,
                                   stream));
   }
   return 0;
+}
+
+// One flag round, closing exchange e = epoch_base (the caller enqueued its stores into buffer parity e & 1 before it):
+// every rank's flag slot e & 1 receives epoch e + 1, the exchange is counted, and the stream waits for every rank's signal.
+int Model::flag_round(cudaStream_t stream) {
+  const unsigned int counter = xch_.epoch_base;
+  KvFlagArgs f;
+  for (int r = 0; r < 8; ++r) f.flags[r] = r < xch_.world ? xch_.peer_flags[r] : nullptr;
+  f.rank = xch_.rank; f.world = xch_.world; f.epoch = counter + 1; f.slot = counter & 1;
+  xch_.epoch_base += 1;  // the stores are enqueued: every rank counts this exchange, whatever happens below
+  if (int rc = kv_signal_run(f, stream)) return rc;
+  return kv_wait_run(f, stream);
 }
 
 // One more exchange of the global epoch sequence (DESIGN.md section 7): counter e = epoch_base stores into parity e & 1 of
@@ -1276,12 +1336,7 @@ int Model::window_exchange(const bf16* latents, const long long* ts_idx, const b
   a.chw = 4ll * h * w;
   a.latents = latents; a.ts = ts_idx; a.x0_prev = x0_prev; a.lower_order_nums = lower_order_nums;
   if (int rc = window_scatter_run(a, xch_.kv_bytes, stream)) return rc;
-  KvFlagArgs f;
-  for (int r = 0; r < 8; ++r) f.flags[r] = r < xch_.world ? xch_.peer_flags[r] : nullptr;
-  f.rank = xch_.rank; f.world = xch_.world; f.epoch = counter + 1; f.slot = par;
-  xch_.epoch_base += 1;  // the stores are enqueued: every rank counts this exchange, whatever happens below
-  if (int rc = kv_signal_run(f, stream)) return rc;
-  if (int rc = kv_wait_run(f, stream)) return rc;
+  if (int rc = flag_round(stream)) return rc;
   const char* g = static_cast<const char*>(xch_.kv[par]);
   const WindowResultLayout L = window_result_layout(F_total, a.chw, dpm);
   D4D_CUDA_OK(cudaMemcpyAsync(latents_out, g, L.x0, cudaMemcpyDeviceToDevice, stream));

@@ -65,7 +65,10 @@ struct PlanShape {
   std::vector<int> domains;
   // frame-sharded window (DESIGN.md section 7): this rank owns F of F_total frames per CFG half
   int F_total = 0, rank = 0, world = 1;
-  bool pose_shared_neg = false;  // skeleton batch = [1 CFG-negative image | F positive images] (window step)
+  // the first pose_neg images of the batch are CFG-negative, whose skeletons are all one constant image: the skeleton
+  // batch is [1 negative image | B - pose_neg positive images], encoded once and broadcast (window step: F of 2F, or
+  // the whole batch on the negative rank of the CFG-split window)
+  int pose_neg = 0;
 };
 
 struct Plan {
@@ -87,7 +90,7 @@ struct Plan {
   const bf16* sample = nullptr;
   const long long* timestep = nullptr;
   const bf16* skeletons = nullptr;
-  bf16* out = nullptr;
+  NchwDst out = {};
   ~Plan();
 };
 
@@ -145,14 +148,19 @@ class Model {
   // F_total > F: frame-sharded window (needs exchange_open); B, F are the LOCAL batch / frames
   int forward(const bf16* sample, const long long* timestep, const bf16* skeletons, const int* domain_ids,
               int n_domains, int B, int F, int h, int w, bf16* out, cudaStream_t stream, int F_total = 0,
-              bool pose_shared_neg = false);
+              int pose_neg = 0);
+  // the same forward, its output stored into every out.p[i]
+  int forward(const bf16* sample, const long long* timestep, const bf16* skeletons, const int* domain_ids,
+              int n_domains, int B, int F, int h, int w, const NchwDst& out, cudaStream_t stream, int F_total,
+              int pose_neg);
   int exchange_alloc(size_t kv_bytes, unsigned char* handles_out /* 3 x 64 bytes */);
   int exchange_open(int rank, int world, const unsigned char* all_handles /* world x 3 x 64 bytes */);
   // num_steps x (assemble -> UNet -> CFG + scheduler step) on the window's F frames; latents, ts_idx and the solver state
-  // of `step` are updated in place.
+  // of `step` are updated in place.  cfg_split (guidance > 1, needs exchange_open with world 1 or 2): this rank runs the
+  // UNet on its CFG half only and the halves meet in the exchange buffers (DESIGN.md section 7).
   int denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
                      long long* ts_idx, const WindowStep& step, float guidance, int domain, int F, int h, int w,
-                     int num_steps, cudaStream_t stream, int F_total);
+                     int num_steps, cudaStream_t stream, int F_total, bool cfg_split = false);
   // frame-sharded sliding loop: this rank's F updated frames (+ DPM-Solver++ state when x0_prev != nullptr) to every rank,
   // one flag round (one more exchange of the epoch sequence), then the gathered F_total frames to the *_out buffers
   int window_exchange(const bf16* latents, const long long* ts_idx, const bf16* x0_prev, const int* lower_order_nums, int F,
@@ -163,7 +171,7 @@ class Model {
               int B, int F, int h, int w, bf16* out, cudaStream_t stream, float* ms_by_kind, int* launches_by_kind,
               double* flops_by_kind);
   int get_plan(const int* domain_ids, int n_domains, int B, int F, int h, int w, Plan** out, int F_total = 0,
-               bool pose_shared_neg = false);
+               int pose_neg = 0);
   // debug: run the forward up to tap `tap` and copy that activation out as NCHW bf16 [B, C, H, W]; out == nullptr only
   // reports name / dims.  Returns 1 when tap is out of range.
   int debug_tap(const bf16* sample, const long long* timestep, const bf16* skeletons, const int* domain_ids, int n_domains,
@@ -200,8 +208,10 @@ class Model {
   void need(const std::string& key, std::vector<int64_t> shape);
   // checks and binds the per-call externals of p, then enqueues ops[0 .. n); timed: events[i] is recorded before op i and
   // events[n] after the last
-  int run_ops(Plan& p, const bf16* sample, const long long* timestep, const bf16* skeletons, bf16* out, size_t n,
+  int run_ops(Plan& p, const bf16* sample, const long long* timestep, const bf16* skeletons, const NchwDst& out, size_t n,
               cudaStream_t stream, bool timed = false);
+  // closes exchange epoch_base: signal it to every rank, count it, wait for every rank's signal
+  int flag_round(cudaStream_t stream);
   int cin_pad() const { return 16; }
   int kp_in() const { return 192; }
 };

@@ -135,10 +135,11 @@ class B200Diffuman4DPipeline:
     def _window_step(self, *, latents, pixel_values_latents, plucker_embeds_latents, skeletons_latents,
                      cond_masks_latents, timestep_indices, domain: str, guidance_scale: float,
                      num_inference_steps: int = 1, solver_state: Optional[SolverState] = None,
-                     F_total: Optional[int] = None):
+                     F_total: Optional[int] = None, cfg_split: bool = False):
         """``denoise_window``'s checks and library call.  ``F_total`` given: the tensors hold this rank's frames of a
-        frame-sharded window of ``F_total`` frames (``FrameShardedPipeline.denoise_window``)."""
-        name = self.scheduler.window_entry_points[F_total is not None]
+        frame-sharded window of ``F_total`` frames (``FrameShardedPipeline.denoise_window``).  ``cfg_split``: the whole
+        window, with this rank running the UNet on its CFG half (``CFGSplitPipeline.denoise_window``)."""
+        name = self.scheduler.window_entry_points[2 if cfg_split else F_total is not None]
         if name is None:
             raise NotImplementedError(f"the frame-sharded window does not run the {self.scheduler.name} scheduler")
         if domain not in _DOMAIN_IDS:

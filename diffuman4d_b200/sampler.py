@@ -16,7 +16,8 @@ Multi-GPU (one process per GPU, SURVEY 8e row 1): the tasks of a round are indep
 (src/samplers/sampling_runner.py:26-43).  Pinned against the reference sampler run end to end on stubs
 (tests/golden/gen_golden.py::gen_sampler -> tests/test_sampler.py).  Alternatively (``execute_tasks(frame_sharded=True)``
 with a ``sharded.FrameShardedPipeline``) every rank runs every task with each window split over the ranks by frames, which
-keeps all GPUs busy when a round has fewer tasks than GPUs (DESIGN.md section 7).
+keeps all GPUs busy when a round has fewer tasks than GPUs (DESIGN.md section 7); ``execute_tasks(cfg_split=True)`` with a
+``cfg_split.CFGSplitPipeline`` does the same with each window step split by CFG half over two ranks.
 
 The dataset object supplies ``scene_label`` and ``get_item(scene_label, spa_labels, tem_labels, input_spa_labels)`` exactly
 like the reference's ``SpaTemDataset`` (src/data/spatem_dataset.py:76-212); pipelines supply
@@ -230,20 +231,29 @@ class B200SlidingIterativeSampler:
             self.save_fn(sample, self.output_dir)
         return sample
 
-    def execute_tasks(self, rank: int = 0, world: int = 1, group=None, pipe_idx: int = 0, frame_sharded: bool = False):
+    def execute_tasks(self, rank: int = 0, world: int = 1, group=None, pipe_idx: int = 0, frame_sharded: bool = False,
+                      cfg_split: bool = False):
         """All rounds.  ``world > 1`` (inside an initialised ``torch.distributed`` job): this rank runs its share of every
         round, then the ranks all-gather the cells they updated (the round barrier of RUN:53-55).
 
         ``frame_sharded=True``: ``pipelines[pipe_idx]`` is a ``FrameShardedPipeline`` and every rank of its process group
         runs every task, each window split over the ranks by frames.  Every rank's grid ends up identical, so there is no
         per-round exchange; ``rank`` / ``world`` / ``group`` are not used (the pipeline's group defines the ranks), and
-        ``save_fn`` runs on the pipeline's rank 0 only."""
+        ``save_fn`` runs on the pipeline's rank 0 only.
+
+        ``cfg_split=True``: the same, with a ``cfg_split.CFGSplitPipeline`` whose ranks each run one CFG half of every
+        window step."""
         save_fn = self.save_fn
-        if frame_sharded:
+        if frame_sharded and cfg_split:
+            raise ValueError("frame_sharded and cfg_split are two different multi-GPU modes; pass one of them")
+        if frame_sharded or cfg_split:
+            from .cfg_split import CFGSplitPipeline
             from .sharded import FrameShardedPipeline
             pipe = self.pipelines[pipe_idx]
-            if not isinstance(pipe, FrameShardedPipeline):
-                raise ValueError("frame_sharded=True needs a FrameShardedPipeline in pipelines[pipe_idx]")
+            cls = FrameShardedPipeline if frame_sharded else CFGSplitPipeline
+            if not isinstance(pipe, cls):
+                raise ValueError(f"{'frame_sharded' if frame_sharded else 'cfg_split'}=True needs a {cls.__name__} in "
+                                 "pipelines[pipe_idx]")
             rank, world, save_fn = 0, 1, (save_fn if pipe.rank == 0 else None)
         saver = _AsyncSaver(save_fn, self.output_dir) if (self.async_save and save_fn is not None) else None
         try:

@@ -18,8 +18,8 @@ epsilon form.  ``DPMSingleTables`` / ``DPMSingleState`` do the same for ``DPMSol
 (``cfg_dpm_single_kernel``, up to third order), whose history is the last two data predictions and the sample the frame's
 current block started from.
 
-Each tables class names the C entry points of its window step (``window_entry_points``: plain and frame-sharded, None
-where there is none) and the bf16 state planes they take, in ABI order (``state_planes``; None for the stateless DDIM).
+Each tables class names the C entry points of its window step (``window_entry_points``: plain, frame-sharded and
+CFG-split, None where there is none) and the bf16 state planes they take, in ABI order (``state_planes``; None for the stateless DDIM).
 """
 from __future__ import annotations
 
@@ -37,7 +37,7 @@ _PRED = {"epsilon": 0, "v_prediction": 1, "sample": 2}
 
 class DDIMTables:
     init_noise_sigma = 1.0  # DDIM: scale_model_input is the identity, init sigma 1 (reference PIPE:189,376)
-    window_entry_points = ("d4d_denoise_window", "d4d_denoise_window_sharded")
+    window_entry_points = ("d4d_denoise_window", "d4d_denoise_window_sharded", "d4d_denoise_window_cfg_split")
     state_planes = None     # stateless: one table serves every frame
 
     def __init__(self, cfg: SchedulerConfig = None, device="cuda:0"):
@@ -210,7 +210,8 @@ class DPMSolverTables(_MultistepTables):
     """Timesteps, sigmas and step coefficients of ``DPMSolverMultistepScheduler`` (diffusers 0.33.1) for
     ``cfg_dpm_kernel``."""
     name = "DPM-Solver++"
-    window_entry_points = ("d4d_denoise_window_dpm", "d4d_denoise_window_dpm_sharded")
+    window_entry_points = ("d4d_denoise_window_dpm", "d4d_denoise_window_dpm_sharded",
+                          "d4d_denoise_window_dpm_cfg_split")
     state_planes = ("x0_prev",)
     _struct = D4DDpmSched
 
@@ -356,7 +357,7 @@ class UniPCTables(_MultistepTables):
     ``cfg_unipc_kernel``."""
     name = "UniPC"
     # no frame-sharded window: its window-result exchange carries DPM-Solver++'s state only
-    window_entry_points = ("d4d_denoise_window_unipc", None)
+    window_entry_points = ("d4d_denoise_window_unipc", None, "d4d_denoise_window_unipc_cfg_split")
     _struct = D4DUniPCSched
 
     def __init__(self, cfg: UniPCConfig = None, device="cuda:0"):
@@ -450,7 +451,7 @@ class PNDMTables:
     name = "PNDM"
     init_noise_sigma = 1.0  # upstream: init_noise_sigma 1, scale_model_input is the identity
     # no frame-sharded window: its window-result exchange carries DPM-Solver++'s state only
-    window_entry_points = ("d4d_denoise_window_pndm", None)
+    window_entry_points = ("d4d_denoise_window_pndm", None, "d4d_denoise_window_pndm_cfg_split")
     state_planes = ("ets0", "ets1", "ets2", "ets3", "cur_sample")
 
     def __init__(self, cfg: PNDMConfig = None, device="cuda:0"):
@@ -591,7 +592,7 @@ class DEISTables(_MultistepTables):
     name = "DEIS"
     solver_orders = (1, 2, 3)
     # no frame-sharded window: its window-result exchange carries DPM-Solver++'s state only
-    window_entry_points = ("d4d_denoise_window_deis", None)
+    window_entry_points = ("d4d_denoise_window_deis", None, "d4d_denoise_window_deis_cfg_split")
     final_sigmas_type = "sigma_min"   # upstream's table always ends on the sigma of the first training timestep
     _struct = D4DDeisSched
 
@@ -699,7 +700,8 @@ class DPMSingleTables(_MultistepTables):
     name = "DPM-Solver++ singlestep"
     solver_orders = (1, 2, 3)
     # no frame-sharded window: its window-result exchange carries DPM-Solver++ multistep's state only
-    window_entry_points = ("d4d_denoise_window_dpm_single", None)
+    window_entry_points = ("d4d_denoise_window_dpm_single", None,
+                          "d4d_denoise_window_dpm_single_cfg_split")
     _struct = D4DDpmSingleSched
 
     def __init__(self, cfg: DPMSingleConfig = None, device="cuda:0"):

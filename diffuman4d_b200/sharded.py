@@ -32,6 +32,22 @@ def exchange_bytes(cfg, F_total: int, h: int, w: int, cfg_halves: int = 2) -> in
                 * pad_head_dim(cfg.head_dim(m.level)) * 2 for m in modules(cfg) if m.is3d), default=0)
 
 
+def open_exchange(pipe: B200Diffuman4DPipeline, nbytes: int, group=None):
+    """Allocates this rank's exchange buffers (``nbytes`` each) on ``pipe``'s handle, all-gathers the cudaIpc handles over
+    ``group`` and maps the peers' buffers.  Returns ``(rank, world)``.  Every rank of the group calls it (SPMD)."""
+    rank, world = dist.get_rank(group), dist.get_world_size(group)
+    mine = (C.c_ubyte * 192)()
+    with torch.cuda.device(pipe.device):
+        check(lib().d4d_exchange_alloc(pipe.unet._h, nbytes, mine), "d4d_exchange_alloc")
+    blobs: List[bytes] = [b""] * world
+    dist.all_gather_object(blobs, bytes(mine), group=group)
+    allh = (C.c_ubyte * (192 * world)).from_buffer_copy(b"".join(blobs))
+    with torch.cuda.device(pipe.device):
+        check(lib().d4d_exchange_open(pipe.unet._h, rank, world, allh), "d4d_exchange_open")
+    dist.barrier(group=group)
+    return rank, world
+
+
 def window_result_bytes(F_total: int, h: int, w: int, dpm: bool = True) -> int:
     """Size of one gathered window result (``d4d_window_exchange``): latents (and DPM-Solver++ ``x0_prev``) bf16
     [F_total, 4, h, w], int64 timestep indices (and int32 ``lower_order_nums``) [F_total]."""
@@ -47,21 +63,11 @@ class FrameShardedPipeline:
             raise RuntimeError("torch.distributed must be initialised (one process per GPU)")
         self.pipe = pipe
         self.group = group
-        self.rank = dist.get_rank(group)
-        self.world = dist.get_world_size(group)
-        if self.world > 8:
+        if dist.get_world_size(group) > 8:
             raise ValueError("at most 8 ranks (one NVSwitch domain)")
         # the buffers also carry the window results of the sliding loop, far smaller than any real model's K/V
         kv_bytes = max(exchange_bytes(pipe.unet.config, max_frames, h, w), window_result_bytes(max_frames, h, w))
-        mine = (C.c_ubyte * 192)()
-        with torch.cuda.device(pipe.device):
-            check(lib().d4d_exchange_alloc(pipe.unet._h, kv_bytes, mine), "d4d_exchange_alloc")
-        blobs: List[bytes] = [b""] * self.world
-        dist.all_gather_object(blobs, bytes(mine), group=group)
-        allh = (C.c_ubyte * (192 * self.world)).from_buffer_copy(b"".join(blobs))
-        with torch.cuda.device(pipe.device):
-            check(lib().d4d_exchange_open(pipe.unet._h, self.rank, self.world, allh), "d4d_exchange_open")
-        dist.barrier(group=group)
+        self.rank, self.world = open_exchange(pipe, kv_bytes, group)
 
     def frames(self, F_total: int):
         return frame_shard(F_total, self.rank, self.world)

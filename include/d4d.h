@@ -491,6 +491,53 @@ int d4d_op_window_scatter(const void* latents, const int64_t* timestep_indices, 
                           const int32_t* lower_order_nums, int F_local, int F_total, int height, int width, int world,
                           int rank, void* const* dst, size_t dst_bytes, void* stream);
 
+/* ---- multi-GPU: CFG-split window (d4d_version() 113 and later) ------------------------------------------------------
+ * With classifier-free guidance on, the two halves of a window's UNet batch (F negative images, then F positive ones)
+ * never read each other; they meet in the CFG combine.  One process per GPU, world = 2: rank k runs the UNet on CFG half
+ * k only (rank 0 the negative half, rank 1 the positive half) and its output permute stores the half's noise
+ * [F,out_channels,h,w] at rows [k*F, (k+1)*F) of BOTH ranks' exchange buffers (d4d_exchange_alloc / d4d_exchange_open,
+ * the same peer buffers and epoch sequence as the frame-sharded window).  One flag round publishes them; then every rank
+ * runs the unchanged CFG + scheduler step of d4d_denoise_window on the whole window, reading the gathered [2F] noise
+ * in place.  The ranks compute the step from the same bits, so they end with identical latents, timestep indices and
+ * solver state, and nothing else is exchanged.
+ *   - Arguments are those of the single-GPU counterpart (d4d_denoise_window, _dpm, _unipc, _pndm, _deis, _dpm_single):
+ *     EVERY rank passes the whole window and the whole window's solver state, and all of it is updated in place alike
+ *     on every rank.  Results are bit-identical to the single-GPU call.
+ *   - SPMD: both ranks make the same calls in the same order, with the same guidance_scale.  guidance_scale <= 1 has no
+ *     halves: the call runs the single-GPU step on every rank and exchanges nothing.
+ *   - Each exchange buffer (kv_bytes of d4d_exchange_alloc) must hold 2 * F * out_channels * h * w bf16; a larger window,
+ *     or a handle opened with world > 2, returns 1 before any launch.
+ *   - world = 1 (rank 0 on its own buffers) is a loopback on one GPU: the rank runs half 0, then half 1, into its own
+ *     buffer, followed by the flag round. */
+int d4d_denoise_window_cfg_split(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                 const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                 const d4d_sched* sched, float guidance_scale, int domain, int F, int height, int width,
+                                 int num_steps, void* stream);
+int d4d_denoise_window_dpm_cfg_split(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                     const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                     const d4d_dpm_sched* sched, float guidance_scale, int domain, int F, int height,
+                                     int width, int num_steps, void* x0_prev, int32_t* lower_order_nums, void* stream);
+int d4d_denoise_window_unipc_cfg_split(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                       const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                       const d4d_unipc_sched* sched, float guidance_scale, int domain, int F, int height,
+                                       int width, int num_steps, void* x0_prev, void* x0_prev2, void* last_sample,
+                                       int32_t* lower_order_nums, void* stream);
+int d4d_denoise_window_pndm_cfg_split(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                      const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                      const d4d_pndm_sched* sched, float guidance_scale, int domain, int F, int height,
+                                      int width, int num_steps, void* ets0, void* ets1, void* ets2, void* ets3,
+                                      void* cur_sample, int32_t* counter, void* stream);
+int d4d_denoise_window_deis_cfg_split(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                      const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                      const d4d_deis_sched* sched, float guidance_scale, int domain, int F, int height,
+                                      int width, int num_steps, void* m_prev, void* m_prev2, int32_t* lower_order_nums,
+                                      void* stream);
+int d4d_denoise_window_dpm_single_cfg_split(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                            const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                            const d4d_dpm_single_sched* sched, float guidance_scale, int domain, int F,
+                                            int height, int width, int num_steps, void* x0_prev, void* x0_prev2,
+                                            void* cur_sample, int32_t* lower_order_nums, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
