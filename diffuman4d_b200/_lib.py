@@ -22,6 +22,8 @@ EXPORTS = [
     "d4d_denoise_window_dpm_single", "d4d_cfg_dpm_single_step",
     "d4d_denoise_window_cfg_split", "d4d_denoise_window_dpm_cfg_split", "d4d_denoise_window_unipc_cfg_split",
     "d4d_denoise_window_pndm_cfg_split", "d4d_denoise_window_deis_cfg_split", "d4d_denoise_window_dpm_single_cfg_split",
+    "d4d_denoise_window_cfg_grid", "d4d_denoise_window_dpm_cfg_grid", "d4d_denoise_window_unipc_cfg_grid",
+    "d4d_denoise_window_pndm_cfg_grid", "d4d_denoise_window_deis_cfg_grid", "d4d_denoise_window_dpm_single_cfg_grid",
 ]
 
 
@@ -127,10 +129,11 @@ def _load(path: str) -> C.CDLL:
                                           i32, vp, vp, vp, vp]
     l.d4d_denoise_window_dpm_single.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.POINTER(D4DDpmSingleSched), f32, i32, i32,
                                                 i32, i32, i32, vp, vp, vp, vp, vp]
-    # the CFG-split window steps take their single-GPU counterparts' arguments
+    # the CFG-split and CFG-grid window steps take their single-GPU counterparts' arguments
     for name in ("d4d_denoise_window", "d4d_denoise_window_dpm", "d4d_denoise_window_unipc", "d4d_denoise_window_pndm",
                  "d4d_denoise_window_deis", "d4d_denoise_window_dpm_single"):
-        getattr(l, name + "_cfg_split").argtypes = getattr(l, name).argtypes
+        for mode in ("_cfg_split", "_cfg_grid"):
+            getattr(l, name + mode).argtypes = getattr(l, name).argtypes
     l.d4d_assemble_input.argtypes = [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]
     l.d4d_cfg_ddim_step.argtypes = [vp, vp, vp, vp, vp, C.POINTER(D4DSched), f32, i32, i32, i32, i32, vp, vp]
     l.d4d_cfg_dpm_step.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, C.POINTER(D4DDpmSched), f32, i32, i32, i32, i32, vp, vp]
@@ -179,7 +182,7 @@ def _load(path: str) -> C.CDLL:
                 "d4d_denoise_window_sharded", "d4d_denoise_window_dpm_sharded", "d4d_window_exchange", "d4d_debug_tap",
                 "d4d_denoise_window_unipc", "d4d_conv_tile_choice", "d4d_gemm_tile_choice", "d4d_denoise_window_pndm",
                 "d4d_cfg_pndm_step", "d4d_denoise_window_deis", "d4d_cfg_deis_step", "d4d_denoise_window_dpm_single",
-                "d4d_cfg_dpm_single_step") or name.endswith("_cfg_split"):
+                "d4d_cfg_dpm_single_step") or name.endswith(("_cfg_split", "_cfg_grid")):
             fn.restype = C.c_int
     return l
 

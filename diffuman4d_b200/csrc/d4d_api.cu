@@ -54,11 +54,12 @@ int unet_forward(d4d_handle* h, const void* sample, const int64_t* timestep, con
 }
 
 // every d4d_denoise_window* entry point: `step` names the scheduler table and the frames' solver state; F_total = 0 runs
-// the single-GPU plan; cfg_split runs this rank's CFG half (the *_cfg_split entry points)
+// the single-GPU plan; mode kSplit runs this rank's CFG half (the *_cfg_split entry points), kGrid its frame shard of
+// its CFG half (the *_cfg_grid entry points)
 int denoise_window(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker, const void* skeletons,
                    const void* cond_mask, int64_t* timestep_indices, const d4d::WindowStep& step, float guidance_scale,
                    int domain, int F, int F_total, int height, int width, int num_steps, void* stream,
-                   bool cfg_split = false) {
+                   d4d::CfgMode mode = d4d::CfgMode::kWhole) {
   D4D_API_BEGIN
   D4D_REQUIRE(h != nullptr && step.tables() > 0, "null argument");
   DeviceGuard g(h->model->device());
@@ -66,7 +67,7 @@ int denoise_window(d4d_handle* h, void* latents, const void* pixel_latents, cons
                                   static_cast<const bf16*>(plucker), static_cast<const bf16*>(skeletons),
                                   static_cast<const bf16*>(cond_mask), reinterpret_cast<long long*>(timestep_indices),
                                   step, guidance_scale, domain, F, height, width, num_steps,
-                                  static_cast<cudaStream_t>(stream), F_total, cfg_split);
+                                  static_cast<cudaStream_t>(stream), F_total, mode);
   D4D_API_END
 }
 
@@ -149,7 +150,7 @@ d4d::StepArgs step_args(const void* noise, const void* latents, const void* cond
 extern "C" {
 
 const char* d4d_last_error(void) { return d4d::g_last_error.c_str(); }
-int d4d_version(void) { return 113; }
+int d4d_version(void) { return 114; }
 
 int d4d_create(const d4d_config* cfg, int device, d4d_handle** out) {
   D4D_API_BEGIN
@@ -689,7 +690,7 @@ int d4d_denoise_window_cfg_split(d4d_handle* h, void* latents, const void* pixel
                                  const d4d_sched* sched, float guidance_scale, int domain, int F, int height, int width,
                                  int num_steps, void* stream) {
   return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, ddim_step(sched),
-                        guidance_scale, domain, F, 0, height, width, num_steps, stream, true);
+                        guidance_scale, domain, F, 0, height, width, num_steps, stream, d4d::CfgMode::kSplit);
 }
 
 int d4d_denoise_window_dpm_cfg_split(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
@@ -698,7 +699,7 @@ int d4d_denoise_window_dpm_cfg_split(d4d_handle* h, void* latents, const void* p
                                      int width, int num_steps, void* x0_prev, int32_t* lower_order_nums, void* stream) {
   return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
                         dpm_step(sched, x0_prev, lower_order_nums), guidance_scale, domain, F, 0, height, width, num_steps,
-                        stream, true);
+                        stream, d4d::CfgMode::kSplit);
 }
 
 int d4d_denoise_window_unipc_cfg_split(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
@@ -708,7 +709,7 @@ int d4d_denoise_window_unipc_cfg_split(d4d_handle* h, void* latents, const void*
                                        int32_t* lower_order_nums, void* stream) {
   return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
                         unipc_step(sched, x0_prev, x0_prev2, last_sample, lower_order_nums), guidance_scale, domain, F, 0,
-                        height, width, num_steps, stream, true);
+                        height, width, num_steps, stream, d4d::CfgMode::kSplit);
 }
 
 int d4d_denoise_window_pndm_cfg_split(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
@@ -718,7 +719,7 @@ int d4d_denoise_window_pndm_cfg_split(d4d_handle* h, void* latents, const void* 
                                       void* cur_sample, int32_t* counter, void* stream) {
   return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
                         pndm_step(sched, ets0, ets1, ets2, ets3, cur_sample, counter), guidance_scale, domain, F, 0, height,
-                        width, num_steps, stream, true);
+                        width, num_steps, stream, d4d::CfgMode::kSplit);
 }
 
 int d4d_denoise_window_deis_cfg_split(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
@@ -728,7 +729,7 @@ int d4d_denoise_window_deis_cfg_split(d4d_handle* h, void* latents, const void* 
                                       void* stream) {
   return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
                         deis_step(sched, m_prev, m_prev2, lower_order_nums), guidance_scale, domain, F, 0, height, width,
-                        num_steps, stream, true);
+                        num_steps, stream, d4d::CfgMode::kSplit);
 }
 
 int d4d_denoise_window_dpm_single_cfg_split(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
@@ -738,7 +739,64 @@ int d4d_denoise_window_dpm_single_cfg_split(d4d_handle* h, void* latents, const 
                                             void* cur_sample, int32_t* lower_order_nums, void* stream) {
   return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
                         dpm_single_step(sched, x0_prev, x0_prev2, cur_sample, lower_order_nums), guidance_scale, domain, F,
-                        0, height, width, num_steps, stream, true);
+                        0, height, width, num_steps, stream, d4d::CfgMode::kSplit);
+}
+
+int d4d_denoise_window_cfg_grid(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                const d4d_sched* sched, float guidance_scale, int domain, int F, int height, int width,
+                                int num_steps, void* stream) {
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices, ddim_step(sched),
+                        guidance_scale, domain, F, 0, height, width, num_steps, stream, d4d::CfgMode::kGrid);
+}
+
+int d4d_denoise_window_dpm_cfg_grid(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                    const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                    const d4d_dpm_sched* sched, float guidance_scale, int domain, int F, int height,
+                                    int width, int num_steps, void* x0_prev, int32_t* lower_order_nums, void* stream) {
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
+                        dpm_step(sched, x0_prev, lower_order_nums), guidance_scale, domain, F, 0, height, width, num_steps,
+                        stream, d4d::CfgMode::kGrid);
+}
+
+int d4d_denoise_window_unipc_cfg_grid(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                      const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                      const d4d_unipc_sched* sched, float guidance_scale, int domain, int F, int height,
+                                      int width, int num_steps, void* x0_prev, void* x0_prev2, void* last_sample,
+                                      int32_t* lower_order_nums, void* stream) {
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
+                        unipc_step(sched, x0_prev, x0_prev2, last_sample, lower_order_nums), guidance_scale, domain, F, 0,
+                        height, width, num_steps, stream, d4d::CfgMode::kGrid);
+}
+
+int d4d_denoise_window_pndm_cfg_grid(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                     const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                     const d4d_pndm_sched* sched, float guidance_scale, int domain, int F, int height,
+                                     int width, int num_steps, void* ets0, void* ets1, void* ets2, void* ets3,
+                                     void* cur_sample, int32_t* counter, void* stream) {
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
+                        pndm_step(sched, ets0, ets1, ets2, ets3, cur_sample, counter), guidance_scale, domain, F, 0, height,
+                        width, num_steps, stream, d4d::CfgMode::kGrid);
+}
+
+int d4d_denoise_window_deis_cfg_grid(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                     const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                     const d4d_deis_sched* sched, float guidance_scale, int domain, int F, int height,
+                                     int width, int num_steps, void* m_prev, void* m_prev2, int32_t* lower_order_nums,
+                                     void* stream) {
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
+                        deis_step(sched, m_prev, m_prev2, lower_order_nums), guidance_scale, domain, F, 0, height, width,
+                        num_steps, stream, d4d::CfgMode::kGrid);
+}
+
+int d4d_denoise_window_dpm_single_cfg_grid(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                           const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                           const d4d_dpm_single_sched* sched, float guidance_scale, int domain, int F,
+                                           int height, int width, int num_steps, void* x0_prev, void* x0_prev2,
+                                           void* cur_sample, int32_t* lower_order_nums, void* stream) {
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
+                        dpm_single_step(sched, x0_prev, x0_prev2, cur_sample, lower_order_nums), guidance_scale, domain, F,
+                        0, height, width, num_steps, stream, d4d::CfgMode::kGrid);
 }
 
 int d4d_exchange_alloc(d4d_handle* h, size_t kv_bytes, unsigned char* handles_out) {

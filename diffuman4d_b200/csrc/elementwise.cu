@@ -258,8 +258,12 @@ __global__ void assemble_kernel(const AssembleArgs a, int Cin) {
   // the rows of frame f's positive and negative images (-1: not written); the positive half is the LAST half when cfg
   // (torch.cat([negative, positive]))
   const bool whole = a.half < 0;
-  const int pos_img = whole ? (a.cfg ? a.F + f : f) : (a.half == 1 ? f : -1);
-  const int neg_img = whole ? (a.cfg ? f : -1) : (a.half == 0 ? f : -1);
+  const bool shard = !whole && a.n_f > 0;
+  const bool rows = !shard || (f >= a.f0 && f < a.f0 + a.n_f);  // frame f has sample rows
+  if (!rows && !is_cond) return;                                // nothing to write for frame f
+  const int fr = shard ? f - a.f0 : f;
+  const int pos_img = !rows ? -1 : whole ? (a.cfg ? a.F + f : f) : (a.half == 1 ? fr : -1);
+  const int neg_img = !rows ? -1 : whole ? (a.cfg ? f : -1) : (a.half == 0 ? fr : -1);
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     long long t = 0;
     if (!is_cond) {

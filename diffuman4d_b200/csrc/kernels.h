@@ -197,6 +197,9 @@ struct AssembleArgs {
   // [0, F), the rows the whole batch has at [k*F, (k+1)*F) (cfg is then not read).  Every mode overwrites the cond frames'
   // latents in place alike.
   int half = -1;
+  // with a half and n_f > 0: only frames [f0, f0 + n_f) get sample rows, at rows [0, n_f) (a frame shard of the CFG
+  // grid); the cond frames of all F frames are still overwritten in place
+  int f0 = 0, n_f = 0;
   bf16* latents;            // [F,4,h,w]  (cond frames are overwritten in place like the reference)
   const bf16* pixel;        // [F,4,h,w]
   const bf16* plucker;      // [F,6,h,w]

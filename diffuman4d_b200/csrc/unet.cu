@@ -61,7 +61,7 @@ const struct { const char* path; int cin, cout, k; } kPoseLayers[8] = {
 std::string plan_key(const PlanShape& s) {
   std::string k = std::to_string(s.B) + "_" + std::to_string(s.F) + "_" + std::to_string(s.h) + "_" + std::to_string(s.w) + "_";
   for (int d : s.domains) k += d ? 't' : 's';
-  if (s.F_total > 0) k += "_sh" + std::to_string(s.F_total);
+  if (s.F_total > 0) k += "_sh" + std::to_string(s.F_total) + "_g" + std::to_string(s.kv_rank0) + "x" + std::to_string(s.kv_world);
   return s.pose_neg > 0 ? k + "_pn" + std::to_string(s.pose_neg) : k;
 }
 
@@ -633,14 +633,16 @@ class PlanBuilder {
     return out;
   }
 
-  // Frame-sharded 3-D attention: the QKV GEMM epilogue stores its K|V columns straight into every rank's gathered
-  // K/V buffer (peer memory), a flag round makes them visible, attention reads all F_total frames locally.
+  // Frame-sharded 3-D attention: the QKV GEMM epilogue stores its K|V columns straight into the gathered K/V buffer of
+  // every rank of the plan's K/V group (peer memory), a flag round of every rank makes them visible, attention reads all
+  // F_total frames locally.
   void sharded_qkv_attention(const AttnW& a, const XfW& x, const bf16* normed, bf16* qkv, bf16* o, int M, int batch, int seq) {
     const int Cp = x.heads * x.dpad;
     const Exchange& X = m_.xch_;
+    const PlanShape& sh = p_.shape;
     const int idx = p_.n3d++;
     const long long rows_local = seq;                                   // F_loc * hw tokens per CFG half
-    const long long rows_global = static_cast<long long>(seq) / p_.shape.F * p_.shape.F_total;
+    const long long rows_global = static_cast<long long>(seq) / sh.F * sh.F_total;
     if (static_cast<size_t>(batch) * rows_global * 2 * Cp * sizeof(bf16) > X.kv_bytes) {
       set_error("K/V exchange buffer too small for this window (d4d_exchange_alloc)");
       if (!rc_) rc_ = 1;
@@ -652,9 +654,9 @@ class PlanBuilder {
     AttnLaunch A[2];
     for (int par = 0; par < 2; ++par) {
       GemmDesc d = linear(a.qkv, normed, M, qkv);
-      d.kv_world = X.world; d.kv_col0 = Cp; d.kv_ld = 2 * Cp;
-      d.kv_rows_local = rows_local; d.kv_rows_global = rows_global; d.kv_row_offset = static_cast<long long>(X.rank) * rows_local;
-      for (int r = 0; r < X.world; ++r) d.kv_dst[r] = static_cast<bf16*>(X.peer_kv[par][r]);
+      d.kv_world = sh.kv_world; d.kv_col0 = Cp; d.kv_ld = 2 * Cp;
+      d.kv_rows_local = rows_local; d.kv_rows_global = rows_global; d.kv_row_offset = static_cast<long long>(sh.shard) * rows_local;
+      for (int r = 0; r < sh.kv_world; ++r) d.kv_dst[r] = static_cast<bf16*>(X.peer_kv[par][sh.kv_rank0 + r]);
       if (int rc = gemm_prepare(d, &G[par])) { if (!rc_) rc_ = rc; return; }
       AttnDesc t;
       t.q = qkv; t.ld_qkv = 3 * Cp;
@@ -663,6 +665,8 @@ class PlanBuilder {
       t.heads = x.heads; t.head_dim = x.dpad; t.scale = 1.0f / sqrtf(static_cast<float>(x.d));
       if (int rc = attn_prepare(t, &A[par])) { if (!rc_) rc_ = rc; return; }
     }
+    // the flag round spans every rank, also those outside the K/V group: the CFG grid's noise store crosses groups, and
+    // the write-after-read argument of DESIGN.md section 7 needs every exchange to wait for every rank
     KvFlagArgs fa;
     for (int r = 0; r < 8; ++r) fa.flags[r] = r < X.world ? X.peer_flags[r] : nullptr;
     fa.rank = X.rank; fa.world = X.world; fa.epoch = 0; fa.slot = 0;
@@ -718,10 +722,12 @@ class PlanBuilder {
     groupnorm(in, nullptr, B, 1e-6f, x.gn, 0, n);
     bf16* t = alloc(static_cast<size_t>(M) * C);
     gemm(linear(x.pin, n, M, t));
-    // attn1 (3-D when num_frames > 1: batch = B / num_frames sequences of num_frames*hw tokens)
+    // attn1 (3-D when the window has more than one frame: batch = B / num_frames sequences of num_frames*hw local
+    // tokens; a frame-sharded rank may hold a single frame of a larger window, and still attends over all F_total)
+    const int window_frames = p_.shape.F_total > 0 ? p_.shape.F_total : p_.shape.F;
     layernorm(t, M, C, x.ln1, n);
     bf16* t1 = alloc(static_cast<size_t>(M) * C);
-    self_attention(x.a1, x, n, t, t1, M, B / num_frames, num_frames * hw, num_frames > 1);
+    self_attention(x.a1, x, n, t, t1, M, B / num_frames, num_frames * hw, x.is3d && window_frames > 1);
     release(t);
     if (x.has2) {  // attn2 with encoder_hidden_states=None: per-image self-attention
       layernorm(t1, M, C, x.ln2, n);
@@ -803,7 +809,7 @@ class PlanBuilder {
       if (!dry_) {
         std::vector<float> hp(B);
         for (int dmn = 0; dmn < sh.n_domains; ++dmn)
-          for (int f = 0; f < F; ++f) hp[dmn * F + f] = sh.domains[dmn] == 0 ? 0.f : static_cast<float>((sh.rank * F + f) % std::max(1, (sh.F_total > 0 ? sh.F_total : F) / 2));
+          for (int f = 0; f < F; ++f) hp[dmn * F + f] = sh.domains[dmn] == 0 ? 0.f : static_cast<float>((sh.shard * F + f) % std::max(1, (sh.F_total > 0 ? sh.F_total : F) / 2));
         if (cudaMemcpy(pos, hp.data(), sizeof(float) * B, cudaMemcpyHostToDevice) != cudaSuccess) rc_ = 2;
       }
       op([=](cudaStream_t s) { return sinusoid_run(pos, B, C0, 1, 0.f, tsin, s); });
@@ -1011,7 +1017,8 @@ Plan* Model::find_plan(int n_domains, int B, int F, int h, int w) {
   return nullptr;
 }
 
-int Model::get_plan(const int* domain_ids, int n_domains, int B, int F, int h, int w, Plan** out, int F_total, int pose_neg) {
+int Model::get_plan(const int* domain_ids, int n_domains, int B, int F, int h, int w, Plan** out, int F_total, int pose_neg,
+                    int kv_world) {
   if (!finalized_) {
     set_error("weights not finalized (call d4d_finalize_weights)");
     return 3;
@@ -1027,14 +1034,20 @@ int Model::get_plan(const int* domain_ids, int n_domains, int B, int F, int h, i
   for (int i = 0; i < n_domains; ++i) D4D_REQUIRE(domain_ids[i] == 0 || domain_ids[i] == 1, "Invalid domain for temporal embedding");
   // every *_sharded call runs the sharded plan, also with world = 1 (rank 0 exchanging with itself)
   const bool sharded = F_total > 0;
-  if (sharded) {
-    D4D_REQUIRE(xch_.ready && xch_.world >= 1, "frame-sharded forward needs d4d_exchange_open first");
-    D4D_REQUIRE(F * xch_.world == F_total, "F_total must equal world * local frames");
-  }
   PlanShape s;
   s.n_domains = n_domains; s.B = B; s.F = F; s.h = h; s.w = w;
   s.domains.assign(domain_ids, domain_ids + n_domains);
-  if (sharded) { s.F_total = F_total; s.rank = xch_.rank; s.world = xch_.world; }
+  if (sharded) {
+    D4D_REQUIRE(xch_.ready && xch_.world >= 1, "frame-sharded forward needs d4d_exchange_open first");
+    // the K/V group: kv_world consecutive ranks, this rank's frame shard its place in them (0: every rank)
+    if (kv_world == 0) kv_world = xch_.world;
+    D4D_REQUIRE(kv_world >= 1 && xch_.world % kv_world == 0, "the K/V group size must divide the world");
+    D4D_REQUIRE(F * kv_world == F_total, "F_total must equal the K/V group size * local frames");
+    s.F_total = F_total;
+    s.kv_world = kv_world;
+    s.kv_rank0 = xch_.rank / kv_world * kv_world;
+    s.shard = xch_.rank - s.kv_rank0;
+  }
   D4D_REQUIRE(pose_neg >= 0 && pose_neg <= B, "pose_neg must be in [0, B]");
   s.pose_neg = cfg_.enable_pose_encoder ? pose_neg : 0;
   const std::string key = plan_key(s);
@@ -1093,9 +1106,9 @@ int Model::forward(const bf16* sample, const long long* timestep, const bf16* sk
 
 int Model::forward(const bf16* sample, const long long* timestep, const bf16* skeletons, const int* domain_ids,
                    int n_domains, int B, int F, int h, int w, const NchwDst& out, cudaStream_t stream, int F_total,
-                   int pose_neg) {
+                   int pose_neg, int kv_world) {
   Plan* p = nullptr;
-  if (int rc = get_plan(domain_ids, n_domains, B, F, h, w, &p, F_total, pose_neg)) return rc;
+  if (int rc = get_plan(domain_ids, n_domains, B, F, h, w, &p, F_total, pose_neg, kv_world)) return rc;
   if (int rc = run_ops(*p, sample, timestep, skeletons, out, p->ops.size(), stream)) return rc;
   xch_.epoch_base += static_cast<unsigned int>(p->n3d);
   return 0;
@@ -1195,23 +1208,38 @@ int Model::profile(const bf16* sample, const long long* timestep, const bf16* sk
 
 int Model::denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
                           long long* ts_idx, const WindowStep& step, float guidance, int domain, int F, int h, int w,
-                          int num_steps, cudaStream_t stream, int F_total, bool cfg_split) {
+                          int num_steps, cudaStream_t stream, int F_total, CfgMode mode) {
   D4D_REQUIRE(latents && pixel && plucker && mask && ts_idx && step.tables() == 1, "null argument");
   D4D_REQUIRE(domain == 0 || domain == 1, "Invalid domain");
   const bool cfg_on = guidance > 1.0f;
-  const bool split = cfg_split && cfg_on;  // guidance <= 1 has no halves: the plain step runs and nothing is exchanged
+  // guidance <= 1 has no halves: the plain step runs and nothing is exchanged
+  const bool split = mode != CfgMode::kWhole && cfg_on;
   const int B = cfg_on ? 2 * F : F;
   const bool pose = cfg_.enable_pose_encoder != 0;
   const int Cin = 4 + 6 + (pose ? 0 : 4) + 1;
   const int Co = cfg_.out_channels;
   D4D_REQUIRE(Cin == cfg_.in_channels, "in_channels does not match the latent/plucker/skeleton/mask channel layout");
   D4D_REQUIRE(skeletons != nullptr, "skeletons required");
+  const int world = xch_.world;
+  if (mode == CfgMode::kGrid)
+    D4D_REQUIRE(world == 1 || world == 2 || world == 4 || world == 6 || world == 8,
+                "the CFG grid runs on 2 * R ranks with R in {1, 2, 3, 4} (or 1 as a loopback)");
+  // frame shards per CFG half: R > 1 only on a grid of 4, 6 or 8 ranks
+  const int R = mode == CfgMode::kGrid && world > 1 ? world / 2 : 1;
+  Plan* grid_plan = nullptr;  // R > 1: this rank's plan, built before any launch (it refuses a too small K/V buffer)
   if (split) {
     D4D_REQUIRE(xch_.ready, "the CFG-split window needs d4d_exchange_open first");
-    D4D_REQUIRE(xch_.world <= 2, "the CFG-split window runs on 1 (loopback) or 2 ranks");
+    D4D_REQUIRE(mode == CfgMode::kGrid || world <= 2, "the CFG-split window runs on 1 (loopback) or 2 ranks");
     D4D_REQUIRE(F > 0 && h > 0 && w > 0, "empty window");
+    D4D_REQUIRE(F % R == 0, "the window's frames (" + std::to_string(F) + ") must be divisible by the frame shards per CFG "
+                "half (" + std::to_string(R) + ")");
     D4D_REQUIRE(2ull * F * Co * h * w * sizeof(bf16) <= xch_.kv_bytes,
                 "the window's noise (2 * F * out_channels * h * w bf16) does not fit the exchange buffer (d4d_exchange_alloc)");
+    if (R > 1) {
+      const int doms1[1] = {domain};
+      const int k = xch_.rank / R;
+      if (int rc = get_plan(doms1, 1, F / R, F / R, h, w, &grid_plan, F, pose && k == 0 ? F / R : 0, R)) return rc;
+    }
   }
   D4D_CUDA_OK(cudaSetDevice(device_));
   const std::string key = std::to_string(B) + "_" + std::to_string(F) + "_" + std::to_string(h) + "_" + std::to_string(w);
@@ -1258,23 +1286,31 @@ int Model::denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker,
     a.n_steps = n_steps; a.F = F; a.h = h; a.w = w; a.cfg = cfg_on ? 1 : 0;
     a.sample = wb.sample; a.timestep_out = wb.timestep;
     if (split) {
-      // CFG split (DESIGN.md section 7): the UNet on this rank's half k (a loopback runs both), its noise stored at rows
-      // [k*F, (k+1)*F) of exchange e's buffer parity on every rank; one flag round; the step reads the gathered [2F] noise
-      // in place.  Every rank then computes the step from the same bits.
-      const unsigned int e = xch_.epoch_base;
-      const int k0 = xch_.world == 1 ? 0 : xch_.rank, k1 = xch_.world == 1 ? 2 : xch_.rank + 1;
+      // CFG split / grid (DESIGN.md section 7): the UNet on this rank's half k (a loopback runs both) of its frame shard r
+      // (Fr = F / R frames), its noise stored at rows [k*F + r*Fr, k*F + (r+1)*Fr) of the exchange buffer parity that
+      // follows the forward's n3d K/V exchanges, on every rank; one flag round; the step reads the gathered [2F] noise in
+      // place.  Every rank then computes the step from the same bits.
+      const int Fr = F / R, r = xch_.rank % R;
+      const int k0 = world == 1 ? 0 : xch_.rank / R, k1 = world == 1 ? 2 : k0 + 1;
+      const unsigned int n3d = grid_plan ? static_cast<unsigned int>(grid_plan->n3d) : 0u;
       for (int k = k0; k < k1; ++k) {
         a.half = k;
+        // a grid rank writes sample rows for its frame shard only, but overwrites every cond frame's latents, so that
+        // every rank's whole-window latents stay those of the single-GPU step
+        if (R > 1) { a.f0 = r * Fr; a.n_f = Fr; }
         if (int rc = assemble_input_run(a, stream)) return rc;
+        const unsigned int e = xch_.epoch_base + n3d;
         NchwDst dst = {};
-        dst.n = xch_.world;
-        for (int r = 0; r < xch_.world; ++r)
-          dst.p[r] = static_cast<bf16*>(xch_.peer_kv[e & 1][r]) + static_cast<size_t>(k) * F * Co * hw;
-        // every negative skeleton is the constant image wb.skel[0]: the negative half encodes it once (pose_neg = F)
-        const bf16* skel_in = pose ? (k == 0 ? wb.skel : skeletons) : nullptr;
-        if (int rc = forward(wb.sample, wb.timestep, skel_in, doms, 1, F, F, h, w, dst, stream, 0, pose && k == 0 ? F : 0))
+        dst.n = world;
+        for (int g = 0; g < world; ++g)
+          dst.p[g] = static_cast<bf16*>(xch_.peer_kv[e & 1][g]) + (static_cast<size_t>(k) * F + r * Fr) * Co * hw;
+        // every negative skeleton is the constant image wb.skel[0]: the negative half encodes it once (pose_neg = Fr)
+        const bf16* skel_in = pose ? (k == 0 ? wb.skel : skeletons + static_cast<size_t>(r) * Fr * 3 * 64 * hw) : nullptr;
+        if (int rc = forward(wb.sample, wb.timestep, skel_in, doms, 1, Fr, Fr, h, w, dst, stream, R > 1 ? F : 0,
+                             pose && k == 0 ? Fr : 0, R > 1 ? R : 0))
           return rc;
       }
+      const unsigned int e = xch_.epoch_base;  // the exchange the flag round closes: the noise's buffer parity
       if (int rc = flag_round(stream)) return rc;
       sa.noise = static_cast<const bf16*>(xch_.kv[e & 1]);
     } else {

@@ -63,8 +63,10 @@ struct PlanOp { std::function<int(cudaStream_t)> run; OpKind kind; int launches;
 struct PlanShape {
   int n_domains = 0, B = 0, F = 0, h = 0, w = 0;
   std::vector<int> domains;
-  // frame-sharded window (DESIGN.md section 7): this rank owns F of F_total frames per CFG half
-  int F_total = 0, rank = 0, world = 1;
+  // frame-sharded plan (DESIGN.md section 7): this rank owns frames [shard * F, (shard + 1) * F) of F_total per CFG half,
+  // and the 3-D layers store their K|V rows into the kv_world ranks kv_rank0 .. kv_rank0 + kv_world - 1: every rank for
+  // the frame-sharded window (shard = rank), the R ranks of this rank's CFG half for the CFG grid (shard = rank % R)
+  int F_total = 0, shard = 0, kv_rank0 = 0, kv_world = 1;
   // the first pose_neg images of the batch are CFG-negative, whose skeletons are all one constant image: the skeleton
   // batch is [1 negative image | B - pose_neg positive images], encoded once and broadcast (window step: F of 2F, or
   // the whole batch on the negative rank of the CFG-split window)
@@ -128,6 +130,11 @@ struct WindowStep {
   }
 };
 
+// Where a window step runs its two CFG halves (DESIGN.md section 7): both on this rank (kWhole); one per rank of a world
+// of 2, or both on a loopback world of 1 (kSplit, the CFG-split window); or each half frame-sharded over the R = world / 2
+// ranks k*R .. k*R + R - 1 of half k (kGrid, the CFG grid; with R = 1 it is the CFG split).
+enum class CfgMode { kWhole, kSplit, kGrid };
+
 struct Exchange {  // K/V exchange buffers in peer memory (cudaIpc), two parities
   bool ready = false;
   int rank = 0, world = 1;
@@ -149,18 +156,20 @@ class Model {
   int forward(const bf16* sample, const long long* timestep, const bf16* skeletons, const int* domain_ids,
               int n_domains, int B, int F, int h, int w, bf16* out, cudaStream_t stream, int F_total = 0,
               int pose_neg = 0);
-  // the same forward, its output stored into every out.p[i]
+  // the same forward, its output stored into every out.p[i]; kv_world > 0 (with F_total): the 3-D layers exchange K|V
+  // within this rank's group of kv_world consecutive ranks only (the CFG grid), 0: with every rank
   int forward(const bf16* sample, const long long* timestep, const bf16* skeletons, const int* domain_ids,
               int n_domains, int B, int F, int h, int w, const NchwDst& out, cudaStream_t stream, int F_total,
-              int pose_neg);
+              int pose_neg, int kv_world = 0);
   int exchange_alloc(size_t kv_bytes, unsigned char* handles_out /* 3 x 64 bytes */);
   int exchange_open(int rank, int world, const unsigned char* all_handles /* world x 3 x 64 bytes */);
   // num_steps x (assemble -> UNet -> CFG + scheduler step) on the window's F frames; latents, ts_idx and the solver state
-  // of `step` are updated in place.  cfg_split (guidance > 1, needs exchange_open with world 1 or 2): this rank runs the
-  // UNet on its CFG half only and the halves meet in the exchange buffers (DESIGN.md section 7).
+  // of `step` are updated in place.  mode kSplit (guidance > 1, needs exchange_open with world 1 or 2): this rank runs the
+  // UNet on its CFG half only and the halves meet in the exchange buffers; kGrid (world 1, 2, 4, 6 or 8): this rank runs
+  // it on its frame shard of its CFG half (DESIGN.md section 7).
   int denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
                      long long* ts_idx, const WindowStep& step, float guidance, int domain, int F, int h, int w,
-                     int num_steps, cudaStream_t stream, int F_total, bool cfg_split = false);
+                     int num_steps, cudaStream_t stream, int F_total, CfgMode mode = CfgMode::kWhole);
   // frame-sharded sliding loop: this rank's F updated frames (+ DPM-Solver++ state when x0_prev != nullptr) to every rank,
   // one flag round (one more exchange of the epoch sequence), then the gathered F_total frames to the *_out buffers
   int window_exchange(const bf16* latents, const long long* ts_idx, const bf16* x0_prev, const int* lower_order_nums, int F,
@@ -171,7 +180,7 @@ class Model {
               int B, int F, int h, int w, bf16* out, cudaStream_t stream, float* ms_by_kind, int* launches_by_kind,
               double* flops_by_kind);
   int get_plan(const int* domain_ids, int n_domains, int B, int F, int h, int w, Plan** out, int F_total = 0,
-               int pose_neg = 0);
+               int pose_neg = 0, int kv_world = 0);
   // debug: run the forward up to tap `tap` and copy that activation out as NCHW bf16 [B, C, H, W]; out == nullptr only
   // reports name / dims.  Returns 1 when tap is out of range.
   int debug_tap(const bf16* sample, const long long* timestep, const bf16* skeletons, const int* domain_ids, int n_domains,

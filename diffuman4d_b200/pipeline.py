@@ -102,7 +102,11 @@ class B200Diffuman4DPipeline:
 
     @property
     def do_classifier_free_guidance(self):
-        return self._guidance_scale > 1 and self.unet.config.time_cond_proj_dim is None
+        return self.has_cfg_halves(self._guidance_scale)
+
+    def has_cfg_halves(self, guidance_scale) -> bool:
+        """Whether a window step at ``guidance_scale`` runs the UNet on two CFG halves (otherwise on the F frames once)."""
+        return guidance_scale > 1 and self.unet.config.time_cond_proj_dim is None
 
     @property
     def _multistep(self) -> bool:
@@ -135,11 +139,16 @@ class B200Diffuman4DPipeline:
     def _window_step(self, *, latents, pixel_values_latents, plucker_embeds_latents, skeletons_latents,
                      cond_masks_latents, timestep_indices, domain: str, guidance_scale: float,
                      num_inference_steps: int = 1, solver_state: Optional[SolverState] = None,
-                     F_total: Optional[int] = None, cfg_split: bool = False):
+                     F_total: Optional[int] = None, cfg_split: bool = False, cfg_grid: bool = False):
         """``denoise_window``'s checks and library call.  ``F_total`` given: the tensors hold this rank's frames of a
         frame-sharded window of ``F_total`` frames (``FrameShardedPipeline.denoise_window``).  ``cfg_split``: the whole
-        window, with this rank running the UNet on its CFG half (``CFGSplitPipeline.denoise_window``)."""
-        name = self.scheduler.window_entry_points[2 if cfg_split else F_total is not None]
+        window, with this rank running the UNet on its CFG half (``CFGSplitPipeline.denoise_window``).  ``cfg_grid``: the
+        whole window, with this rank running the UNet on its frame shard of its CFG half
+        (``CFGGridPipeline.denoise_window``)."""
+        if cfg_grid:
+            name = self.scheduler.window_entry_points[0] + "_cfg_grid"
+        else:
+            name = self.scheduler.window_entry_points[2 if cfg_split else F_total is not None]
         if name is None:
             raise NotImplementedError(f"the frame-sharded window does not run the {self.scheduler.name} scheduler")
         if domain not in _DOMAIN_IDS:

@@ -169,7 +169,7 @@ def launches(cfg, F: int, h: int, w: int, halves: int = 2, ranks: int = 1) -> Li
         elif m.type == "transformer":
             C, M = m.cout, B * n
             gemm(m.path, "proj_in", lvl, M, C, C, ("bias",), algo=2.0 * C * C * M)
-            self_attention(m, "", m.is3d and Fl > 1)
+            self_attention(m, "", m.is3d and F > 1)   # 3-D over the window, also when a rank holds one frame
             if m.attn2:
                 self_attention(m, "attn2 ", False)
             gemm(m.path, "ff1 geglu", lvl, M, 8 * C, C, ("bias", "geglu"), algo=16.0 * C * C * M, category="ff")

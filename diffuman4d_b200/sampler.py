@@ -17,7 +17,8 @@ Multi-GPU (one process per GPU, SURVEY 8e row 1): the tasks of a round are indep
 (tests/golden/gen_golden.py::gen_sampler -> tests/test_sampler.py).  Alternatively (``execute_tasks(frame_sharded=True)``
 with a ``sharded.FrameShardedPipeline``) every rank runs every task with each window split over the ranks by frames, which
 keeps all GPUs busy when a round has fewer tasks than GPUs (DESIGN.md section 7); ``execute_tasks(cfg_split=True)`` with a
-``cfg_split.CFGSplitPipeline`` does the same with each window step split by CFG half over two ranks.
+``cfg_split.CFGSplitPipeline`` does the same with each window step split by CFG half over two ranks (or, with a
+``cfg_split.CFGGridPipeline``, by CFG half and frames over 2R ranks).
 
 The dataset object supplies ``scene_label`` and ``get_item(scene_label, spa_labels, tem_labels, input_spa_labels)`` exactly
 like the reference's ``SpaTemDataset`` (src/data/spatem_dataset.py:76-212); pipelines supply
@@ -242,7 +243,7 @@ class B200SlidingIterativeSampler:
         ``save_fn`` runs on the pipeline's rank 0 only.
 
         ``cfg_split=True``: the same, with a ``cfg_split.CFGSplitPipeline`` whose ranks each run one CFG half of every
-        window step."""
+        window step, or a ``cfg_split.CFGGridPipeline`` whose ranks each run a frame shard of one CFG half."""
         save_fn = self.save_fn
         if frame_sharded and cfg_split:
             raise ValueError("frame_sharded and cfg_split are two different multi-GPU modes; pass one of them")

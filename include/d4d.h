@@ -538,6 +538,50 @@ int d4d_denoise_window_dpm_single_cfg_split(d4d_handle* h, void* latents, const 
                                             int height, int width, int num_steps, void* x0_prev, void* x0_prev2,
                                             void* cur_sample, int32_t* lower_order_nums, void* stream);
 
+/* ---- multi-GPU: CFG grid, the CFG-split window on 2 x R ranks (d4d_version() 114 and later) -------------------------
+ * The CFG-split window with each CFG half frame-sharded over R ranks.  One process per GPU, world = 2R with R in
+ * {1, 2, 3, 4}: global rank g runs CFG half k = g / R (ranks 0 .. R-1 the negative half) on frame shard r = g % R, frames
+ * [r*F/R, (r+1)*F/R) of the window.  At each 3-D attention layer the rank's fused-QKV GEMM epilogue stores its K|V rows
+ * into the gathered K/V buffers of the R ranks of its half only (the frame-sharded window's scatter, within the half); the
+ * output permute stores the rank's noise [F/R,out_channels,h,w] at rows [k*F + r*F/R, k*F + (r+1)*F/R) of EVERY rank's
+ * exchange buffer.  One flag round publishes the noise; then every rank runs the unchanged CFG + scheduler step of
+ * d4d_denoise_window on the whole window, reading the gathered [2F] noise in place, as in the CFG split.  Every flag round,
+ * those of the K/V layers included, waits for all 2R ranks.
+ *   - Arguments, SPMD rules, guidance_scale <= 1 and the whole-window state are those of the *_cfg_split counterpart;
+ *     results are bit-identical to the single-GPU call on every rank.
+ *   - With R = 1 (world 1 or 2) the call is the CFG-split window, the same code and the same bits.
+ *   - Returns 1 before any launch for a world other than 1, 2, 4, 6 or 8; with guidance_scale > 1, for F not divisible by
+ *     R, or an exchange buffer (kv_bytes of d4d_exchange_alloc) smaller than the larger of 2 * F * out_channels * h * w
+ *     bf16 and, for R > 1, one CFG half's largest 3-D K|V layer at F frames (sharded.exchange_bytes with one half). */
+int d4d_denoise_window_cfg_grid(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                const d4d_sched* sched, float guidance_scale, int domain, int F, int height, int width,
+                                int num_steps, void* stream);
+int d4d_denoise_window_dpm_cfg_grid(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                    const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                    const d4d_dpm_sched* sched, float guidance_scale, int domain, int F, int height,
+                                    int width, int num_steps, void* x0_prev, int32_t* lower_order_nums, void* stream);
+int d4d_denoise_window_unipc_cfg_grid(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                      const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                      const d4d_unipc_sched* sched, float guidance_scale, int domain, int F, int height,
+                                      int width, int num_steps, void* x0_prev, void* x0_prev2, void* last_sample,
+                                      int32_t* lower_order_nums, void* stream);
+int d4d_denoise_window_pndm_cfg_grid(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                     const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                     const d4d_pndm_sched* sched, float guidance_scale, int domain, int F, int height,
+                                     int width, int num_steps, void* ets0, void* ets1, void* ets2, void* ets3,
+                                     void* cur_sample, int32_t* counter, void* stream);
+int d4d_denoise_window_deis_cfg_grid(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                     const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                     const d4d_deis_sched* sched, float guidance_scale, int domain, int F, int height,
+                                     int width, int num_steps, void* m_prev, void* m_prev2, int32_t* lower_order_nums,
+                                     void* stream);
+int d4d_denoise_window_dpm_single_cfg_grid(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                           const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                           const d4d_dpm_single_sched* sched, float guidance_scale, int domain, int F,
+                                           int height, int width, int num_steps, void* x0_prev, void* x0_prev2,
+                                           void* cur_sample, int32_t* lower_order_nums, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
