@@ -24,6 +24,8 @@ EXPORTS = [
     "d4d_denoise_window_pndm_cfg_split", "d4d_denoise_window_deis_cfg_split", "d4d_denoise_window_dpm_single_cfg_split",
     "d4d_denoise_window_cfg_grid", "d4d_denoise_window_dpm_cfg_grid", "d4d_denoise_window_unipc_cfg_grid",
     "d4d_denoise_window_pndm_cfg_grid", "d4d_denoise_window_deis_cfg_grid", "d4d_denoise_window_dpm_single_cfg_grid",
+    "d4d_denoise_window_ddpm", "d4d_denoise_window_ddpm_sharded", "d4d_denoise_window_ddpm_cfg_split",
+    "d4d_denoise_window_ddpm_cfg_grid", "d4d_cfg_ddpm_step", "d4d_op_ddpm_noise",
 ]
 
 
@@ -80,6 +82,13 @@ class D4DDpmSingleSched(C.Structure):
     ]
 
 
+class D4DDdpmSched(C.Structure):
+    _fields_ = [
+        ("timesteps_table", C.c_void_p), ("coefs", C.c_void_p), ("n_steps", C.c_int32), ("prediction_type", C.c_int32),
+        ("clip_sample", C.c_int32), ("clip_sample_range", C.c_float), ("emulate_bf16", C.c_int32), ("seed", C.c_uint64),
+    ]
+
+
 class D4DError(RuntimeError):
     pass
 
@@ -129,9 +138,11 @@ def _load(path: str) -> C.CDLL:
                                           i32, vp, vp, vp, vp]
     l.d4d_denoise_window_dpm_single.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.POINTER(D4DDpmSingleSched), f32, i32, i32,
                                                 i32, i32, i32, vp, vp, vp, vp, vp]
+    l.d4d_denoise_window_ddpm.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.POINTER(D4DDdpmSched), f32, i32, i32, i32, i32,
+                                          i32, vp, vp]
     # the CFG-split and CFG-grid window steps take their single-GPU counterparts' arguments
     for name in ("d4d_denoise_window", "d4d_denoise_window_dpm", "d4d_denoise_window_unipc", "d4d_denoise_window_pndm",
-                 "d4d_denoise_window_deis", "d4d_denoise_window_dpm_single"):
+                 "d4d_denoise_window_deis", "d4d_denoise_window_dpm_single", "d4d_denoise_window_ddpm"):
         for mode in ("_cfg_split", "_cfg_grid"):
             getattr(l, name + mode).argtypes = getattr(l, name).argtypes
     l.d4d_assemble_input.argtypes = [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]
@@ -145,6 +156,8 @@ def _load(path: str) -> C.CDLL:
                                     vp, vp]
     l.d4d_cfg_dpm_single_step.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.POINTER(D4DDpmSingleSched), f32, i32,
                                           i32, i32, i32, vp, vp]
+    l.d4d_cfg_ddpm_step.argtypes = [vp, vp, vp, vp, vp, vp, C.POINTER(D4DDdpmSched), f32, i32, i32, i32, i32, vp, vp]
+    l.d4d_op_ddpm_noise.argtypes = [C.c_uint64, vp, vp, i32, i32, i32, vp, vp]
     l.d4d_op_gemm.argtypes = [vp, i32, i32, vp, i32, i32, vp, i32, i32, f32p, vp, i32, i32, vp, i32, vp, i32, i32,
                               i32, f32, i32, vp, i32, vp]
     l.d4d_op_gemm_tiled.argtypes = [vp, i32, i32, vp, i32, i32, vp, i32, i32, f32p, vp, i32, i32, vp, i32, vp, i32, i32,
@@ -172,6 +185,8 @@ def _load(path: str) -> C.CDLL:
                                              i32, i32, vp]
     l.d4d_denoise_window_dpm_sharded.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.POINTER(D4DDpmSched), f32, i32, i32, i32,
                                                  i32, i32, i32, vp, vp, vp]
+    l.d4d_denoise_window_ddpm_sharded.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.POINTER(D4DDdpmSched), f32, i32, i32, i32,
+                                                  i32, i32, i32, vp, vp]
     l.d4d_window_exchange.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp]
     l.d4d_op_window_scatter.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, C.c_size_t, vp]
     for name in EXPORTS:
@@ -182,7 +197,8 @@ def _load(path: str) -> C.CDLL:
                 "d4d_denoise_window_sharded", "d4d_denoise_window_dpm_sharded", "d4d_window_exchange", "d4d_debug_tap",
                 "d4d_denoise_window_unipc", "d4d_conv_tile_choice", "d4d_gemm_tile_choice", "d4d_denoise_window_pndm",
                 "d4d_cfg_pndm_step", "d4d_denoise_window_deis", "d4d_cfg_deis_step", "d4d_denoise_window_dpm_single",
-                "d4d_cfg_dpm_single_step") or name.endswith(("_cfg_split", "_cfg_grid")):
+                "d4d_cfg_dpm_single_step", "d4d_denoise_window_ddpm", "d4d_denoise_window_ddpm_sharded",
+                "d4d_cfg_ddpm_step") or name.endswith(("_cfg_split", "_cfg_grid")):
             fn.restype = C.c_int
     return l
 

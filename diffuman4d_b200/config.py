@@ -210,3 +210,21 @@ class DPMSingleConfig:
     lower_order_final: bool = False
     final_sigmas_type: str = "zero"       # or "sigma_min"
     timestep_spacing: str = "linspace"    # the only spacing upstream has
+
+
+@dataclass
+class DDPMConfig:
+    """DDPM scheduler knobs (upstream diffusers==0.33.1 ``DDPMScheduler`` defaults) that the fused step implements:
+    ancestral sampling with a fixed variance ("fixed_small", "fixed_small_log" or "fixed_large"), no thresholding, betas
+    from a linear or scaled-linear schedule, DDIM's timestep spacings.  The noise of each step is counter-based
+    (include/d4d.h ``d4d_ddpm_sched``), not torch's RNG stream."""
+    num_train_timesteps: int = 1000
+    beta_start: float = 0.0001
+    beta_end: float = 0.02
+    beta_schedule: str = "linear"         # or "scaled_linear"
+    variance_type: str = "fixed_small"    # or "fixed_small_log", "fixed_large"
+    clip_sample: bool = True
+    clip_sample_range: float = 1.0
+    prediction_type: str = "epsilon"      # or "v_prediction", "sample"
+    timestep_spacing: str = "leading"     # or "linspace", "trailing"
+    steps_offset: int = 0

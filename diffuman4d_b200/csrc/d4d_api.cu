@@ -131,6 +131,13 @@ d4d::WindowStep dpm_single_step(const d4d_dpm_single_sched* sched, void* x0_prev
   return s;
 }
 
+d4d::WindowStep ddpm_step(const d4d_ddpm_sched* sched, const int64_t* frame_ids) {
+  d4d::WindowStep s;
+  s.ddpm = sched;
+  s.state.frame_ids = reinterpret_cast<const long long*>(frame_ids);
+  return s;
+}
+
 // the step arguments of every d4d_cfg_*_step entry point
 d4d::StepArgs step_args(const void* noise, const void* latents, const void* cond_mask, const int64_t* timestep_indices,
                         int64_t* timestep_indices_out, float guidance_scale, int cfg, int F, int height, int width,
@@ -150,7 +157,7 @@ d4d::StepArgs step_args(const void* noise, const void* latents, const void* cond
 extern "C" {
 
 const char* d4d_last_error(void) { return d4d::g_last_error.c_str(); }
-int d4d_version(void) { return 114; }
+int d4d_version(void) { return 115; }
 
 int d4d_create(const d4d_config* cfg, int device, d4d_handle** out) {
   D4D_API_BEGIN
@@ -306,6 +313,14 @@ int d4d_denoise_window_dpm_single(d4d_handle* h, void* latents, const void* pixe
                         0, height, width, num_steps, stream);
 }
 
+int d4d_denoise_window_ddpm(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                            const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                            const d4d_ddpm_sched* sched, float guidance_scale, int domain, int F, int height, int width,
+                            int num_steps, const int64_t* frame_ids, void* stream) {
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
+                        ddpm_step(sched, frame_ids), guidance_scale, domain, F, 0, height, width, num_steps, stream);
+}
+
 int d4d_assemble_input(void* latents, const void* pixel_latents, const void* plucker, const void* skel_latents,
                        const void* cond_mask, const int64_t* timestep_indices, const int64_t* timesteps_table,
                        int n_steps, int F, int height, int width, int cfg, void* sample_out, int64_t* timestep_out,
@@ -413,6 +428,29 @@ int d4d_cfg_dpm_single_step(const void* noise, const void* latents, const void* 
   return d4d::cfg_step_run(step_args(noise, latents, cond_mask, timestep_indices, timestep_indices_out, guidance_scale, cfg,
                                      F, height, width, latents_out),
                            *sched, st, static_cast<cudaStream_t>(stream));
+  D4D_API_END
+}
+
+int d4d_cfg_ddpm_step(const void* noise, const void* latents, const void* cond_mask, const int64_t* timestep_indices,
+                      int64_t* timestep_indices_out, const int64_t* frame_ids, const d4d_ddpm_sched* sched,
+                      float guidance_scale, int cfg, int F, int height, int width, void* latents_out, void* stream) {
+  D4D_API_BEGIN
+  D4D_REQUIRE(sched != nullptr, "null argument");
+  d4d::SolverState st;
+  st.frame_ids = reinterpret_cast<const long long*>(frame_ids);
+  return d4d::cfg_step_run(step_args(noise, latents, cond_mask, timestep_indices, timestep_indices_out, guidance_scale, cfg,
+                                     F, height, width, latents_out),
+                           *sched, st, static_cast<cudaStream_t>(stream));
+  D4D_API_END
+}
+
+int d4d_op_ddpm_noise(uint64_t seed, const int64_t* frame_ids, const int64_t* timestep_indices, int F, int height,
+                      int width, float* out, void* stream) {
+  D4D_API_BEGIN
+  D4D_REQUIRE(height > 0 && width > 0, "latent height/width");
+  return d4d::ddpm_noise_run(seed, reinterpret_cast<const long long*>(frame_ids),
+                             reinterpret_cast<const long long*>(timestep_indices), F, height * width, out,
+                             static_cast<cudaStream_t>(stream));
   D4D_API_END
 }
 
@@ -653,6 +691,16 @@ int d4d_denoise_window_dpm_sharded(d4d_handle* h, void* latents, const void* pix
                         width, num_steps, stream);
 }
 
+int d4d_denoise_window_ddpm_sharded(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                    const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                    const d4d_ddpm_sched* sched, float guidance_scale, int domain, int F_local,
+                                    int F_total, int height, int width, int num_steps, const int64_t* frame_ids,
+                                    void* stream) {
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
+                        ddpm_step(sched, frame_ids), guidance_scale, domain, F_local, F_total, height, width, num_steps,
+                        stream);
+}
+
 int d4d_window_exchange(d4d_handle* h, const void* latents_local, const int64_t* timestep_indices_local,
                         const void* x0_prev_local, const int32_t* lower_order_nums_local, int F_local, int F_total,
                         int height, int width, void* latents_out, int64_t* timestep_indices_out, void* x0_prev_out,
@@ -742,6 +790,15 @@ int d4d_denoise_window_dpm_single_cfg_split(d4d_handle* h, void* latents, const 
                         0, height, width, num_steps, stream, d4d::CfgMode::kSplit);
 }
 
+int d4d_denoise_window_ddpm_cfg_split(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                      const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                      const d4d_ddpm_sched* sched, float guidance_scale, int domain, int F, int height,
+                                      int width, int num_steps, const int64_t* frame_ids, void* stream) {
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
+                        ddpm_step(sched, frame_ids), guidance_scale, domain, F, 0, height, width, num_steps, stream,
+                        d4d::CfgMode::kSplit);
+}
+
 int d4d_denoise_window_cfg_grid(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
                                 const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
                                 const d4d_sched* sched, float guidance_scale, int domain, int F, int height, int width,
@@ -797,6 +854,15 @@ int d4d_denoise_window_dpm_single_cfg_grid(d4d_handle* h, void* latents, const v
   return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
                         dpm_single_step(sched, x0_prev, x0_prev2, cur_sample, lower_order_nums), guidance_scale, domain, F,
                         0, height, width, num_steps, stream, d4d::CfgMode::kGrid);
+}
+
+int d4d_denoise_window_ddpm_cfg_grid(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                     const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                     const d4d_ddpm_sched* sched, float guidance_scale, int domain, int F, int height,
+                                     int width, int num_steps, const int64_t* frame_ids, void* stream) {
+  return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
+                        ddpm_step(sched, frame_ids), guidance_scale, domain, F, 0, height, width, num_steps, stream,
+                        d4d::CfgMode::kGrid);
 }
 
 int d4d_exchange_alloc(d4d_handle* h, size_t kv_bytes, unsigned char* handles_out) {

@@ -2,6 +2,7 @@
 // tensor-core kernels, the pose-encoder's small-channel convolutions, and the fused pipeline pieces
 // (input assembly, CFG combine + per-frame scheduler step).  All global traffic is 128-bit where the
 // layout allows it.
+#include "ddpm_noise.cuh"
 #include "kernels.h"
 
 namespace d4d {
@@ -360,13 +361,32 @@ __device__ __forceinline__ bool step_frame(const StepArgs& a, int n_steps, const
   return true;
 }
 
-// The model output at element j of the frames: the CFG combine u + g * (c - u) of the two halves, or the one prediction.
+// The CFG combine u + g * (c - u) of the two halves' predictions u (negative) and c (positive).
+template <bool EMU>
+__device__ __forceinline__ float cfg_combine(const StepArgs& a, float u, float c) {
+  return rnd<EMU>(u + rnd<EMU>(a.guidance * rnd<EMU>(c - u)));
+}
+
+// The model output at element j of the frames: the CFG combine of the two halves, or the one prediction.
 template <bool EMU>
 __device__ __forceinline__ float model_output(const StepArgs& a, size_t j) {
   if (!a.cfg) return __bfloat162float(a.noise[j]);
-  const float u = __bfloat162float(a.noise[j]);
-  const float c = __bfloat162float(a.noise[static_cast<size_t>(a.F) * a.chw + j]);
-  return rnd<EMU>(u + rnd<EMU>(a.guidance * rnd<EMU>(c - u)));
+  return cfg_combine<EMU>(a, __bfloat162float(a.noise[j]),
+                          __bfloat162float(a.noise[static_cast<size_t>(a.F) * a.chw + j]));
+}
+
+// four consecutive bf16 as fp32 (one 8-byte load; p 8-byte aligned), and the reverse, rounding to nearest
+__device__ __forceinline__ void load_bf16x4(const bf16* p, float v[4]) {
+  const uint2 r = *reinterpret_cast<const uint2*>(p);
+  v[0] = __uint_as_float(r.x << 16); v[1] = __uint_as_float(r.x & 0xFFFF0000u);
+  v[2] = __uint_as_float(r.y << 16); v[3] = __uint_as_float(r.y & 0xFFFF0000u);
+}
+__device__ __forceinline__ void store_bf16x4(bf16* p, const float v[4]) {
+  const __nv_bfloat162 lo = __floats2bfloat162_rn(v[0], v[1]), hi = __floats2bfloat162_rn(v[2], v[3]);
+  uint2 r;
+  r.x = *reinterpret_cast<const unsigned int*>(&lo);
+  r.y = *reinterpret_cast<const unsigned int*>(&hi);
+  *reinterpret_cast<uint2*>(p) = r;
 }
 
 // convert_model_output: the data prediction of model output m at sample x (alpha_t, sigma_t of the step), computed in
@@ -403,6 +423,53 @@ __global__ void cfg_ddim_kernel(const StepArgs a, const d4d_sched s) {
     const float dir = rnd<EMU>(sdir * eps);
     const float prev = rnd<EMU>(rnd<EMU>(sa_prev * x0) + dir);
     a.out[base + i] = __float2bfloat16_rn(prev);
+  }
+}
+
+// upstream DDPMScheduler.step (fixed variances): x0 by prediction type, the clip, the posterior mean c0 * x0 + c1 * x and,
+// on rows with t > 0, std * z with z of ddpm_noise.cuh keyed by the frame's task index st.frame_ids[f] and its row.  A
+// thread steps four consecutive elements, the four draws of one Philox call, with 8-byte loads and stores.
+template <bool EMU>
+__global__ void cfg_ddpm_kernel(const StepArgs a, const d4d_ddpm_sched s, const SolverState st) {
+  long long idx;
+  int lon;
+  if (!step_frame(a, s.n_steps, nullptr, nullptr, 0, idx, lon)) return;
+  const size_t base = static_cast<size_t>(blockIdx.y) * a.chw;
+  const float* k = s.coefs + idx * kDdpmCoefs;
+  const float sa = k[0], sb = k[1], c0 = k[2], c1 = k[3], std = k[4];
+  const bool noisy = k[5] != 0.f;
+  const uint32_t frame = static_cast<uint32_t>(st.frame_ids[blockIdx.y]);
+  for (int q = blockIdx.x * blockDim.x + threadIdx.x; q < a.chw / 4; q += gridDim.x * blockDim.x) {
+    double z[4] = {0.0, 0.0, 0.0, 0.0};
+    if (noisy) ddpm_normal4(s.seed, static_cast<uint32_t>(q), frame, static_cast<uint32_t>(idx), z);
+    const size_t e = base + 4 * static_cast<size_t>(q);
+    float x[4], m[4], prev[4];
+    load_bf16x4(a.latents + e, x);
+    load_bf16x4(a.noise + e, m);
+    if (a.cfg) {
+      float c[4];
+      load_bf16x4(a.noise + static_cast<size_t>(a.F) * a.chw + e, c);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) m[j] = cfg_combine<EMU>(a, m[j], c[j]);
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      float x0 = data_prediction<EMU>(s.prediction_type, x[j], m[j], sa, sb);
+      if (s.clip_sample) x0 = fminf(fmaxf(x0, -s.clip_sample_range), s.clip_sample_range);
+      prev[j] = rnd<EMU>(rnd<EMU>(c0 * x0) + rnd<EMU>(c1 * x[j]));
+      if (noisy) prev[j] = rnd<EMU>(prev[j] + rnd<EMU>(std * round_noise<EMU>(z[j])));
+    }
+    store_bf16x4(a.out + e, prev);
+  }
+}
+
+__global__ void ddpm_noise_kernel(unsigned long long seed, const long long* __restrict__ frame_ids,
+                                  const long long* __restrict__ ts_idx, int quads, float* __restrict__ out) {
+  const int f = blockIdx.y;
+  for (int q = blockIdx.x * blockDim.x + threadIdx.x; q < quads; q += gridDim.x * blockDim.x) {
+    double z[4];
+    ddpm_normal4(seed, static_cast<uint32_t>(q), static_cast<uint32_t>(frame_ids[f]), static_cast<uint32_t>(ts_idx[f]), z);
+    for (int j = 0; j < 4; ++j) out[(static_cast<size_t>(f) * quads + q) * 4 + j] = round_noise<false>(z[j]);
   }
 }
 
@@ -906,6 +973,30 @@ int cfg_step_run(const StepArgs& a, const d4d_dpm_single_sched& s, const SolverS
   D4D_REQUIRE((st.x0_prev2 != nullptr) == (s.solver_order == 3), "x0_prev2 is given exactly when solver_order is 3");
   if (!launch) return 0;
   return launch_step(cfg_dpm_single_kernel<true>, cfg_dpm_single_kernel<false>, s.emulate_bf16, stream, a, s, st);
+}
+
+int cfg_step_run(const StepArgs& a, const d4d_ddpm_sched& s, const SolverState& st, cudaStream_t stream, bool launch) {
+  if (int rc = check_step(a, s.timesteps_table, s.coefs, s.n_steps, s.prediction_type, nullptr)) return rc;
+  D4D_REQUIRE(st.frame_ids != nullptr, "null argument");
+  const auto aligned8 = [](const void* p) { return reinterpret_cast<uintptr_t>(p) % 8 == 0; };
+  D4D_REQUIRE(aligned8(a.noise) && aligned8(a.latents) && aligned8(a.out),
+              "the DDPM step needs 8-byte aligned noise, latents and output");
+  if (!launch) return 0;
+  // a thread steps four elements: a grid sized by the quads of a frame, not its elements
+  dim3 grid(min(64, blocks_for(a.chw / 4, 256)), a.F);
+  (s.emulate_bf16 ? cfg_ddpm_kernel<true> : cfg_ddpm_kernel<false>)<<<grid, 256, 0, stream>>>(a, s, st);
+  D4D_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int ddpm_noise_run(unsigned long long seed, const long long* frame_ids, const long long* ts_idx, int F, int hw, float* out,
+                   cudaStream_t stream) {
+  D4D_REQUIRE(frame_ids && ts_idx && out, "null argument");
+  D4D_REQUIRE(F > 0 && hw > 0, "the frame count and latent size must be positive");
+  dim3 grid(min(64, blocks_for(hw, 256)), F);
+  ddpm_noise_kernel<<<grid, 256, 0, stream>>>(seed, frame_ids, ts_idx, hw, out);
+  D4D_CUDA_OK(cudaGetLastError());
+  return 0;
 }
 
 }  // namespace d4d

@@ -216,15 +216,16 @@ int assemble_input_run(const AssembleArgs& a, cudaStream_t stream);
 
 // a-13 + a-14: CFG combine + per-frame scheduler step (pipeline_diffuman4d.py:408-423): DDIM, DPM-Solver++ (dpmsolver++ /
 // midpoint, order <= 2), UniPC (predict_x0, bh1 / bh2, order <= 2; the UniC corrector of the frame's previous step,
-// then the UniP predictor), PNDM (skip_prk_steps: the PLMS steps), DEIS (deis / logrho, order <= 3) or DPM-Solver++
-// singlestep (dpmsolver++ / midpoint, order <= 3).  The scheduler's constants, step count, prediction type and bf16
-// emulation come from its table struct in include/d4d.h, passed as it is; the multistep solvers' coefficient rows are
-// laid out there too.
+// then the UniP predictor), PNDM (skip_prk_steps: the PLMS steps), DEIS (deis / logrho, order <= 3), DPM-Solver++
+// singlestep (dpmsolver++ / midpoint, order <= 3) or DDPM (ancestral sampling with the counter-based noise of
+// ddpm_noise.cuh).  The scheduler's constants, step count, prediction type and bf16 emulation come from its table struct
+// in include/d4d.h, passed as it is; the coefficient rows of the schedulers that have them are laid out there too.
 constexpr int kDpmCoefs = 6;
 constexpr int kUniPCCoefs = 14;
 constexpr int kPndmCoefs = 10;
 constexpr int kDeisCoefs = 11;
 constexpr int kDpmSingleCoefs = 13;
+constexpr int kDdpmCoefs = 6;
 struct StepArgs {
   const bf16* noise;        // [(cfg?2:1)*F,4,h,w]
   const bf16* latents;      // [F,4,h,w]
@@ -248,6 +249,7 @@ struct SolverState {
   bf16* cur_sample = nullptr;
   bf16* m_prev = nullptr;       // [F,4,h,w]: each frame's previous DEIS model output, in its epsilon form
   bf16* m_prev2 = nullptr;      // [F,4,h,w]: the one before (DEIS at solver_order 3)
+  const long long* frame_ids = nullptr;  // [F]: each frame's index in its task, DDPM's noise counter (no history)
   // [F]: steps each frame has taken, capped at solver_order (PNDM: uncapped, its `counter`)
   const int* lower_order_nums = nullptr;
   int* lower_order_nums_out = nullptr;    // [F]: the advanced counts (may not alias lower_order_nums)
@@ -264,6 +266,11 @@ int cfg_step_run(const StepArgs& a, const d4d_deis_sched& s, const SolverState& 
                  bool launch = true);
 int cfg_step_run(const StepArgs& a, const d4d_dpm_single_sched& s, const SolverState& st, cudaStream_t stream,
                  bool launch = true);
+int cfg_step_run(const StepArgs& a, const d4d_ddpm_sched& s, const SolverState& st, cudaStream_t stream,
+                 bool launch = true);
+// The DDPM step's noise alone, in fp32: out [F,4,h,w] for frames frame_ids [F] at timestep indices ts_idx [F]
+int ddpm_noise_run(unsigned long long seed, const long long* frame_ids, const long long* ts_idx, int F, int hw, float* out,
+                   cudaStream_t stream);
 
 // cross-rank K/V arrival flags (frame-sharded window): signal = system-scope release of `epoch` into slot `my_rank` of
 // every rank's flag array; wait = acquire-spin until all `world` slots of the local array reach `epoch`

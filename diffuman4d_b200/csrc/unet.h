@@ -109,7 +109,7 @@ struct WindowBufs {  // scratch of d4d_denoise_window for one (F, h, w, cfg)
 // The scheduler of a window step: exactly one of the tables is set.  The stateful schedulers (DPM-Solver++, UniPC,
 // PNDM, DEIS, DPM-Solver++ singlestep) also get the window frames' solver state, read and updated in place: the order
 // counts are read from state.lower_order_nums and the advanced ones end up in state.lower_order_nums_out, both the
-// caller's array.
+// caller's array.  DDPM gets the frames' task indices in state.frame_ids.
 struct WindowStep {
   const d4d_sched* ddim = nullptr;
   const d4d_dpm_sched* dpm = nullptr;
@@ -117,16 +117,18 @@ struct WindowStep {
   const d4d_pndm_sched* pndm = nullptr;
   const d4d_deis_sched* deis = nullptr;
   const d4d_dpm_single_sched* dpm_single = nullptr;
+  const d4d_ddpm_sched* ddpm = nullptr;
   SolverState state;
   // the number of tables set (a valid step has one)
   int tables() const {
     return (ddim != nullptr) + (dpm != nullptr) + (unipc != nullptr) + (pndm != nullptr) + (deis != nullptr) +
-           (dpm_single != nullptr);
+           (dpm_single != nullptr) + (ddpm != nullptr);
   }
   // fn(table) with whichever table is set
   template <typename Fn>
   int with_table(Fn&& fn) const {
-    return ddim ? fn(*ddim) : dpm ? fn(*dpm) : unipc ? fn(*unipc) : pndm ? fn(*pndm) : deis ? fn(*deis) : fn(*dpm_single);
+    return ddim ? fn(*ddim) : dpm ? fn(*dpm) : unipc ? fn(*unipc) : pndm ? fn(*pndm) : deis ? fn(*deis)
+           : dpm_single ? fn(*dpm_single) : fn(*ddpm);
   }
 };
 

@@ -19,7 +19,7 @@ from typing import Callable, List, Optional, Union
 
 import torch
 
-from .config import (DEISConfig, DPMSingleConfig, DPMSolverConfig, PNDMConfig, SchedulerConfig, UNetConfig,
+from .config import (DDPMConfig, DEISConfig, DPMSingleConfig, DPMSolverConfig, PNDMConfig, SchedulerConfig, UNetConfig,
                      UniPCConfig)
 from .pipeline import B200Diffuman4DPipeline
 from .unet import B200MultiviewUNet
@@ -252,8 +252,43 @@ def dpm_single_config_from_json(d: dict) -> DPMSingleConfig:
         final_sigmas_type=d.get("final_sigmas_type", "zero"))
 
 
+def ddpm_config_from_json(d: dict) -> DDPMConfig:
+    """Map a diffusers ``DDPMScheduler`` config; every knob the fused step does not implement raises
+    ``NotImplementedError`` naming the key."""
+    def refuse(key, why):
+        raise NotImplementedError(f"DDPMScheduler {key}={d.get(key)!r} is not supported by the CUDA path ({why})")
+
+    def want(key, allowed, default):
+        v = d.get(key, default)
+        if v not in allowed:
+            refuse(key, f"supported: {allowed}")
+        return v
+
+    if d.get("thresholding", False):
+        refuse("thresholding", "dynamic thresholding is not implemented")
+    if d.get("rescale_betas_zero_snr", False):
+        refuse("rescale_betas_zero_snr", "zero-SNR rescaling is not implemented")
+    if d.get("trained_betas") is not None:
+        refuse("trained_betas", "betas come from beta_schedule")
+    vt = d.get("variance_type", "fixed_small")
+    if vt in ("learned", "learned_range"):
+        refuse("variance_type", "a learned variance needs a UNet with 2 * out_channels outputs")
+    if vt == "fixed_large_log":
+        refuse("variance_type", "upstream takes the square root of a log there")
+    want("variance_type", ("fixed_small", "fixed_small_log", "fixed_large"), "fixed_small")
+    want("beta_schedule", ("linear", "scaled_linear"), "linear")
+    want("prediction_type", ("epsilon", "v_prediction", "sample"), "epsilon")
+    want("timestep_spacing", ("leading", "linspace", "trailing"), "leading")
+    return DDPMConfig(
+        num_train_timesteps=d.get("num_train_timesteps", 1000), beta_start=d.get("beta_start", 0.0001),
+        beta_end=d.get("beta_end", 0.02), beta_schedule=d.get("beta_schedule", "linear"), variance_type=vt,
+        clip_sample=d.get("clip_sample", True), clip_sample_range=d.get("clip_sample_range", 1.0),
+        prediction_type=d.get("prediction_type", "epsilon"), timestep_spacing=d.get("timestep_spacing", "leading"),
+        steps_offset=d.get("steps_offset", 0))
+
+
 def scheduler_config_from_json(d: dict) -> Union[SchedulerConfig, DPMSolverConfig, UniPCConfig, PNDMConfig, DEISConfig,
-                                                 DPMSingleConfig]:
+                                                 DPMSingleConfig, DDPMConfig]:
     cls = d.get("_class_name", "DDIMScheduler")
     if cls == "DPMSolverMultistepScheduler":
         return dpm_solver_config_from_json(d)
@@ -265,9 +300,11 @@ def scheduler_config_from_json(d: dict) -> Union[SchedulerConfig, DPMSolverConfi
         return deis_config_from_json(d)
     if cls == "DPMSolverSinglestepScheduler":
         return dpm_single_config_from_json(d)
+    if cls == "DDPMScheduler":
+        return ddpm_config_from_json(d)
     if cls != "DDIMScheduler":
         raise NotImplementedError(
-            f"scheduler {cls} is not fused on the CUDA path (DDIMScheduler, DPMSolverMultistepScheduler, "
+            f"scheduler {cls} is not fused on the CUDA path (DDIMScheduler, DDPMScheduler, DPMSolverMultistepScheduler, "
             "UniPCMultistepScheduler, PNDMScheduler, DEISMultistepScheduler and DPMSolverSinglestepScheduler only); run "
             "the reference's Python scheduler loop for other classes")
     if d.get("thresholding", False):

@@ -367,3 +367,34 @@ def cfg_dpm_single_step(noise: torch.Tensor, latents: torch.Tensor, cond_mask: t
     return _multistep_step("d4d_cfg_dpm_single_step", noise, latents, cond_mask, timestep_indices,
                            [("x0_prev", x0_prev), ("x0_prev2", x0_prev2), ("cur_sample", cur_sample)], lower_order_nums,
                            sched, guidance_scale, cfg)
+
+
+def cfg_ddpm_step(noise: torch.Tensor, latents: torch.Tensor, cond_mask: torch.Tensor, timestep_indices: torch.Tensor,
+                  frame_ids: torch.Tensor, sched, guidance_scale: float, cfg: bool):
+    """One CFG + DDPM step of F frames (``sched``: a ``d4d_ddpm_sched`` from ``DDPMTables.c_struct``, which carries the
+    noise seed).  ``noise`` [(cfg?2:1)*F,4,h,w]; ``frame_ids`` int64 [F]: each frame's index in its task.  Returns (new
+    latents, advanced timestep indices)."""
+    _bf16c(noise, "noise"), _bf16c(latents, "latents"), _bf16c(cond_mask, "cond_mask")
+    F, _, h, w = latents.shape
+    for name, t in (("timestep_indices", timestep_indices), ("frame_ids", frame_ids)):
+        if t.dtype != torch.int64 or not t.is_cuda or not t.is_contiguous() or t.numel() != F:
+            raise ValueError(f"{name} must be a contiguous CUDA int64 [F] tensor")
+    out = torch.empty_like(latents)
+    ti_out = torch.empty_like(timestep_indices)
+    check(lib().d4d_cfg_ddpm_step(_p(noise), _p(latents), _p(cond_mask), _p(timestep_indices), _p(ti_out), _p(frame_ids),
+                                  C.byref(sched), float(guidance_scale), int(cfg), F, h, w, _p(out), _stream()),
+          "d4d_cfg_ddpm_step")
+    return out, ti_out
+
+
+def ddpm_noise(seed: int, frame_ids: torch.Tensor, timestep_indices: torch.Tensor, h: int, w: int) -> torch.Tensor:
+    """The DDPM step's noise z of frames ``frame_ids`` (int64 [F]) at ``timestep_indices`` (int64 [F]) for the task
+    ``seed``, rounded once to fp32: [F, 4, h, w]."""
+    F = frame_ids.numel()
+    for name, t in (("frame_ids", frame_ids), ("timestep_indices", timestep_indices)):
+        if t.dtype != torch.int64 or not t.is_cuda or not t.is_contiguous() or t.numel() != F:
+            raise ValueError(f"{name} must be a contiguous CUDA int64 [F] tensor")
+    out = torch.empty(F, 4, h, w, dtype=torch.float32, device=frame_ids.device)
+    check(lib().d4d_op_ddpm_noise(int(seed) & 0xFFFFFFFFFFFFFFFF, _p(frame_ids), _p(timestep_indices), F, h, w, _p(out),
+                                  _stream()), "d4d_op_ddpm_noise")
+    return out

@@ -5,9 +5,10 @@ Seams (SURVEY.md section 8b):
        (reference src/diffusers/pipelines/diffuman4d/pipeline_diffuman4d.py:345-425): input assembly, UNet, CFG
        combine and the F per-frame scheduler steps run as ONE C-ABI call (no per-frame host sync).  The scheduler is DDIM
        (``SchedulerConfig``), DPM-Solver++ (``DPMSolverConfig``), UniPC (``UniPCConfig``), PNDM (``PNDMConfig``), DEIS
-       (``DEISConfig``) or DPM-Solver++ singlestep (``DPMSingleConfig``); the stateful ones keep a per-frame history on
-       the device (``DPMSolverState`` / ``UniPCState`` / ``PNDMState`` / ``DEISState`` / ``DPMSingleState``) in place of
-       the reference's per-frame scheduler copies.
+       (``DEISConfig``), DPM-Solver++ singlestep (``DPMSingleConfig``) or DDPM (``DDPMConfig``); the stateful ones keep a
+       per-frame history on the device (``DPMSolverState`` / ``UniPCState`` / ``PNDMState`` / ``DEISState`` /
+       ``DPMSingleState``) in place of the reference's per-frame scheduler copies, and DDPM's per-frame handles carry
+       the task's noise seed and the frames' indices in the task (``DDPMTask``).
   B-4  ``sliding_iterative_denoise`` == PIPE:439-559: same arguments, same ValueErrors, same returned dict.  The VAE
        (stock AutoencoderKL, out of scope per SURVEY section 8f) is pluggable: pass ``vae`` with ``encode_latents(x)`` /
        ``decode_latents(z)`` callables, or feed latents directly (``pixel_values_latents=...``).
@@ -23,9 +24,9 @@ from typing import Callable, List, Optional, Union
 import torch
 
 from ._lib import check, lib
-from .config import DEISConfig, DPMSingleConfig, DPMSolverConfig, PNDMConfig, SchedulerConfig, UniPCConfig
-from .scheduler import (DDIMTables, DEISTables, DPMSingleTables, DPMSolverFrame, DPMSolverTables, PNDMTables,
-                        SolverState, UniPCTables)
+from .config import DDPMConfig, DEISConfig, DPMSingleConfig, DPMSolverConfig, PNDMConfig, SchedulerConfig, UniPCConfig
+from .scheduler import (DDIMTables, DDPMFrames, DDPMTables, DEISTables, DPMSingleTables, DPMSolverFrame, DPMSolverTables,
+                        PNDMTables, SolverState, UniPCTables, draw_seed)
 from .unet import _DOMAIN_IDS, B200MultiviewUNet
 
 
@@ -68,7 +69,7 @@ def resize_conditions(plucker_embeds: torch.Tensor, cond_masks: torch.Tensor, h:
 class B200Diffuman4DPipeline:
     def __init__(self, unet: B200MultiviewUNet,
                  scheduler_config: Union[SchedulerConfig, DPMSolverConfig, UniPCConfig, PNDMConfig, DEISConfig,
-                                         DPMSingleConfig, None] = None,
+                                         DPMSingleConfig, DDPMConfig, None] = None,
                  vae=None, emulate_bf16_scheduler: bool = False):
         self.unet = unet
         self.vae = vae
@@ -84,6 +85,8 @@ class B200Diffuman4DPipeline:
             self.scheduler = DEISTables(scheduler_config, device=self.device)
         elif isinstance(scheduler_config, DPMSingleConfig):
             self.scheduler = DPMSingleTables(scheduler_config, device=self.device)
+        elif isinstance(scheduler_config, DDPMConfig):
+            self.scheduler = DDPMTables(scheduler_config, device=self.device)
         else:
             self.scheduler = DDIMTables(scheduler_config, device=self.device)
         self.emulate_bf16_scheduler = emulate_bf16_scheduler
@@ -112,13 +115,23 @@ class B200Diffuman4DPipeline:
     def _multistep(self) -> bool:
         return self.scheduler.state_planes is not None
 
+    @property
+    def _ddpm(self) -> bool:
+        return isinstance(self.scheduler, DDPMTables)
+
+    @property
+    def _per_frame(self) -> bool:
+        """Whether ``parepare_schedulers`` hands out per-frame handles (a multistep solver or DDPM)."""
+        return self._multistep or self._ddpm
+
     def parepare_schedulers(self, num_inference_steps: int, num_frames: int):
         """PIPE:265-271.  The per-frame deep copies exist in the reference only because scheduler objects are
         stateful; DDIM is stateless, so one table serves all frames.  DPM-Solver++ (multistep and singlestep), UniPC,
         PNDM and DEIS get a fresh (zeroed) device state for the frames, and one ``DPMSolverFrame`` handle per frame in
-        place of each copy."""
+        place of each copy.  DDPM's handles belong to a fresh ``DDPMTask``, whose noise seed is drawn when the task first
+        runs (``__call__`` or the sliding loop)."""
         ts = self.scheduler.set_timesteps(num_inference_steps)
-        if self._multistep:
+        if self._per_frame:
             return self.scheduler.new_state(num_frames).frames(), ts
         return [self.scheduler] * num_frames, ts
 
@@ -129,7 +142,8 @@ class B200Diffuman4DPipeline:
         """One window: ``num_inference_steps`` x (assemble -> UNet -> CFG -> per-frame scheduler step).  ``latents``
         [F,4,h,w] and ``timestep_indices`` [F] (int64, device) are updated IN PLACE and returned.  With DPM-Solver++,
         UniPC, PNDM, DEIS or DPM-Solver++ singlestep, ``solver_state`` is the window frames' ``DPMSolverState`` /
-        ``UniPCState`` / ``PNDMState`` / ``DEISState`` / ``DPMSingleState`` (``take``), also updated in place."""
+        ``UniPCState`` / ``PNDMState`` / ``DEISState`` / ``DPMSingleState`` (``take``), also updated in place.  With
+        DDPM it is the window's ``DDPMFrames`` (``DDPMTask.take``): the task's noise seed and the frames' task indices."""
         return self._window_step(latents=latents, pixel_values_latents=pixel_values_latents,
                                  plucker_embeds_latents=plucker_embeds_latents, skeletons_latents=skeletons_latents,
                                  cond_masks_latents=cond_masks_latents, timestep_indices=timestep_indices, domain=domain,
@@ -168,13 +182,24 @@ class B200Diffuman4DPipeline:
         plk = prep(plucker_embeds_latents, "plucker_embeds_latents")
         skl = prep(skeletons_latents, "skeletons")
         msk = prep(cond_masks_latents, "cond_masks_latents")
-        sched = self.scheduler.c_struct(self.emulate_bf16_scheduler)
+        extra = []
+        if self._ddpm:   # the noise seed in the table struct, the frames' task indices after num_inference_steps
+            st = solver_state
+            if not isinstance(st, DDPMFrames):
+                raise ValueError("the DDPM scheduler needs the window's DDPMFrames as solver_state")
+            ids = st.frame_ids
+            if not (ids.is_cuda and ids.dtype == torch.int64 and ids.is_contiguous() and ids.numel() == F_):
+                raise ValueError("solver_state.frame_ids must be a contiguous CUDA int64 [F] tensor")
+            sched = self.scheduler.c_struct(self.emulate_bf16_scheduler, st.seed)
+            extra.append(ids.data_ptr())
+        else:
+            sched = self.scheduler.c_struct(self.emulate_bf16_scheduler)
         self._guidance_scale = guidance_scale
         g = guidance_scale if self.do_classifier_free_guidance else 1.0
         frames = (F_,) if F_total is None else (F_, F_total)
         args = [self.unet._h, latents.data_ptr(), pix.data_ptr(), plk.data_ptr(), skl.data_ptr(), msk.data_ptr(),
                 timestep_indices.data_ptr(), C.byref(sched), float(g), _DOMAIN_IDS[domain], *frames, h, w,
-                int(num_inference_steps)]
+                int(num_inference_steps), *extra]
         if self._multistep:   # the state planes in ABI order (None: passed as NULL), then lower_order_nums
             st = solver_state
             if st is None:
@@ -216,13 +241,15 @@ class B200Diffuman4DPipeline:
         lat = (latents * self.scheduler.init_noise_sigma).to(device=self.device, dtype=torch.bfloat16).contiguous().clone()
         ti = timestep_indices.to(device=self.device, dtype=torch.int64).contiguous().clone()
         task, frames, window_state = None, None, None
-        if self._multistep:   # the frames' solver history travels with the `schedulers` handles
+        if self._per_frame:   # the frames' solver history or task indices travel with the `schedulers` handles
             if len(schedulers) != F_ or not all(isinstance(s, DPMSolverFrame) for s in schedulers):
                 raise ValueError("schedulers must be the per-frame handles of parepare_schedulers, one per frame")
             task = schedulers[0].state
             if any(s.state is not task for s in schedulers):
                 raise ValueError("schedulers must all come from one parepare_schedulers call")
             frames = torch.tensor([s.index for s in schedulers], dtype=torch.int64)
+            if self._ddpm and task.seed is None:
+                task.seed = int(draw_seed(unused.get("generator"), self.device).item())
             window_state = task.take(frames, *lat.shape[2:])
         self.denoise_window(latents=lat, pixel_values_latents=pixel_values_latents,
                             plucker_embeds_latents=plucker_embeds_latents, skeletons_latents=skeletons_latents,
@@ -263,7 +290,7 @@ class B200Diffuman4DPipeline:
                  share_noise: Optional[Callable] = None):
         """The B-4 loop around ``window_step(window, lw, tiw, sw, conds, ...) -> (lw, sw)``, which returns the window's
         updated latents and solver state (``FrameShardedPipeline`` runs it on a frame shard).  ``share_noise`` is applied
-        to freshly drawn initial noise."""
+        to freshly drawn initial noise and, with DDPM, to every task's noise seed."""
         dev = self.device
         if (window_size * num_denoising_steps) % sliding_stride != 0:
             raise ValueError(
@@ -312,7 +339,12 @@ class B200Diffuman4DPipeline:
         latents = (latents.to(dev, torch.bfloat16) * self.scheduler.init_noise_sigma).contiguous().clone()
 
         schedulers, _ = self.parepare_schedulers(num_inference_steps, n)   # a fresh solver state per task (PIPE:501)
-        task = schedulers[0].state if self._multistep else None
+        task = schedulers[0].state if self._per_frame else None
+        if self._ddpm:   # the task's noise seed, drawn after the initial noise; rank 0's on every rank
+            seed = draw_seed(generator, dev)
+            if share_noise is not None:
+                share_noise(seed)
+            task.seed = int(seed.item())
         target_windows, input_windows = build_windows(target_indices, input_indices, domain, window_size,
                                                       sliding_stride, sliding_shift, bidirectional)
         it = zip(target_windows, input_windows)

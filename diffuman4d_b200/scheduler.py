@@ -16,7 +16,10 @@ outputs, the sample of the frame's first step and its step counter.  ``DEISTable
 ``DEISMultistepScheduler`` (``cfg_deis_kernel``, up to third order), whose history is the last two model outputs in their
 epsilon form.  ``DPMSingleTables`` / ``DPMSingleState`` do the same for ``DPMSolverSinglestepScheduler``
 (``cfg_dpm_single_kernel``, up to third order), whose history is the last two data predictions and the sample the frame's
-current block started from.
+current block started from.  ``DDPMTables`` does the same for ``DDPMScheduler`` (``cfg_ddpm_kernel``), which keeps no
+history but draws noise: ``DDPMTask`` holds a task's noise seed and hands out one handle per frame, which knows the
+frame's index in the task; a window's ``DDPMFrames`` (``take``) carry the seed and the window frames' task indices, the
+two things besides the timestep index and element that the device noise is a function of.
 
 Each tables class names the C entry points of its window step (``window_entry_points``: plain, frame-sharded and
 CFG-split, None where there is none) and the bf16 state planes they take, in ABI order (``state_planes``; None for the stateless DDIM).
@@ -29,8 +32,8 @@ import dataclasses
 import numpy as np
 import torch
 
-from ._lib import D4DDeisSched, D4DDpmSched, D4DDpmSingleSched, D4DPndmSched, D4DSched, D4DUniPCSched
-from .config import DEISConfig, DPMSingleConfig, DPMSolverConfig, PNDMConfig, SchedulerConfig, UniPCConfig
+from ._lib import D4DDdpmSched, D4DDeisSched, D4DDpmSched, D4DDpmSingleSched, D4DPndmSched, D4DSched, D4DUniPCSched
+from .config import DDPMConfig, DEISConfig, DPMSingleConfig, DPMSolverConfig, PNDMConfig, SchedulerConfig, UniPCConfig
 
 _PRED = {"epsilon": 0, "v_prediction": 1, "sample": 2}
 
@@ -55,19 +58,8 @@ class DDIMTables:
         self._timesteps_dev = None
 
     def set_timesteps(self, n: int, device=None):
-        c = self.config
-        T = c.num_train_timesteps
-        if n > T:
-            raise ValueError(f"`num_inference_steps`: {n} cannot be larger than `self.config.train_timesteps`: {T}")
+        ts = ddim_timesteps(self.config, n)
         self.num_inference_steps = n
-        if c.timestep_spacing == "leading":
-            ts = (np.arange(0, n) * (T // n)).round()[::-1].copy().astype(np.int64) + c.steps_offset
-        elif c.timestep_spacing == "trailing":
-            ts = np.round(np.arange(T, 0, -T / n)).astype(np.int64) - 1
-        elif c.timestep_spacing == "linspace":
-            ts = np.linspace(0, T - 1, n).round()[::-1].copy().astype(np.int64)
-        else:
-            raise ValueError(f"{c.timestep_spacing} is not supported")
         self.timesteps = torch.from_numpy(ts)
         self._timesteps_dev = None
         return self.timesteps
@@ -91,6 +83,20 @@ class DDIMTables:
         s.clip_sample_range = float(c.clip_sample_range)
         s.emulate_bf16 = int(emulate_bf16)
         return s
+
+
+def ddim_timesteps(c, n: int) -> np.ndarray:
+    """``DDIMScheduler.set_timesteps(n)`` timesteps (``DDPMScheduler`` spaces its timesteps the same way)."""
+    T = c.num_train_timesteps
+    if n > T:
+        raise ValueError(f"`num_inference_steps`: {n} cannot be larger than `self.config.train_timesteps`: {T}")
+    if c.timestep_spacing == "leading":
+        return (np.arange(0, n) * (T // n)).round()[::-1].copy().astype(np.int64) + c.steps_offset
+    if c.timestep_spacing == "trailing":
+        return np.round(np.arange(T, 0, -T / n)).astype(np.int64) - 1
+    if c.timestep_spacing == "linspace":
+        return np.linspace(0, T - 1, n).round()[::-1].copy().astype(np.int64)
+    raise ValueError(f"{c.timestep_spacing} is not supported")
 
 
 def _betas(c) -> torch.Tensor:
@@ -741,3 +747,135 @@ class DPMSingleState(SolverState):
         super().__init__(num_frames, device, tuple(p for p in _dpm_single_planes(solver_order) if p), lower_order_nums,
                          x0_prev=x0_prev, x0_prev2=x0_prev2, cur_sample=cur_sample)
         self.solver_order = solver_order
+
+
+# ---- DDPM -------------------------------------------------------------------------------------------------------------
+DDPM_COEFS = 6   # row layout in include/d4d.h ``d4d_ddpm_sched``
+DDPM_VARIANCE_TYPES = ("fixed_small", "fixed_small_log", "fixed_large")
+
+
+def ddpm_step_coefficients(alphas_cumprod: torch.Tensor, timesteps, variance_type: str) -> torch.Tensor:
+    """[n, 6] coefficients of ``cfg_ddpm_kernel`` (layout in include/d4d.h ``d4d_ddpm_sched``) for the timesteps, each
+    evaluated on 0-dim tensors of ``alphas_cumprod``'s dtype in the order ``DDPMScheduler``'s ``step`` /
+    ``_get_variance`` evaluate them.  The previous timestep is the next entry of ``timesteps`` (upstream
+    ``previous_timestep``), or -1 after the last one, where the previous alpha product is 1."""
+    if variance_type not in DDPM_VARIANCE_TYPES:
+        raise NotImplementedError(f"variance_type {variance_type!r}: the fused step implements {DDPM_VARIANCE_TYPES}")
+    ts = [int(t) for t in timesteps]
+    one = torch.tensor(1.0, dtype=alphas_cumprod.dtype)
+    out = torch.zeros(len(ts), DDPM_COEFS, dtype=alphas_cumprod.dtype)
+    for i, t in enumerate(ts):
+        prev_t = ts[i + 1] if i + 1 < len(ts) else -1
+        alpha_prod_t = alphas_cumprod[t]
+        alpha_prod_t_prev = alphas_cumprod[prev_t] if prev_t >= 0 else one
+        beta_prod_t = 1 - alpha_prod_t
+        beta_prod_t_prev = 1 - alpha_prod_t_prev
+        current_alpha_t = alpha_prod_t / alpha_prod_t_prev
+        current_beta_t = 1 - current_alpha_t
+        x0_coeff = (alpha_prod_t_prev ** 0.5 * current_beta_t) / beta_prod_t
+        sample_coeff = current_alpha_t ** 0.5 * beta_prod_t_prev / beta_prod_t
+        variance = torch.clamp((1 - alpha_prod_t_prev) / (1 - alpha_prod_t) * current_beta_t, min=1e-20)
+        if variance_type == "fixed_small":
+            std = variance ** 0.5
+        elif variance_type == "fixed_small_log":
+            std = torch.exp(0.5 * torch.log(variance))
+        else:
+            std = current_beta_t ** 0.5
+        out[i] = torch.stack([alpha_prod_t ** 0.5, beta_prod_t ** 0.5, x0_coeff, sample_coeff, std,
+                              torch.tensor(float(t > 0), dtype=out.dtype)])
+    return out
+
+
+def draw_seed(generator=None, device="cpu") -> torch.Tensor:
+    """One 64-bit noise seed, an int64 [1] tensor on ``device`` drawn from ``generator`` (the default generator of
+    ``device`` when None)."""
+    info = torch.iinfo(torch.int64)
+    return torch.randint(info.min, info.max, (1,), generator=generator, device=device, dtype=torch.int64)
+
+
+class DDPMTables:
+    """Timesteps and step coefficients of ``DDPMScheduler`` (diffusers 0.33.1; fixed variances) for ``cfg_ddpm_kernel``.
+    Stateless like DDIM, but the step draws noise keyed by the task's seed and the frame's index in its task, so frames
+    get ``DDPMTask`` handles (``new_state``)."""
+    name = "DDPM"
+    init_noise_sigma = 1.0  # upstream: init_noise_sigma 1, scale_model_input is the identity
+    window_entry_points = ("d4d_denoise_window_ddpm", "d4d_denoise_window_ddpm_sharded",
+                          "d4d_denoise_window_ddpm_cfg_split")
+    state_planes = None     # no history
+
+    def __init__(self, cfg: DDPMConfig = None, device="cuda:0"):
+        self.config = c = cfg or DDPMConfig()
+        if c.prediction_type not in _PRED:
+            raise ValueError(f"prediction_type given as {c.prediction_type} must be one of {list(_PRED)}")
+        if c.variance_type not in DDPM_VARIANCE_TYPES:
+            raise NotImplementedError(f"variance_type {c.variance_type!r}: the fused step implements "
+                                      f"{DDPM_VARIANCE_TYPES}")
+        self.alphas_cumprod = torch.cumprod(1.0 - _betas(c), dim=0)
+        self.device = torch.device(device)
+        self.num_inference_steps = None
+        self.timesteps = None          # host int64 [n]
+        self.coefs = None              # host fp32 [n, 6]
+        self._dev = None
+
+    def set_timesteps(self, n: int, device=None):
+        ts = ddim_timesteps(self.config, n)
+        self.num_inference_steps = n
+        self.timesteps = torch.from_numpy(ts)
+        self.coefs = ddpm_step_coefficients(self.alphas_cumprod, ts, self.config.variance_type)
+        self._dev = None
+        return self.timesteps
+
+    def c_struct(self, emulate_bf16: bool = False, seed: int = 0) -> D4DDdpmSched:
+        if self.timesteps is None:
+            raise ValueError("call set_timesteps first")
+        if self._dev is None:
+            self._dev = (self.timesteps.to(self.device), self.coefs.to(self.device).contiguous())
+        c = self.config
+        s = D4DDdpmSched()
+        s.timesteps_table = self._dev[0].data_ptr()
+        s.coefs = self._dev[1].data_ptr()
+        s.n_steps = int(self.num_inference_steps)
+        s.prediction_type = _PRED[c.prediction_type]
+        s.clip_sample = int(c.clip_sample)
+        s.clip_sample_range = float(c.clip_sample_range)
+        s.emulate_bf16 = int(emulate_bf16)
+        s.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        return s
+
+    def new_state(self, num_frames: int) -> "DDPMTask":
+        return DDPMTask(num_frames, self.device)
+
+
+class DDPMTask:
+    """One DDPM task: its noise ``seed`` (an int, None until drawn) and ``num_frames``.  ``frames`` hands out the
+    per-frame handles of ``parepare_schedulers``; ``take`` gives a window's ``DDPMFrames``.  Nothing is stored back
+    (``put`` is a no-op): DDPM keeps no history."""
+
+    def __init__(self, num_frames: int, device, seed: int = None):
+        self.num_frames = num_frames
+        self.device = torch.device(device)
+        self.seed = seed
+
+    def frames(self) -> list:
+        return [DPMSolverFrame(self, i) for i in range(self.num_frames)]
+
+    def take(self, index: torch.Tensor, h: int = None, w: int = None) -> "DDPMFrames":
+        if self.seed is None:
+            raise ValueError("the DDPM task has no noise seed yet")
+        return DDPMFrames(self.seed, index.to(device=self.device, dtype=torch.int64).contiguous())
+
+    def put(self, index: torch.Tensor, window):
+        pass
+
+
+class DDPMFrames:
+    """The frames of one window of a DDPM task, as the step needs them: the task's ``seed`` and ``frame_ids``, the
+    frames' indices in the task (int64 [F] on the device)."""
+    __slots__ = ("seed", "frame_ids")
+
+    def __init__(self, seed: int, frame_ids: torch.Tensor):
+        self.seed, self.frame_ids = seed, frame_ids
+
+    def shard(self, lo: int, hi: int) -> "DDPMFrames":
+        """Frames ``[lo, hi)`` of the window (a rank's frame shard)."""
+        return DDPMFrames(self.seed, self.frame_ids[lo:hi].contiguous())

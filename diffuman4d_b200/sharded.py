@@ -4,7 +4,7 @@ One process per GPU (torch.distributed).  Rank r owns frames [r*F/R, (r+1)*F/R) 
 frame stay on the rank).  Everything except 3-D attention is per image and needs no communication; at each 3-D block
 the fused-QKV GEMM epilogue stores K|V straight into every rank's gathered buffer over NVLink (peer memory mapped with
 cudaIpc) -- there is no NCCL call on the data path.  torch.distributed is used to exchange the IPC handles, and once
-per task to share freshly drawn initial noise.
+per task to share freshly drawn initial noise and, with DDPM, the task's noise seed.
 
 ``sliding_iterative_denoise`` runs whole tasks this way: every rank holds the whole task, steps its shard of each
 window, and the window-result exchange (``d4d_window_exchange``, the same peer buffers) hands every rank the updated
@@ -21,7 +21,7 @@ import torch.distributed as dist
 from ._lib import check, lib
 from .pipeline import B200Diffuman4DPipeline, _check_inplace, build_windows
 from .plan import modules, pad_head_dim
-from .scheduler import DPMSolverState
+from .scheduler import DDPMFrames, DPMSolverState
 from .sharding import frame_shard
 
 
@@ -130,7 +130,8 @@ class FrameShardedPipeline:
         pix, plk, skl, msk = conds
         self.denoise_window(latents=lat, pixel_values_latents=pix, plucker_embeds_latents=plk, skeletons_latents=skl,
                             cond_masks_latents=msk, timestep_indices=ts, F_total=F_total, solver_state=state, **kw)
-        return self.window_exchange(lat, ts, state, F_total)
+        # DDPM's frames carry no state to exchange
+        return self.window_exchange(lat, ts, state if isinstance(state, DPMSolverState) else None, F_total)
 
     def _task_window(self, window, lw, tiw, sw, conds, **kw):
         """``B200Diffuman4DPipeline._task_window`` on this rank's shard: slice, step, exchange; the gathered window
@@ -139,7 +140,9 @@ class FrameShardedPipeline:
         lo, hi = self.frames(F_total)
         mine = window[lo:hi]
         state = None
-        if sw is not None:
+        if isinstance(sw, DDPMFrames):   # the local frames' task indices key their noise
+            state = sw.shard(lo, hi)
+        elif sw is not None:
             state = DPMSolverState(hi - lo, sw.device, sw.x0_prev[lo:hi].contiguous(),
                                    sw.lower_order_nums[lo:hi].contiguous())
         lat, _, out = self._step_and_exchange(lw[lo:hi].contiguous(), tiw[lo:hi].contiguous(), state,

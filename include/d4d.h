@@ -186,6 +186,34 @@ typedef struct d4d_dpm_single_sched {
   int32_t emulate_bf16;             /* 1: round like the reference's bf16 eager maths (history and every op in bf16) */
 } d4d_dpm_single_sched;
 
+/* DDPM constants for the fused step (upstream diffusers DDPMScheduler with variance_type "fixed_small",
+ * "fixed_small_log" or "fixed_large", no thresholding; d4d_version() 115 and later).  Ancestral sampling: the step adds
+ * std * z on rows with t > 0, so it is the first stochastic step.  z is a pure function of the task's 64-bit `seed`, the
+ * frame's index in its task (the `frame_ids` argument), the frame's timestep index before the step and the element:
+ * Philox4x32-10 with key = seed (low word first) and counter (e / 4, frame id, timestep index, 0) for element e of the
+ * frame's [4,h,w] latent, which takes word e % 4; a word x maps to u = (x + 0.5) * 2^-32, Box-Muller turns (u0, u1) into
+ * z0, z1 and (u2, u3) into z2, z3 in fp64, and the result is rounded once (to bf16 with emulate_bf16, as upstream draws
+ * the noise in the model output's dtype; to fp32 otherwise).  No rank, window position or launch order enters it, so
+ * every multi-GPU mode draws the single-GPU bits.  DDPM keeps no history; a frame's step index is its timestep index.
+ * coefs row i (fp32), computed on the host in the upstream scheduler's fp32 order of operations (the device evaluates no
+ * pow / log / exp), with t = timesteps[i], a_t = alphas_cumprod[t], a_prev = alphas_cumprod[timesteps[i + 1]] (1 after
+ * the last row), beta = 1 - a_t / a_prev:
+ *   [0] a_t^0.5   [1] (1 - a_t)^0.5                        (x0 by prediction type; epsilon divides by [0] like upstream)
+ *   [2] a_prev^0.5 * beta / (1 - a_t)   [3] (a_t / a_prev)^0.5 * (1 - a_prev) / (1 - a_t)   (x' = [2] * x0 + [3] * x)
+ *   [4] the noise std: fixed_small (max((1 - a_prev) / (1 - a_t) * beta, 1e-20))^0.5, fixed_small_log
+ *       exp(0.5 * log(that)), fixed_large beta^0.5
+ *   [5] 1 if t > 0 (the row adds std * z), else 0 */
+typedef struct d4d_ddpm_sched {
+  const int64_t* timesteps_table;   /* device, [n_steps]  (scheduler.timesteps after set_timesteps) */
+  const float* coefs;               /* device, [n_steps][6], see above */
+  int32_t n_steps;
+  int32_t prediction_type;          /* 0 epsilon, 1 v_prediction, 2 sample */
+  int32_t clip_sample;
+  float clip_sample_range;
+  int32_t emulate_bf16;             /* 1: round like the reference's bf16 eager maths (every op and the noise in bf16) */
+  uint64_t seed;                    /* the task's noise seed */
+} d4d_ddpm_sched;
+
 const char* d4d_last_error(void);
 int d4d_version(void);
 
@@ -294,6 +322,15 @@ int d4d_denoise_window_dpm_single(d4d_handle* h, void* latents, const void* pixe
                                   int width, int num_steps, void* x0_prev, void* x0_prev2, void* cur_sample,
                                   int32_t* lower_order_nums, void* stream);
 
+/* The same window step with a DDPM scheduler (d4d_version() 115 and later).  Arguments as d4d_denoise_window, plus
+ *   frame_ids  device int64 [F]: each window frame's index in its task, which keys its noise (see d4d_ddpm_sched)
+ * DDPM keeps no history: nothing but the latents and timestep indices is updated.  The step reads and writes four
+ * elements at a time: latents must be 8-byte aligned (a call with unaligned latents returns 1 before any launch). */
+int d4d_denoise_window_ddpm(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                            const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                            const d4d_ddpm_sched* sched, float guidance_scale, int domain, int F, int height, int width,
+                            int num_steps, const int64_t* frame_ids, void* stream);
+
 /* ---- building blocks of B-3, exported for parity tests ------------------------------------------------ */
 int d4d_assemble_input(void* latents, const void* pixel_latents, const void* plucker, const void* skel_latents,
                        const void* cond_mask, const int64_t* timestep_indices, const int64_t* timesteps_table,
@@ -338,6 +375,17 @@ int d4d_cfg_dpm_single_step(const void* noise, const void* latents, const void* 
                             void* x0_prev2, void* cur_sample, const int32_t* lower_order_nums,
                             int32_t* lower_order_nums_out, const d4d_dpm_single_sched* sched, float guidance_scale,
                             int cfg, int F, int height, int width, void* latents_out, void* stream);
+
+/* One CFG + DDPM step of the frames (d4d_version() 115 and later); frame_ids [F] as d4d_denoise_window_ddpm.
+ * timestep_indices_out receives the advanced indices (it may not alias the input); latents_out may alias latents.
+ * noise, latents and latents_out must be 8-byte aligned. */
+int d4d_cfg_ddpm_step(const void* noise, const void* latents, const void* cond_mask, const int64_t* timestep_indices,
+                      int64_t* timestep_indices_out, const int64_t* frame_ids, const d4d_ddpm_sched* sched,
+                      float guidance_scale, int cfg, int F, int height, int width, void* latents_out, void* stream);
+/* The DDPM step's noise alone (d4d_version() 115 and later): out fp32 [F,4,h,w] receives z of frames frame_ids [F]
+ * (device int64) at timestep indices timestep_indices [F] (device int64) for `seed`, rounded once to fp32. */
+int d4d_op_ddpm_noise(uint64_t seed, const int64_t* frame_ids, const int64_t* timestep_indices, int F, int height,
+                      int width, float* out, void* stream);
 
 /* ---- op-level entry points (each is one hot-path kernel; used by tests/ and bench.py) ------------------
  * d4d_op_gemm:   out[M,N] = act((A|A2)[M,K1+K2] . W[N,K]^T + bias + rowvec[row/rows_per_image]) * scale + residual
@@ -460,6 +508,13 @@ int d4d_denoise_window_sharded(d4d_handle* h, void* latents, const void* pixel_l
                                const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
                                const d4d_sched* sched, float guidance_scale, int domain, int F_local, int F_total,
                                int height, int width, int num_steps, void* stream);
+/* d4d_denoise_window_ddpm on a frame shard (d4d_version() 115 and later): frame_ids [F_local] holds the LOCAL frames'
+ * indices in their task. */
+int d4d_denoise_window_ddpm_sharded(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                    const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                    const d4d_ddpm_sched* sched, float guidance_scale, int domain, int F_local,
+                                    int F_total, int height, int width, int num_steps, const int64_t* frame_ids,
+                                    void* stream);
 /* d4d_denoise_window_dpm on a frame shard (d4d_version() 106 and later): x0_prev [F_local,4,h,w] and lower_order_nums
  * [F_local] hold the LOCAL frames' solver state. */
 int d4d_denoise_window_dpm_sharded(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
@@ -469,7 +524,7 @@ int d4d_denoise_window_dpm_sharded(d4d_handle* h, void* latents, const void* pix
                                    void* stream);
 /* Window-result exchange of the frame-sharded sliding loop (d4d_version() 106 and later): after a window step every rank
  * passes its F_local updated frames -- latents [F_local,4,h,w], timestep indices int64 [F_local] and, with DPM-Solver++,
- * x0_prev [F_local,4,h,w] and lower_order_nums int32 [F_local] (both NULL for DDIM) -- and receives the whole window,
+ * x0_prev [F_local,4,h,w] and lower_order_nums int32 [F_local] (both NULL for DDIM and DDPM) -- and receives the whole window,
  * F_total = world * F_local frames in window order, in latents_out / timestep_indices_out / x0_prev_out /
  * lower_order_nums_out (NULL exactly when the inputs are).  The frames are stored into every rank's exchange buffer at
  * row rank * F_local (d4d_op_window_scatter), one flag round publishes them, and each rank copies the gathered window out.
@@ -537,6 +592,11 @@ int d4d_denoise_window_dpm_single_cfg_split(d4d_handle* h, void* latents, const 
                                             const d4d_dpm_single_sched* sched, float guidance_scale, int domain, int F,
                                             int height, int width, int num_steps, void* x0_prev, void* x0_prev2,
                                             void* cur_sample, int32_t* lower_order_nums, void* stream);
+/* (d4d_version() 115 and later) frame_ids [F]: the whole window's, as d4d_denoise_window_ddpm */
+int d4d_denoise_window_ddpm_cfg_split(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                      const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                      const d4d_ddpm_sched* sched, float guidance_scale, int domain, int F, int height,
+                                      int width, int num_steps, const int64_t* frame_ids, void* stream);
 
 /* ---- multi-GPU: CFG grid, the CFG-split window on 2 x R ranks (d4d_version() 114 and later) -------------------------
  * The CFG-split window with each CFG half frame-sharded over R ranks.  One process per GPU, world = 2R with R in
@@ -581,6 +641,11 @@ int d4d_denoise_window_dpm_single_cfg_grid(d4d_handle* h, void* latents, const v
                                            const d4d_dpm_single_sched* sched, float guidance_scale, int domain, int F,
                                            int height, int width, int num_steps, void* x0_prev, void* x0_prev2,
                                            void* cur_sample, int32_t* lower_order_nums, void* stream);
+/* (d4d_version() 115 and later) frame_ids [F]: the whole window's, as d4d_denoise_window_ddpm */
+int d4d_denoise_window_ddpm_cfg_grid(d4d_handle* h, void* latents, const void* pixel_latents, const void* plucker,
+                                     const void* skeletons, const void* cond_mask, int64_t* timestep_indices,
+                                     const d4d_ddpm_sched* sched, float guidance_scale, int domain, int F, int height,
+                                     int width, int num_steps, const int64_t* frame_ids, void* stream);
 
 #ifdef __cplusplus
 }

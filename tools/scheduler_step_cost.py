@@ -1,16 +1,16 @@
-"""What the DPM-Solver++, UniPC, PNDM, DEIS and singlestep DPM-Solver++ steps cost against DDIM in the window step of
+"""What the DPM-Solver++, UniPC, PNDM, DEIS, singlestep DPM-Solver++ and DDPM steps cost against DDIM in the window step of
 bench.py's workload (W16 @ 64x64 latents, CFG 2.0, SD-2.1 channel layout, random weights), on one GPU in one process.
 
-The six pipelines share one UNet; rounds alternate DDIM, DPM-Solver++, UniPC, PNDM, DEIS and singlestep DPM-Solver++ so
-that clock drift hits all alike.
+The seven pipelines share one UNet; rounds alternate DDIM, DPM-Solver++, UniPC, PNDM, DEIS, singlestep DPM-Solver++ and
+DDPM, in an order rotated by one arm each round, so that clock drift and the position in a round hit all alike.
 Each step restores its inputs (latents, timestep indices and, for the multistep schedulers, the frames' solver state) from
 device copies and then makes ONE public ``denoise_window`` call.  The multistep frames start with a full history, so the
 timed step is the second-order one; the UniPC target frames also sit two steps further into the schedule, so that both
 its corrector and its predictor run at order 2, the PNDM frames have taken five steps, so that they combine four
 model outputs, the DEIS (solver_order 3) frames sit at the UniPC rows with a full history, so that every one takes
 the third-order step, and the singlestep (solver_order 3) frames sit on third-order rows of its order list with a full
-history, so that every one takes the third-order update from its block's start sample.  Also times the six fused step
-kernels alone.  Prints one JSON line (and writes it to --out) with the
+history, so that every one takes the third-order update from its block's start sample; every DDPM target frame sits on a
+row with t > 0, so that every one draws its noise.  Also times the seven fused step kernels alone.  Prints one JSON line (and writes it to --out) with the
 card's name, power limit and max SM clock beside the numbers.
 
     python tools/scheduler_step_cost.py --rounds 8 --steps 10 --out /tmp/scheduler_step_cost.json
@@ -43,10 +43,11 @@ def main():
     from bench import WORKLOAD, gpu_identity, synth_inputs
     from diffuman4d_b200 import ops
     from diffuman4d_b200._lib import check, lib
-    from diffuman4d_b200.config import (DEISConfig, DPMSingleConfig, DPMSolverConfig, PNDMConfig, SchedulerConfig,
-                                        UNetConfig, UniPCConfig)
+    from diffuman4d_b200.config import (DDPMConfig, DEISConfig, DPMSingleConfig, DPMSolverConfig, PNDMConfig,
+                                        SchedulerConfig, UNetConfig, UniPCConfig)
     from diffuman4d_b200.pipeline import B200Diffuman4DPipeline
-    from diffuman4d_b200.scheduler import DEISState, DPMSingleState, DPMSolverState, PNDMState, UniPCState
+    from diffuman4d_b200.scheduler import (DDPMTask, DEISState, DPMSingleState, DPMSolverState, PNDMState,
+                                           UniPCState)
     from diffuman4d_b200.unet import B200MultiviewUNet
     from diffuman4d_b200.weights import random_state_dict
 
@@ -62,7 +63,8 @@ def main():
     pndm = B200Diffuman4DPipeline(unet, PNDMConfig())
     deis = B200Diffuman4DPipeline(unet, DEISConfig(solver_order=3))
     single = B200Diffuman4DPipeline(unet, DPMSingleConfig(solver_order=3))
-    for p in (ddim, dpm, unipc, pndm, deis, single):
+    ddpm = B200Diffuman4DPipeline(unet, DDPMConfig())
+    for p in (ddim, dpm, unipc, pndm, deis, single, ddpm):
         p.parepare_schedulers(wl["n_steps"], F)
 
     inp = {k: (v.to(torch.bfloat16) if v.dtype.is_floating_point else v).to(dev)
@@ -88,6 +90,7 @@ def main():
     assert all(single.scheduler.order_list[int(i)] == 3 for i in ts_single[n_cond:])
     cur_init = torch.randn(F, 4, h, w, device=dev, generator=g).to(torch.bfloat16)
     state_s = DPMSingleState(F, dev, solver_order=3).take(torch.arange(F), h, w)
+    frames_p = DDPMTask(F, dev, seed=1234).take(torch.arange(F))   # every target row has t > 0: the noise is drawn
 
     def window(p, solver_state=None, ts_init=inp["ts"]):
         def step():
@@ -111,7 +114,7 @@ def main():
                 solver_state.last_sample.copy_(last_init)
                 solver_state.x0_prev.copy_(x0_init)
                 solver_state.lower_order_nums.copy_(lon2_init)
-            elif solver_state is not None:
+            elif isinstance(solver_state, DPMSolverState):   # DDPM's frames have no state to restore
                 solver_state.x0_prev.copy_(x0_init)
                 solver_state.lower_order_nums.copy_(lon_init)
             p.denoise_window(latents=lat, pixel_values_latents=inp["pixel"], plucker_embeds_latents=inp["plucker"],
@@ -123,6 +126,7 @@ def main():
     noise = torch.randn(2 * F, 4, h, w, device=dev, generator=g).to(torch.bfloat16)
     ddim_s, dpm_s, unipc_s = ddim.scheduler.c_struct(), dpm.scheduler.c_struct(), unipc.scheduler.c_struct()
     pndm_s, deis_s, single_s = pndm.scheduler.c_struct(), deis.scheduler.c_struct(), single.scheduler.c_struct()
+    ddpm_s = ddpm.scheduler.c_struct(False, frames_p.seed)
     out = torch.empty_like(lat)
     ts_out = torch.empty_like(ts)
     x0_k, lon_k = x0_init.clone(), lon_init.clone()
@@ -154,6 +158,9 @@ def main():
     def single_kernel():
         ops.cfg_dpm_single_step(noise, lat, inp["mask"], ts_s, x0_s, x02_s, cur_s, lon_s, single_s, wl["guidance"], True)
 
+    def ddpm_kernel():
+        ops.cfg_ddpm_step(noise, lat, inp["mask"], ts, frames_p.frame_ids, ddpm_s, wl["guidance"], True)
+
     def timed(fn, n):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
@@ -165,22 +172,24 @@ def main():
 
     arms = {"ddim": window(ddim), "dpm_solver++": window(dpm, state), "unipc": window(unipc, state_u, ts_unipc),
             "pndm": window(pndm, state_p), "deis": window(deis, state_d, ts_unipc),
-            "dpm_single": window(single, state_s, ts_single)}
+            "dpm_single": window(single, state_s, ts_single), "ddpm": window(ddpm, frames_p)}
     for fn in arms.values():                                             # warm-up: plans, buffers, clocks
         for _ in range(3):
             fn()
     torch.cuda.synchronize()
     per_round = {k: [] for k in arms}
-    kernel = {"ddim": [], "dpm_solver++": [], "unipc": [], "pndm": [], "deis": [], "dpm_single": []}
-    for _ in range(args.rounds):
-        for k, fn in arms.items():
-            per_round[k].append(timed(fn, args.steps))
+    kernel = {"ddim": [], "dpm_solver++": [], "unipc": [], "pndm": [], "deis": [], "dpm_single": [], "ddpm": []}
+    names = list(arms)
+    for r in range(args.rounds):
+        for k in names[r % len(names):] + names[:r % len(names)]:   # rotated: no arm always runs first in a round
+            per_round[k].append(timed(arms[k], args.steps))
         kernel["ddim"].append(timed(ddim_kernel, args.kernel_iters))
         kernel["dpm_solver++"].append(timed(dpm_kernel, args.kernel_iters))
         kernel["unipc"].append(timed(unipc_kernel, args.kernel_iters))
         kernel["pndm"].append(timed(pndm_kernel, args.kernel_iters))
         kernel["deis"].append(timed(deis_kernel, args.kernel_iters))
         kernel["dpm_single"].append(timed(single_kernel, args.kernel_iters))
+        kernel["ddpm"].append(timed(ddpm_kernel, args.kernel_iters))
     med = {k: statistics.median(v) for k, v in per_round.items()}
     kmed = {k: statistics.median(v) for k, v in kernel.items()}
     res = {"workload": wl["name"], "gpu": gpu_identity(0), "rounds": args.rounds, "steps_per_round": args.steps,
@@ -192,10 +201,11 @@ def main():
            "pndm_minus_ddim_ms": med["pndm"] - med["ddim"],
            "deis_minus_ddim_ms": med["deis"] - med["ddim"],
            "dpm_single_minus_ddim_ms": med["dpm_single"] - med["ddim"],
+           "ddpm_minus_ddim_ms": med["ddpm"] - med["ddim"],
            "step_kernel_us_median": {k: 1e3 * v for k, v in kmed.items()},
            "note": "DPM-Solver++ and UniPC steps timed in their second-order branches (every frame has a full history, "
                    "UniPC corrects at order 2), PNDM in its four-output branch, DEIS and singlestep DPM-Solver++ in "
-                   "their third-order branches; the kernel-only multistep times include the op wrappers' output "
+                   "their third-order branches, DDPM with noise drawn on every target frame; the kernel-only multistep times include the op wrappers' output "
                    "allocations"}
     line = json.dumps(res)
     print(line)
