@@ -26,6 +26,7 @@ EXPORTS = [
     "d4d_denoise_window_pndm_cfg_grid", "d4d_denoise_window_deis_cfg_grid", "d4d_denoise_window_dpm_single_cfg_grid",
     "d4d_denoise_window_ddpm", "d4d_denoise_window_ddpm_sharded", "d4d_denoise_window_ddpm_cfg_split",
     "d4d_denoise_window_ddpm_cfg_grid", "d4d_cfg_ddpm_step", "d4d_op_ddpm_noise",
+    "d4d_unet_forward_cfg_split", "d4d_unet_forward_cfg_grid",
 ]
 
 
@@ -145,6 +146,9 @@ def _load(path: str) -> C.CDLL:
                  "d4d_denoise_window_deis", "d4d_denoise_window_dpm_single", "d4d_denoise_window_ddpm"):
         for mode in ("_cfg_split", "_cfg_grid"):
             getattr(l, name + mode).argtypes = getattr(l, name).argtypes
+    # the UNet alone on the CFG split and grid takes d4d_unet_forward's arguments
+    for mode in ("_cfg_split", "_cfg_grid"):
+        getattr(l, "d4d_unet_forward" + mode).argtypes = l.d4d_unet_forward.argtypes
     l.d4d_assemble_input.argtypes = [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]
     l.d4d_cfg_ddim_step.argtypes = [vp, vp, vp, vp, vp, C.POINTER(D4DSched), f32, i32, i32, i32, i32, vp, vp]
     l.d4d_cfg_dpm_step.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, C.POINTER(D4DDpmSched), f32, i32, i32, i32, i32, vp, vp]

@@ -15,6 +15,10 @@ every rank runs the plain single-GPU step, exchanges nothing, and gains nothing 
 ``CFGGridPipeline`` runs the same window step on 2R ranks (R = 1, 2, 3 or 4): each CFG half is frame-sharded over R
 ranks, whose 3-D attention layers exchange K|V among themselves like the frame-sharded window, and every rank's noise
 shard still lands in every rank's exchange buffer, so the step stays replicated and no solver state moves.
+
+Both also run the UNet alone (seam B-2): ``unet_forward`` and the ``.unet`` object, a drop-in ``pipeline.unet``, forward
+the reference's CFG batch [F negative | F positive] with each rank on its share and hand every rank the whole noise.  A
+caller that keeps the reference's own scheduler loop on every rank thus gets the split or the grid for any scheduler.
 """
 from __future__ import annotations
 
@@ -26,6 +30,7 @@ import torch.distributed as dist
 from .pipeline import B200Diffuman4DPipeline, build_windows
 from .sharded import FrameShardedPipeline, exchange_bytes, open_exchange
 from .sharding import frame_shard
+from .unet import UNetMultiviewConditionOutput
 
 
 def noise_exchange_bytes(cfg, max_frames: int, h: int, w: int) -> int:
@@ -67,7 +72,8 @@ class CFGSplitPipeline:
         self._check_world(dist.get_world_size(group))
         self.pipe = pipe
         self.group = group
-        self.rank, self.world = open_exchange(pipe, self._exchange_bytes(pipe.unet.config, max_frames, h, w), group)
+        self.exchange_nbytes = self._exchange_bytes(pipe.unet.config, max_frames, h, w)
+        self.rank, self.world = open_exchange(pipe, self.exchange_nbytes, group)
 
     @staticmethod
     def _check_world(world: int):
@@ -85,6 +91,36 @@ class CFGSplitPipeline:
         ``B200Diffuman4DPipeline.denoise_window``, on the whole window on every rank.  SPMD: both ranks make the same
         calls with the same arguments."""
         return self.pipe._window_step(cfg_split=True, **kw)
+
+    # B-2 ---------------------------------------------------------------------------------------------------------
+    _unet_entry = "d4d_unet_forward_cfg_split"
+
+    def _check_unet_batch(self, n_domains: int, F: int, h: int, w: int):
+        """Raises what the library's CFG forward refuses, before any library call: other than one or two domains, or
+        two domains whose gathered noise does not fit the exchange buffer."""
+        if n_domains not in (1, 2):
+            raise ValueError("the CFG split / grid forward takes one domain (no CFG halves) or two (the CFG batch "
+                             f"[F negative | F positive]), not {n_domains}")
+        if n_domains == 2:
+            need = noise_exchange_bytes(self.pipe.unet.config, F, h, w)
+            if need > self.exchange_nbytes:
+                raise ValueError(f"the batch's noise ({need} bytes) does not fit the exchange buffer "
+                                 f"({self.exchange_nbytes} bytes); construct the pipeline with a larger max_frames")
+
+    def unet_forward(self, sample, timestep, skeletons=None, domains=None, num_frames: int = 1):
+        """B-2 with this rank forwarding its share of the batch: the arguments and checks of
+        ``B200MultiviewUNet.forward``, and a new [B, out_channels, h, w] tensor of the whole batch's noise on every rank,
+        bit-identical to the single-GPU forward.  Two domains are the reference's CFG batch [F negative | F positive]
+        (``num_frames`` = F), one domain a batch without CFG halves, which every rank forwards whole.  SPMD: every rank
+        makes the same calls with the whole batch."""
+        return self.pipe.unet._forward(sample, timestep, skeletons, domains, num_frames, cfg_entry=self._unet_entry,
+                                       cfg_check=self._check_unet_batch)
+
+    @property
+    def unet(self) -> "CFGSplitUNet":
+        """A drop-in ``pipeline.unet`` (seam B-2) that runs ``unet_forward``: ``pipeline.register_modules(unet=sp.unet)``
+        on every rank."""
+        return CFGSplitUNet(self)
 
     def _task_window(self, window, lw, tiw, sw, conds, **kw):
         """``B200Diffuman4DPipeline._task_window`` with the CFG-split step."""
@@ -124,6 +160,18 @@ class CFGGridPipeline(CFGSplitPipeline):
             raise ValueError(f"the CFG grid runs on 2 * R ranks with R in 1..4 (or 1 as a loopback), not {world}")
 
     _exchange_bytes = staticmethod(grid_exchange_bytes)
+    _unet_entry = "d4d_unet_forward_cfg_grid"
+
+    def _check_unet_batch(self, n_domains: int, F: int, h: int, w: int):
+        """``CFGSplitPipeline._check_unet_batch``; with two domains, also F divisible by R and, for R > 1, one half's
+        largest 3-D K|V layer within the exchange buffer."""
+        super()._check_unet_batch(n_domains, F, h, w)
+        if n_domains == 2:
+            grid_noise_rows(F, self.rank, self.world)
+            need = exchange_bytes(self.pipe.unet.config, F, h, w, cfg_halves=1)
+            if grid_cell(self.rank, self.world)[2] > 1 and need > self.exchange_nbytes:
+                raise ValueError(f"one CFG half's K/V layers ({need} bytes) do not fit the exchange buffer "
+                                 f"({self.exchange_nbytes} bytes); construct the pipeline with a larger max_frames")
 
     def denoise_window(self, **kw):
         """B-3 with this rank running the UNet on its frame shard of its CFG half: the arguments, checks and in-place
@@ -156,3 +204,39 @@ class CFGGridPipeline(CFGSplitPipeline):
             num_denoising_steps=num_denoising_steps, alternation_rounds=alternation_rounds,
             guidance_scale=guidance_scale, tqdm=tqdm, pixel_values_latents=pixel_values_latents,
             skeletons_latents=skeletons_latents, generator=generator)
+
+
+class CFGSplitUNet:
+    """``pipeline.unet`` for the reference's ``Diffuman4DPipeline.__call__`` (seam B-2, SURVEY.md section 8b) on the CFG
+    split or grid: the call signature of ``B200MultiviewUNet`` and its ``.config``, ``.dtype``, ``.device`` and
+    ``.to()``, with every forward run by ``CFGSplitPipeline.unet_forward``.  SPMD: every rank runs the same loop, so a
+    stochastic scheduler must be seeded the same on every rank."""
+
+    def __init__(self, split: CFGSplitPipeline):
+        self._split = split
+
+    @property
+    def config(self):
+        return self._split.pipe.unet.config
+
+    @property
+    def dtype(self):
+        return self._split.pipe.unet.dtype
+
+    @property
+    def device(self):
+        return self._split.pipe.unet.device
+
+    def to(self, *args, **kwargs):
+        """``B200MultiviewUNet.to``: accepted for interface compatibility; the model is pinned to its GPU."""
+        self._split.pipe.unet.to(*args, **kwargs)
+        return self
+
+    def eval(self):
+        return self
+
+    def forward(self, sample, timestep, skeletons=None, domains=None, num_frames: int = 1, return_dict: bool = True):
+        out = self._split.unet_forward(sample, timestep, skeletons, domains, num_frames)
+        return UNetMultiviewConditionOutput(sample=out) if return_dict else (out,)
+
+    __call__ = forward

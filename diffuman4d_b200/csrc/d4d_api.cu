@@ -53,6 +53,19 @@ int unet_forward(d4d_handle* h, const void* sample, const int64_t* timestep, con
   D4D_API_END
 }
 
+// d4d_unet_forward_cfg_split (mode kSplit) and d4d_unet_forward_cfg_grid (kGrid)
+int unet_forward_cfg(d4d_handle* h, const void* sample, const int64_t* timestep, const void* skeletons,
+                     const int32_t* domain_ids, int n_domains, int B, int F, int height, int width, void* out, void* stream,
+                     d4d::CfgMode mode) {
+  D4D_API_BEGIN
+  D4D_REQUIRE(h != nullptr, "null handle");
+  DeviceGuard g(h->model->device());
+  return h->model->unet_forward_cfg(static_cast<const bf16*>(sample), reinterpret_cast<const long long*>(timestep),
+                                    static_cast<const bf16*>(skeletons), domain_ids, n_domains, B, F, height, width,
+                                    static_cast<bf16*>(out), static_cast<cudaStream_t>(stream), mode);
+  D4D_API_END
+}
+
 // every d4d_denoise_window* entry point: `step` names the scheduler table and the frames' solver state; F_total = 0 runs
 // the single-GPU plan; mode kSplit runs this rank's CFG half (the *_cfg_split entry points), kGrid its frame shard of
 // its CFG half (the *_cfg_grid entry points)
@@ -157,7 +170,7 @@ d4d::StepArgs step_args(const void* noise, const void* latents, const void* cond
 extern "C" {
 
 const char* d4d_last_error(void) { return d4d::g_last_error.c_str(); }
-int d4d_version(void) { return 115; }
+int d4d_version(void) { return 116; }
 
 int d4d_create(const d4d_config* cfg, int device, d4d_handle** out) {
   D4D_API_BEGIN
@@ -863,6 +876,20 @@ int d4d_denoise_window_ddpm_cfg_grid(d4d_handle* h, void* latents, const void* p
   return denoise_window(h, latents, pixel_latents, plucker, skeletons, cond_mask, timestep_indices,
                         ddpm_step(sched, frame_ids), guidance_scale, domain, F, 0, height, width, num_steps, stream,
                         d4d::CfgMode::kGrid);
+}
+
+int d4d_unet_forward_cfg_split(d4d_handle* h, const void* sample, const int64_t* timestep, const void* skeletons,
+                               const int32_t* domain_ids, int n_domains, int B, int F, int height, int width, void* out,
+                               void* stream) {
+  return unet_forward_cfg(h, sample, timestep, skeletons, domain_ids, n_domains, B, F, height, width, out, stream,
+                          d4d::CfgMode::kSplit);
+}
+
+int d4d_unet_forward_cfg_grid(d4d_handle* h, const void* sample, const int64_t* timestep, const void* skeletons,
+                              const int32_t* domain_ids, int n_domains, int B, int F, int height, int width, void* out,
+                              void* stream) {
+  return unet_forward_cfg(h, sample, timestep, skeletons, domain_ids, n_domains, B, F, height, width, out, stream,
+                          d4d::CfgMode::kGrid);
 }
 
 int d4d_exchange_alloc(d4d_handle* h, size_t kv_bytes, unsigned char* handles_out) {

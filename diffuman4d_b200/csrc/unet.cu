@@ -1220,27 +1220,12 @@ int Model::denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker,
   const int Co = cfg_.out_channels;
   D4D_REQUIRE(Cin == cfg_.in_channels, "in_channels does not match the latent/plucker/skeleton/mask channel layout");
   D4D_REQUIRE(skeletons != nullptr, "skeletons required");
-  const int world = xch_.world;
   if (mode == CfgMode::kGrid)
-    D4D_REQUIRE(world == 1 || world == 2 || world == 4 || world == 6 || world == 8,
-                "the CFG grid runs on 2 * R ranks with R in {1, 2, 3, 4} (or 1 as a loopback)");
-  // frame shards per CFG half: R > 1 only on a grid of 4, 6 or 8 ranks
-  const int R = mode == CfgMode::kGrid && world > 1 ? world / 2 : 1;
-  Plan* grid_plan = nullptr;  // R > 1: this rank's plan, built before any launch (it refuses a too small K/V buffer)
-  if (split) {
-    D4D_REQUIRE(xch_.ready, "the CFG-split window needs d4d_exchange_open first");
-    D4D_REQUIRE(mode == CfgMode::kGrid || world <= 2, "the CFG-split window runs on 1 (loopback) or 2 ranks");
-    D4D_REQUIRE(F > 0 && h > 0 && w > 0, "empty window");
-    D4D_REQUIRE(F % R == 0, "the window's frames (" + std::to_string(F) + ") must be divisible by the frame shards per CFG "
-                "half (" + std::to_string(R) + ")");
-    D4D_REQUIRE(2ull * F * Co * h * w * sizeof(bf16) <= xch_.kv_bytes,
-                "the window's noise (2 * F * out_channels * h * w bf16) does not fit the exchange buffer (d4d_exchange_alloc)");
-    if (R > 1) {
-      const int doms1[1] = {domain};
-      const int k = xch_.rank / R;
-      if (int rc = get_plan(doms1, 1, F / R, F / R, h, w, &grid_plan, F, pose && k == 0 ? F / R : 0, R)) return rc;
-    }
-  }
+    if (int rc = cfg_world_check(mode)) return rc;
+  const int doms[2] = {domain, domain};
+  int R = 1;  // frame shards per CFG half: R > 1 only on a grid of 4, 6 or 8 ranks
+  if (split)
+    if (int rc = cfg_split_prepare(mode, doms, F, h, w, true, &R)) return rc;
   D4D_CUDA_OK(cudaSetDevice(device_));
   const std::string key = std::to_string(B) + "_" + std::to_string(F) + "_" + std::to_string(h) + "_" + std::to_string(w);
   auto it = wbufs_.find(key);
@@ -1260,7 +1245,6 @@ int Model::denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker,
   WindowBufs& wb = *it->second;
   const bool multistep = step.state.lower_order_nums != nullptr;
   if (multistep && !wb.order_tmp) D4D_CUDA_OK(cudaMalloc(&wb.order_tmp, sizeof(int) * F));
-  const int doms[2] = {domain, domain};
   const int hw = h * w;
   // The scheduler step runs in place (each element is read and written by the same thread); the counters go through
   // ts_tmp / order_tmp, since a kernel may not overwrite the counters its other blocks still read.
@@ -1286,33 +1270,28 @@ int Model::denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker,
     a.n_steps = n_steps; a.F = F; a.h = h; a.w = w; a.cfg = cfg_on ? 1 : 0;
     a.sample = wb.sample; a.timestep_out = wb.timestep;
     if (split) {
-      // CFG split / grid (DESIGN.md section 7): the UNet on this rank's half k (a loopback runs both) of its frame shard r
-      // (Fr = F / R frames), its noise stored at rows [k*F + r*Fr, k*F + (r+1)*Fr) of the exchange buffer parity that
-      // follows the forward's n3d K/V exchanges, on every rank; one flag round; the step reads the gathered [2F] noise in
-      // place.  Every rank then computes the step from the same bits.
-      const int Fr = F / R, r = xch_.rank % R;
-      const int k0 = world == 1 ? 0 : xch_.rank / R, k1 = world == 1 ? 2 : k0 + 1;
-      const unsigned int n3d = grid_plan ? static_cast<unsigned int>(grid_plan->n3d) : 0u;
+      // CFG split / grid (DESIGN.md section 7): this rank assembles the input rows of its frame shard r (Fr = F / R
+      // frames) of its half k (a loopback both halves), half k at rows [k*F, k*F + Fr) of the window's buffers, and
+      // forwards them; the step reads the gathered [2F] noise in place.  Every rank then computes the step from the same
+      // bits.
+      const int Fr = F / R;
+      int k0, k1, r;
+      cfg_cell(R, &k0, &k1, &r);
+      CfgHalfRows rows[2];
       for (int k = k0; k < k1; ++k) {
         a.half = k;
         // a grid rank writes sample rows for its frame shard only, but overwrites every cond frame's latents, so that
         // every rank's whole-window latents stay those of the single-GPU step
         if (R > 1) { a.f0 = r * Fr; a.n_f = Fr; }
+        a.sample = wb.sample + static_cast<size_t>(k) * F * Cin * hw;
+        a.timestep_out = wb.timestep + static_cast<size_t>(k) * F;
         if (int rc = assemble_input_run(a, stream)) return rc;
-        const unsigned int e = xch_.epoch_base + n3d;
-        NchwDst dst = {};
-        dst.n = world;
-        for (int g = 0; g < world; ++g)
-          dst.p[g] = static_cast<bf16*>(xch_.peer_kv[e & 1][g]) + (static_cast<size_t>(k) * F + r * Fr) * Co * hw;
-        // every negative skeleton is the constant image wb.skel[0]: the negative half encodes it once (pose_neg = Fr)
-        const bf16* skel_in = pose ? (k == 0 ? wb.skel : skeletons + static_cast<size_t>(r) * Fr * 3 * 64 * hw) : nullptr;
-        if (int rc = forward(wb.sample, wb.timestep, skel_in, doms, 1, Fr, Fr, h, w, dst, stream, R > 1 ? F : 0,
-                             pose && k == 0 ? Fr : 0, R > 1 ? R : 0))
-          return rc;
+        rows[k].sample = a.sample;
+        rows[k].timestep = a.timestep_out;
+        // every negative skeleton is the constant image wb.skel[0]: the negative half encodes it once
+        if (pose) rows[k].skeletons = k == 0 ? wb.skel : skeletons + static_cast<size_t>(r) * Fr * 3 * 64 * hw;
       }
-      const unsigned int e = xch_.epoch_base;  // the exchange the flag round closes: the noise's buffer parity
-      if (int rc = flag_round(stream)) return rc;
-      sa.noise = static_cast<const bf16*>(xch_.kv[e & 1]);
+      if (int rc = cfg_split_forward(rows, doms, F, h, w, R, true, stream, &sa.noise)) return rc;
     } else {
       if (int rc = assemble_input_run(a, stream)) return rc;
       const bf16* skel_in = nullptr;
@@ -1348,6 +1327,113 @@ int Model::flag_round(cudaStream_t stream) {
   xch_.epoch_base += 1;  // the stores are enqueued: every rank counts this exchange, whatever happens below
   if (int rc = kv_signal_run(f, stream)) return rc;
   return kv_wait_run(f, stream);
+}
+
+int Model::cfg_split_prepare(CfgMode mode, const int* domain_ids, int F, int h, int w, bool neg_const, int* R_out) {
+  const int world = xch_.world;
+  D4D_REQUIRE(xch_.ready, "the CFG-split window needs d4d_exchange_open first");
+  if (int rc = cfg_world_check(mode)) return rc;
+  D4D_REQUIRE(F > 0 && h > 0 && w > 0, "empty window");
+  for (int k = 0; k < 2; ++k)  // both halves on every rank, so that no rank goes on alone
+    D4D_REQUIRE(domain_ids[k] == 0 || domain_ids[k] == 1, "Invalid domain for temporal embedding");
+  const int R = mode == CfgMode::kGrid && world > 1 ? world / 2 : 1;
+  D4D_REQUIRE(F % R == 0, "the window's frames (" + std::to_string(F) + ") must be divisible by the frame shards per CFG "
+              "half (" + std::to_string(R) + ")");
+  D4D_REQUIRE(2ull * F * cfg_.out_channels * h * w * sizeof(bf16) <= xch_.kv_bytes,
+              "the window's noise (2 * F * out_channels * h * w bf16) does not fit the exchange buffer (d4d_exchange_alloc)");
+  const bool pose = cfg_.enable_pose_encoder != 0;
+  const int Fr = F / R;
+  int k0, k1, r;
+  cfg_cell(R, &k0, &k1, &r);
+  for (int k = k0; k < k1; ++k) {
+    Plan* p = nullptr;
+    if (int rc = get_plan(domain_ids + k, 1, Fr, Fr, h, w, &p, R > 1 ? F : 0, pose && neg_const && k == 0 ? Fr : 0,
+                          R > 1 ? R : 0))
+      return rc;
+  }
+  *R_out = R;
+  return 0;
+}
+
+int Model::cfg_world_check(CfgMode mode) const {
+  const int world = xch_.world;
+  if (mode == CfgMode::kGrid)
+    D4D_REQUIRE(world == 1 || world == 2 || world == 4 || world == 6 || world == 8,
+                "the CFG grid runs on 2 * R ranks with R in {1, 2, 3, 4} (or 1 as a loopback)");
+  D4D_REQUIRE(mode == CfgMode::kGrid || world <= 2, "the CFG-split window runs on 1 (loopback) or 2 ranks");
+  return 0;
+}
+
+void Model::cfg_cell(int R, int* k0, int* k1, int* r) const {
+  *k0 = xch_.world == 1 ? 0 : xch_.rank / R;
+  *k1 = xch_.world == 1 ? 2 : *k0 + 1;
+  *r = xch_.rank % R;
+}
+
+int Model::cfg_split_forward(const CfgHalfRows* rows, const int* domain_ids, int F, int h, int w, int R, bool neg_const,
+                             cudaStream_t stream, const bf16** noise) {
+  const bool pose = cfg_.enable_pose_encoder != 0;
+  const int Co = cfg_.out_channels, Fr = F / R, world = xch_.world;
+  const size_t hw = static_cast<size_t>(h) * w;
+  int k0, k1, r;
+  cfg_cell(R, &k0, &k1, &r);
+  for (int k = k0; k < k1; ++k) {
+    const int F_total = R > 1 ? F : 0, pose_neg = pose && neg_const && k == 0 ? Fr : 0, kv_world = R > 1 ? R : 0;
+    Plan* p = nullptr;  // built by cfg_split_prepare
+    if (int rc = get_plan(domain_ids + k, 1, Fr, Fr, h, w, &p, F_total, pose_neg, kv_world)) return rc;
+    // the noise goes to the exchange buffer parity that follows the forward's n3d K/V exchanges, on every rank
+    const unsigned int e = xch_.epoch_base + static_cast<unsigned int>(p->n3d);
+    NchwDst dst = {};
+    dst.n = world;
+    for (int g = 0; g < world; ++g)
+      dst.p[g] = static_cast<bf16*>(xch_.peer_kv[e & 1][g]) + (static_cast<size_t>(k) * F + r * Fr) * Co * hw;
+    if (int rc = forward(rows[k].sample, rows[k].timestep, rows[k].skeletons, domain_ids + k, 1, Fr, Fr, h, w, dst, stream,
+                         F_total, pose_neg, kv_world))
+      return rc;
+  }
+  const unsigned int e = xch_.epoch_base;  // the exchange the flag round closes: the noise's buffer parity
+  if (int rc = flag_round(stream)) return rc;
+  *noise = static_cast<const bf16*>(xch_.kv[e & 1]);
+  return 0;
+}
+
+int Model::unet_forward_cfg(const bf16* sample, const long long* timestep, const bf16* skeletons, const int* domain_ids,
+                            int n_domains, int B, int F, int h, int w, bf16* out, cudaStream_t stream, CfgMode mode) {
+  D4D_REQUIRE(sample && timestep && domain_ids && out, "null argument");
+  D4D_REQUIRE(n_domains == 1 || n_domains == 2,
+              "the CFG split / grid forward takes one domain (no CFG halves) or two (the CFG batch [F negative | F "
+              "positive]), not " + std::to_string(n_domains));
+  if (n_domains * F != B) {
+    // same message as the reference's ValueError (unet_multiview_condition.py:524-525)
+    set_error("num_frames: " + std::to_string(F) + " * len(domains): " + std::to_string(n_domains) + " != len(emb): " + std::to_string(B));
+    return 1;
+  }
+  if (int rc = cfg_world_check(mode)) return rc;
+  // no halves: every rank runs the plain forward and exchanges nothing, like the window step at guidance <= 1
+  if (n_domains == 1) return forward(sample, timestep, skeletons, domain_ids, 1, B, F, h, w, out, stream);
+  D4D_REQUIRE(!cfg_.enable_pose_encoder || skeletons != nullptr, "skeletons are required when enable_pose_encoder");
+  // B-2 cannot assume that the negative skeletons are constant: every half forwards the caller's rows (pose_neg = 0)
+  int R = 1;
+  if (int rc = cfg_split_prepare(mode, domain_ids, F, h, w, false, &R)) return rc;
+  D4D_CUDA_OK(cudaSetDevice(device_));
+  const size_t hw = static_cast<size_t>(h) * w;
+  const int Fr = F / R;
+  int k0, k1, r;
+  cfg_cell(R, &k0, &k1, &r);
+  CfgHalfRows rows[2];
+  for (int k = k0; k < k1; ++k) {
+    const size_t row = static_cast<size_t>(k) * F + static_cast<size_t>(r) * Fr;  // grid_noise_rows's first row
+    rows[k].sample = sample + row * cfg_.in_channels * hw;
+    rows[k].timestep = timestep + row;
+    if (cfg_.enable_pose_encoder) rows[k].skeletons = skeletons + row * 3 * 64 * hw;
+  }
+  const bf16* noise = nullptr;
+  if (int rc = cfg_split_forward(rows, domain_ids, F, h, w, R, false, stream, &noise)) return rc;
+  // Write-after-read (DESIGN.md section 7): `noise` is parity e & 1 of this rank's exchange buffer, and the next write to
+  // it by any rank is exchange e + 2, which waits for this rank's signal of exchange e + 1.  That signal is enqueued on
+  // this stream after the copy, so no rank can overwrite the rows before they are read.
+  D4D_CUDA_OK(cudaMemcpyAsync(out, noise, sizeof(bf16) * B * cfg_.out_channels * hw, cudaMemcpyDeviceToDevice, stream));
+  return 0;
 }
 
 // One more exchange of the global epoch sequence (DESIGN.md section 7): counter e = epoch_base stores into parity e & 1 of

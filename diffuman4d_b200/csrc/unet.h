@@ -137,6 +137,14 @@ struct WindowStep {
 // ranks k*R .. k*R + R - 1 of half k (kGrid, the CFG grid; with R = 1 it is the CFG split).
 enum class CfgMode { kWhole, kSplit, kGrid };
 
+// The rows of one CFG half that a rank of the CFG split / grid forwards: sample [n, Cin, h, w], timestep [n] and, with the
+// pose encoder, skeletons [n, 3, 8h, 8w], n = F / R (its frame shard of the half's F frames).
+struct CfgHalfRows {
+  const bf16* sample = nullptr;
+  const long long* timestep = nullptr;
+  const bf16* skeletons = nullptr;
+};
+
 struct Exchange {  // K/V exchange buffers in peer memory (cudaIpc), two parities
   bool ready = false;
   int rank = 0, world = 1;
@@ -172,6 +180,11 @@ class Model {
   int denoise_window(bf16* latents, const bf16* pixel, const bf16* plucker, const bf16* skeletons, const bf16* mask,
                      long long* ts_idx, const WindowStep& step, float guidance, int domain, int F, int h, int w,
                      int num_steps, cudaStream_t stream, int F_total, CfgMode mode = CfgMode::kWhole);
+  // B-2 on the CFG split (kSplit) or grid (kGrid): sample [B, Cin, h, w] is the reference's batch, and every rank gets the
+  // whole noise [B, out_channels, h, w] in `out`.  n_domains 2: [F negative | F positive]; this rank forwards its rows
+  // (cfg_split_forward) and the gathered noise is copied out.  n_domains 1: the plain forward, nothing exchanged.
+  int unet_forward_cfg(const bf16* sample, const long long* timestep, const bf16* skeletons, const int* domain_ids,
+                       int n_domains, int B, int F, int h, int w, bf16* out, cudaStream_t stream, CfgMode mode);
   // frame-sharded sliding loop: this rank's F updated frames (+ DPM-Solver++ state when x0_prev != nullptr) to every rank,
   // one flag round (one more exchange of the epoch sequence), then the gathered F_total frames to the *_out buffers
   int window_exchange(const bf16* latents, const long long* ts_idx, const bf16* x0_prev, const int* lower_order_nums, int F,
@@ -223,6 +236,21 @@ class Model {
               cudaStream_t stream, bool timed = false);
   // closes exchange epoch_base: signal it to every rank, count it, wait for every rank's signal
   int flag_round(cudaStream_t stream);
+  // The CFG split / grid forward of F frames per CFG half (domain_ids[k]: half k's domain), before any launch: the
+  // mode's world, F divisible by R, the noise within the exchange buffer, and this rank's plans built (a grid plan
+  // refuses a K/V buffer too small for one half's 3-D layers).  *R: the frame shards per half.  neg_const: the negative
+  // half's skeletons are one constant image, encoded once (the window step); otherwise the caller's rows.
+  int cfg_split_prepare(CfgMode mode, const int* domain_ids, int F, int h, int w, bool neg_const, int* R);
+  // the worlds a mode runs: the split 1 (loopback) or 2 ranks, the grid 1, 2, 4, 6 or 8
+  int cfg_world_check(CfgMode mode) const;
+  // the CFG halves [k0, k1) this rank forwards (both on a loopback) and its frame shard r of R per half
+  void cfg_cell(int R, int* k0, int* k1, int* r) const;
+  // The UNet on rows[k] for each half k this rank runs, each half's noise stored at rows [k*F + r*F/R, k*F + (r+1)*F/R)
+  // of every rank's exchange buffer, then one flag round.  *noise: this rank's buffer that holds the gathered
+  // [2F, out_channels, h, w] noise; reads of it enqueued before this rank's next exchange signal are safe (DESIGN.md
+  // section 7).
+  int cfg_split_forward(const CfgHalfRows* rows, const int* domain_ids, int F, int h, int w, int R, bool neg_const,
+                        cudaStream_t stream, const bf16** noise);
   int cin_pad() const { return 16; }
   int kp_in() const { return 192; }
 };

@@ -9,7 +9,7 @@ from __future__ import annotations
 
 import ctypes as C
 from types import SimpleNamespace
-from typing import Dict, List, Optional, Union
+from typing import Callable, Dict, List, Optional, Union
 
 import torch
 
@@ -123,9 +123,12 @@ class B200MultiviewUNet:
 
     __call__ = forward
 
-    def _forward(self, sample, timestep, skeletons, domains, num_frames: int, F_total: Optional[int] = None):
+    def _forward(self, sample, timestep, skeletons, domains, num_frames: int, F_total: Optional[int] = None,
+                 cfg_entry: Optional[str] = None, cfg_check: Optional[Callable[[int, int, int, int], None]] = None):
         """``forward``'s checks and library call.  ``F_total`` given: ``num_frames`` are this rank's frames of a
-        frame-sharded window of ``F_total`` frames (``FrameShardedPipeline.unet_forward``)."""
+        frame-sharded window of ``F_total`` frames (``FrameShardedPipeline.unet_forward``).  ``cfg_entry`` given: the
+        CFG split or grid entry point with ``forward``'s arguments (``CFGSplitPipeline.unet_forward``), after
+        ``cfg_check(n_domains, num_frames, H, W)`` has raised whatever that entry point would refuse."""
         cfg = self.config
         if not torch.is_tensor(sample) or sample.dim() != 4:
             raise ValueError("sample must be [B, C, H, W]")
@@ -142,6 +145,8 @@ class B200MultiviewUNet:
             dom = (C.c_int32 * len(domains))(*[_DOMAIN_IDS[d] for d in domains])
         except KeyError as e:
             raise ValueError(f"Invalid domain for temporal embedding: {e.args[0]}") from None
+        if cfg_check is not None:
+            cfg_check(len(domains), num_frames, H, W)
         if not torch.is_tensor(timestep):
             timestep = torch.tensor([timestep], dtype=torch.int64, device=self._device)
         timestep = timestep.to(device=self._device, dtype=torch.int64).reshape(-1)
@@ -161,7 +166,10 @@ class B200MultiviewUNet:
         out = torch.empty(B, cfg.out_channels, H, W, device=self._device, dtype=torch.bfloat16)
         with torch.cuda.device(self._device):
             stream = torch.cuda.current_stream().cuda_stream
-            if F_total is None:
+            if cfg_entry is not None:
+                check(getattr(lib(), cfg_entry)(self._h, sample.data_ptr(), timestep.data_ptr(), sk, dom, len(domains),
+                                                B, num_frames, H, W, out.data_ptr(), stream), cfg_entry)
+            elif F_total is None:
                 check(lib().d4d_unet_forward(self._h, sample.data_ptr(), timestep.data_ptr(), sk, dom, len(domains), B,
                                              num_frames, H, W, out.data_ptr(), stream), "d4d_unet_forward")
             else:

@@ -647,6 +647,27 @@ int d4d_denoise_window_ddpm_cfg_grid(d4d_handle* h, void* latents, const void* p
                                      const d4d_ddpm_sched* sched, float guidance_scale, int domain, int F, int height,
                                      int width, int num_steps, const int64_t* frame_ids, void* stream);
 
+/* ---- multi-GPU: the UNet alone on the CFG split and the CFG grid (d4d_version() 116 and later) ------------------------
+ * B-2 (a drop-in pipeline.unet) on the ranks of the CFG split or grid, for callers that run their own scheduler loop.  The
+ * arguments are d4d_unet_forward's, and so is the result: every rank gets the whole noise out [B, out_channels, h, w].
+ *   - n_domains == 2: the reference's CFG batch, [F negative | F positive] images, half k of domain domain_ids[k].  Rank g
+ *     forwards rows [k*F + r*F/R, k*F + (r+1)*F/R) of sample, timestep and skeletons (k, r and R as for the CFG grid; the
+ *     split is R = 1; a loopback, world 1, forwards all 2F rows) and stores their noise into every rank's exchange buffer;
+ *     one flag round publishes it, and the gathered noise is copied into out.  The negative half's skeletons are the
+ *     caller's rows, not assumed constant.  Needs d4d_exchange_open first.
+ *   - n_domains == 1: no CFG halves; every rank runs d4d_unet_forward on the whole batch and exchanges nothing.
+ *   - SPMD: every rank makes the same calls with the same (whole-batch) arguments; the result is bit-identical to
+ *     d4d_unet_forward on one GPU on every rank.
+ *   - Returns 1 before any launch for n_domains other than 1 or 2, B != n_domains * F, a world the mode does not run
+ *     (split: 1 or 2; grid: 1, 2, 4, 6 or 8), and with n_domains == 2 for F not divisible by R or noise
+ *     (2 * F * out_channels * h * w bf16) larger than the exchange buffer. */
+int d4d_unet_forward_cfg_split(d4d_handle* h, const void* sample, const int64_t* timestep, const void* skeletons,
+                               const int32_t* domain_ids, int n_domains, int B, int F, int height, int width, void* out,
+                               void* stream);
+int d4d_unet_forward_cfg_grid(d4d_handle* h, const void* sample, const int64_t* timestep, const void* skeletons,
+                              const int32_t* domain_ids, int n_domains, int B, int F, int height, int width, void* out,
+                              void* stream);
+
 #ifdef __cplusplus
 }
 #endif
